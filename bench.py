@@ -211,7 +211,7 @@ def _peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback 6650 GB/s (B200_PROFILING.md)"
+        return 3350.0, "fallback 3350 GB/s (H100 SXM data sheet, HBM3)"
 
 
 # Algorithmic bytes per launch of each kernel of the JPEG path, per image of the megabatch (DESIGN.md 4; px = pixels of the image,
@@ -301,7 +301,21 @@ def jpeg_e2e_only(args, L, torch, dist, world, datas, params, threads, e2e_threa
     return {"value": e2e["value"], "ms_total": 0.0, "launches": 0, "roofline": None, "e2e": e2e, "not_settled": 0, "encoder_retries": 0, "out_bytes_per_image": 0, "in_bytes_per_image": 0}
 
 
-def jpeg_workload(args, L, torch, dist, world, rank, datas, params, lossless, threads, e2e_threads, with_kernels=True):
+DUMP_SAMPLE = 4          # output files written in full by --dump-outputs (a seeded choice among the batch)
+
+
+def dump_pipe_outputs(pipe, sizes, out_dir):
+    """What a caller of the resident pipe receives after the last timed step: every image's output size and, for a fixed
+    seeded sample of images, the whole output JPEG file (bytes as float32, at most a few MB each)."""
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "jpeg_out_sizes.npy"), np.asarray(sizes, dtype=np.float64))
+    pick = np.sort(np.random.default_rng(0).choice(len(sizes), size=min(DUMP_SAMPLE, len(sizes)), replace=False))
+    for i in pick:
+        f = np.frombuffer(pipe.fetch(int(i)), dtype=np.uint8)
+        np.save(os.path.join(out_dir, f"jpeg_out_{int(i):04d}.npy"), f.astype(np.float32))
+
+
+def jpeg_workload(args, L, torch, dist, world, rank, datas, params, lossless, threads, e2e_threads, with_kernels=True, dump_dir=None):
     """Resident full-path rate (`value`), per-kernel table, and the C-ABI rate (`e2e`) of one JPEG re-encode configuration."""
     px = W4K * H4K
     B = args.batch
@@ -312,6 +326,8 @@ def jpeg_workload(args, L, torch, dist, world, rank, datas, params, lossless, th
     pipe = L.JpegPipe(work, params, group=args.group)
     ms_total, launches = time_pipe(torch, dist, world, pipe, stream, args.steps, args.warmup)
     sizes, not_settled, retries = pipe.finish()
+    if dump_dir and rank == 0:
+        dump_pipe_outputs(pipe, sizes, dump_dir)
     value = world * B * MP_PER_IMAGE * args.steps / (ms_total / 1e3)
     if args.only_value:
         if rank == 0:
@@ -442,11 +458,11 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--batch", type=int, default=128, help="images per step per GPU, device-resident leg (128 x ~1.5 MB of scan bytes > L2)")
     ap.add_argument("--group", type=int, default=8, help="images per launch sequence (megabatch) in the device-resident leg")
-    ap.add_argument("--e2e-batch", type=int, default=1024, help="images per step per GPU (C-ABI leg); one blocking b200_compress_batch call per step, so every step pays one pipeline fill and drain (~8 ms): 256 images per step under-reports the steady-state rate by ~10 %")
+    ap.add_argument("--e2e-batch", type=int, default=1024, help="images per step per GPU (C-ABI leg); one blocking b200_compress_batch call per step, so every step pays one pipeline fill and drain: a small batch under-reports the steady-state rate")
     ap.add_argument("--unique", type=int, default=64, help="unique synthetic sources per rank, cycled to fill a batch")
     ap.add_argument("--configs", default=None, help="comma list of BASELINE configs to run (1 = the headline; 2,3,4 = sub-records); default 1,2,3,4 on one GPU, 1 under torchrun")
     ap.add_argument("--png-unique", type=int, default=4); ap.add_argument("--png-batch", type=int, default=64)
-    ap.add_argument("--png-threads", type=int, default=0, help="callers in flight for the PNG leg (default: twice the usable cores, 16..48: a caller spends 0.2 s inflating on its core and then waits for its share of the device, which is the bound -- measured 16 / 24 / 32 / 48 callers: 429 / 466 / 479 / 493 MP/s)")
+    ap.add_argument("--png-threads", type=int, default=0, help="callers in flight for the PNG leg (default: twice the usable cores, 16..24: a caller spends its inflate on its core and then waits for its share of the device, which is the bound; each caller's slot holds ~2.6 GB of device buffers for a 4096x4096 image, so 24 stay well inside the H100's 80 GB)")
     ap.add_argument("--webp-unique", type=int, default=8); ap.add_argument("--webp-batch", type=int, default=64)
     ap.add_argument("--cpu-seconds", type=float, default=6.0, help="minimum CPU work per cpu_baseline sample")
     ap.add_argument("--skip-cpu-baseline", action="store_true")
@@ -454,6 +470,7 @@ def main():
     ap.add_argument("--only-e2e", action="store_true", help="diagnostics: skip the device-resident leg and the per-kernel table")
     ap.add_argument("--only-value", action="store_true", help="diagnostics: the device-resident leg only (prints a short JSON line)")
     ap.add_argument("--only-configs", action="store_true", help="diagnostics: skip configs[1]; prints {\"configs\": {...}} for the sub-records named by --configs")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None, help="after the timed steps of configs[1], write rank 0's outputs of the last step as DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     rank, world, local_rank = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
@@ -481,7 +498,7 @@ def main():
     L = load_pkg()
     torch.cuda.set_device(local_rank)
     if L.lib().b200_init_device(local_rank) != 0:
-        raise SystemExit("bench.py: no B200 visible -- the product has no CPU fallback")
+        raise SystemExit("bench.py: no H100 visible -- the product has no CPU fallback")
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     # quant tables: computed on rank 0, broadcast over NCCL (the only collective of this path), checked locally
@@ -493,7 +510,7 @@ def main():
 
     clocks = ClockSampler(local_rank)
     clocks.start()
-    r1 = None if args.only_configs else jpeg_workload(args, L, torch, dist, world, rank, datas, p, False, threads, e2e_threads)
+    r1 = None if args.only_configs else jpeg_workload(args, L, torch, dist, world, rank, datas, p, False, threads, e2e_threads, dump_dir=args.dump_outputs)
     clk = clocks.stop()
 
     sub = {}
@@ -513,11 +530,13 @@ def main():
                 rec["cpu_baseline"] = {"value": round(v, 2), "unit": "MP/s", "cores": cores, "kind": "port", "sample": f"{k} of the same 4K inputs, {cores} threads, oracle jpeg_lossless, {cdt:.1f} s"}
             sub["2"] = rec
         if 3 in which:
+            release_slots(L, local_rank)
             rec, _ = config_png_run(args, L, cores, png_datas)
             if not args.skip_cpu_baseline:
                 rec["cpu_baseline"] = cpu_png(png_datas, L, cores, args.cpu_seconds)
             sub["3"] = rec
         if 4 in which:
+            release_slots(L, local_rank)
             rec, _ = config_webp_run(args, L, cores, webp_datas)
             if not args.skip_cpu_baseline:
                 rec["cpu_baseline"] = cpu_webp(webp_datas, cores, args.cpu_seconds)
@@ -540,7 +559,7 @@ def main():
             "config": {"workload": "configs[1]: 3840x2160 RGB JPEG q90 4:2:0 -> -q 80 --jpeg-chroma-subsampling 4:2:0 (progressive, optimised Huffman)",
                        "value_scope": "FULL device path, inputs resident: entropy-coded scans in HBM -> Huffman decode -> K1-K5 transform -> Huffman encode -> entropy-coded scans in HBM (b200_jpeg_pipe_*); no host wait inside the timed region",
                        "images_per_step_per_gpu": B, "megabatch": args.group, "unique_sources_per_gpu": len(datas), "parallelism": f"dp{world} (images sharded, no collective on the path)",
-                       "l2": f"per step and GPU {B * r1['in_bytes_per_image'] / 1e6:.0f} MB of scan bytes are read and {B * 2 * W4K * H4K * 3 / 1e9:.1f} GB of coefficients pass through HBM (L2 = 126 MB): nothing of a step survives in L2 to the next"},
+                       "l2": f"per step and GPU {B * r1['in_bytes_per_image'] / 1e6:.0f} MB of scan bytes are read and {B * 2 * W4K * H4K * 3 / 1e9:.1f} GB of coefficients pass through HBM (H100 L2 = 50 MB): nothing of a step survives in L2 to the next"},
             "images_per_sec": round(r1["value"] / MP_PER_IMAGE, 1),
             "e2e": r1["e2e"], "gpu_launches": r1["launches"] * args.steps, "roofline": r1["roofline"], "cpu_baseline": cpu, "clocks": clk,
             "decoder_not_settled": r1["not_settled"], "encoder_retries": r1["encoder_retries"],
@@ -552,16 +571,24 @@ def main():
         dist.destroy_process_group()
 
 
+def release_slots(L, device):
+    """Free the device buffers the previous legs' slots keep (they only grow): each leg then starts from its own footprint,
+    which the 80 GB of an H100 needs when a PNG and a JPEG leg would otherwise share the same slots."""
+    L.lib().b200_shutdown()
+    if L.lib().b200_init_device(device) != 0:
+        raise SystemExit("bench.py: re-initialising the device failed")
+
+
 def config_png_run(args, L, cores, datas):
     w = h = 4096
     mp = w * h / 1e6
     p = L.default_params(); p.png_optimize = 1; p.png_optimization_level = 3
     n = args.png_batch
     work = [datas[i % len(datas)] for i in range(n)]
-    nt = args.png_threads if args.png_threads > 0 else min(48, max(2 * cores, 16))
+    nt = args.png_threads if args.png_threads > 0 else min(24, max(2 * cores, 16))
     L.compress_batch(work[:min(n, nt)], p, nt, copy=False)
     bi = L.BatchInputs(work)
-    steps = max(1, args.steps // 5)
+    steps = args.steps
     t0 = time.perf_counter()
     out_bytes = 0
     for _ in range(steps):
@@ -592,7 +619,7 @@ def config_webp_run(args, L, cores, datas):
     nt = max(cores, 16)
     with ThreadPoolExecutor(nt) as ex:
         list(ex.map(conv, work[:nt]))
-        steps = max(1, args.steps // 3)
+        steps = args.steps
         d2h0 = L.lib().b200_webp_d2h_bytes()
         t0 = time.perf_counter()
         out_bytes = 0

@@ -1,8 +1,8 @@
 """ctypes binding of libb200caesium.so (include/b200_caesium.h).
 
 This is the only way Python code in this repo reaches the product: through the same C-ABI a
-Rust maintainer would bind at /root/reference/src/compressor.rs:287-306.  There is no Python or
-CPU fallback -- if the shared library is missing, loading raises; if no B200 is visible, every
+Rust maintainer would bind at caesium-clt's src/compressor.rs:287-306.  There is no Python or
+CPU fallback -- if the shared library is missing, loading raises; if no H100 is visible, every
 codec call returns B200_ERR_NO_DEVICE.
 """
 import ctypes as C
@@ -50,7 +50,7 @@ class B200Error(RuntimeError):
 
 
 def build(force=False):
-    """Compile the CUDA + C++ sources in-tree (nvcc -gencode arch=compute_100a,code=sm_100a)."""
+    """Compile the CUDA + C++ sources in-tree (nvcc -gencode arch=compute_90a,code=sm_90a)."""
     if force:
         subprocess.check_call(["make", "-C", _HERE, "-s", "clean"])
     subprocess.check_call(["make", "-C", _HERE, "-s", "-j8"])

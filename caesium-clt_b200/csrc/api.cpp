@@ -1,6 +1,6 @@
 // api.cpp -- the C-ABI of include/b200_caesium.h: format dispatch, parameter mapping and error mapping that
 // libcaesium's lib.rs performs behind caesium::{compress,convert,compress_to_size}_in_memory
-// (call sites /root/reference/src/compressor.rs:287-306).  No CPU codec fallback exists anywhere below.
+// (call sites caesium-clt's src/compressor.rs:287-306).  No CPU codec fallback exists anywhere below.
 #include "../../include/b200_caesium.h"
 #include <atomic>
 #include <chrono>
@@ -49,16 +49,18 @@ b200_status make_status(int code, const std::string &msg)
 // a header the reader refused: RGB-coded sources are "recognised but not on this path" (code 3), everything else is corrupt input
 b200_status header_status(const std::string &err) { return make_status(err.compare(0, 9, "RGB-coded") == 0 ? B200_ERR_UNSUPPORTED : B200_ERR_CORRUPT_INPUT, err); }
 
-std::once_flag g_once;
-std::string g_init_err;
 int g_forced_device = -1, g_forced_ngpus = 0;
 std::atomic<int> g_entropy_mode{-1};     // -1 unset (env B200_ENTROPY); bit 0 = device entropy encoder, bit 1 = device entropy decoder (default 3)
 
+// runtime_init is idempotent while initialised, so after b200_shutdown (which frees every slot's device buffers) the next call
+// initialises again: a long-running host can hand the memory of one workload's slots back before starting another
 bool ensure_runtime(std::string &err)
 {
-    std::call_once(g_once, [] { runtime_init(g_forced_ngpus, g_forced_device, g_init_err); });
-    if (runtime_device_count() <= 0) { err = g_init_err.empty() ? "no CUDA device available; this build has no CPU fallback" : g_init_err; return false; }
-    return true;
+    if (runtime_device_count() > 0) return true;
+    std::string e;
+    if (runtime_init(g_forced_ngpus, g_forced_device, e) > 0) return true;
+    err = e.empty() ? "no CUDA device available; this build has no CPU fallback" : e;
+    return false;
 }
 
 void layout_from_geom(const JpegGeom &g, b200_jpeg_layout *l)
@@ -816,7 +818,7 @@ void b200_shutdown(void) { print_trace(); runtime_shutdown(); }
 int b200_device_count(void) { return runtime_device_count(); }
 long long b200_device_jobs(int index) { return runtime_device_jobs(index); }
 int b200_device_numa_node(int index) { return index < 0 || index >= runtime_device_count() ? -1 : device_numa_node(runtime_device_ordinal(index)); }
-const char *b200_version(void) { return "b200-caesium 0.1.0 (sm_100a)"; }
+const char *b200_version(void) { return "b200-caesium 0.1.0 (sm_90a)"; }
 void b200_free(void *p) { free(p); }
 int b200_set_entropy_mode(int mode) { if (mode < 0 || mode > 3) return B200_ERR_INVALID_ARGUMENT; g_entropy_mode.store(mode); return B200_OK; }
 

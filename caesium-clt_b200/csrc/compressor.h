@@ -1,4 +1,4 @@
-// compressor.h -- C++ mirror of caesiumclt's host side around the codec boundary (/root/reference/src/compressor.rs).
+// compressor.h -- C++ mirror of caesiumclt's host side around the codec boundary (caesium-clt's src/compressor.rs).
 // The reference host is Rust; no cargo/rustc exists in this image, so the same interface is kept here in C++ (same
 // names, argument meaning, messages and policies) on top of the C-ABI, for the b200clt CLI and the tests.  A Rust
 // maintainer keeps the original file and swaps only the three caesium::* calls (INTEGRATION.md).

@@ -1,5 +1,5 @@
 // compressor_c.cpp -- plain-C hooks over the C++ host mirror (compressor.h) so the Python tests can drive the same
-// cases the reference's inline unit tests cover (/root/reference/src/compressor.rs:607-1109).  Built into libb200clt.so.
+// cases the reference's inline unit tests cover (caesium-clt's src/compressor.rs:607-1109).  Built into libb200clt.so.
 #include <cstring>
 #include <string>
 #include "compressor.h"

@@ -1,5 +1,5 @@
 // dfl_core.h -- the DEFLATE block coder of the lossless PNG path (libcaesium png::lossless -> oxipng -> deflate,
-// /root/reference/src/compressor.rs:428,436-437) written ONCE as __host__ __device__ code: png_host.cpp's deflate_tokens()
+// caesium-clt's src/compressor.rs:428,436-437) written ONCE as __host__ __device__ code: png_host.cpp's deflate_tokens()
 // (the CPU writer, and the twin the GPU tests compare against) and png_deflate.cu's kernels (the device writer) run the same
 // bodies, so their output is identical bit for bit.  Per block of tokens: symbol statistics -> length-limited Huffman code
 // lengths (limit 15, code-length code limit 7) -> canonical codes (stored bit-reversed for LSB-first output) -> the dynamic

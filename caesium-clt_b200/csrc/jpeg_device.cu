@@ -1,5 +1,5 @@
 // jpeg_device.cu -- see jpeg_device.h.  Device runtime for the JPEG path of caesium::compress_in_memory
-// (/root/reference/src/compressor.rs:305): one pool of "slots" per GPU so that the blocking, one-image-per-thread
+// (caesium-clt's src/compressor.rs:305): one pool of "slots" per GPU so that the blocking, one-image-per-thread
 // callers of the reference's rayon map (compressor.rs:81-83) each get a private stream, pinned staging buffers and
 // HBM buffers; images are sharded round-robin over the initialised GPUs (no cross-GPU traffic on this path).
 #include <cuda_runtime.h>
@@ -155,7 +155,7 @@ int runtime_init(int n_gpus, int only_device, std::string &err)
         if (blocking && cudaSetDevice(o) == cudaSuccess) { cudaSetDeviceFlags(cudaDeviceScheduleBlockingSync); cudaGetLastError(); }
         cudaDeviceProp prop;
         if (cudaGetDeviceProperties(&prop, o) != cudaSuccess) { err = "cudaGetDeviceProperties failed"; return 0; }
-        if (prop.major != 10) { err = "device " + std::to_string(o) + " is sm_" + std::to_string(prop.major) + std::to_string(prop.minor) + "; this library ships sm_100a kernels only"; for (auto *d : g_devs) delete d; g_devs.clear(); return 0; }
+        if (prop.major != 9 || prop.minor != 0) { err = "device " + std::to_string(o) + " is sm_" + std::to_string(prop.major) + std::to_string(prop.minor) + "; this library ships sm_90a kernels only"; for (auto *d : g_devs) delete d; g_devs.clear(); return 0; }
         auto *d = new DevicePool(); d->ordinal = o; g_devs.push_back(d);
     }
     g_inited = true;

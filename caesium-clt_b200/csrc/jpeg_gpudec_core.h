@@ -1,7 +1,7 @@
 // jpeg_gpudec_core.h -- parallel decoding of a baseline (sequential Huffman, single interleaved or single-component
 // scan, no restart markers) JPEG entropy-coded segment, written as __host__ __device__ code shared by the CUDA kernels
 // (jpeg_gpudec.cu) and the serial CPU emulation in tests/emul/.  This is the decode half of SURVEY.md §8f rank 1; it
-// replaces the host's jdhuff.c-style loop in front of caesium::compress_in_memory (/root/reference/src/compressor.rs:305).
+// replaces the host's jdhuff.c-style loop in front of caesium::compress_in_memory (caesium-clt's src/compressor.rs:305).
 //
 // Method (self-synchronising Huffman decoding, Klein & Wiseman 2003; Weissenberger & Schmidt 2018): the unstuffed bit
 // stream is cut into subsequences of SUBSEQ_BITS bits.  A decoder state is (p, k, b) = bit position of the next

@@ -2,7 +2,7 @@
 // optimised Huffman tables), written once as __host__ __device__ code: jpeg_gpuenc.cu wraps these bodies in CUDA
 // kernels; tests/emul/ runs the very same bodies in plain loops on the CPU to validate the formulation without a GPU.
 // This is SURVEY.md §8f rank 1 ("GPU-side Huffman encode"): it removes the host entropy-coding wall behind
-// caesium::compress_in_memory (/root/reference/src/compressor.rs:305).  Output bits are identical to jpeg_host.cpp's
+// caesium::compress_in_memory (caesium-clt's src/compressor.rs:305).  Output bits are identical to jpeg_host.cpp's
 // sequential writer (and therefore to oracle/jpeg_oracle.c).
 //
 // Formulation.  A scan is a sequence of blocks j = 0..n-1 in scan order.  Each block owns up to three consecutive

@@ -1,5 +1,5 @@
 // jpeg_host.cpp -- see jpeg_host.h.  Upstream behaviour restated (mozjpeg 4.x via mozjpeg-sys 2.2.1,
-// /root/reference/Cargo.lock:1035; reached from /root/reference/src/compressor.rs:305): jdmarker.c (markers),
+// caesium-clt's Cargo.lock:1035; reached from caesium-clt's src/compressor.rs:305): jdmarker.c (markers),
 // jdhuff.c / jdphuff.c (entropy decode), jchuff.c / jcphuff.c (entropy encode, optimised tables),
 // jcmarker.c (file layout), jccoefct.c / jctrans.c (dummy blocks), jcparam.c (quality scaling, sampling).
 #include "jpeg_host.h"

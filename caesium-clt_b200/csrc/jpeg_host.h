@@ -1,7 +1,7 @@
 // jpeg_host.h -- host half of the JPEG path: marker parsing, Huffman decode to zigzag coefficient
 // buffers, and Huffman encode from them (entropy coding stays on the host per BASELINE.json's north_star;
 // it is what mozjpeg's jdhuff.c/jdphuff.c/jchuff.c/jcphuff.c do below caesium::compress_in_memory,
-// /root/reference/src/compressor.rs:305).  Written for throughput: 64-bit bit buffers, lookahead tables,
+// caesium-clt's src/compressor.rs:305).  Written for throughput: 64-bit bit buffers, lookahead tables,
 // token streams shared by the statistics and emission passes.
 #pragma once
 #include <cstdint>

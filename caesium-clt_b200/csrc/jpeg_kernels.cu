@@ -1,5 +1,5 @@
-// jpeg_kernels.cu -- hand-written sm_100a kernels for the JPEG transform stages of
-// caesium::compress_in_memory (call site /root/reference/src/compressor.rs:305; SURVEY.md §8a row a6):
+// jpeg_kernels.cu -- hand-written sm_90a kernels for the JPEG transform stages of
+// caesium::compress_in_memory (call site caesium-clt's src/compressor.rs:305; SURVEY.md §8a row a6):
 //   K1 dequantise + 8x8 inverse DCT          K2 chroma upsample ("fancy" triangle filter)
 //   K4 chroma box downsample                 K5 forward DCT + quantise + zigzag
 // and the fusions the no-resize path uses (K1->K5 for full-resolution components, K2->K4->K5 for 4:2:0 chroma).

@@ -4,7 +4,7 @@
 // on a set of streams, without a single host wait: scan bytes in HBM -> scan bytes in HBM.  This is what bench.py reports as
 // `value` (SURVEY.md 8d: inputs resident when the timed region starts); b200_compress_batch runs the same launch sequences with
 // the H2D / D2H copies and the file assembly around them (bench.py's `e2e`).  Reference path: caesium::compress_in_memory,
-// /root/reference/src/compressor.rs:305.
+// caesium-clt's src/compressor.rs:305.
 #include <cuda_runtime.h>
 #include <map>
 #include <memory>

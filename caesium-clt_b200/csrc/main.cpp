@@ -1,4 +1,4 @@
-// main.cpp -- b200clt: a C++ stand-in for caesiumclt's main.rs (flags of /root/reference/src/options.rs:47-190,
+// main.cpp -- b200clt: a C++ stand-in for caesiumclt's main.rs (flags of caesium-clt's src/options.rs:47-190,
 // flow of main.rs:43-113, JSON of main.rs:15-34,164-187) so the drop-in path can be exercised end to end on boxes
 // without a Rust toolchain.  Presentation (progress bars, colours) is deliberately not reproduced.
 #include <cerrno>
@@ -73,7 +73,7 @@ int main(int argc, char **argv)
         else if (a == "--strip-icc") o.strip_icc = true;
         else if (a == "--min-savings") { MinSavingsThreshold t; std::string e; if (!parse_min_savings(need(i), t, e)) return usage(e.c_str()); o.min_savings = t; }
         else if (a == "--threads") threads = (int)num(i, 0, 4096);
-        else if (a == "--gpus") n_gpus = (int)num(i, 0, 64);          // extension: number of B200s to shard over (0 = all)
+        else if (a == "--gpus") n_gpus = (int)num(i, 0, 64);          // extension: number of GPUs to shard over (0 = all)
         else if (a == "--timing") timing = true;                 // extension: print MP/s to stderr
         else if (a == "--dry-run" || a == "-d") dry_run = true;
         else if (a == "-Q" || a == "--quiet") quiet = true;

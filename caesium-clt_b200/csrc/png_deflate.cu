@@ -6,7 +6,7 @@
 //   k_dfl_len     per block: bits of every 256-token chunk -> chunk offsets inside the block, block size in bits
 //   k_dfl_scan    block sizes -> start bit of every block, total size                 (one CTA)
 //   k_dfl_emit    per block: header, tokens, end-of-block code, OR-ed LSB-first into the zeroed output words
-// Reference path: caesium::compress_in_memory -> png::lossless -> oxipng (/root/reference/src/compressor.rs:428,436-437).
+// Reference path: caesium::compress_in_memory -> png::lossless -> oxipng (caesium-clt's src/compressor.rs:428,436-437).
 #include <cuda_runtime.h>
 #include <cstdint>
 #include "dfl_core.h"

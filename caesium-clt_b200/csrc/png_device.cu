@@ -1,5 +1,5 @@
 // png_device.cu -- device orchestration of the lossless PNG path (libcaesium png::lossless -> oxipng::optimize_from_memory,
-// /root/reference/src/compressor.rs:428,436-437): upload the decoded samples, apply the cheap lossless reductions
+// caesium-clt's src/compressor.rs:428,436-437): upload the decoded samples, apply the cheap lossless reductions
 // (opaque alpha, grey RGB), then for every row-filter strategy of the optimisation preset run K6 (filter) + K7 (match,
 // parse) and estimate the DEFLATE size from the token histogram; the winning strategy's tokens come back to the host,
 // which Huffman-codes and frames them (png_host.cpp).

@@ -1,5 +1,5 @@
 // png_host.h -- host half of the lossless PNG path (libcaesium png::lossless -> oxipng, reached with png.optimize == true,
-// /root/reference/src/compressor.rs:428,436-437): container parsing, inflate + unfilter of the source IDAT, and the
+// caesium-clt's src/compressor.rs:428,436-437): container parsing, inflate + unfilter of the source IDAT, and the
 // DEFLATE bit-packer (dynamic Huffman blocks) + zlib/PNG framing around the LZ77 tokens the device produces.  Row-filter
 // selection (K6) and LZ77 match finding (K7) are CUDA kernels (png_kernels.cu); entropy coding stays here.
 #pragma once

@@ -1,5 +1,5 @@
 // png_kernels.cu -- K6 (row-filter selection) and K7 (LZ77 match finding) for the lossless PNG path, SURVEY.md §8a row a8:
-// the device side of what oxipng 9.1.5 does behind libcaesium png::lossless (/root/reference/src/compressor.rs:428,
+// the device side of what oxipng 9.1.5 does behind libcaesium png::lossless (caesium-clt's src/compressor.rs:428,
 // 436-437): for every filter strategy of the optimisation preset, filter all rows and run the compressor over them.
 // Filtering reads only RAW neighbours (left, up, up-left), so unlike un-filtering it is embarrassingly parallel: one CTA
 // per row scores the five candidate filters (MinSum / Entropy / Bigrams / BigEnt heuristics as histograms in shared
@@ -636,7 +636,7 @@ int launch_png_hashmatch(const uint8_t *d_filt, uint32_t *d_best, size_t n, uint
 {
     cudaStream_t st = (cudaStream_t)stream;
     cudaMemsetAsync(d_work, 0, 256 * 4, st);
-    k_png_bytehist<<<296, 256, 0, st>>>(d_filt, n, d_work);
+    k_png_bytehist<<<264, 256, 0, st>>>(d_filt, n, d_work);          // two CTAs on each of the H100's 132 SMs
     k_png_costs<<<1, 32, 0, st>>>(d_work, n, d_work + 256);
     LT_MARK("k_png_bytehist");
     using Sort = cub::BlockRadixSort<uint16_t, HM_THREADS, HM_ITEMS, uint16_t>;

@@ -1,5 +1,5 @@
 // png_kernels.h -- launchers for K6 (PNG row-filter selection) and K7 (LZ77 match finding), SURVEY.md §8a row a8:
-// the device work of libcaesium png::lossless -> oxipng (/root/reference/src/compressor.rs:428,436-437).
+// the device work of libcaesium png::lossless -> oxipng (caesium-clt's src/compressor.rs:428,436-437).
 #pragma once
 #include <cstdint>
 #include <cstddef>

@@ -1,5 +1,5 @@
 // png_match_core.h -- K7 phase 1 (fixed pixel / row candidates, SURVEY.md §8a row a8; libcaesium png::lossless -> oxipng -> deflate,
-// /root/reference/src/compressor.rs:428,436-437) written once as __host__ __device__ code: png_kernels.cu's k_png_match and the CPU
+// caesium-clt's src/compressor.rs:428,436-437) written once as __host__ __device__ code: png_kernels.cu's k_png_match and the CPU
 // emulation in tests/emul/match_emul.cpp run the same bodies.
 //
 // One CTA owns MATCH_T consecutive positions of the filtered stream.  For every candidate distance the comparison "byte q of the

@@ -1,6 +1,6 @@
 // resize_host.cpp -- host half of K3: the per-axis tap windows and normalised Lanczos3 weights of image 0.25.9
 // imageops/sample.rs (reached via libcaesium resize::resize_image when CSParameters.width/height are set,
-// /root/reference/src/compressor.rs:439-443).  f32 throughout, libm sinf, no FMA contraction (Makefile passes
+// caesium-clt's src/compressor.rs:439-443).  f32 throughout, libm sinf, no FMA contraction (Makefile passes
 // -ffp-contract=off) so the tables match oracle/resize_oracle.c bit for bit.
 #include "resize_kernels.h"
 #include <cmath>

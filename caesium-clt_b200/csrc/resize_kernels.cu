@@ -1,6 +1,6 @@
 // resize_kernels.cu -- K3 (separable Lanczos3 resize) and the colour halves of K2/K4 (YCbCr<->RGB), SURVEY.md §8a
 // rows a6/a9: what libcaesium's resize::resize_image does through image 0.25.9 `resize_exact(.., Lanczos3)` between
-// decode and encode when CSParameters.width/height are set (/root/reference/src/compressor.rs:439-443, :503-536).
+// decode and encode when CSParameters.width/height are set (caesium-clt's src/compressor.rs:439-443, :503-536).
 // Bit-exact with oracle/resize_oracle.c: tap windows and normalised f32 weights are computed on the host with the
 // same libm calls (resize_host.cpp); the kernels accumulate taps in the same order with separately rounded multiply
 // and add (__fmul_rn/__fadd_rn: no FMA contraction), clamp and round half away from zero.  Vertical pass first into

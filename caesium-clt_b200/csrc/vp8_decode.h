@@ -1,6 +1,6 @@
 // vp8_decode.h -- host VP8 key-frame DECODER (lossy WebP input): RIFF container, RFC 6386 bitstream, reconstruction, loop filters and
 // libwebp's RGB output conversion.  libcaesium's webp::compress decodes its input before it re-encodes
-// (caesium::compress_in_memory on a .webp, /root/reference/src/compressor.rs:305; the reference's own tests require
+// (caesium::compress_in_memory on a .webp, caesium-clt's src/compressor.rs:305; the reference's own tests require
 // samples/w0.webp to succeed, :769-787): this is that decode, as format plumbing in front of the device encoder (K8) -- like the
 // PNG inflate.  Bit-exact with libwebp's decoder (tests compare against Pillow).
 #pragma once

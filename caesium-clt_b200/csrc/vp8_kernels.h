@@ -1,5 +1,5 @@
 // vp8_kernels.h -- K8: the device half of the WebP (lossy VP8 key frame) leg, SURVEY.md §8a row a10:
-// caesium::convert_in_memory(.., WebP) (/root/reference/src/compressor.rs:288-292 -> libcaesium webp::compress -> libwebp).
+// caesium::convert_in_memory(.., WebP) (caesium-clt's src/compressor.rs:288-292 -> libcaesium webp::compress -> libwebp).
 // RGB -> Y'CbCr 4:2:0, then per macroblock: intra mode choice, forward DCT/WHT, quantisation, and the decoder-exact
 // reconstruction the next macroblocks predict from.  The boolean entropy coder stays on the host (vp8_host.cpp).
 #pragma once

@@ -2,7 +2,7 @@
 // as __host__ __device__ code: the device generates the frame's decisions in parallel, one thread per macroblock (vp8_kernels.cu,
 // k_vp8_tokens), the host writer (vp8_host.cpp) runs the same bodies when it is handed levels instead of tokens (the stage entry
 // points and the CPU tests), so both produce the same decision list.  WebP leg of caesium::convert_in_memory
-// (/root/reference/src/compressor.rs:288-292 -> libcaesium webp::compress -> libwebp's token pass).
+// (caesium-clt's src/compressor.rs:288-292 -> libcaesium webp::compress -> libwebp's token pass).
 //
 // What makes the pass parallel: a block's context is "did the block above / to the left have coded coefficients", which is a
 // property of those blocks' levels alone -- a 25-bit mask per macroblock (mb_mask), computable before any token exists.  With the

@@ -1,5 +1,5 @@
 // vp8l_alpha.h -- the alpha plane of a lossy WebP: the ALPH chunk of a VP8X file (libcaesium webp::compress on an image with
-// transparency -> libwebp WebPEncodeRGBA: lossy VP8 colour + losslessly coded alpha; /root/reference/src/compressor.rs:288-292, :305).
+// transparency -> libwebp WebPEncodeRGBA: lossy VP8 colour + losslessly coded alpha; caesium-clt's src/compressor.rs:288-292, :305).
 // The plane is coded as a VP8L image stream (WebP lossless bitstream, alpha in the green channel, no transforms, no colour cache,
 // one prefix-code group) from LZ77 tokens the device's K7 kernels produce over the plane.
 #pragma once

@@ -1,6 +1,6 @@
 // vp8l_decode.cpp -- host decoder of the WebP lossless bitstream ("VP8L"): lossless WebP inputs and the alpha plane (ALPH chunk) of
 // lossy ones.  libcaesium's webp::compress decodes its input before it re-encodes (caesium::compress_in_memory on a .webp,
-// /root/reference/src/compressor.rs:305); this is that decode for the files the VP8 key-frame decoder (vp8_decode.cpp) does not
+// caesium-clt's src/compressor.rs:305); this is that decode for the files the VP8 key-frame decoder (vp8_decode.cpp) does not
 // cover -- format plumbing in front of the device encoder, like the PNG inflate.  Written from the format specification (LSB-first
 // bit reader, canonical prefix codes, LZ77 with the 120 neighbourhood distance codes, colour cache, meta prefix image, the four
 // transforms); the tests pin it against libwebp (Pillow) on lossless files and alpha planes of every flavour libwebp writes.

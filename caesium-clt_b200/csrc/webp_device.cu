@@ -1,4 +1,4 @@
-// webp_device.cu -- see webp_device.h.  caesium::convert_in_memory(.., WebP) (/root/reference/src/compressor.rs:288-292).
+// webp_device.cu -- see webp_device.h.  caesium::convert_in_memory(.., WebP) (caesium-clt's src/compressor.rs:288-292).
 #include <cuda_runtime.h>
 #include <cstring>
 #include <chrono>

@@ -1,5 +1,5 @@
 """Sharding of an image list over ranks (one process per GPU) -- the multi-GPU shape of caesiumclt's data-parallel map
-over files (/root/reference/src/compressor.rs:74-101).  Images are independent, so there is no collective on the data
+over files (caesium-clt's src/compressor.rs:74-101).  Images are independent, so there is no collective on the data
 path: each rank takes its shard, and results are put back in input order (par_iter().collect() semantics).  The only
 exchange is the one-time broadcast of the quantisation tables (a handshake, not a bandwidth operation)."""
 

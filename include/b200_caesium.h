@@ -1,9 +1,9 @@
 /*
- * b200_caesium.h -- C-ABI of libb200caesium.so, the B200-native replacement for the
+ * b200_caesium.h -- C-ABI of libb200caesium.so, the H100-native replacement for the
  * `libcaesium` crate calls made by caesiumclt's per-image hot path.
  *
  * The reference has no FFI of its own; the seam is the Rust crate boundary in
- * /root/reference/src/compressor.rs:287-306:
+ * caesium-clt's src/compressor.rs:287-306:
  *     caesium::compress_in_memory(Vec<u8>, &CSParameters)                        (compressor.rs:305)
  *     caesium::convert_in_memory(Vec<u8>, &CSParameters, SupportedFileTypes)     (compressor.rs:289,300)
  *     caesium::compress_to_size_in_memory(Vec<u8>, &mut CSParameters, usize, bool)(compressor.rs:295,298)
@@ -31,7 +31,7 @@ enum {
     B200_ERR_UNSUPPORTED = 3,        /* recognised, but this path is not implemented on the GPU build:
                                         the Rust host may route the file to caesium::* instead */
     B200_ERR_CORRUPT_INPUT = 4,
-    B200_ERR_NO_DEVICE = 5,          /* no CUDA device / sm_100a image -- there is NO CPU fallback */
+    B200_ERR_NO_DEVICE = 5,          /* no CUDA device / sm_90a image -- there is NO CPU fallback */
     B200_ERR_CUDA = 6,
     B200_ERR_OUT_OF_MEMORY = 7,
     B200_ERR_SAME_FORMAT = 8,        /* convert_in_memory asked for the input's own format */
@@ -77,6 +77,7 @@ void b200_params_default(b200_params *p);
 int  b200_init(int n_gpus);
 /* One-process-per-GPU launchers (torchrun): bind the library to exactly this CUDA ordinal. */
 int  b200_init_device(int device_ordinal);
+/* Frees every slot (streams, pinned and device buffers).  Calls made afterwards initialise the library again. */
 void b200_shutdown(void);
 int  b200_device_count(void);         /* devices the library is driving (0 before init / without GPU) */
 /* jobs (megabatches or single images) device `index` (0 .. b200_device_count()-1) has been handed so far, and the NUMA node its

@@ -2,10 +2,10 @@
  * oracle/jpeg_oracle.c -- TEST INFRASTRUCTURE, NOT PRODUCT CODE (see jpeg_oracle.h).
  *
  * Plain-C restatement of the JPEG path below caesiumclt's codec boundary
- * (/root/reference/src/compressor.rs:287-306 -> caesium::compress_in_memory).
+ * (caesium-clt's src/compressor.rs:287-306 -> caesium::compress_in_memory).
  * Upstream routine names (mozjpeg 4.x / libjpeg-turbo lineage, pinned by
- * /root/reference/Cargo.lock:1035 mozjpeg-sys 2.2.1) are cited per function; the
- * sources are not vendored under /root/reference, so each block restates the
+ * caesium-clt's Cargo.lock:1035 mozjpeg-sys 2.2.1) are cited per function; the
+ * sources are not vendored under the caesium-clt sources, so each block restates the
  * published IJG algorithm and is pinned by tests/test_oracle_jpeg.py against
  * libjpeg-turbo (Pillow) and the fixtures' DQT / scan-script known answers.
  */

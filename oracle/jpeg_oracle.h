@@ -2,11 +2,11 @@
  * oracle/jpeg_oracle.h -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  *
  * CPU restatement of the JPEG half of the hot path that caesiumclt reaches through
- * `caesium::compress_in_memory` (/root/reference/src/compressor.rs:305) and, for
+ * `caesium::compress_in_memory` (caesium-clt's src/compressor.rs:305) and, for
  * `--lossless`, the coefficient-domain transcode selected by
- * `parameters.jpeg.optimize` (/root/reference/src/compressor.rs:427).
+ * `parameters.jpeg.optimize` (caesium-clt's src/compressor.rs:427).
  *
- * The arithmetic itself is NOT in /root/reference: it lives in libcaesium 0.20.3
+ * The arithmetic itself is NOT in the caesium-clt sources: it lives in libcaesium 0.20.3
  * (Cargo.lock:892) -> mozjpeg-sys 2.2.1 (Cargo.lock:1035) -> mozjpeg 4.x, whose
  * sources are not vendored.  This file restates the *published* IJG/libjpeg-turbo
  * algorithms those crates execute (names of the upstream routines are cited at each

@@ -2,7 +2,7 @@
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference
 legs may import this module (see oracle/jpeg_oracle.h for what the oracle restates:
-the codec work below /root/reference/src/compressor.rs:287-306).
+the codec work below caesium-clt's src/compressor.rs:287-306).
 """
 import ctypes as C
 import os

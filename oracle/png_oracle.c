@@ -1,8 +1,8 @@
 /* png_oracle.c -- TEST INFRASTRUCTURE ONLY (never linked into or called by the product).
  *
  * CPU restatement of the lossless PNG leg of the hot path: libcaesium png::lossless -> oxipng::optimize_from_memory
- * (/root/reference/src/compressor.rs:428 `parameters.png.optimize`, :436 `optimization_level`, :437 `force_zopfli`).
- * oxipng 9.x and libdeflate are Cargo dependencies that are NOT vendored under /root/reference, so this file restates
+ * (caesium-clt's src/compressor.rs:428 `parameters.png.optimize`, :436 `optimization_level`, :437 `force_zopfli`).
+ * oxipng 9.x and libdeflate are Cargo dependencies that are NOT vendored under the caesium-clt sources, so this file restates
  * their published algorithms: the PNG filters (PNG spec 9.2), oxipng's per-row filter heuristics (RowFilter::MinSum,
  * Entropy, Bigrams, BigEnt; Brute is scored like Entropy -- documented deviation in DESIGN.md), and an LZ77 parse over a
  * fixed candidate set with zlib's one-step lazy evaluation.  Parity status: "pinned by losslessness" -- the product's

@@ -2,7 +2,7 @@
  * oracle/resize_oracle.c -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  *
  * CPU restatement of the resize leg reached through CSParameters.width/height
- * (/root/reference/src/compressor.rs:439-443, :503-536): libcaesium's resize::resize_image calls
+ * (caesium-clt's src/compressor.rs:439-443, :503-536): libcaesium's resize::resize_image calls
  * image 0.25.9 `resize_exact(w, h, FilterType::Lanczos3)` (Cargo.lock:701).  The crate source is not vendored; this
  * follows its published algorithm (imageops/sample.rs: vertical_sample into an f32 image, then horizontal_sample
  * with clamp + round-half-away to u8; lanczos3_kernel = sinc(x) * sinc(x/3) in f32), plus libjpeg's fixed-point

@@ -1,8 +1,8 @@
 /* webp_oracle.c -- TEST INFRASTRUCTURE ONLY (never linked into or called by the product).
  *
  * CPU restatement of the WebP leg of the hot path: caesium::convert_in_memory(.., SupportedFileTypes::WebP)
- * (/root/reference/src/compressor.rs:288-292 -> libcaesium webp::compress -> libwebp, lossy VP8 key frame at
- * `parameters.webp.quality`).  libwebp is a Cargo/C dependency that is NOT vendored under /root/reference; the VP8
+ * (caesium-clt's src/compressor.rs:288-292 -> libcaesium webp::compress -> libwebp, lossy VP8 key frame at
+ * `parameters.webp.quality`).  libwebp is a Cargo/C dependency that is NOT vendored under the caesium-clt sources; the VP8
  * bitstream, its arithmetic ("bool") coder, token tree, transforms and intra predictors are normative (RFC 6386), so the
  * decoder side of every function below is fixed by the standard.  The ENCODER decisions are this project's profile:
  * 16x16 luma prediction only (DC / TM / V / H by least squared error), one segment, token probabilities re-estimated per

@@ -36,7 +36,7 @@ int main(void)
     if (p.jpeg_quality != 80 || p.png_optimization_level != 3 || !p.jpeg_progressive) return 2;
     if (b200_sniff_format(png_sig, 8) != B200_FMT_PNG || b200_sniff_format(jpg_sig, 4) != B200_FMT_JPEG || b200_sniff_format(webp_sig, 12) != B200_FMT_WEBP ||
         b200_sniff_format((const uint8_t *)"nope", 4) != B200_FMT_UNKNOWN) return 3;
-    if (!b200_version() || !strstr(b200_version(), "sm_100a")) return 4;
+    if (!b200_version() || !strstr(b200_version(), "sm_90a")) return 4;
     b200_jpeg_quant_table(80, 0, qt);
     if (qt[0] == 0 || qt[63] == 0) return 5;
     if (b200_webp_qindex(100, f) != 0 || f[0] != 4 || b200_webp_qindex(0, f) != 127 || f[1] != 284) return 6;

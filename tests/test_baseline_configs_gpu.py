@@ -3,7 +3,7 @@
   configs[3]      4096x4096 RGBA PNG --lossless --png-opt-level 3: output decodes to the source pixels; the filtered stream it
                   carries equals the oracle's for one of the level's strategies; K6 / K7 stage outputs == oracle at full size
   configs[4]      6000x4000 JPEG -> -q 85 --width 1920 --format webp: bytes == oracle
-and the reference's own sample files (tests/golden/reference_samples, copied from /root/reference/samples) through the CUDA path:
+and the reference's own sample files (tests/golden/reference_samples, copied from caesium-clt's samples) through the CUDA path:
 bytes == oracle, plus the size facts the reference's tests assert (compressor.rs:1051-1068) on the PRODUCT's output."""
 import io
 import os

@@ -72,7 +72,7 @@ def test_coalesced_calls_return_what_direct_calls_return():
 
 @pytest.mark.gpu
 def test_coalesced_lossy_calls_on_the_gpu_return_what_direct_calls_return():
-    """the same on a B200 with the lossy path: the collector's batch takes the megabatch route (same-shaped files decoded,
+    """the same on an H100 with the lossy path: the collector's batch takes the megabatch route (same-shaped files decoded,
     transformed and encoded together), the direct calls the one-image route -- the bytes must not differ"""
     direct = _run(False, lossy=True)
     merged = _run(True, lossy=True)

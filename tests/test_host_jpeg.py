@@ -56,10 +56,9 @@ def test_host_huffman_decode_matches_oracle(L, O, golden, name):
         assert np.array_equal(np.array(lay.qt[c][:], dtype=np.uint16), j.qtable(c)[ZZ])
 
 
-@pytest.mark.skipif(not os.path.exists("/root/reference/samples/j0.JPG"), reason="/root/reference not mounted")
-@pytest.mark.parametrize("rel", ["j0.JPG", "level_1_0/j1.jpg"])
-def test_host_progressive_decode_on_reference_fixtures(L, O, rel):
-    data = open(os.path.join("/root/reference/samples", rel), "rb").read()
+@pytest.mark.parametrize("rel", ["j0.JPG", "level_1_0/j1.jpg"])       # paths under the reference's samples/
+def test_host_progressive_decode_on_reference_fixtures(L, O, golden, rel):
+    data = golden(os.path.join("reference_samples", os.path.basename(rel)))
     lay, co = L.jpeg_decode_coefficients(data)
     j = O.Jpeg(data)
     for c in range(3):
@@ -146,7 +145,7 @@ def test_corrupt_and_unknown_inputs_return_errors(L, golden):
 
 
 def test_cuda_paths_fail_loudly_without_a_gpu(L, golden):
-    """No CPU fallback: on a box without a B200 the lossy path must return B200_ERR_NO_DEVICE, never pixels."""
+    """No CPU fallback: on a machine without an H100 the lossy path must return B200_ERR_NO_DEVICE, never pixels."""
     if not _no_gpu():
         pytest.skip("a GPU is visible")
     p = L.default_params()

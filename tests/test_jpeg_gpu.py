@@ -1,7 +1,7 @@
-"""GPU parity tests (run with -m gpu on a B200): the CUDA path, called through the C-ABI, against the CPU oracle.
+"""GPU parity tests (run with -m gpu on an H100): the CUDA path, called through the C-ABI, against the CPU oracle.
 
 Bar: bit-exact (integer arithmetic end to end).  Three levels, mirroring how compress_in_memory is assembled
-(/root/reference/src/compressor.rs:305 -> libcaesium jpeg::lossy):
+(caesium-clt's src/compressor.rs:305 -> libcaesium jpeg::lossy):
   1. stage: device dequant/IDCT/resample/FDCT/quantise == oracle coefficients,
   2. file: b200_compress_in_memory output bytes == oracle jpeg_lossy output bytes (and the committed sha256),
   3. full-size: BASELINE config sizes through size-independent properties + sampled block checks.

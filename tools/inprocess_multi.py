@@ -20,7 +20,7 @@ def main():
     small = bench.make_inputs(8, 1000, "jpeg4k")
     work = [datas[i % len(datas)] for i in range(n)]
     L = bench.load_pkg()
-    assert L.lib().b200_init(0) == 0, "no B200 visible"
+    assert L.lib().b200_init(0) == 0, "no H100 visible"
     ndev = L.lib().b200_device_count()
     p = L.default_params(); p.jpeg_quality, p.jpeg_chroma_subsampling, p.jpeg_progressive = 80, 420, 1
     bi = L.BatchInputs(work)
