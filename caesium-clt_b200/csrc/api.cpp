@@ -63,6 +63,72 @@ bool ensure_runtime(std::string &err)
     return false;
 }
 
+// bit 0 = device entropy encoder, bit 1 = device entropy decoder; B200_ENTROPY is read once unless b200_set_entropy_mode chose
+int entropy_mode()
+{
+    if (g_entropy_mode.load() < 0) {
+        const char *e = getenv("B200_ENTROPY");
+        g_entropy_mode.store(!e ? 3 : !strcmp(e, "host") ? 0 : !strcmp(e, "gpuenc") ? 1 : !strcmp(e, "gpudec") ? 2 : 3);
+    }
+    return g_entropy_mode.load();
+}
+
+// One slot of one device (prefer_dev < 0: the next device round-robin), held until the lease goes out of scope.  The runtime
+// must already be up (ensure_runtime): where a leg calls that decides which status a machine without a device answers.
+class SlotLease {
+public:
+    explicit SlotLease(int prefer_dev) : s_(slot_acquire(prefer_dev < 0 ? runtime_next_device() : prefer_dev, err_)) {}
+    ~SlotLease() { slot_release(s_); }
+    SlotLease(const SlotLease &) = delete;
+    SlotLease &operator=(const SlotLease &) = delete;
+    operator Slot *() const { return s_; }
+    Slot *operator->() const { return s_; }
+    b200_status failure() const { return make_status(B200_ERR_CUDA, err_); }      // why no slot could be had
+private:
+    std::string err_;
+    Slot *s_;
+};
+
+// the body of an entry point: no C++ exception crosses the C ABI
+template <class Fn> b200_status guarded(Fn fn)
+{
+    try { return fn(); }
+    catch (const std::exception &e) { return make_status(B200_ERR_OUT_OF_MEMORY, e.what()); }
+    catch (...) { return make_status(B200_ERR_INVALID_ARGUMENT, "unexpected failure"); }
+}
+
+// a result handed to the caller in malloc'ed memory (released with b200_free); *n counts elements
+template <class T> b200_status give(const std::vector<T> &v, T **out, size_t *n)
+{
+    *out = (T *)malloc(v.size() ? v.size() * sizeof(T) : 1);
+    if (!*out) return make_status(B200_ERR_OUT_OF_MEMORY, "out of memory");
+    memcpy(*out, v.data(), v.size() * sizeof(T)); *n = v.size();
+    return ok_status();
+}
+
+// a PNG the decoder refused: interlaced files are "recognised but not on this path", everything else is corrupt input
+b200_status png_status(const std::string &err) { return make_status(err.find("interlace") != std::string::npos ? B200_ERR_UNSUPPORTED : B200_ERR_CORRUPT_INPUT, err); }
+
+// planar 8-bit samples with no JPEG behind them ([nc][h][w]: RGB or one grey plane): 1x1 sampling, one quantisation slot
+JpegGeom planar_geom(uint32_t w, uint32_t h, int nc)
+{
+    JpegGeom g; g.width = (int)w; g.height = (int)h; g.ncomp = nc;
+    for (int c = 0; c < nc; c++) { g.cid[c] = c + 1; g.hs[c] = g.vs[c] = 1; g.tq[c] = 0; }
+    g.finalize();
+    return g;
+}
+JpegGeom with_size(JpegGeom g, uint32_t w, uint32_t h) { g.width = (int)w; g.height = (int)h; g.finalize(); return g; }
+
+// libcaesium resize::resize_image -> compute_dimensions (the source size when neither width nor height is set); source and
+// target must fit the format: both sides at most 65535, the target at most `limit` and not empty
+b200_status target_size(uint32_t w, uint32_t h, const b200_params *p, uint32_t limit, uint32_t &nw, uint32_t &nh, const char *msg)
+{
+    nw = w; nh = h;
+    if (p->width || p->height) compute_resize_dimensions(w, h, p->width, p->height, nw, nh);
+    if (nw == 0 || nh == 0 || nw > limit || nh > limit || w > 65535 || h > 65535) return make_status(B200_ERR_INVALID_ARGUMENT, msg);
+    return ok_status();
+}
+
 void layout_from_geom(const JpegGeom &g, b200_jpeg_layout *l)
 {
     memset(l, 0, sizeof(*l));
@@ -133,109 +199,100 @@ void print_trace()
 }
 
 // ---- JPEG through the device ---------------------------------------------------------------------------------
+// Entropy DECODE on the device for baseline single-scan files (jpeg_gpudec.cu): the scan's bytes go up, the coefficients are
+// born in HBM (on_device).  Progressive / multi-scan / restart-interval files, and the rare stream whose parallel decode does not
+// settle, are Huffman-decoded into s->h_in on the calling thread instead.
+b200_status decode_into_slot(Slot *s, JpegReader &rd, bool &on_device, std::string &err, StageTimer *tm = nullptr)
+{
+    on_device = false;
+    JpegReader::DeviceScan ds;
+    if ((entropy_mode() & 2) && rd.device_decodable(ds)) {
+        if (tm) tm->lap(0);
+        const int r = slot_gpu_decode(s, rd, ds, err);
+        if (tm) tm->lap(1);
+        if (r == 0) on_device = true;
+        else if (r != 1) return make_status(B200_ERR_CUDA, err);
+    }
+    if (!on_device && !rd.decode(s->h_in, err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
+    return ok_status();
+}
+
+// Huffman statistics, table construction, bit packing and 0xFF stuffing of the coefficients in s->d_out on the device
+// (jpeg_gpuenc.cu); the host only frames the scans.  A scan that outgrows its device buffer falls back to the host ENCODER
+// (still the same coefficients from the CUDA transform).
+b200_status encode_from_slot(Slot *s, const JpegGeom &gout, const JpegWriteOptions &wo, const JpegMeta *meta, std::vector<uint8_t> &out, std::string &err,
+                             StageTimer *tm = nullptr)
+{
+    if (slot_gpu_encode(s, gout, wo.progressive, err)) {
+        if (tm) tm->lap(4);
+        const bool ok = jpeg_assemble(gout, wo, meta, s->enc->results.data(), (int)s->enc->results.size(), out, err);
+        if (tm) tm->lap(5);
+        return ok ? ok_status() : make_status(B200_ERR_INVALID_ARGUMENT, err);
+    }
+    if (!s->enc->overflow || !slot_download_coefs(s, (size_t)gout.total_coefs * 2, err)) return make_status(B200_ERR_CUDA, err);
+    jpeg_fill_dummy_blocks(gout, s->h_out);
+    if (!jpeg_write(gout, s->h_out, wo, meta, out, err)) return make_status(B200_ERR_INVALID_ARGUMENT, err);
+    return ok_status();
+}
+
 b200_status jpeg_compress(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
 {
     std::string err;
     JpegReader rd(in, in_len);
     if (!rd.read_header(err)) return header_status(err);
     const JpegGeom &gin = rd.geom();
-    JpegWriteOptions wo; wo.progressive = p->jpeg_progressive != 0; wo.keep_metadata = p->keep_metadata != 0; wo.preserve_icc = p->jpeg_preserve_icc != 0;
+    JpegWriteOptions wo = write_options(p);
     if (p->jpeg_optimize) {
         // libcaesium jpeg::lossless: coefficient-domain transcode.  Baseline single-scan inputs are entropy-decoded and
         // re-encoded (optimal tables, progressive script) by the device coders; the coefficients never leave HBM.
         // Everything else (progressive input, no device) is transcoded on the calling thread -- there is no arithmetic
         // on this path, only entropy coding.
+        wo.copy_jfif = true;
         std::string derr;
         JpegReader::DeviceScan ds;
-        if (g_entropy_mode.load() < 0) {
-            const char *e = getenv("B200_ENTROPY");
-            g_entropy_mode.store(!e ? 3 : !strcmp(e, "host") ? 0 : !strcmp(e, "gpuenc") ? 1 : !strcmp(e, "gpudec") ? 2 : 3);
-        }
-        if (g_entropy_mode.load() == 3 && rd.device_decodable(ds) && ensure_runtime(derr)) {
-            if (Slot *s = slot_acquire(prefer_dev < 0 ? runtime_next_device() : prefer_dev, derr)) {
-                bool done = false;
-                wo.copy_jfif = true;
+        if (entropy_mode() == 3 && rd.device_decodable(ds) && ensure_runtime(derr)) {
+            SlotLease s(prefer_dev);
+            if (s) {
                 if (s->ensure((size_t)gin.total_coefs * 2, 0, 0, 1 << 14, derr) && slot_gpu_decode(s, rd, ds, derr) == 0 &&
-                    slot_gpu_encode(s, gin, wo.progressive, derr, true))
-                    done = jpeg_assemble(gin, wo, &rd.meta(), s->enc->results.data(), (int)s->enc->results.size(), out, derr);
-                slot_release(s);
-                if (done) return ok_status();
+                    slot_gpu_encode(s, gin, wo.progressive, derr, true) &&
+                    jpeg_assemble(gin, wo, &rd.meta(), s->enc->results.data(), (int)s->enc->results.size(), out, derr))
+                    return ok_status();
                 out.clear();
             }
         }
         std::vector<int16_t> coefs((size_t)gin.total_coefs);
         if (!rd.decode(coefs.data(), err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
         jpeg_fill_dummy_blocks(gin, coefs.data());
-        wo.copy_jfif = true;
         if (!jpeg_write(gin, coefs.data(), wo, &rd.meta(), out, err)) return make_status(B200_ERR_INVALID_ARGUMENT, err);
         return ok_status();
     }
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    if (g_entropy_mode.load() < 0) {
-        const char *e = getenv("B200_ENTROPY");
-        g_entropy_mode.store(!e ? 3 : !strcmp(e, "host") ? 0 : !strcmp(e, "gpuenc") ? 1 : !strcmp(e, "gpudec") ? 2 : 3);
-    }
     JpegGeom gout;
     if (!jpeg_output_geom(gin, (int)p->jpeg_quality, (int)p->jpeg_chroma_subsampling, gout, err)) return make_status(B200_ERR_INVALID_ARGUMENT, err);
     const bool resize = p->width || p->height;
-    if (resize) {   // libcaesium resize::resize_image -> compute_dimensions
-        uint32_t nw = 0, nh = 0;
-        compute_resize_dimensions((uint32_t)gin.width, (uint32_t)gin.height, p->width, p->height, nw, nh);
-        if (nw == 0 || nh == 0 || nw > 65535 || nh > 65535) return make_status(B200_ERR_INVALID_ARGUMENT, "invalid target dimensions");
-        gout.width = (int)nw; gout.height = (int)nh; gout.finalize();
+    if (resize) {
+        uint32_t nw, nh;
+        const b200_status st = target_size((uint32_t)gin.width, (uint32_t)gin.height, p, 65535, nw, nh, "invalid target dimensions");
+        if (st.code) return st;
+        gout = with_size(gout, nw, nh);
     }
     ImagePlan plan;
     if (!resize && !plan_image(gin, gout, plan, err)) return make_status(B200_ERR_UNSUPPORTED, err);
     if (resize) { plan.in_bytes = (size_t)gin.total_coefs * 2; plan.out_bytes = (size_t)gout.total_coefs * 2; }
-    Slot *s = slot_acquire(prefer_dev < 0 ? runtime_next_device() : prefer_dev, err);
-    if (!s) return make_status(B200_ERR_CUDA, err);
-    b200_status st = ok_status();
-    do {
-        if (!s->ensure(plan.in_bytes, plan.out_bytes, plan.scratch_bytes(), 1 << 14, err)) { st = make_status(B200_ERR_OUT_OF_MEMORY, err); break; }
-        const int mode = g_entropy_mode.load();
-        const bool gpu_entropy = (mode & 1) != 0;
-        // Entropy DECODE on the device for baseline single-scan files (jpeg_gpudec.cu): the scan's bytes go up, the
-        // coefficients are born in HBM.  Progressive / multi-scan / restart-interval files, and the rare stream whose
-        // parallel decode does not settle, are Huffman-decoded here on the calling thread instead.
-        bool on_device = false;
-        JpegReader::DeviceScan ds;
-        StageTimer tm;
-        if ((mode & 2) && rd.device_decodable(ds)) {
-            tm.lap(0);
-            const int r = slot_gpu_decode(s, rd, ds, err);
-            tm.lap(1);
-            if (r == 0) on_device = true;
-            else if (r != 1) { st = make_status(B200_ERR_CUDA, err); break; }
-        }
-        if (!on_device && !rd.decode(s->h_in, err)) { st = make_status(B200_ERR_CORRUPT_INPUT, err); break; }
-        tm.lap(2);
-        if (!(resize ? slot_transform_resized(s, gin, gout, err, !gpu_entropy, !on_device) : slot_transform(s, gin, gout, err, !gpu_entropy, !on_device))) { st = make_status(B200_ERR_CUDA, err); break; }
-        tm.lap(3);
-        if (gpu_entropy) {
-            // Huffman statistics, table construction, bit packing and 0xFF stuffing on the device (jpeg_gpuenc.cu); the
-            // host only frames the scans.  A scan that outgrows its device buffer falls back to the host ENCODER
-            // (still the same coefficients from the CUDA transform).
-            if (slot_gpu_encode(s, gout, wo.progressive, err)) {
-                tm.lap(4);
-                if (!jpeg_assemble(gout, wo, &rd.meta(), s->enc->results.data(), (int)s->enc->results.size(), out, err)) st = make_status(B200_ERR_INVALID_ARGUMENT, err);
-                tm.lap(5);
-                break;
-            }
-            if (!s->enc || !s->enc->overflow) { st = make_status(B200_ERR_CUDA, err); break; }
-            if (!slot_download_coefs(s, plan.out_bytes, err)) { st = make_status(B200_ERR_CUDA, err); break; }
-        }
-        jpeg_fill_dummy_blocks(gout, s->h_out);
-        if (!jpeg_write(gout, s->h_out, wo, &rd.meta(), out, err)) { st = make_status(B200_ERR_INVALID_ARGUMENT, err); break; }
-    } while (0);
-    slot_release(s);
-    return st;
-}
-
-b200_status give(std::vector<uint8_t> &v, uint8_t **out, size_t *out_len)
-{
-    *out = (uint8_t *)malloc(v.size() ? v.size() : 1);
-    if (!*out) return make_status(B200_ERR_OUT_OF_MEMORY, "out of memory");
-    memcpy(*out, v.data(), v.size()); *out_len = v.size();
+    SlotLease s(prefer_dev);
+    if (!s) return s.failure();
+    if (!s->ensure(plan.in_bytes, plan.out_bytes, plan.scratch_bytes(), 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    const bool gpu_entropy = (entropy_mode() & 1) != 0;
+    bool on_device;
+    StageTimer tm;
+    const b200_status st = decode_into_slot(s, rd, on_device, err, &tm);
+    if (st.code) return st;
+    tm.lap(2);
+    if (!(resize ? slot_transform_resized(s, gin, gout, err, !gpu_entropy, !on_device) : slot_transform(s, gin, gout, err, !gpu_entropy, !on_device))) return make_status(B200_ERR_CUDA, err);
+    tm.lap(3);
+    if (gpu_entropy) return encode_from_slot(s, gout, wo, &rd.meta(), out, err, &tm);
+    jpeg_fill_dummy_blocks(gout, s->h_out);
+    if (!jpeg_write(gout, s->h_out, wo, &rd.meta(), out, err)) return make_status(B200_ERR_INVALID_ARGUMENT, err);
     return ok_status();
 }
 
@@ -256,12 +313,7 @@ void jpeg_compress_group(const uint8_t *const *in, const size_t *in_len, const s
         if (b200_sniff_format(in[i], in_len[i]) != B200_FMT_JPEG) continue;
         rd[k].reset(new JpegReader(in[i], in_len[i]));
         if (!rd[k]->read_header(err) || !rd[k]->device_decodable(ds[k], true)) continue;      // the entropy-coded segment is walked on the device
-        if (!members.empty()) {
-            const JpegGeom &a = rd[members[0]]->geom(), &b = rd[k]->geom();
-            bool same = a.width == b.width && a.height == b.height && a.ncomp == b.ncomp;
-            for (int c = 0; same && c < a.ncomp; c++) same = a.hs[c] == b.hs[c] && a.vs[c] == b.vs[c];
-            if (!same) continue;
-        }
+        if (!members.empty() && !same_shape(rd[members[0]]->geom(), rd[k]->geom())) continue;
         members.push_back(k);
     }
     if (members.size() < 2) return;
@@ -270,40 +322,34 @@ void jpeg_compress_group(const uint8_t *const *in, const size_t *in_len, const s
     JpegGeom gout;
     if (lossless) gout = gin0;
     else if (!jpeg_output_geom(gin0, (int)p->jpeg_quality, (int)p->jpeg_chroma_subsampling, gout, err)) return;
-    Slot *s = slot_acquire(dev, err);
+    SlotLease s(dev);
     if (!s) return;
     const int Kg = (int)members.size();
-    bool ok = false;
-    do {
-        GroupLayout L;
-        if (!slot_group_layout(s, gin0, gout, Kg, L, err)) break;
-        std::vector<GpuDecoder::Item> items((size_t)Kg);
-        std::vector<const JpegGeom *> gins((size_t)Kg);
-        for (int m = 0; m < Kg; m++) {
-            const int k = members[m];
-            items[m].rd = rd[k].get(); items[m].ds = &ds[k]; items[m].result = GpuDecoder::FAILED;
-            items[m].d_coefs = reinterpret_cast<int16_t *>(reinterpret_cast<uint8_t *>(s->d_in) + L.in_stride * m);
-            gins[m] = &rd[k]->geom();
-        }
-        tm.lap(0);
-        JpegWriteOptions wo; wo.progressive = p->jpeg_progressive != 0; wo.keep_metadata = p->keep_metadata != 0; wo.preserve_icc = p->jpeg_preserve_icc != 0;
-        wo.copy_jfif = lossless;
-        if (!slot_run_group(s, items, gins.data(), gout, L, wo.progressive, lossless, err)) break;
-        tm.lap(4);
-        const int spi = s->enc->plan.scans_per_image;
-        for (int m = 0; m < Kg; m++) {
-            const int k = members[m], i = idx[k];
-            if (items[m].result != GpuDecoder::OK) continue;          // not converged: the per-image path decodes it on the host
-            out[i] = nullptr; out_len[i] = 0;
-            if (!jpeg_assemble_malloc(lossless ? rd[k]->geom() : gout, wo, &rd[k]->meta(), s->enc->results.data() + (size_t)m * spi, spi, &out[i], &out_len[i], err)) status[i] = make_status(B200_ERR_INVALID_ARGUMENT, err);
-            else status[i] = ok_status();
-            done[k] = 1;
-        }
-        tm.lap(5);
-        ok = true;
-    } while (0);
-    (void)ok;
-    slot_release(s);
+    GroupLayout L;
+    if (!slot_group_layout(s, gin0, gout, Kg, L, err)) return;
+    std::vector<GpuDecoder::Item> items((size_t)Kg);
+    std::vector<const JpegGeom *> gins((size_t)Kg);
+    for (int m = 0; m < Kg; m++) {
+        const int k = members[m];
+        items[m].rd = rd[k].get(); items[m].ds = &ds[k]; items[m].result = GpuDecoder::FAILED;
+        items[m].d_coefs = L.coefs(*s, m, true);
+        gins[m] = &rd[k]->geom();
+    }
+    tm.lap(0);
+    JpegWriteOptions wo = write_options(p);
+    wo.copy_jfif = lossless;
+    if (!slot_run_group(s, items, gins.data(), gout, L, wo.progressive, lossless, err)) return;
+    tm.lap(4);
+    const int spi = s->enc->plan.scans_per_image;
+    for (int m = 0; m < Kg; m++) {
+        const int k = members[m], i = idx[k];
+        if (items[m].result != GpuDecoder::OK) continue;          // not converged: the per-image path decodes it on the host
+        out[i] = nullptr; out_len[i] = 0;
+        if (!jpeg_assemble_malloc(lossless ? rd[k]->geom() : gout, wo, &rd[k]->meta(), s->enc->results.data() + (size_t)m * spi, spi, &out[i], &out_len[i], err)) status[i] = make_status(B200_ERR_INVALID_ARGUMENT, err);
+        else status[i] = ok_status();
+        done[k] = 1;
+    }
+    tm.lap(5);
 }
 
 // ---- PNG (lossless) through the device ---------------------------------------------------------------------------
@@ -318,27 +364,28 @@ b200_status png_compress(const uint8_t *in, size_t in_len, const b200_params *p,
     PngInfo info; PngIdat idat;
     static const bool verbose = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2;
     const auto t0 = std::chrono::steady_clock::now();
-    if (!png_parse_chunks(in, in_len, p->keep_metadata != 0, info, idat, err)) return make_status(err.find("interlace") != std::string::npos ? B200_ERR_UNSUPPORTED : B200_ERR_CORRUPT_INPUT, err);
+    if (!png_parse_chunks(in, in_len, p->keep_metadata != 0, info, idat, err)) return png_status(err);
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    Slot *s = slot_acquire(prefer_dev < 0 ? runtime_next_device() : prefer_dev, err);
-    if (!s) return make_status(B200_ERR_CUDA, err);
-    if (!s->png) s->png = new PngDevice();
-    // the IDAT stream is inflated straight into the slot's pinned staging buffer; from there on everything is device work
-    // (un-filter, checksum, reductions, filter trials, LZ77, DEFLATE coding) until the finished zlib stream comes back
-    const size_t nin = (info.row_bytes + 1) * (size_t)info.height;
-    size_t cap = 0, got = 0; uint32_t stored_adler = 0;
-    uint8_t *buf = s->png->input_buffer(nin, cap, err);
-    if (!buf) { slot_release(s); return make_status(B200_ERR_OUT_OF_MEMORY, err); }
-    if (!zlib_inflate_to(idat.p, idat.n, buf, cap, nin, &got, &stored_adler, err)) { slot_release(s); return make_status(B200_ERR_CORRUPT_INPUT, err); }
-    if (got < nin) { slot_release(s); return make_status(B200_ERR_CORRUPT_INPUT, "IDAT too short"); }
-    const auto t1 = std::chrono::steady_clock::now();
     std::vector<uint8_t> z;
-    int level = (int)p->png_optimization_level; if (level > 6) level = 6;
-    const bool ok = s->png->compress_filtered(info, got, stored_adler, level, s->stream, z, nullptr, err);
-    const bool corrupt = s->png->corrupt;
-    const double deflate_ms = s->png->last_deflate_ms;
-    slot_release(s);
-    if (!ok) return make_status(corrupt ? B200_ERR_CORRUPT_INPUT : B200_ERR_CUDA, err);
+    auto t1 = t0;
+    double deflate_ms = 0;
+    {   // the slot goes back before the container is written
+        SlotLease s(prefer_dev);
+        if (!s) return s.failure();
+        PngDevice *png = s->png_dev();
+        // the IDAT stream is inflated straight into the slot's pinned staging buffer; from there on everything is device work
+        // (un-filter, checksum, reductions, filter trials, LZ77, DEFLATE coding) until the finished zlib stream comes back
+        const size_t nin = (info.row_bytes + 1) * (size_t)info.height;
+        size_t cap = 0, got = 0; uint32_t stored_adler = 0;
+        uint8_t *buf = png->input_buffer(nin, cap, err);
+        if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+        if (!zlib_inflate_to(idat.p, idat.n, buf, cap, nin, &got, &stored_adler, err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
+        if (got < nin) return make_status(B200_ERR_CORRUPT_INPUT, "IDAT too short");
+        t1 = std::chrono::steady_clock::now();
+        if (!png->compress_filtered(info, got, stored_adler, std::min((int)p->png_optimization_level, 6), s->stream, z, nullptr, err))
+            return make_status(png->corrupt ? B200_ERR_CORRUPT_INPUT : B200_ERR_CUDA, err);
+        deflate_ms = png->last_deflate_ms;
+    }
     const auto t3 = std::chrono::steady_clock::now();
     png_write(info, z, out);
     if (verbose) {
@@ -347,6 +394,40 @@ b200_status png_compress(const uint8_t *in, size_t in_len, const b200_params *p,
                 info.width, info.height, ms(t0, t1), deflate_ms, ms(t1, t3), ms(t3, std::chrono::steady_clock::now()));
     }
     return ok_status();
+}
+
+// 8-bit planar samples ([nc][h][w], nc = 1 or 3) and an optional alpha plane -> lossless PNG (K6 filter selection, K7 LZ77) on the
+// slot's PngDevice.  palette: try png_reduce_palette first.
+b200_status png_from_planes(Slot *s, const uint8_t *planes, int nc, const uint8_t *alpha, uint32_t w, uint32_t h, bool palette, const b200_params *p,
+                            std::vector<uint8_t> &out, std::string &err)
+{
+    const size_t n = (size_t)w * h;
+    const int ch = nc + (alpha ? 1 : 0);
+    std::vector<uint8_t> raw;
+    if (ch == 1) raw.assign(planes, planes + n);
+    else {
+        raw.resize((size_t)ch * n);
+        for (size_t i = 0; i < n; i++) {
+            raw[ch * i] = planes[i]; raw[ch * i + 1] = planes[n + i]; raw[ch * i + 2] = planes[2 * n + i];
+            if (alpha) raw[ch * i + 3] = alpha[i];
+        }
+    }
+    PngInfo info; info.width = w; info.height = h; info.bit_depth = 8; info.color_type = ch == 1 ? 0 : ch == 3 ? 2 : 6; info.channels = ch;
+    info.bits_per_pixel = 8 * ch; info.bpp = ch; info.row_bytes = (size_t)w * ch;
+    if (palette) png_reduce_palette(info, raw);
+    std::vector<uint8_t> z;
+    if (!s->png_dev()->compress(info, raw, std::min((int)p->png_optimization_level, 6), s->stream, z, nullptr, err)) return make_status(B200_ERR_CUDA, err);
+    png_write(info, z, out);
+    return ok_status();
+}
+
+// Lanczos3 (K3) of nc host planes [nc][h][w] to [nc][nh][nw], fetched back into dst
+bool resize_to_host(Slot *s, const uint8_t *src, uint32_t w, uint32_t h, uint32_t nw, uint32_t nh, int nc, std::vector<uint8_t> &dst, std::string &err)
+{
+    const JpegGeom gin = planar_geom(w, h, nc);
+    uint8_t *dp[3] = {nullptr, nullptr, nullptr};
+    dst.resize((size_t)nc * nw * nh);
+    return slot_transform_resized(s, gin, with_size(gin, nw, nh), err, false, false, dp, src) && slot_fetch_planes(s, dp, nc, (size_t)nw * nh, dst.data(), err);
 }
 
 // ---- conversion to WebP (lossy VP8) ----------------------------------------------------------------------------------
@@ -359,43 +440,29 @@ b200_status jpeg_to_webp(const uint8_t *in, size_t in_len, const b200_params *p,
     if (!rd.read_header(err)) return header_status(err);
     const JpegGeom &gin = rd.geom();
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    uint32_t nw = (uint32_t)gin.width, nh = (uint32_t)gin.height;
-    if (p->width || p->height) compute_resize_dimensions((uint32_t)gin.width, (uint32_t)gin.height, p->width, p->height, nw, nh);
-    if (nw == 0 || nh == 0 || nw > 16383 || nh > 16383) return make_status(B200_ERR_INVALID_ARGUMENT, "invalid target dimensions for WebP");
-    JpegGeom gout = gin; gout.width = (int)nw; gout.height = (int)nh; gout.finalize();
-    if (g_entropy_mode.load() < 0) {
-        const char *e = getenv("B200_ENTROPY");
-        g_entropy_mode.store(!e ? 3 : !strcmp(e, "host") ? 0 : !strcmp(e, "gpuenc") ? 1 : !strcmp(e, "gpudec") ? 2 : 3);
-    }
-    Slot *s = slot_acquire(prefer_dev < 0 ? runtime_next_device() : prefer_dev, err);
-    if (!s) return make_status(B200_ERR_CUDA, err);
-    b200_status st = ok_status();
+    uint32_t nw, nh;
+    b200_status st = target_size((uint32_t)gin.width, (uint32_t)gin.height, p, 16383, nw, nh, "invalid target dimensions for WebP");
+    if (st.code) return st;
+    const JpegGeom gout = with_size(gin, nw, nh);
+    SlotLease s(prefer_dev);
+    if (!s) return s.failure();
     static const bool verbose = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2;
     const auto t0 = std::chrono::steady_clock::now();
-    auto t1 = t0, t2 = t0;
-    do {
-        if (!s->ensure((size_t)gin.total_coefs * 2, (size_t)gout.total_coefs * 2, 0, 1 << 14, err)) { st = make_status(B200_ERR_OUT_OF_MEMORY, err); break; }
-        bool on_device = false;
-        JpegReader::DeviceScan ds;
-        if ((g_entropy_mode.load() & 2) && rd.device_decodable(ds)) {
-            const int r = slot_gpu_decode(s, rd, ds, err);
-            if (r == 0) on_device = true; else if (r != 1) { st = make_status(B200_ERR_CUDA, err); break; }
-        }
-        if (!on_device && !rd.decode(s->h_in, err)) { st = make_status(B200_ERR_CORRUPT_INPUT, err); break; }
-        t1 = std::chrono::steady_clock::now();
-        uint8_t *rgb[3] = {nullptr, nullptr, nullptr};
-        if (!slot_transform_resized(s, gin, gout, err, false, !on_device, rgb)) { st = make_status(B200_ERR_CUDA, err); break; }
-        t2 = std::chrono::steady_clock::now();
-        if (!s->webp) s->webp = new WebpDevice();
-        if (!s->webp->encode_planes(rgb[0], rgb[1], rgb[2], (int)nw, (int)nh, (int)p->webp_quality, s->stream, out, err)) { st = make_status(B200_ERR_CUDA, err); break; }
-        if (verbose) {
-            auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
-            fprintf(stderr, "[b200 trace] jpeg %dx%d -> webp %ux%u: segment walk + entropy decode (device %d) %.1f ms, transform + resize launch %.1f ms, VP8 (wait for the device %.1f ms, boolean coder %.1f ms) %.1f ms\n",
-                    gin.width, gin.height, nw, nh, (int)on_device, ms(t0, t1), ms(t1, t2), s->webp->last_wait_ms, s->webp->last_code_ms, ms(t2, std::chrono::steady_clock::now()));
-        }
-    } while (0);
-    slot_release(s);
-    return st;
+    if (!s->ensure((size_t)gin.total_coefs * 2, (size_t)gout.total_coefs * 2, 0, 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    bool on_device;
+    if ((st = decode_into_slot(s, rd, on_device, err)).code) return st;
+    const auto t1 = std::chrono::steady_clock::now();
+    uint8_t *rgb[3] = {nullptr, nullptr, nullptr};
+    if (!slot_transform_resized(s, gin, gout, err, false, !on_device, rgb)) return make_status(B200_ERR_CUDA, err);
+    const auto t2 = std::chrono::steady_clock::now();
+    WebpDevice *webp = s->webp_dev();
+    if (!webp->encode_planes(rgb[0], rgb[1], rgb[2], (int)nw, (int)nh, (int)p->webp_quality, s->stream, out, err)) return make_status(B200_ERR_CUDA, err);
+    if (verbose) {
+        auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
+        fprintf(stderr, "[b200 trace] jpeg %dx%d -> webp %ux%u: segment walk + entropy decode (device %d) %.1f ms, transform + resize launch %.1f ms, VP8 (wait for the device %.1f ms, boolean coder %.1f ms) %.1f ms\n",
+                gin.width, gin.height, nw, nh, (int)on_device, ms(t0, t1), ms(t1, t2), webp->last_wait_ms, webp->last_code_ms, ms(t2, std::chrono::steady_clock::now()));
+    }
+    return ok_status();
 }
 
 // JPEG -> PNG (lossless PNG only: png.optimize): device decode (+ K3 resize) to RGB, samples back to the host as PNG rows, then
@@ -408,45 +475,21 @@ b200_status jpeg_to_png(const uint8_t *in, size_t in_len, const b200_params *p, 
     if (!rd.read_header(err)) return header_status(err);
     const JpegGeom &gin = rd.geom();
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    uint32_t nw = (uint32_t)gin.width, nh = (uint32_t)gin.height;
-    if (p->width || p->height) compute_resize_dimensions((uint32_t)gin.width, (uint32_t)gin.height, p->width, p->height, nw, nh);
-    if (nw == 0 || nh == 0 || nw > 65535 || nh > 65535) return make_status(B200_ERR_INVALID_ARGUMENT, "invalid target dimensions");
-    JpegGeom gout = gin; gout.width = (int)nw; gout.height = (int)nh; gout.finalize();
-    if (g_entropy_mode.load() < 0) {
-        const char *e = getenv("B200_ENTROPY");
-        g_entropy_mode.store(!e ? 3 : !strcmp(e, "host") ? 0 : !strcmp(e, "gpuenc") ? 1 : !strcmp(e, "gpudec") ? 2 : 3);
-    }
-    Slot *s = slot_acquire(prefer_dev < 0 ? runtime_next_device() : prefer_dev, err);
-    if (!s) return make_status(B200_ERR_CUDA, err);
-    b200_status st = ok_status();
+    uint32_t nw, nh;
+    b200_status st = target_size((uint32_t)gin.width, (uint32_t)gin.height, p, 65535, nw, nh, "invalid target dimensions");
+    if (st.code) return st;
+    const JpegGeom gout = with_size(gin, nw, nh);
+    SlotLease s(prefer_dev);
+    if (!s) return s.failure();
+    if (!s->ensure((size_t)gin.total_coefs * 2, (size_t)gout.total_coefs * 2, 0, 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    bool on_device;
+    if ((st = decode_into_slot(s, rd, on_device, err)).code) return st;
     const int nc = gin.ncomp == 1 ? 1 : 3;
-    const size_t n = (size_t)nw * nh;
-    std::vector<uint8_t> planes((size_t)nc * n), raw;
-    do {
-        if (!s->ensure((size_t)gin.total_coefs * 2, (size_t)gout.total_coefs * 2, 0, 1 << 14, err)) { st = make_status(B200_ERR_OUT_OF_MEMORY, err); break; }
-        bool on_device = false;
-        JpegReader::DeviceScan ds;
-        if ((g_entropy_mode.load() & 2) && rd.device_decodable(ds)) {
-            const int r = slot_gpu_decode(s, rd, ds, err);
-            if (r == 0) on_device = true; else if (r != 1) { st = make_status(B200_ERR_CUDA, err); break; }
-        }
-        if (!on_device && !rd.decode(s->h_in, err)) { st = make_status(B200_ERR_CORRUPT_INPUT, err); break; }
-        uint8_t *rgb[3] = {nullptr, nullptr, nullptr};
-        if (!slot_transform_resized(s, gin, gout, err, false, !on_device, rgb)) { st = make_status(B200_ERR_CUDA, err); break; }
-        if (!slot_fetch_planes(s, rgb, nc, n, planes.data(), err)) { st = make_status(B200_ERR_CUDA, err); break; }
-        raw.resize((size_t)nc * n);
-        if (nc == 1) raw = planes;
-        else for (size_t i = 0; i < n; i++) { raw[3 * i] = planes[i]; raw[3 * i + 1] = planes[n + i]; raw[3 * i + 2] = planes[2 * n + i]; }
-        PngInfo info; info.width = nw; info.height = nh; info.bit_depth = 8; info.color_type = nc == 1 ? 0 : 2; info.channels = nc;
-        info.bits_per_pixel = 8 * nc; info.bpp = nc; info.row_bytes = (size_t)nw * nc;
-        if (!s->png) s->png = new PngDevice();
-        std::vector<uint8_t> z;
-        int level = (int)p->png_optimization_level; if (level > 6) level = 6;
-        if (!s->png->compress(info, raw, level, s->stream, z, nullptr, err)) { st = make_status(B200_ERR_CUDA, err); break; }
-        png_write(info, z, out);
-    } while (0);
-    slot_release(s);
-    return st;
+    uint8_t *rgb[3] = {nullptr, nullptr, nullptr};
+    std::vector<uint8_t> planes((size_t)nc * nw * nh);
+    if (!slot_transform_resized(s, gin, gout, err, false, !on_device, rgb) || !slot_fetch_planes(s, rgb, nc, (size_t)nw * nh, planes.data(), err))
+        return make_status(B200_ERR_CUDA, err);
+    return png_from_planes(s, planes.data(), nc, nullptr, nw, nh, false, p, out, err);
 }
 
 // Decoded PNG samples -> 8-bit planar samples on the host: palette looked up, sub-byte greys scaled, 16-bit -> high byte,
@@ -481,42 +524,27 @@ b200_status planes_to_jpeg(const std::vector<uint8_t> &planes, uint32_t w, uint3
 {
     std::string err;
     if (w > 65535 || h > 65535) return make_status(B200_ERR_INVALID_ARGUMENT, "image too large for JPEG");
-    JpegGeom gin; gin.width = (int)w; gin.height = (int)h; gin.ncomp = nc;
-    for (int c = 0; c < nc; c++) { gin.cid[c] = c + 1; gin.hs[c] = gin.vs[c] = 1; gin.tq[c] = 0; }
-    gin.finalize();
+    const JpegGeom gin = planar_geom(w, h, nc);
     JpegGeom gout;
     if (!jpeg_output_geom(gin, (int)p->jpeg_quality, (int)p->jpeg_chroma_subsampling, gout, err)) return make_status(B200_ERR_INVALID_ARGUMENT, err);
     if (p->width || p->height) {
-        uint32_t nw = 0, nh = 0;
-        compute_resize_dimensions(w, h, p->width, p->height, nw, nh);
-        if (nw == 0 || nh == 0 || nw > 65535 || nh > 65535) return make_status(B200_ERR_INVALID_ARGUMENT, "invalid target dimensions");
-        gout.width = (int)nw; gout.height = (int)nh; gout.finalize();
+        uint32_t nw, nh;
+        const b200_status st = target_size(w, h, p, 65535, nw, nh, "invalid target dimensions");
+        if (st.code) return st;
+        gout = with_size(gout, nw, nh);
     }
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    Slot *s = slot_acquire(prefer_dev < 0 ? runtime_next_device() : prefer_dev, err);
-    if (!s) return make_status(B200_ERR_CUDA, err);
-    b200_status st = ok_status();
-    JpegWriteOptions wo; wo.progressive = p->jpeg_progressive != 0;
-    do {
-        if (!slot_transform_resized(s, gin, gout, err, false, false, nullptr, planes.data())) { st = make_status(B200_ERR_CUDA, err); break; }
-        if (slot_gpu_encode(s, gout, wo.progressive, err)) {
-            if (!jpeg_assemble(gout, wo, nullptr, s->enc->results.data(), (int)s->enc->results.size(), out, err)) st = make_status(B200_ERR_INVALID_ARGUMENT, err);
-            break;
-        }
-        if (!s->enc || !s->enc->overflow) { st = make_status(B200_ERR_CUDA, err); break; }
-        if (!slot_download_coefs(s, (size_t)gout.total_coefs * 2, err)) { st = make_status(B200_ERR_CUDA, err); break; }
-        jpeg_fill_dummy_blocks(gout, s->h_out);
-        if (!jpeg_write(gout, s->h_out, wo, nullptr, out, err)) st = make_status(B200_ERR_INVALID_ARGUMENT, err);
-    } while (0);
-    slot_release(s);
-    return st;
+    SlotLease s(prefer_dev);
+    if (!s) return s.failure();
+    if (!slot_transform_resized(s, gin, gout, err, false, false, nullptr, planes.data())) return make_status(B200_ERR_CUDA, err);
+    return encode_from_slot(s, gout, write_options(p), nullptr, out, err);      // no source metadata: only `progressive` matters
 }
 
 b200_status png_to_jpeg(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
 {
     std::string err;
     PngInfo info; std::vector<uint8_t> raw;
-    if (!png_decode(in, in_len, false, info, raw, err)) return make_status(err.find("interlace") != std::string::npos ? B200_ERR_UNSUPPORTED : B200_ERR_CORRUPT_INPUT, err);
+    if (!png_decode(in, in_len, false, info, raw, err)) return png_status(err);
     std::vector<uint8_t> planes; int nc = 3;
     png_expand_planar(info, raw, true, planes, nc);
     return planes_to_jpeg(planes, info.width, info.height, nc, p, prefer_dev, out);
@@ -529,49 +557,35 @@ b200_status rgb_to_webp(const std::vector<uint8_t> &rgb, uint32_t w, uint32_t h,
                         const std::vector<uint8_t> *alpha = nullptr)
 {
     std::string err;
-    uint32_t nw = w, nh = h;
-    if (p->width || p->height) compute_resize_dimensions(w, h, p->width, p->height, nw, nh);
-    if (nw == 0 || nh == 0 || nw > 16383 || nh > 16383 || w > 65535 || h > 65535) return make_status(B200_ERR_INVALID_ARGUMENT, "invalid dimensions for WebP");
+    uint32_t nw, nh;
+    const b200_status st = target_size(w, h, p, 16383, nw, nh, "invalid dimensions for WebP");
+    if (st.code) return st;
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    Slot *s = slot_acquire(prefer_dev < 0 ? runtime_next_device() : prefer_dev, err);
-    if (!s) return make_status(B200_ERR_CUDA, err);
-    if (!s->webp) s->webp = new WebpDevice();
-    bool ok;
-    if (nw == w && nh == h) ok = s->webp->encode_host_rgb(rgb.data(), (int)nw, (int)nh, (int)p->webp_quality, s->stream, out, err);
-    else {   // through the resize leg (K3 Lanczos3) first
-        JpegGeom gin; gin.width = (int)w; gin.height = (int)h; gin.ncomp = 3;
-        for (int c = 0; c < 3; c++) { gin.cid[c] = c + 1; gin.hs[c] = gin.vs[c] = 1; gin.tq[c] = 0; }
-        gin.finalize();
-        JpegGeom gout = gin; gout.width = (int)nw; gout.height = (int)nh; gout.finalize();
+    SlotLease s(prefer_dev);
+    if (!s) return s.failure();
+    WebpDevice *webp = s->webp_dev();
+    const bool resize = nw != w || nh != h;
+    if (!resize) {
+        if (!webp->encode_host_rgb(rgb.data(), (int)nw, (int)nh, (int)p->webp_quality, s->stream, out, err)) return make_status(B200_ERR_CUDA, err);
+    } else {   // through the resize leg (K3 Lanczos3) first
+        const JpegGeom gin = planar_geom(w, h, 3);
         uint8_t *planes[3] = {nullptr, nullptr, nullptr};
-        ok = slot_transform_resized(s, gin, gout, err, false, false, planes, rgb.data()) &&
-             s->webp->encode_planes(planes[0], planes[1], planes[2], (int)nw, (int)nh, (int)p->webp_quality, s->stream, out, err);
+        if (!slot_transform_resized(s, gin, with_size(gin, nw, nh), err, false, false, planes, rgb.data()) ||
+            !webp->encode_planes(planes[0], planes[1], planes[2], (int)nw, (int)nh, (int)p->webp_quality, s->stream, out, err)) return make_status(B200_ERR_CUDA, err);
     }
-    if (ok && alpha) {
-        const size_t n = (size_t)nw * nh;
-        std::vector<uint8_t> resized;
-        const uint8_t *ap = alpha->data();
-        if (nw != w || nh != h) {
-            JpegGeom gin; gin.width = (int)w; gin.height = (int)h; gin.ncomp = 1; gin.cid[0] = 1; gin.hs[0] = gin.vs[0] = 1; gin.tq[0] = 0; gin.finalize();
-            JpegGeom gout = gin; gout.width = (int)nw; gout.height = (int)nh; gout.finalize();
-            uint8_t *planes[3] = {nullptr, nullptr, nullptr};
-            resized.resize(n);
-            ok = slot_transform_resized(s, gin, gout, err, false, false, planes, alpha->data()) && slot_fetch_planes(s, planes, 1, n, resized.data(), err);
-            ap = resized.data();
-        }
-        bool opaque = true;
-        for (size_t i = 0; ok && i < n; i++) if (ap[i] != 0xFF) { opaque = false; break; }
-        if (ok && !opaque) {
-            if (!s->png) s->png = new PngDevice();
-            std::vector<uint32_t> tokens; std::vector<uint8_t> alph, wrapped, residual;
-            const int filter = webp_alpha_choose_filter(ap, (int)nw, (int)nh, residual);
-            ok = s->png->plane_tokens(filter ? residual.data() : ap, n, (int)nw, s->stream, tokens, err);
-            if (ok && !(vp8l_alpha_from_tokens(tokens.data(), tokens.size(), (int)nw, (int)nh, alph, filter) && webp_wrap_alpha(out, alph, (int)nw, (int)nh, wrapped))) { ok = false; err = "alpha plane could not be coded"; }
-            if (ok) out.swap(wrapped);
-        }
-    }
-    slot_release(s);
-    return ok ? ok_status() : make_status(B200_ERR_CUDA, err);
+    if (!alpha) return ok_status();
+    const size_t n = (size_t)nw * nh;
+    std::vector<uint8_t> resized;
+    if (resize && !resize_to_host(s, alpha->data(), w, h, nw, nh, 1, resized, err)) return make_status(B200_ERR_CUDA, err);
+    const uint8_t *ap = resize ? resized.data() : alpha->data();
+    if (std::all_of(ap, ap + n, [](uint8_t v) { return v == 0xFF; })) return ok_status();
+    std::vector<uint32_t> tokens; std::vector<uint8_t> alph, wrapped, residual;
+    const int filter = webp_alpha_choose_filter(ap, (int)nw, (int)nh, residual);
+    if (!s->png_dev()->plane_tokens(filter ? residual.data() : ap, n, (int)nw, s->stream, tokens, err)) return make_status(B200_ERR_CUDA, err);
+    if (!(vp8l_alpha_from_tokens(tokens.data(), tokens.size(), (int)nw, (int)nh, alph, filter) && webp_wrap_alpha(out, alph, (int)nw, (int)nh, wrapped)))
+        return make_status(B200_ERR_CUDA, "alpha plane could not be coded");
+    out.swap(wrapped);
+    return ok_status();
 }
 
 // The transparency of decoded PNG samples as one 8-bit plane (alpha channel: high byte of a 16-bit sample; tRNS: the palette's
@@ -636,10 +650,10 @@ b200_status png_to_webp(const uint8_t *in, size_t in_len, const b200_params *p, 
 {
     std::string err;
     PngInfo info; std::vector<uint8_t> raw;
-    if (!png_decode(in, in_len, false, info, raw, err)) return make_status(err.find("interlace") != std::string::npos ? B200_ERR_UNSUPPORTED : B200_ERR_CORRUPT_INPUT, err);
-    uint32_t nw = info.width, nh = info.height;
-    if (p->width || p->height) compute_resize_dimensions(info.width, info.height, p->width, p->height, nw, nh);
-    if (nw == 0 || nh == 0 || nw > 16383 || nh > 16383 || info.width > 65535 || info.height > 65535) return make_status(B200_ERR_INVALID_ARGUMENT, "invalid dimensions for WebP");
+    if (!png_decode(in, in_len, false, info, raw, err)) return png_status(err);
+    uint32_t nw, nh;
+    const b200_status st = target_size(info.width, info.height, p, 16383, nw, nh, "invalid dimensions for WebP");
+    if (st.code) return st;
     // transparency (alpha channel, tRNS) travels as the file's alpha plane: VP8X + ALPH next to the lossy frame
     std::vector<uint8_t> alpha;
     const bool has_alpha = png_extract_alpha(info, raw, alpha);
@@ -653,56 +667,47 @@ b200_status rgb_to_png(const std::vector<uint8_t> &rgb, uint32_t w, uint32_t h, 
                        const std::vector<uint8_t> *alpha = nullptr)
 {
     std::string err;
-    uint32_t nw = w, nh = h;
-    if (p->width || p->height) compute_resize_dimensions(w, h, p->width, p->height, nw, nh);
-    if (nw == 0 || nh == 0 || nw > 65535 || nh > 65535 || w > 65535 || h > 65535) return make_status(B200_ERR_INVALID_ARGUMENT, "invalid target dimensions");
+    uint32_t nw, nh;
+    const b200_status st = target_size(w, h, p, 65535, nw, nh, "invalid target dimensions");
+    if (st.code) return st;
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    Slot *s = slot_acquire(prefer_dev < 0 ? runtime_next_device() : prefer_dev, err);
-    if (!s) return make_status(B200_ERR_CUDA, err);
-    b200_status st = ok_status();
-    const size_t n = (size_t)nw * nh;
-    std::vector<uint8_t> planes, raw(3 * n);
-    const uint8_t *src = rgb.data();
-    do {
-        if (nw != w || nh != h) {
-            JpegGeom gin; gin.width = (int)w; gin.height = (int)h; gin.ncomp = 3;
-            for (int c = 0; c < 3; c++) { gin.cid[c] = c + 1; gin.hs[c] = gin.vs[c] = 1; gin.tq[c] = 0; }
-            gin.finalize();
-            JpegGeom gout = gin; gout.width = (int)nw; gout.height = (int)nh; gout.finalize();
-            uint8_t *dp[3] = {nullptr, nullptr, nullptr};
-            planes.resize(3 * n);
-            if (!slot_transform_resized(s, gin, gout, err, false, false, dp, rgb.data()) || !slot_fetch_planes(s, dp, 3, n, planes.data(), err)) { st = make_status(B200_ERR_CUDA, err); break; }
-            src = planes.data();
-        }
-        PngInfo info; info.width = nw; info.height = nh; info.bit_depth = 8;
-        if (!alpha) {
-            for (size_t i = 0; i < n; i++) { raw[3 * i] = src[i]; raw[3 * i + 1] = src[n + i]; raw[3 * i + 2] = src[2 * n + i]; }
-            info.color_type = 2; info.channels = 3; info.bits_per_pixel = 24; info.bpp = 3; info.row_bytes = (size_t)nw * 3;
-        } else {
-            // transparency stays: RGBA samples (the alpha plane takes the same Lanczos3 as the colour planes)
-            std::vector<uint8_t> ra;
-            const uint8_t *ap = alpha->data();
-            if (nw != w || nh != h) {
-                JpegGeom gin; gin.width = (int)w; gin.height = (int)h; gin.ncomp = 1; gin.cid[0] = 1; gin.hs[0] = gin.vs[0] = 1; gin.tq[0] = 0; gin.finalize();
-                JpegGeom gout = gin; gout.width = (int)nw; gout.height = (int)nh; gout.finalize();
-                uint8_t *dp[3] = {nullptr, nullptr, nullptr};
-                ra.resize(n);
-                if (!slot_transform_resized(s, gin, gout, err, false, false, dp, alpha->data()) || !slot_fetch_planes(s, dp, 1, n, ra.data(), err)) { st = make_status(B200_ERR_CUDA, err); break; }
-                ap = ra.data();
-            }
-            raw.resize(4 * n);
-            for (size_t i = 0; i < n; i++) { raw[4 * i] = src[i]; raw[4 * i + 1] = src[n + i]; raw[4 * i + 2] = src[2 * n + i]; raw[4 * i + 3] = ap[i]; }
-            info.color_type = 6; info.channels = 4; info.bits_per_pixel = 32; info.bpp = 4; info.row_bytes = (size_t)nw * 4;
-        }
-        png_reduce_palette(info, raw);
-        if (!s->png) s->png = new PngDevice();
-        std::vector<uint8_t> z;
-        int level = (int)p->png_optimization_level; if (level > 6) level = 6;
-        if (!s->png->compress(info, raw, level, s->stream, z, nullptr, err)) { st = make_status(B200_ERR_CUDA, err); break; }
-        png_write(info, z, out);
-    } while (0);
-    slot_release(s);
-    return st;
+    SlotLease s(prefer_dev);
+    if (!s) return s.failure();
+    const uint8_t *src = rgb.data(), *ap = alpha ? alpha->data() : nullptr;
+    std::vector<uint8_t> planes, ra;
+    if (nw != w || nh != h) {   // transparency stays: the alpha plane takes the same Lanczos3 as the colour planes
+        if (!resize_to_host(s, src, w, h, nw, nh, 3, planes, err) || (ap && !resize_to_host(s, ap, w, h, nw, nh, 1, ra, err))) return make_status(B200_ERR_CUDA, err);
+        src = planes.data();
+        if (ap) ap = ra.data();
+    }
+    return png_from_planes(s, src, 3, ap, nw, nh, true, p, out, err);
+}
+
+// libcaesium convert_in_memory for a source of format src: the conversions this path takes, the refusals in the reference's order
+b200_status convert_dispatch(const uint8_t *in, size_t in_len, uint32_t src, uint32_t fmt, const b200_params *p, std::vector<uint8_t> &out)
+{
+    if (src == B200_FMT_UNKNOWN) return make_status(B200_ERR_UNKNOWN_FORMAT, "Unknown file type");
+    if (src == fmt) return make_status(B200_ERR_SAME_FORMAT, "Cannot convert to the same format");
+    if (fmt == B200_FMT_PNG && src == B200_FMT_JPEG) return jpeg_to_png(in, in_len, p, -1, out);
+    if (src == B200_FMT_WEBP && (fmt == B200_FMT_JPEG || fmt == B200_FMT_PNG)) {
+        // WebP source: decoded on the calling thread (vp8_decode.cpp), then the same back ends as a PNG source
+        if (fmt == B200_FMT_JPEG && p->jpeg_optimize) return make_status(B200_ERR_UNSUPPORTED, "lossless conversion to JPEG is outside the GPU path (route to caesium::convert_in_memory)");
+        if (fmt == B200_FMT_PNG && !p->png_optimize) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::convert_in_memory)");
+        WebpInfo wi; std::vector<uint8_t> rgb, alpha;
+        const b200_status s = webp_decode_status(in, in_len, wi, rgb, &alpha);
+        if (s.code) return s;
+        // a JPEG has no alpha (the image crate's to_rgb8 drops it); a PNG keeps it as an RGBA image
+        return fmt == B200_FMT_JPEG ? planes_to_jpeg(rgb, (uint32_t)wi.width, (uint32_t)wi.height, 3, p, -1, out)
+                                    : rgb_to_png(rgb, (uint32_t)wi.width, (uint32_t)wi.height, p, -1, out, alpha.empty() ? nullptr : &alpha);
+    }
+    const bool to_webp = fmt == B200_FMT_WEBP, png_to_jpg = fmt == B200_FMT_JPEG && src == B200_FMT_PNG;
+    if (!to_webp && !png_to_jpg) return make_status(B200_ERR_UNSUPPORTED, "this conversion is outside the GPU path (route to caesium::convert_in_memory)");
+    if (to_webp && p->webp_lossless) return make_status(B200_ERR_UNSUPPORTED, "lossless WebP (VP8L) is outside the GPU path (route to caesium::convert_in_memory)");
+    if (png_to_jpg && p->jpeg_optimize) return make_status(B200_ERR_UNSUPPORTED, "lossless conversion to JPEG is outside the GPU path (route to caesium::convert_in_memory)");
+    if (png_to_jpg) return png_to_jpeg(in, in_len, p, -1, out);
+    if (src == B200_FMT_JPEG) return jpeg_to_webp(in, in_len, p, -1, out);
+    if (src == B200_FMT_PNG) return png_to_webp(in, in_len, p, -1, out);
+    return make_status(B200_ERR_UNSUPPORTED, "conversion from this format is outside the GPU path (route to caesium::convert_in_memory)");
 }
 
 b200_status compress_dispatch(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
@@ -754,8 +759,7 @@ static b200_status jpeg_to_size(const uint8_t *in, size_t in_len, b200_params *p
     if (!rd.read_header(err)) return header_status(err);
     const JpegGeom &gin = rd.geom();
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    if (g_entropy_mode.load() < 0) { const char *e = getenv("B200_ENTROPY"); g_entropy_mode.store(!e ? 3 : !strcmp(e, "host") ? 0 : !strcmp(e, "gpuenc") ? 1 : !strcmp(e, "gpudec") ? 2 : 3); }
-    if (params->width || params->height || (g_entropy_mode.load() & 1) == 0) {
+    if (params->width || params->height || (entropy_mode() & 1) == 0) {
         // resize, or the host-entropy mode: every try is a whole compress call (the resized planes are not kept between tries)
         auto size_at = [&](int q, auto want, size_t &sz, std::vector<uint8_t> &cur) {
             b200_params p = *params; p.jpeg_quality = (uint32_t)q; p.jpeg_optimize = 0;
@@ -765,40 +769,31 @@ static b200_status jpeg_to_size(const uint8_t *in, size_t in_len, b200_params *p
         };
         return bisect_quality(size_at, max_output_size, return_smallest, &params->jpeg_quality, result);
     }
-    Slot *s = slot_acquire(runtime_next_device(), err);
-    if (!s) return make_status(B200_ERR_CUDA, err);
-    b200_status st = ok_status();
-    do {
-        JpegGeom g0;
-        if (!jpeg_output_geom(gin, 80, (int)params->jpeg_chroma_subsampling, g0, err)) { st = make_status(B200_ERR_INVALID_ARGUMENT, err); break; }
-        ImagePlan plan;
-        if (!plan_image(gin, g0, plan, err)) { st = make_status(B200_ERR_UNSUPPORTED, err); break; }
-        if (!s->ensure(plan.in_bytes, plan.out_bytes, plan.scratch_bytes(), 1 << 14, err)) { st = make_status(B200_ERR_OUT_OF_MEMORY, err); break; }
-        bool resident = false;                      // coefficients already in s->d_in?
-        JpegReader::DeviceScan ds;
-        if ((g_entropy_mode.load() & 2) && rd.device_decodable(ds)) {
-            const int r = slot_gpu_decode(s, rd, ds, err);
-            if (r == 0) resident = true; else if (r != 1) { st = make_status(B200_ERR_CUDA, err); break; }
+    SlotLease s(-1);
+    if (!s) return s.failure();
+    JpegGeom g0;
+    if (!jpeg_output_geom(gin, 80, (int)params->jpeg_chroma_subsampling, g0, err)) return make_status(B200_ERR_INVALID_ARGUMENT, err);
+    ImagePlan plan;
+    if (!plan_image(gin, g0, plan, err)) return make_status(B200_ERR_UNSUPPORTED, err);
+    if (!s->ensure(plan.in_bytes, plan.out_bytes, plan.scratch_bytes(), 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    bool resident;                                  // coefficients already in s->d_in?
+    const b200_status st = decode_into_slot(s, rd, resident, err);
+    if (st.code) return st;
+    const JpegWriteOptions wo = write_options(params);
+    auto size_at = [&](int q, auto want, size_t &sz, std::vector<uint8_t> &cur) -> b200_status {
+        JpegGeom gout; std::string e2;
+        if (!jpeg_output_geom(gin, q, (int)params->jpeg_chroma_subsampling, gout, e2)) return make_status(B200_ERR_INVALID_ARGUMENT, e2);
+        if (!slot_transform(s, gin, gout, e2, false, !resident)) return make_status(B200_ERR_CUDA, e2);
+        resident = true;                            // the first try uploaded them if the host decoded
+        if (!slot_gpu_encode_sizes(s, gout, wo.progressive, e2)) return make_status(B200_ERR_CUDA, e2);
+        sz = jpeg_assembled_size(gout, wo, &rd.meta(), s->enc->results.data(), (int)s->enc->results.size());
+        if (want(sz)) {
+            if (!slot_gpu_fetch(s, e2)) return make_status(B200_ERR_CUDA, e2);
+            if (!jpeg_assemble(gout, wo, &rd.meta(), s->enc->results.data(), (int)s->enc->results.size(), cur, e2)) return make_status(B200_ERR_INVALID_ARGUMENT, e2);
         }
-        if (!resident && !rd.decode(s->h_in, err)) { st = make_status(B200_ERR_CORRUPT_INPUT, err); break; }
-        JpegWriteOptions wo; wo.progressive = params->jpeg_progressive != 0; wo.keep_metadata = params->keep_metadata != 0; wo.preserve_icc = params->jpeg_preserve_icc != 0;
-        auto size_at = [&](int q, auto want, size_t &sz, std::vector<uint8_t> &cur) -> b200_status {
-            JpegGeom gout; std::string e2;
-            if (!jpeg_output_geom(gin, q, (int)params->jpeg_chroma_subsampling, gout, e2)) return make_status(B200_ERR_INVALID_ARGUMENT, e2);
-            if (!slot_transform(s, gin, gout, e2, false, !resident)) return make_status(B200_ERR_CUDA, e2);
-            resident = true;                        // the first try uploaded them if the host decoded
-            if (!slot_gpu_encode_sizes(s, gout, wo.progressive, e2)) return make_status(B200_ERR_CUDA, e2);
-            sz = jpeg_assembled_size(gout, wo, &rd.meta(), s->enc->results.data(), (int)s->enc->results.size());
-            if (want(sz)) {
-                if (!slot_gpu_fetch(s, e2)) return make_status(B200_ERR_CUDA, e2);
-                if (!jpeg_assemble(gout, wo, &rd.meta(), s->enc->results.data(), (int)s->enc->results.size(), cur, e2)) return make_status(B200_ERR_INVALID_ARGUMENT, e2);
-            }
-            return ok_status();
-        };
-        st = bisect_quality(size_at, max_output_size, return_smallest, &params->jpeg_quality, result);
-    } while (0);
-    slot_release(s);
-    return st;
+        return ok_status();
+    };
+    return bisect_quality(size_at, max_output_size, return_smallest, &params->jpeg_quality, result);
 }
 
 } // namespace
@@ -921,57 +916,23 @@ b200_status b200_compress_in_memory(const uint8_t *in, size_t in_len, const b200
 {
     if (!in || !params || !out || !out_len) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
     *out = nullptr; *out_len = 0;
-    if (coalesce_mode() && b200_sniff_format(in, in_len) == B200_FMT_JPEG) {
-        try { return coalesced_compress(in, in_len, params, out, out_len); }
-        catch (const std::exception &e) { return make_status(B200_ERR_OUT_OF_MEMORY, e.what()); } catch (...) { return make_status(B200_ERR_INVALID_ARGUMENT, "unexpected failure"); }
-    }
-    try {
+    if (coalesce_mode() && b200_sniff_format(in, in_len) == B200_FMT_JPEG) return guarded([&] { return coalesced_compress(in, in_len, params, out, out_len); });
+    return guarded([&] {
         std::vector<uint8_t> v;
-        b200_status s = compress_dispatch(in, in_len, params, -1, v);
-        if (s.code) return s;
-        return give(v, out, out_len);
-    } catch (const std::exception &e) { return make_status(B200_ERR_OUT_OF_MEMORY, e.what()); } catch (...) { return make_status(B200_ERR_INVALID_ARGUMENT, "unexpected failure"); }
+        const b200_status s = compress_dispatch(in, in_len, params, -1, v);
+        return s.code ? s : give(v, out, out_len);
+    });
 }
 
 b200_status b200_convert_in_memory(const uint8_t *in, size_t in_len, const b200_params *params, uint32_t fmt, uint8_t **out, size_t *out_len)
 {
     if (!in || !params || !out || !out_len) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
     *out = nullptr; *out_len = 0;
-    uint32_t src = b200_sniff_format(in, in_len);
-    if (src == B200_FMT_UNKNOWN) return make_status(B200_ERR_UNKNOWN_FORMAT, "Unknown file type");
-    if (src == fmt) return make_status(B200_ERR_SAME_FORMAT, "Cannot convert to the same format");
-    const bool to_webp = fmt == B200_FMT_WEBP, png_to_jpg = fmt == B200_FMT_JPEG && src == B200_FMT_PNG, jpg_to_png = fmt == B200_FMT_PNG && src == B200_FMT_JPEG;
-    if (jpg_to_png) {
-        try { std::vector<uint8_t> v; b200_status s = jpeg_to_png(in, in_len, params, -1, v); if (s.code) return s; return give(v, out, out_len); }
-        catch (const std::exception &e) { return make_status(B200_ERR_OUT_OF_MEMORY, e.what()); }
-    }
-    if (src == B200_FMT_WEBP && (fmt == B200_FMT_JPEG || fmt == B200_FMT_PNG)) {
-        // WebP source: decoded on the calling thread (vp8_decode.cpp), then the same back ends as a PNG source
-        try {
-            if (fmt == B200_FMT_JPEG && params->jpeg_optimize) return make_status(B200_ERR_UNSUPPORTED, "lossless conversion to JPEG is outside the GPU path (route to caesium::convert_in_memory)");
-            if (fmt == B200_FMT_PNG && !params->png_optimize) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::convert_in_memory)");
-            WebpInfo wi; std::vector<uint8_t> rgb, alpha, v;
-            b200_status s = webp_decode_status(in, in_len, wi, rgb, &alpha);
-            if (s.code) return s;
-            // a JPEG has no alpha (the image crate's to_rgb8 drops it); a PNG keeps it as an RGBA image
-            s = fmt == B200_FMT_JPEG ? planes_to_jpeg(rgb, (uint32_t)wi.width, (uint32_t)wi.height, 3, params, -1, v)
-                                     : rgb_to_png(rgb, (uint32_t)wi.width, (uint32_t)wi.height, params, -1, v, alpha.empty() ? nullptr : &alpha);
-            if (s.code) return s;
-            return give(v, out, out_len);
-        } catch (const std::exception &e) { return make_status(B200_ERR_OUT_OF_MEMORY, e.what()); }
-    }
-    if (!to_webp && !png_to_jpg) return make_status(B200_ERR_UNSUPPORTED, "this conversion is outside the GPU path (route to caesium::convert_in_memory)");
-    if (to_webp && params->webp_lossless) return make_status(B200_ERR_UNSUPPORTED, "lossless WebP (VP8L) is outside the GPU path (route to caesium::convert_in_memory)");
-    if (png_to_jpg && params->jpeg_optimize) return make_status(B200_ERR_UNSUPPORTED, "lossless conversion to JPEG is outside the GPU path (route to caesium::convert_in_memory)");
-    try {
+    return guarded([&] {
         std::vector<uint8_t> v;
-        b200_status s = png_to_jpg ? png_to_jpeg(in, in_len, params, -1, v)
-                      : src == B200_FMT_JPEG ? jpeg_to_webp(in, in_len, params, -1, v)
-                      : src == B200_FMT_PNG ? png_to_webp(in, in_len, params, -1, v)
-                      : make_status(B200_ERR_UNSUPPORTED, "conversion from this format is outside the GPU path (route to caesium::convert_in_memory)");
-        if (s.code) return s;
-        return give(v, out, out_len);
-    } catch (const std::exception &e) { return make_status(B200_ERR_OUT_OF_MEMORY, e.what()); }
+        const b200_status s = convert_dispatch(in, in_len, b200_sniff_format(in, in_len), fmt, params, v);
+        return s.code ? s : give(v, out, out_len);
+    });
 }
 
 // WebP: the source is decoded once, its RGB uploaded once (resized once if asked); every try runs K8 at the try's quality and the
@@ -984,31 +945,23 @@ static b200_status webp_to_size(const uint8_t *in, size_t in_len, b200_params *p
     b200_status st = webp_decode_status(in, in_len, wi, rgb, &alpha);
     if (st.code) return st;
     if (!alpha.empty()) return make_status(B200_ERR_UNSUPPORTED, "compress_to_size on a WebP with an alpha plane is outside the GPU path (route to caesium::compress_to_size_in_memory)");
-    uint32_t w = (uint32_t)wi.width, h = (uint32_t)wi.height, nw = w, nh = h;
-    if (params->width || params->height) compute_resize_dimensions(w, h, params->width, params->height, nw, nh);
-    if (nw == 0 || nh == 0 || nw > 16383 || nh > 16383) return make_status(B200_ERR_INVALID_ARGUMENT, "invalid dimensions for WebP");
+    uint32_t nw, nh;
+    if ((st = target_size((uint32_t)wi.width, (uint32_t)wi.height, params, 16383, nw, nh, "invalid dimensions for WebP")).code) return st;
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    Slot *s = slot_acquire(runtime_next_device(), err);
-    if (!s) return make_status(B200_ERR_CUDA, err);
-    if (!s->webp) s->webp = new WebpDevice();
-    do {
-        uint8_t *planes[3] = {nullptr, nullptr, nullptr};
-        JpegGeom gin; gin.width = (int)w; gin.height = (int)h; gin.ncomp = 3;
-        for (int c = 0; c < 3; c++) { gin.cid[c] = c + 1; gin.hs[c] = gin.vs[c] = 1; gin.tq[c] = 0; }
-        gin.finalize();
-        JpegGeom gout = gin; gout.width = (int)nw; gout.height = (int)nh; gout.finalize();
-        // the (possibly resized) RGB planes stay in the slot's scratch memory for all tries
-        if (!slot_transform_resized(s, gin, gout, err, false, false, planes, rgb.data())) { st = make_status(B200_ERR_CUDA, err); break; }
-        auto size_at = [&](int q, auto want, size_t &sz, std::vector<uint8_t> &cur) -> b200_status {
-            std::string e2; (void)want;
-            if (!s->webp->encode_planes(planes[0], planes[1], planes[2], (int)nw, (int)nh, q, s->stream, cur, e2)) return make_status(B200_ERR_CUDA, e2);
-            sz = cur.size();
-            return ok_status();
-        };
-        st = bisect_quality(size_at, max_output_size, return_smallest, &params->webp_quality, result);
-    } while (0);
-    slot_release(s);
-    return st;
+    SlotLease s(-1);
+    if (!s) return s.failure();
+    WebpDevice *webp = s->webp_dev();
+    uint8_t *planes[3] = {nullptr, nullptr, nullptr};
+    const JpegGeom gin = planar_geom((uint32_t)wi.width, (uint32_t)wi.height, 3);
+    // the (possibly resized) RGB planes stay in the slot's scratch memory for all tries
+    if (!slot_transform_resized(s, gin, with_size(gin, nw, nh), err, false, false, planes, rgb.data())) return make_status(B200_ERR_CUDA, err);
+    auto size_at = [&](int q, auto want, size_t &sz, std::vector<uint8_t> &cur) -> b200_status {
+        std::string e2; (void)want;
+        if (!webp->encode_planes(planes[0], planes[1], planes[2], (int)nw, (int)nh, q, s->stream, cur, e2)) return make_status(B200_ERR_CUDA, e2);
+        sz = cur.size();
+        return ok_status();
+    };
+    return bisect_quality(size_at, max_output_size, return_smallest, &params->webp_quality, result);
 }
 
 b200_status b200_compress_to_size_in_memory(const uint8_t *in, size_t in_len, b200_params *params, size_t max_output_size, uint8_t return_smallest,
@@ -1016,7 +969,7 @@ b200_status b200_compress_to_size_in_memory(const uint8_t *in, size_t in_len, b2
 {
     if (!in || !params || !out || !out_len) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
     *out = nullptr; *out_len = 0;
-    try {
+    return guarded([&] {
         // input already small enough is returned unchanged
         if (in_len <= max_output_size) { std::vector<uint8_t> v(in, in + in_len); return give(v, out, out_len); }
         uint32_t fmt = b200_sniff_format(in, in_len);
@@ -1026,9 +979,8 @@ b200_status b200_compress_to_size_in_memory(const uint8_t *in, size_t in_len, b2
         else if (fmt == B200_FMT_WEBP) s = webp_to_size(in, in_len, params, max_output_size, return_smallest != 0, result);
         else if (fmt == B200_FMT_PNG) s = make_status(B200_ERR_UNSUPPORTED, "compress_to_size on a PNG bisects the lossy (imagequant) quality, which is outside the GPU path (route to caesium::compress_to_size_in_memory)");
         else s = make_status(fmt == B200_FMT_UNKNOWN ? B200_ERR_UNKNOWN_FORMAT : B200_ERR_UNSUPPORTED, "compress_to_size for this format is outside the GPU path (route to caesium::compress_to_size_in_memory)");
-        if (s.code) return s;
-        return give(result, out, out_len);
-    } catch (const std::exception &e) { return make_status(B200_ERR_OUT_OF_MEMORY, e.what()); } catch (...) { return make_status(B200_ERR_INVALID_ARGUMENT, "unexpected failure"); }
+        return s.code ? s : give(result, out, out_len);
+    });
 }
 
 int b200_compress_batch(const uint8_t *const *in, const size_t *in_len, int n, const b200_params *params, int n_threads,
@@ -1040,19 +992,18 @@ int b200_compress_batch(const uint8_t *const *in, const size_t *in_len, int n, c
     std::atomic<int> failed{0};
     { std::string e; ensure_runtime(e); }
     const int ndev = std::max(1, runtime_device_count());
-    if (g_entropy_mode.load() < 0) { const char *e = getenv("B200_ENTROPY"); g_entropy_mode.store(!e ? 3 : !strcmp(e, "host") ? 0 : !strcmp(e, "gpuenc") ? 1 : !strcmp(e, "gpudec") ? 2 : 3); }
     // Megabatches: with both entropy stages on the device, consecutive images are processed K at a time -- one launch
     // sequence (decode rounds, transform, encode passes) for the whole group instead of one per image.  Images that do not
     // fit the group path (other formats, progressive input, resize, odd one out in shape) go through the per-image path.
     int K = 8; { const char *e = getenv("B200_MEGABATCH"); if (e) K = std::max(1, std::min(64, atoi(e))); }
-    const bool grouped = runtime_device_count() > 0 && g_entropy_mode.load() == 3 && K > 1 && ((!params->width && !params->height) || params->jpeg_optimize);
+    const bool grouped = runtime_device_count() > 0 && entropy_mode() == 3 && K > 1 && ((!params->width && !params->height) || params->jpeg_optimize);
     auto one = [&](int i, int dev) {
         out[i] = nullptr; out_len[i] = 0;
-        try {
+        status[i] = guarded([&] {
             std::vector<uint8_t> v;
-            status[i] = compress_dispatch(in[i], in_len[i], params, dev, v);
-            if (!status[i].code) status[i] = give(v, &out[i], &out_len[i]);
-        } catch (const std::exception &e) { status[i] = make_status(B200_ERR_OUT_OF_MEMORY, e.what()); } catch (...) { status[i] = make_status(B200_ERR_INVALID_ARGUMENT, "unexpected failure"); }
+            const b200_status s = compress_dispatch(in[i], in_len[i], params, dev, v);
+            return s.code ? s : give(v, &out[i], &out_len[i]);
+        });
         if (status[i].code) failed++;
     };
     auto run_threads = [](int nt, const std::function<void()> &fn) {
@@ -1160,19 +1111,15 @@ b200_status b200_jpeg_requantize(const b200_jpeg_layout *in_layout, const int16_
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
     ImagePlan plan;
     if (!plan_image(gin, gout, plan, err)) return make_status(B200_ERR_UNSUPPORTED, err);
-    Slot *s = slot_acquire(runtime_next_device(), err);
-    if (!s) return make_status(B200_ERR_CUDA, err);
-    b200_status st = ok_status();
-    do {
-        if (!s->ensure(plan.in_bytes, plan.out_bytes, plan.scratch_bytes(), 1 << 14, err)) { st = make_status(B200_ERR_OUT_OF_MEMORY, err); break; }
-        memcpy(s->h_in, in_coefs, plan.in_bytes);
-        memset(s->h_out, 0, plan.out_bytes);
-        if (!slot_transform(s, gin, gout, err)) { st = make_status(B200_ERR_CUDA, err); break; }
-        jpeg_fill_dummy_blocks(gout, s->h_out);
-        memcpy(out_coefs, s->h_out, plan.out_bytes);
-    } while (0);
-    slot_release(s);
-    return st;
+    SlotLease s(-1);
+    if (!s) return s.failure();
+    if (!s->ensure(plan.in_bytes, plan.out_bytes, plan.scratch_bytes(), 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    memcpy(s->h_in, in_coefs, plan.in_bytes);
+    memset(s->h_out, 0, plan.out_bytes);
+    if (!slot_transform(s, gin, gout, err)) return make_status(B200_ERR_CUDA, err);
+    jpeg_fill_dummy_blocks(gout, s->h_out);
+    memcpy(out_coefs, s->h_out, plan.out_bytes);
+    return ok_status();
 }
 
 b200_status b200_jpeg_encode_coefficients(const b200_jpeg_layout *layout, const int16_t *coefs, int progressive, uint8_t **out, size_t *out_len)
@@ -1192,21 +1139,16 @@ b200_status b200_jpeg_encode_coefficients_device(const b200_jpeg_layout *layout,
     std::string err; JpegGeom g;
     if (!geom_from_layout(layout, g, err)) return make_status(B200_ERR_INVALID_ARGUMENT, err);
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    Slot *s = slot_acquire(runtime_next_device(), err);
-    if (!s) return make_status(B200_ERR_CUDA, err);
-    b200_status st = ok_status();
+    SlotLease s(-1);
+    if (!s) return s.failure();
+    const size_t bytes = (size_t)g.total_coefs * 2;
+    if (!s->ensure(256, bytes, 256, 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    memcpy(s->h_out, coefs, bytes);
+    if (!slot_upload_out_coefs(s, bytes, err)) return make_status(B200_ERR_CUDA, err);
+    JpegWriteOptions wo; wo.progressive = progressive != 0;
+    if (!slot_gpu_encode(s, g, wo.progressive, err)) return make_status(B200_ERR_CUDA, err);
     std::vector<uint8_t> v;
-    do {
-        const size_t bytes = (size_t)g.total_coefs * 2;
-        if (!s->ensure(256, bytes, 256, 1 << 14, err)) { st = make_status(B200_ERR_OUT_OF_MEMORY, err); break; }
-        memcpy(s->h_out, coefs, bytes);
-        if (!slot_upload_out_coefs(s, bytes, err)) { st = make_status(B200_ERR_CUDA, err); break; }
-        JpegWriteOptions wo; wo.progressive = progressive != 0;
-        if (!slot_gpu_encode(s, g, wo.progressive, err)) { st = make_status(B200_ERR_CUDA, err); break; }
-        if (!jpeg_assemble(g, wo, nullptr, s->enc->results.data(), (int)s->enc->results.size(), v, err)) { st = make_status(B200_ERR_INVALID_ARGUMENT, err); break; }
-    } while (0);
-    slot_release(s);
-    if (st.code) return st;
+    if (!jpeg_assemble(g, wo, nullptr, s->enc->results.data(), (int)s->enc->results.size(), v, err)) return make_status(B200_ERR_INVALID_ARGUMENT, err);
     return give(v, out, out_len);
 }
 
@@ -1216,16 +1158,12 @@ b200_status b200_jpeg_decode_planes(const b200_jpeg_layout *in_layout, const int
     std::string err; JpegGeom gin;
     if (!geom_from_layout(in_layout, gin, err)) return make_status(B200_ERR_INVALID_ARGUMENT, err);
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    Slot *s = slot_acquire(runtime_next_device(), err);
-    if (!s) return make_status(B200_ERR_CUDA, err);
-    b200_status st = ok_status();
-    do {
-        if (!s->ensure((size_t)gin.total_coefs * 2, 256, 256, 1 << 14, err)) { st = make_status(B200_ERR_OUT_OF_MEMORY, err); break; }
-        memcpy(s->h_in, in_coefs, (size_t)gin.total_coefs * 2);
-        if (!slot_decode_planes(s, gin, planes, err)) { st = make_status(B200_ERR_CUDA, err); break; }
-    } while (0);
-    slot_release(s);
-    return st;
+    SlotLease s(-1);
+    if (!s) return s.failure();
+    if (!s->ensure((size_t)gin.total_coefs * 2, 256, 256, 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    memcpy(s->h_in, in_coefs, (size_t)gin.total_coefs * 2);
+    if (!slot_decode_planes(s, gin, planes, err)) return make_status(B200_ERR_CUDA, err);
+    return ok_status();
 }
 
 void b200_jpeg_quant_table(int quality, int which, uint16_t out[64]) { jpeg_quant_table(quality, which, out); }
@@ -1275,12 +1213,12 @@ b200_status b200_jpeg_pipe_create(const uint8_t *const *in, const size_t *in_len
     *pipe = nullptr;
     std::string err;
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    try {
+    return guarded([&] {
         JpegPipe *P = pipe_create(in, in_len, n, params, group > 0 ? group : 8, err);
         if (!P) return make_status(B200_ERR_INVALID_ARGUMENT, err);
         *pipe = new b200_jpeg_pipe{P};
-    } catch (const std::exception &e) { return make_status(B200_ERR_OUT_OF_MEMORY, e.what()); }
-    return ok_status();
+        return ok_status();
+    });
 }
 b200_status b200_jpeg_pipe_run(b200_jpeg_pipe *p, void *cuda_stream, int which, int *launches)
 {
@@ -1313,71 +1251,60 @@ b200_status b200_jpeg_pipe_kernel_times(b200_jpeg_pipe *p, int iters, char *text
 void b200_jpeg_pipe_destroy(b200_jpeg_pipe *p) { if (p) { pipe_destroy(p->p); delete p; } }
 
 // ---- PNG stage entry points ----------------------------------------------------------------------------------------
+// palette_rgba / npalette set: the samples are first reduced to a palette where png_reduce_palette finds one
+static b200_status png_decode_abi(const uint8_t *in, size_t in_len, b200_png_info *info, uint8_t **raw, uint8_t *palette_rgba, int *npalette)
+{
+    std::string err; PngInfo pi; std::vector<uint8_t> r;
+    if (!png_decode(in, in_len, false, pi, r, err)) return png_status(err);
+    if (npalette) {
+        *npalette = 0;
+        if (png_reduce_palette(pi, r)) {
+            *npalette = (int)(pi.plte.size() / 3);
+            for (int k = 0; k < *npalette; k++) {
+                palette_rgba[4 * k] = pi.plte[3 * k]; palette_rgba[4 * k + 1] = pi.plte[3 * k + 1]; palette_rgba[4 * k + 2] = pi.plte[3 * k + 2];
+                palette_rgba[4 * k + 3] = (size_t)k < pi.trns.size() ? pi.trns[k] : 255;
+            }
+        }
+    }
+    info->width = pi.width; info->height = pi.height; info->bit_depth = pi.bit_depth; info->color_type = pi.color_type; info->bpp = pi.bpp; info->row_bytes = pi.row_bytes;
+    size_t n;
+    return give(r, raw, &n);
+}
 b200_status b200_png_decode(const uint8_t *in, size_t in_len, b200_png_info *info, uint8_t **raw)
 {
     if (!in || !info || !raw) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
-    std::string err; PngInfo pi; std::vector<uint8_t> r;
-    if (!png_decode(in, in_len, false, pi, r, err)) return make_status(err.find("interlace") != std::string::npos ? B200_ERR_UNSUPPORTED : B200_ERR_CORRUPT_INPUT, err);
-    info->width = pi.width; info->height = pi.height; info->bit_depth = pi.bit_depth; info->color_type = pi.color_type; info->bpp = pi.bpp; info->row_bytes = pi.row_bytes;
-    *raw = (uint8_t *)malloc(r.size() ? r.size() : 1);
-    if (!*raw) return make_status(B200_ERR_OUT_OF_MEMORY, "malloc failed");
-    memcpy(*raw, r.data(), r.size());
-    return ok_status();
+    return png_decode_abi(in, in_len, info, raw, nullptr, nullptr);
 }
 b200_status b200_png_decode_reduced(const uint8_t *in, size_t in_len, b200_png_info *info, uint8_t **raw, uint8_t *palette_rgba, int *npalette)
 {
     if (!in || !info || !raw || !palette_rgba || !npalette) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
-    std::string err; PngInfo pi; std::vector<uint8_t> r;
-    if (!png_decode(in, in_len, false, pi, r, err)) return make_status(err.find("interlace") != std::string::npos ? B200_ERR_UNSUPPORTED : B200_ERR_CORRUPT_INPUT, err);
-    *npalette = 0;
-    if (png_reduce_palette(pi, r)) {
-        *npalette = (int)(pi.plte.size() / 3);
-        for (int k = 0; k < *npalette; k++) {
-            palette_rgba[4 * k] = pi.plte[3 * k]; palette_rgba[4 * k + 1] = pi.plte[3 * k + 1]; palette_rgba[4 * k + 2] = pi.plte[3 * k + 2];
-            palette_rgba[4 * k + 3] = (size_t)k < pi.trns.size() ? pi.trns[k] : 255;
-        }
-    }
-    info->width = pi.width; info->height = pi.height; info->bit_depth = pi.bit_depth; info->color_type = pi.color_type; info->bpp = pi.bpp; info->row_bytes = pi.row_bytes;
-    *raw = (uint8_t *)malloc(r.size() ? r.size() : 1);
-    if (!*raw) return make_status(B200_ERR_OUT_OF_MEMORY, "malloc failed");
-    memcpy(*raw, r.data(), r.size());
-    return ok_status();
+    return png_decode_abi(in, in_len, info, raw, palette_rgba, npalette);
 }
 b200_status b200_png_filter(const uint8_t *raw, int h, int row_bytes, int bpp, int strategy, uint8_t *filtered)
 {
     if (!raw || !filtered || h <= 0 || row_bytes <= 0 || bpp < 1 || bpp > 8 || strategy < 0 || strategy > 9) return make_status(B200_ERR_INVALID_ARGUMENT, "invalid argument");
     std::string err;
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    Slot *s = slot_acquire(runtime_next_device(), err);              // makes the slot's device current for this thread
-    if (!s) return make_status(B200_ERR_CUDA, err);
-    const bool ok = png_stage_filter(raw, h, row_bytes, bpp, strategy, filtered, err);
-    slot_release(s);
-    return ok ? ok_status() : make_status(B200_ERR_CUDA, err);
+    SlotLease s(-1);                                                 // makes the slot's device current for this thread
+    if (!s) return s.failure();
+    return png_stage_filter(raw, h, row_bytes, bpp, strategy, filtered, err) ? ok_status() : make_status(B200_ERR_CUDA, err);
 }
 b200_status b200_png_lz77(const uint8_t *filtered, size_t n, int bpp, int stride, uint32_t **tokens, size_t *ntokens, uint32_t *hist)
 {
     if (!filtered || !n || !tokens || !ntokens || !hist || bpp < 1 || stride < 1) return make_status(B200_ERR_INVALID_ARGUMENT, "invalid argument");
     std::string err;
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    Slot *s = slot_acquire(runtime_next_device(), err);
-    if (!s) return make_status(B200_ERR_CUDA, err);
+    SlotLease s(-1);
+    if (!s) return s.failure();
     std::vector<uint32_t> t;
-    const bool ok = png_stage_lz77(filtered, n, bpp, stride, t, hist, err);
-    slot_release(s);
-    if (!ok) return make_status(B200_ERR_CUDA, err);
-    *tokens = (uint32_t *)malloc(t.size() * 4 + 4);
-    if (!*tokens) return make_status(B200_ERR_OUT_OF_MEMORY, "malloc failed");
-    memcpy(*tokens, t.data(), t.size() * 4); *ntokens = t.size();
-    return ok_status();
+    if (!png_stage_lz77(filtered, n, bpp, stride, t, hist, err)) return make_status(B200_ERR_CUDA, err);
+    return give(t, tokens, ntokens);
 }
 b200_status b200_png_deflate_tokens(const uint32_t *tokens, size_t ntokens, uint32_t adler, uint8_t **out, size_t *out_len)
 {
     if ((!tokens && ntokens) || !out || !out_len) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
     std::vector<uint8_t> z; deflate_tokens(tokens, ntokens, adler, z);
-    *out = (uint8_t *)malloc(z.size() + 1);
-    if (!*out) return make_status(B200_ERR_OUT_OF_MEMORY, "malloc failed");
-    memcpy(*out, z.data(), z.size()); *out_len = z.size();
-    return ok_status();
+    return give(z, out, out_len);
 }
 int b200_webp_alpha_filter(const uint8_t *alpha, int width, int height, uint8_t *filtered)
 {
@@ -1392,20 +1319,14 @@ b200_status b200_webp_alpha_chunk(const uint32_t *tokens, size_t ntokens, int wi
     if (!tokens || !out || !out_len || width < 1 || height < 1 || width > 16383 || height > 16383 || filter < 0 || filter > 3) return make_status(B200_ERR_INVALID_ARGUMENT, "invalid argument");
     std::vector<uint8_t> a;
     if (!vp8l_alpha_from_tokens(tokens, ntokens, width, height, a, filter)) return make_status(B200_ERR_INVALID_ARGUMENT, "the tokens do not cover the plane");
-    *out = (uint8_t *)malloc(a.size() + 1);
-    if (!*out) return make_status(B200_ERR_OUT_OF_MEMORY, "malloc failed");
-    memcpy(*out, a.data(), a.size()); *out_len = a.size();
-    return ok_status();
+    return give(a, out, out_len);
 }
 b200_status b200_webp_wrap_alpha(const uint8_t *simple_file, size_t file_len, const uint8_t *alph, size_t alph_len, int width, int height, uint8_t **out, size_t *out_len)
 {
     if (!simple_file || !alph || !out || !out_len || width < 1 || height < 1 || width > 16383 || height > 16383) return make_status(B200_ERR_INVALID_ARGUMENT, "invalid argument");
     std::vector<uint8_t> f(simple_file, simple_file + file_len), a(alph, alph + alph_len), o;
     if (!webp_wrap_alpha(f, a, width, height, o)) return make_status(B200_ERR_INVALID_ARGUMENT, "not a simple lossy WebP file");
-    *out = (uint8_t *)malloc(o.size() + 1);
-    if (!*out) return make_status(B200_ERR_OUT_OF_MEMORY, "malloc failed");
-    memcpy(*out, o.data(), o.size()); *out_len = o.size();
-    return ok_status();
+    return give(o, out, out_len);
 }
 // ---- WebP stage entry points -----------------------------------------------------------------------------------------
 b200_status b200_webp_encode_rgb(const uint8_t *rgb, int w, int h, int quality, uint8_t **out, size_t *out_len, int16_t *levels, uint8_t *modes)
@@ -1414,32 +1335,30 @@ b200_status b200_webp_encode_rgb(const uint8_t *rgb, int w, int h, int quality, 
     *out = nullptr; *out_len = 0;
     std::string err;
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    Slot *s = slot_acquire(runtime_next_device(), err);
-    if (!s) return make_status(B200_ERR_CUDA, err);
-    if (!s->webp) s->webp = new WebpDevice();
+    SlotLease s(-1);
+    if (!s) return s.failure();
     std::vector<uint8_t> v;
-    const bool ok = s->webp->encode_host_rgb(rgb, w, h, quality, s->stream, v, err, levels, modes);
-    slot_release(s);
-    return ok ? give(v, out, out_len) : make_status(B200_ERR_CUDA, err);
+    if (!s->webp_dev()->encode_host_rgb(rgb, w, h, quality, s->stream, v, err, levels, modes)) return make_status(B200_ERR_CUDA, err);
+    return give(v, out, out_len);
 }
 b200_status b200_webp_decode(const uint8_t *in, size_t in_len, int *width, int *height, uint8_t **rgb)
 {
     if (!in || !width || !height || !rgb) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
     *rgb = nullptr;
-    try {
+    return guarded([&] {
         WebpInfo wi; std::vector<uint8_t> v, a;
-        b200_status s = webp_decode_status(in, in_len, wi, v, &a);
+        const b200_status s = webp_decode_status(in, in_len, wi, v, &a);
         if (s.code) return s;
         *width = wi.width; *height = wi.height;
         size_t n = 0;
         return give(v, rgb, &n);
-    } catch (const std::exception &e) { return make_status(B200_ERR_OUT_OF_MEMORY, e.what()); }
+    });
 }
 b200_status b200_webp_decode_rgba(const uint8_t *in, size_t in_len, int *width, int *height, uint8_t **rgb, uint8_t **alpha)
 {
     if (!in || !width || !height || !rgb || !alpha) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
     *rgb = nullptr; *alpha = nullptr;
-    try {
+    return guarded([&] {
         WebpInfo wi; std::vector<uint8_t> v, a;
         b200_status s = webp_decode_status(in, in_len, wi, v, &a);
         if (s.code) return s;
@@ -1449,7 +1368,7 @@ b200_status b200_webp_decode_rgba(const uint8_t *in, size_t in_len, int *width, 
         s = give(v, rgb, &n);
         if (s.code) { free(*alpha); *alpha = nullptr; }
         return s;
-    } catch (const std::exception &e) { return make_status(B200_ERR_OUT_OF_MEMORY, e.what()); }
+    });
 }
 b200_status b200_webp_write_levels(int w, int h, int quality, const int16_t *levels, const uint8_t *modes, uint8_t **out, size_t *out_len)
 {
@@ -1473,30 +1392,27 @@ b200_status b200_png_device_times(const uint8_t *in, size_t in_len, int level, i
     PngInfo info0; PngIdat idat;
     if (!png_parse_chunks(in, in_len, false, info0, idat, err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    Slot *s = slot_acquire(runtime_next_device(), err);
-    if (!s) return make_status(B200_ERR_CUDA, err);
-    if (!s->png) s->png = new PngDevice();
-    b200_status st = ok_status();
     std::map<std::string, std::pair<double, int>> acc;
-    do {
+    {
+        SlotLease s(-1);
+        if (!s) return s.failure();
+        PngDevice *png = s->png_dev();
         const size_t nin = (info0.row_bytes + 1) * (size_t)info0.height;
         size_t bcap = 0, got = 0; uint32_t adler = 0;
-        uint8_t *buf = s->png->input_buffer(nin, bcap, err);
-        if (!buf) { st = make_status(B200_ERR_OUT_OF_MEMORY, err); break; }
-        if (!zlib_inflate_to(idat.p, idat.n, buf, bcap, nin, &got, &adler, err) || got < nin) { st = make_status(B200_ERR_CORRUPT_INPUT, err.empty() ? "IDAT too short" : err); break; }
+        uint8_t *buf = png->input_buffer(nin, bcap, err);
+        if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+        if (!zlib_inflate_to(idat.p, idat.n, buf, bcap, nin, &got, &adler, err) || got < nin) return make_status(B200_ERR_CORRUPT_INPUT, err.empty() ? "IDAT too short" : err);
         std::vector<uint8_t> z;
         for (int it = 0; it <= iters; it++) {          // iteration 0 warms buffers up and is not counted
             PngInfo info = info0;
             LaunchTimer lt; lt.begin((cudaStream_t)s->stream);
             tl_launch_timer = it ? &lt : nullptr;
-            const bool ok = s->png->compress_filtered(info, got, adler, level < 0 ? 0 : level > 6 ? 6 : level, s->stream, z, nullptr, err);
+            const bool ok = png->compress_filtered(info, got, adler, level < 0 ? 0 : level > 6 ? 6 : level, s->stream, z, nullptr, err);
             tl_launch_timer = nullptr;
-            if (!ok) { st = make_status(B200_ERR_CUDA, err); break; }
+            if (!ok) return make_status(B200_ERR_CUDA, err);
             if (it) lt.collect(acc);
         }
-    } while (0);
-    slot_release(s);
-    if (st.code) return st;
+    }
     std::string out;
     for (auto &kv : acc) { char b[160]; snprintf(b, sizeof b, "%s %.6f %d\n", kv.first.c_str(), kv.second.first / kv.second.second, kv.second.second / iters); out += b; }
     if (out.size() + 1 > cap) return make_status(B200_ERR_INVALID_ARGUMENT, "text buffer too small");

@@ -170,16 +170,24 @@ void runtime_shutdown()
     std::lock_guard<std::mutex> lk(g_mu);
     for (auto *d : g_devs) {
         cudaSetDevice(d->ordinal);
-        for (Slot *s : d->free_slots) {
-            if (s->stream) cudaStreamDestroy((cudaStream_t)s->stream);
-            drop_graphs(s);
-            cudaFreeHost(s->h_in); cudaFreeHost(s->h_out); cudaFree(s->d_in); cudaFree(s->d_out); cudaFree(s->d_scratch); cudaFreeHost(s->h_par); cudaFree(s->d_par); delete s->enc; delete s->dec; delete s->png; delete s->webp;
-            delete s;
-        }
+        for (Slot *s : d->free_slots) delete s;
         delete d;
     }
     g_devs.clear(); g_inited = false;
 }
+
+Slot::~Slot()
+{
+    if (stream) cudaStreamDestroy((cudaStream_t)stream);
+    drop_graphs(this);
+    cudaFreeHost(h_in); cudaFreeHost(h_out); cudaFree(d_in); cudaFree(d_out); cudaFree(d_scratch); cudaFreeHost(h_par); cudaFree(d_par);
+    delete enc; delete dec; delete png; delete webp;
+}
+
+GpuEncoder *Slot::encoder() { if (!enc) enc = new GpuEncoder(); return enc; }
+GpuDecoder *Slot::decoder() { if (!dec) dec = new GpuDecoder(); return dec; }
+PngDevice *Slot::png_dev() { if (!png) png = new PngDevice(); return png; }
+WebpDevice *Slot::webp_dev() { if (!webp) webp = new WebpDevice(); return webp; }
 
 int runtime_device_count() { std::lock_guard<std::mutex> lk(g_mu); return g_inited ? (int)g_devs.size() : 0; }
 long long runtime_device_jobs(int i) { return g_devs.empty() || i < 0 || i >= (int)g_devs.size() ? 0 : g_devs[(size_t)i]->jobs.load(); }
@@ -314,8 +322,7 @@ bool slot_transform_group_prepare(Slot *s, const JpegGeom *const *gins, const Jp
         if (!plan_image(gin, gout, plan, err)) return false;
         uint16_t *dq = reinterpret_cast<uint16_t *>(s->h_par + o_dq) + 256 * k;
         for (int c = 0; c < gin.ncomp; c++) memcpy(dq + 64 * c, gin.qt[gin.tq[c]], 128);
-        append_image_work(gin, gout, plan, reinterpret_cast<const int16_t *>(reinterpret_cast<const uint8_t *>(s->d_in) + L.in_stride * k),
-                          reinterpret_cast<int16_t *>(reinterpret_cast<uint8_t *>(s->d_out) + L.out_stride * k), s->d_scratch + L.scratch_stride * k,
+        append_image_work(gin, gout, plan, L.coefs(*s, k, true), L.coefs(*s, k, false), s->d_scratch + L.scratch_stride * k,
                           reinterpret_cast<const uint16_t *>(s->d_par + o_dq) + 256 * k, reinterpret_cast<const QuantDev *>(s->d_par + o_q), wl);
     }
     const size_t nw = flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + o_work));
@@ -388,18 +395,15 @@ template <class Fn> static bool capture_graph(cudaStream_t st, void *&exec_out, 
 bool slot_run_group(Slot *s, std::vector<GpuDecoder::Item> &items, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, bool progressive,
                     bool lossless, std::string &err)
 {
-    if (!s->dec) s->dec = new GpuDecoder();
-    if (!s->enc) s->enc = new GpuEncoder();
     cudaStream_t st = (cudaStream_t)s->stream;
     const auto t0 = std::chrono::steady_clock::now();
     // ---- host half of all three stages (pinned staging, descriptors, plans); nothing touches the stream yet
-    if (!s->dec->prepare(items, st, err)) return false;
+    if (!s->decoder()->prepare(items, st, err)) return false;
     if (!lossless && !slot_transform_group_prepare(s, gins, gout, L, err)) return false;
     std::vector<int16_t *> bases((size_t)L.K);
-    for (int k = 0; k < L.K; k++) bases[k] = lossless ? reinterpret_cast<int16_t *>(reinterpret_cast<uint8_t *>(s->d_in) + L.in_stride * k)
-                                                      : reinterpret_cast<int16_t *>(reinterpret_cast<uint8_t *>(s->d_out) + L.out_stride * k);
+    for (int k = 0; k < L.K; k++) bases[k] = L.coefs(*s, k, lossless);
     // a re-encode at lower quality (or a transcode with optimal tables) does not grow: the inputs' entropy-coded size sizes the output buffers
-    if (!s->enc->prepare(gout, progressive, bases.data(), L.K, st, s->dec->raw_bytes(), err)) return false;
+    if (!s->encoder()->prepare(gout, progressive, bases.data(), L.K, st, s->dec->raw_bytes(), err)) return false;
     const auto t1 = std::chrono::steady_clock::now();
     auto front = [&]() { return s->dec->upload(st, err) && s->dec->enqueue(st, err) && (lossless || slot_transform_group_enqueue(s, err)) &&
                                 s->enc->upload(st, err) && s->enc->enqueue_front(st, true, err) && s->enc->enqueue_sizes(st, err); };
@@ -433,21 +437,6 @@ bool slot_run_group(Slot *s, std::vector<GpuDecoder::Item> &items, const JpegGeo
     return true;
 }
 
-bool slot_decode_group(Slot *s, std::vector<GpuDecoder::Item> &items, std::string &err)
-{
-    if (!s->dec) s->dec = new GpuDecoder();
-    return s->dec->decode(items, s->stream, err);
-}
-
-bool slot_encode_group(Slot *s, const JpegGeom &gout, bool progressive, const GroupLayout &L, std::string &err, bool from_input)
-{
-    if (!s->enc) s->enc = new GpuEncoder();
-    std::vector<int16_t *> bases((size_t)L.K);
-    for (int k = 0; k < L.K; k++) bases[k] = from_input ? reinterpret_cast<int16_t *>(reinterpret_cast<uint8_t *>(s->d_in) + L.in_stride * k)
-                                                        : reinterpret_cast<int16_t *>(reinterpret_cast<uint8_t *>(s->d_out) + L.out_stride * k);
-    return s->enc->encode(gout, progressive, bases.data(), L.K, s->stream, true, err);
-}
-
 bool slot_download_coefs(Slot *s, size_t out_bytes, std::string &err)
 {
     cudaStream_t st = (cudaStream_t)s->stream;
@@ -458,10 +447,9 @@ bool slot_download_coefs(Slot *s, size_t out_bytes, std::string &err)
 
 int slot_gpu_decode(Slot *s, const JpegReader &rd, const JpegReader::DeviceScan &ds, std::string &err)
 {   // 0 = coefficients are in s->d_in, 1 = not converged (decode on the host instead), 2 = failure
-    if (!s->dec) s->dec = new GpuDecoder();
     std::vector<GpuDecoder::Item> items(1);
     items[0].rd = &rd; items[0].ds = &ds; items[0].d_coefs = s->d_in; items[0].result = GpuDecoder::FAILED;
-    if (!s->dec->decode(items, s->stream, err)) return 2;
+    if (!s->decoder()->decode(items, s->stream, err)) return 2;
     return (int)items[0].result;
 }
 
@@ -474,16 +462,15 @@ bool slot_upload_out_coefs(Slot *s, size_t bytes, std::string &err)
 
 bool slot_gpu_encode(Slot *s, const JpegGeom &gout, bool progressive, std::string &err, bool from_input)
 {
-    if (!s->enc) s->enc = new GpuEncoder();
     int16_t *base = from_input ? s->d_in : s->d_out;
-    return s->enc->encode(gout, progressive, &base, 1, s->stream, true, err);
+    return s->encoder()->encode(gout, progressive, &base, 1, s->stream, true, err);
 }
 
 bool slot_gpu_encode_sizes(Slot *s, const JpegGeom &gout, bool progressive, std::string &err)
 {
-    if (!s->enc) s->enc = new GpuEncoder();
+    GpuEncoder *enc = s->encoder();
     int16_t *base = s->d_out;
-    return s->enc->prepare(gout, progressive, &base, 1, s->stream, 0, err) && s->enc->upload(s->stream, err) && s->enc->enqueue(s->stream, true, err) && s->enc->finish(s->stream, false, err);
+    return enc->prepare(gout, progressive, &base, 1, s->stream, 0, err) && enc->upload(s->stream, err) && enc->enqueue(s->stream, true, err) && enc->finish(s->stream, false, err);
 }
 bool slot_gpu_fetch(Slot *s, std::string &err) { return s->enc && s->enc->finish(s->stream, true, err); }
 

@@ -58,6 +58,15 @@ struct Slot {
     void *graph_front = nullptr, *graph_back = nullptr; unsigned long long graph_sig = 0; bool graphs_broken = false;
     bool ensure(size_t in_bytes, size_t out_bytes, size_t scratch_bytes, size_t par_bytes, std::string &err);
     bool ensure_device(size_t in_bytes, size_t out_bytes, size_t scratch_bytes, size_t par_bytes, std::string &err);
+    // the coders, created on first use
+    GpuEncoder *encoder();
+    GpuDecoder *decoder();
+    PngDevice *png_dev();
+    WebpDevice *webp_dev();
+    Slot() = default;
+    Slot(const Slot &) = delete;
+    Slot &operator=(const Slot &) = delete;
+    ~Slot();        // destroys the stream and frees every buffer; the caller has made the slot's device current and its stream idle
 };
 
 int  runtime_init(int n_gpus, int only_device, std::string &err);   // returns device count (>0) or 0 with err
@@ -76,16 +85,27 @@ bool slot_download_coefs(Slot *s, size_t out_bytes, std::string &err);
 // Entropy-decode a baseline single-scan file on the device into s->d_in (0 ok, 1 not converged -> host decode, 2 failed)
 int slot_gpu_decode(Slot *s, const JpegReader &rd, const JpegReader::DeviceScan &ds, std::string &err);
 // ---- megabatch (K same-shaped images per launch sequence; used by b200_compress_batch) ---------------------------------
-struct GroupLayout { int K = 0; size_t in_stride = 0, out_stride = 0, scratch_stride = 0; };
+struct GroupLayout {
+    int K = 0; size_t in_stride = 0, out_stride = 0, scratch_stride = 0;
+    // image k's coefficients: its input in s.d_in, or its output in s.d_out
+    int16_t *coefs(const Slot &s, int k, bool input) const
+    {
+        return reinterpret_cast<int16_t *>(reinterpret_cast<uint8_t *>(input ? s.d_in : s.d_out) + (input ? in_stride : out_stride) * k);
+    }
+};
 bool slot_group_layout(Slot *s, const JpegGeom &gin, const JpegGeom &gout, int K, GroupLayout &L, std::string &err);   // sizes + ensure()
-bool slot_decode_group(Slot *s, std::vector<GpuDecoder::Item> &items, std::string &err);      // items[k].d_coefs = d_in + k * in_stride
+// one launch sequence serves images of one size, component count and sampling
+inline bool same_shape(const JpegGeom &a, const JpegGeom &b)
+{
+    bool same = a.width == b.width && a.height == b.height && a.ncomp == b.ncomp;
+    for (int c = 0; same && c < a.ncomp; c++) same = a.hs[c] == b.hs[c] && a.vs[c] == b.vs[c];
+    return same;
+}
 // decode -> (transform) -> encode of one megabatch enqueued back to back, one idle host wait at the end; results in s->enc->results,
 // items[k].result says which images the device decoder settled
 bool slot_run_group(Slot *s, std::vector<GpuDecoder::Item> &items, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, bool progressive,
                     bool lossless, std::string &err);
 bool slot_transform_group(Slot *s, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, std::string &err);
-// results in s->enc->results; from_input = encode the coefficients in d_in (lossless transcode) instead of d_out
-bool slot_encode_group(Slot *s, const JpegGeom &gout, bool progressive, const GroupLayout &L, std::string &err, bool from_input = false);
 // H2D of s->h_out into s->d_out (entry point that encodes caller-supplied coefficients on the device)
 bool slot_upload_out_coefs(Slot *s, size_t bytes, std::string &err);
 // Entropy-code the output coefficients sitting in s->d_out on the device; result in s->enc->results

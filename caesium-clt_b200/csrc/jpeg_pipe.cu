@@ -45,13 +45,11 @@ struct JpegPipe {
 JpegPipe::~JpegPipe()
 {
     for (auto &g : groups) {
-        Slot &s = g->slot;
-        if (s.stream) { cudaStreamSynchronize((cudaStream_t)s.stream); cudaStreamDestroy((cudaStream_t)s.stream); }
-        cudaFreeHost(s.h_in); cudaFreeHost(s.h_out); cudaFree(s.d_in); cudaFree(s.d_out); cudaFree(s.d_scratch); cudaFreeHost(s.h_par); cudaFree(s.d_par);
-        delete s.enc; delete s.dec;
+        if (g->slot.stream) cudaStreamSynchronize((cudaStream_t)g->slot.stream);
         if (g->done) cudaEventDestroy(g->done);
     }
     if (fork) cudaEventDestroy(fork);
+    groups.clear();             // ~Slot: streams and buffers
 }
 
 JpegPipe *pipe_create(const uint8_t *const *in, const size_t *in_len, int n, const b200_params *p, int K, std::string &err)
@@ -59,16 +57,13 @@ JpegPipe *pipe_create(const uint8_t *const *in, const size_t *in_len, int n, con
     if (n <= 0 || K <= 0) { err = "empty pipe"; return nullptr; }
     std::unique_ptr<JpegPipe> P(new JpegPipe());
     P->n = n; P->K = K; P->lossless = p->jpeg_optimize != 0; P->progressive = p->jpeg_progressive != 0;
-    P->wo.progressive = P->progressive; P->wo.keep_metadata = p->keep_metadata != 0; P->wo.preserve_icc = p->jpeg_preserve_icc != 0; P->wo.copy_jfif = P->lossless;
+    P->wo = write_options(p); P->wo.copy_jfif = P->lossless;
     P->rd.resize((size_t)n); P->ds.resize((size_t)n);
     for (int i = 0; i < n; i++) {
         P->rd[i].reset(new JpegReader(in[i], in_len[i]));
         if (!P->rd[i]->read_header(err)) return nullptr;
         if (!P->rd[i]->device_decodable(P->ds[i])) { err = "input " + std::to_string(i) + " is not a baseline single-scan JPEG (the resident pipe takes only those)"; return nullptr; }
-        const JpegGeom &a = P->rd[0]->geom(), &b = P->rd[i]->geom();
-        bool same = a.width == b.width && a.height == b.height && a.ncomp == b.ncomp;
-        for (int c = 0; same && c < a.ncomp; c++) same = a.hs[c] == b.hs[c] && a.vs[c] == b.vs[c];
-        if (!same) { err = "inputs of a resident pipe must share one shape"; return nullptr; }
+        if (!same_shape(P->rd[0]->geom(), P->rd[i]->geom())) { err = "inputs of a resident pipe must share one shape"; return nullptr; }
     }
     const JpegGeom &gin0 = P->rd[0]->geom();
     if (P->lossless) P->gout = gin0;
@@ -91,14 +86,13 @@ JpegPipe *pipe_create(const uint8_t *const *in, const size_t *in_len, int n, con
             const int i = i0 + m;
             G->members.push_back(i);
             G->items[m].rd = P->rd[i].get(); G->items[m].ds = &P->ds[i]; G->items[m].result = GpuDecoder::FAILED;
-            G->items[m].d_coefs = reinterpret_cast<int16_t *>(reinterpret_cast<uint8_t *>(G->slot.d_in) + G->L.in_stride * m);
+            G->items[m].d_coefs = G->L.coefs(G->slot, m, true);
             G->gins[m] = &P->rd[i]->geom();
-            G->bases[m] = P->lossless ? G->items[m].d_coefs : reinterpret_cast<int16_t *>(reinterpret_cast<uint8_t *>(G->slot.d_out) + G->L.out_stride * m);
+            G->bases[m] = G->L.coefs(G->slot, m, P->lossless);
             raw += P->ds[i].ecs_end - P->ds[i].ecs_begin;
         }
-        G->slot.dec = new GpuDecoder(); G->slot.enc = new GpuEncoder();
-        if (!G->slot.dec->prepare(G->items, st, err) || !G->slot.dec->upload(st, err)) return nullptr;       // entropy-coded bytes + tables go up here, once
-        if (!G->slot.enc->prepare(P->gout, P->progressive, G->bases.data(), Kg, st, raw, err) || !G->slot.enc->upload(st, err)) return nullptr;
+        if (!G->slot.decoder()->prepare(G->items, st, err) || !G->slot.dec->upload(st, err)) return nullptr;       // entropy-coded bytes + tables go up here, once
+        if (!G->slot.encoder()->prepare(P->gout, P->progressive, G->bases.data(), Kg, st, raw, err) || !G->slot.enc->upload(st, err)) return nullptr;
         if (cudaStreamSynchronize(st) != cudaSuccess) { err = "upload failed"; return nullptr; }
         P->groups.push_back(std::move(G));
     }

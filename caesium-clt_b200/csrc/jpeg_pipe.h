@@ -6,8 +6,15 @@
 #include <string>
 #include <vector>
 #include "../../include/b200_caesium.h"
+#include "jpeg_host.h"
 
 namespace b200 {
+// the JPEG writer's options from the C ABI's parameters; copying the source's JFIF header is each caller's choice
+inline JpegWriteOptions write_options(const b200_params *p)
+{
+    JpegWriteOptions wo; wo.progressive = p->jpeg_progressive != 0; wo.keep_metadata = p->keep_metadata != 0; wo.preserve_icc = p->jpeg_preserve_icc != 0;
+    return wo;
+}
 struct JpegPipe;
 JpegPipe *pipe_create(const uint8_t *const *in, const size_t *in_len, int n, const b200_params *p, int group_size, std::string &err);
 // which: 0 whole path, 1 entropy decode only, 2 transform only, 3 entropy encode only (2 / 3 need a prior whole run)

@@ -350,3 +350,22 @@ def test_compress_webp_inputs_with_alpha_and_lossless(L, O):
     png = np.asarray(pil_pixels(L.convert_in_memory(lossy_alpha, pp, FMT_PNG)).convert("RGBA"))
     assert np.array_equal(png[:, :, 3], O.resize_plane(np.ascontiguousarray(dec[:, :, 3]), nw, nh))
     assert np.array_equal(png[:, :, 0], O.resize_plane(np.ascontiguousarray(dec[:, :, 0]), nw, nh))
+
+
+def test_convert_webp_to_png_with_resize_matches_oracle(L, O):
+    """WebP -> lossless PNG at width=100, for an opaque file and one with an alpha plane: every channel of the PNG is the oracle's
+    Lanczos3 of the decoded source's channel."""
+    import io
+    from PIL import Image
+    from pngutil import pil_pixels
+    h, w = 150, 210
+    img = np.concatenate([synth(h, w, 3, seed=12, kind="photo"), _soft_alpha(h, w, 3)[:, :, None]], axis=2)
+    b = io.BytesIO(); Image.fromarray(img).save(b, "WEBP", quality=85, alpha_quality=100); lossy_alpha = b.getvalue()
+    p = L.default_params(); p.png_optimize = 1; p.width = 100
+    for src, mode in ((_sample("w0.webp"), "RGB"), (lossy_alpha, "RGBA")):
+        dec = np.asarray(Image.open(io.BytesIO(src)).convert(mode))
+        nw, nh = O.compute_dimensions(dec.shape[1], dec.shape[0], 100, 0)
+        png = np.asarray(pil_pixels(L.convert_in_memory(src, p, FMT_PNG)).convert(mode))
+        assert png.shape == (nh, nw, len(mode)), mode
+        for c in range(len(mode)):
+            assert np.array_equal(png[:, :, c], O.resize_plane(np.ascontiguousarray(dec[:, :, c]), nw, nh)), (mode, c)
