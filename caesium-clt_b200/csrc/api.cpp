@@ -26,6 +26,7 @@
 #include "png_device.h"
 #include "vp8_host.h"
 #include "webp_device.h"
+#include "vp8l_device.h"
 #include "vp8_decode.h"
 #include "vp8l_alpha.h"
 #include "jpeg_pipe.h"
@@ -635,9 +636,53 @@ b200_status webp_decode_status(const uint8_t *in, size_t in_len, WebpInfo &info,
     if (rc) return make_status(B200_ERR_CORRUPT_INPUT, err);
     return ok_status();
 }
+// webp.lossless: decode as above, K3 on the RGB and alpha planes when width / height are set, then the lossless encoder (VP8L:
+// subtract-green, per-tile predictors, colour cache, LZ77 at neighbourhood distances -- vp8l_kernels.cu).  Exact: RGB under fully
+// transparent pixels is kept.  Like the lossy leg, no metadata is kept.
+b200_status webp_lossless_compress(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
+{
+    std::string err;
+    static const bool verbose = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2;
+    const auto t0 = std::chrono::steady_clock::now();
+    WebpInfo info; std::vector<uint8_t> rgb, alpha;
+    b200_status st = webp_decode_status(in, in_len, info, rgb, &alpha);
+    if (st.code) return st;
+    const uint32_t w = (uint32_t)info.width, h = (uint32_t)info.height;
+    uint32_t nw, nh;
+    if ((st = target_size(w, h, p, 16383, nw, nh, "invalid dimensions for WebP")).code) return st;
+    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
+    SlotLease s(prefer_dev);
+    if (!s) return s.failure();
+    const auto t1 = std::chrono::steady_clock::now();
+    const uint8_t *src = rgb.data(), *ap = alpha.empty() ? nullptr : alpha.data();
+    std::vector<uint8_t> planes, ra;
+    if (nw != w || nh != h) {
+        if (!resize_to_host(s, src, w, h, nw, nh, 3, planes, err) || (ap && !resize_to_host(s, ap, w, h, nw, nh, 1, ra, err))) return make_status(B200_ERR_CUDA, err);
+        src = planes.data();
+        if (ap) ap = ra.data();
+    }
+    const auto t2 = std::chrono::steady_clock::now();
+    Vp8lDevice *v = s->vp8l_dev();
+    LaunchTimer lt;
+    if (verbose) { lt.begin((cudaStream_t)s->stream); tl_launch_timer = &lt; }
+    const bool ok = v->encode(src, ap, (int)nw, (int)nh, s->stream, out, err);
+    tl_launch_timer = nullptr;
+    if (!ok) return make_status(B200_ERR_CUDA, err);
+    if (verbose) {
+        auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
+        std::map<std::string, std::pair<double, int>> acc;
+        lt.collect(acc);
+        std::string kt;
+        for (auto &kv : acc) { char b[96]; snprintf(b, sizeof b, " %s=%.4f", kv.first.c_str(), kv.second.first); kt += b; }
+        fprintf(stderr, "[b200 trace] webp-lossless %ux%u -> %ux%u: host decode %.3f ms, resize %.3f ms, device encode %.3f ms (analysis wait %.3f, cache bits %d, codes + emission %.3f); kernels ms:%s\n",
+                w, h, nw, nh, ms(t0, t1), ms(t1, t2), ms(t2, std::chrono::steady_clock::now()), v->last_analyse_ms, v->last_cache_bits, v->last_code_ms, kt.c_str());
+    }
+    return ok_status();
+}
+
 b200_status webp_compress(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
 {
-    if (p->webp_lossless) return make_status(B200_ERR_UNSUPPORTED, "lossless WebP (VP8L) is outside the GPU path (route to caesium::compress_in_memory)");
+    if (p->webp_lossless) return webp_lossless_compress(in, in_len, p, prefer_dev, out);
     WebpInfo info; std::vector<uint8_t> rgb, alpha;
     b200_status st = webp_decode_status(in, in_len, info, rgb, &alpha);
     if (st.code) return st;

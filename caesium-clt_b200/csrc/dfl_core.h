@@ -57,9 +57,13 @@ DFL_HD int dist_sym(int d)
 // scratch: order[n] (symbols), w[2n] (node weights), parent[2n]; all <= MAXSYM
 struct HuffScratch { uint16_t order[MAXSYM]; uint64_t w[2 * MAXSYM]; int16_t parent[2 * MAXSYM]; uint8_t depth[2 * MAXSYM]; };
 
+// the same for alphabets of up to N symbols (VP8L's green alphabet with a colour cache has up to 1304)
+template <int N> struct HuffScratchN { uint16_t order[N]; uint64_t w[2 * N]; int16_t parent[2 * N]; uint8_t depth[2 * N]; };
+
 // leaves (symbols with a non-zero count) sorted by (frequency, symbol) ascending into S.order; returns their number.  Insertion
 // sort: m <= 286.  (The device sorts the litlen alphabet with the whole warp instead -- png_deflate.cu -- into the same order.)
-DFL_HD int huff_sort_leaves(const uint32_t *freq, int n, HuffScratch &S)
+template <class Scratch>
+DFL_HD int huff_sort_leaves(const uint32_t *freq, int n, Scratch &S)
 {
     int m = 0;
     for (int i = 0; i < n; i++) if (freq[i]) S.order[m++] = (uint16_t)i;
@@ -73,7 +77,8 @@ DFL_HD int huff_sort_leaves(const uint32_t *freq, int n, HuffScratch &S)
 }
 
 // code lengths from the sorted leaves S.order[0 .. m)
-DFL_HD void huff_lengths_sorted(const uint32_t *freq, int n, int m, int limit, uint8_t *len, HuffScratch &S)
+template <class Scratch>
+DFL_HD void huff_lengths_sorted(const uint32_t *freq, int n, int m, int limit, uint8_t *len, Scratch &S)
 {
     for (int i = 0; i < n; i++) len[i] = 0;
     if (m == 0) return;
@@ -117,7 +122,8 @@ DFL_HD void huff_lengths_sorted(const uint32_t *freq, int n, int m, int limit, u
     }
 }
 
-DFL_HD void huff_lengths(const uint32_t *freq, int n, int limit, uint8_t *len, HuffScratch &S)
+template <class Scratch>
+DFL_HD void huff_lengths(const uint32_t *freq, int n, int limit, uint8_t *len, Scratch &S)
 {
     const int m = huff_sort_leaves(freq, n, S);
     huff_lengths_sorted(freq, n, m, limit, len, S);

@@ -19,6 +19,7 @@
 #include "jpeg_gpudec.h"
 #include "png_device.h"
 #include "webp_device.h"
+#include "vp8l_device.h"
 #include "stream_wait.h"
 #include "launch_timer.h"
 
@@ -181,13 +182,14 @@ Slot::~Slot()
     if (stream) cudaStreamDestroy((cudaStream_t)stream);
     drop_graphs(this);
     cudaFreeHost(h_in); cudaFreeHost(h_out); cudaFree(d_in); cudaFree(d_out); cudaFree(d_scratch); cudaFreeHost(h_par); cudaFree(d_par);
-    delete enc; delete dec; delete png; delete webp;
+    delete enc; delete dec; delete png; delete webp; delete vp8l;
 }
 
 GpuEncoder *Slot::encoder() { if (!enc) enc = new GpuEncoder(); return enc; }
 GpuDecoder *Slot::decoder() { if (!dec) dec = new GpuDecoder(); return dec; }
 PngDevice *Slot::png_dev() { if (!png) png = new PngDevice(); return png; }
 WebpDevice *Slot::webp_dev() { if (!webp) webp = new WebpDevice(); return webp; }
+Vp8lDevice *Slot::vp8l_dev() { if (!vp8l) vp8l = new Vp8lDevice(); return vp8l; }
 
 int runtime_device_count() { std::lock_guard<std::mutex> lk(g_mu); return g_inited ? (int)g_devs.size() : 0; }
 long long runtime_device_jobs(int i) { return g_devs.empty() || i < 0 || i >= (int)g_devs.size() ? 0 : g_devs[(size_t)i]->jobs.load(); }

@@ -52,6 +52,7 @@ struct Slot {
     class GpuDecoder *dec = nullptr;                                                     // device entropy decoder (lazy)
     struct PngDevice *png = nullptr;                                                     // lossless PNG state (lazy, png_device.cu)
     struct WebpDevice *webp = nullptr;                                                   // WebP / VP8 state (lazy, webp_device.cu)
+    struct Vp8lDevice *vp8l = nullptr;                                                   // lossless WebP / VP8L state (lazy, vp8l_encode.cpp)
     // megabatch path: transform work lists of the current megabatch, and the captured launch sequence (two CUDA graphs, see
     // slot_run_group) with the signature it was captured for
     WorkLists group_wl; size_t group_par_bytes = 0, group_work_off = 0;
@@ -63,6 +64,7 @@ struct Slot {
     GpuDecoder *decoder();
     PngDevice *png_dev();
     WebpDevice *webp_dev();
+    Vp8lDevice *vp8l_dev();
     Slot() = default;
     Slot(const Slot &) = delete;
     Slot &operator=(const Slot &) = delete;

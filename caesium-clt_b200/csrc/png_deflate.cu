@@ -12,6 +12,7 @@
 #include "dfl_core.h"
 #include "png_deflate.h"
 #include "launch_timer.h"
+#include "dev_bits.h"
 
 namespace b200 {
 
@@ -128,22 +129,6 @@ __global__ void __launch_bounds__(1024) k_dfl_scan(const unsigned long long *__r
     }
     if (threadIdx.x == 0) { total[0] = carry; total[1] = *ntok_p; }
 }
-
-struct DevBits {                // LSB-first writer into zeroed 32-bit words shared with neighbours: every flush is an atomic OR
-    uint32_t *words; unsigned long long wpos; unsigned long long acc; int n;
-    __device__ __forceinline__ DevBits(uint32_t *w, unsigned long long bitpos) : words(w), wpos(bitpos >> 5), acc(0), n((int)(bitpos & 31)) {}
-    __device__ __forceinline__ void put32(uint32_t v, int k)      // k <= 32, n < 32 on entry
-    {
-        if (!k) return;
-        acc |= (unsigned long long)v << n; n += k;
-        if (n >= 32) { const uint32_t w = (uint32_t)acc; if (w) atomicOr(&words[wpos], w); wpos++; acc >>= 32; n -= 32; }
-    }
-    __device__ __forceinline__ void put(unsigned long long v, int k)   // k <= 48
-    {
-        if (k > 32) { put32((uint32_t)v, 32); put32((uint32_t)(v >> 32), k - 32); } else put32((uint32_t)v, k);
-    }
-    __device__ __forceinline__ void finish() { if (n > 0) { const uint32_t w = (uint32_t)acc; if (w) atomicOr(&words[wpos], w); } }
-};
 
 __global__ void __launch_bounds__(DFL_THREADS) k_dfl_emit(const uint32_t *__restrict__ tok, const uint32_t *__restrict__ ntok_p, int block_tokens, const BlockTables *__restrict__ tabs,
                                                            const EmitTables *__restrict__ emit, const uint32_t *__restrict__ chunk_off, const unsigned long long *__restrict__ block_bits,

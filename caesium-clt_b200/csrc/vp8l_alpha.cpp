@@ -1,76 +1,25 @@
 // vp8l_alpha.cpp -- see vp8l_alpha.h.  WebP lossless bitstream (the "VP8L" specification: LSB-first bits, canonical prefix codes
 // of at most 15 bits, five codes per group: green + length prefixes, red, blue, alpha, distance prefixes), restricted to what an
 // alpha plane needs: no transforms, no colour cache, no meta prefix image; red / blue / alpha are single-symbol codes (zero bits).
+// The prefix-code writer here (vp8l_writer.h) also serves the lossless WebP encoder (vp8l_encode.cpp).
 #include "vp8l_alpha.h"
-#include "dfl_core.h"
+#include "vp8l_writer.h"
 #include <cstring>
 
 namespace b200 {
-namespace {
 
-struct BitsLsb {
-    std::vector<uint8_t> &o; uint64_t acc = 0; int n = 0;
-    explicit BitsLsb(std::vector<uint8_t> &out) : o(out) {}
-    void put(uint32_t v, int nb)
-    {
-        if (!nb) return;
-        acc |= (uint64_t)(v & (nb >= 32 ? 0xFFFFFFFFu : ((1u << nb) - 1u))) << n; n += nb;
-        while (n >= 8) { o.push_back((uint8_t)acc); acc >>= 8; n -= 8; }
-    }
-    void flush() { if (n > 0) { o.push_back((uint8_t)acc); acc = 0; n = 0; } }
-};
-
-// the specification's prefix coding of lengths and distance codes: value >= 1 -> (prefix symbol, extra bit count, extra bits)
-inline void prefix_of(uint32_t v, int &sym, int &nx, uint32_t &xv)
-{
-    const uint32_t d = v - 1;
-    if (d < 4) { sym = (int)d; nx = 0; xv = 0; return; }
-    const int hb = dfl::hibit(d);
-    sym = 2 * hb + (int)((d >> (hb - 1)) & 1u); nx = hb - 1; xv = d & ((1u << nx) - 1u);
-}
-
-// distance codes 1..120 name a pixel of the neighbourhood: (dy << 4) | (8 - dx)  (table of the specification, section 5.2.2)
-const uint8_t kCodeToPlane[120] = {
-    0x18, 0x07, 0x17, 0x19, 0x28, 0x06, 0x27, 0x29, 0x16, 0x1a, 0x26, 0x2a, 0x38, 0x05, 0x37, 0x39, 0x15, 0x1b, 0x36, 0x3a,
-    0x25, 0x2b, 0x48, 0x04, 0x47, 0x49, 0x14, 0x1c, 0x35, 0x3b, 0x46, 0x4a, 0x24, 0x2c, 0x58, 0x45, 0x4b, 0x34, 0x3c, 0x03,
-    0x57, 0x59, 0x13, 0x1d, 0x56, 0x5a, 0x23, 0x2d, 0x44, 0x4c, 0x55, 0x5b, 0x33, 0x3d, 0x68, 0x02, 0x67, 0x69, 0x12, 0x1e,
-    0x66, 0x6a, 0x22, 0x2e, 0x54, 0x5c, 0x43, 0x4d, 0x65, 0x6b, 0x32, 0x3e, 0x78, 0x01, 0x77, 0x79, 0x53, 0x5d, 0x11, 0x1f,
-    0x64, 0x6c, 0x42, 0x4e, 0x76, 0x7a, 0x21, 0x2f, 0x75, 0x7b, 0x31, 0x3f, 0x63, 0x6d, 0x52, 0x5e, 0x00, 0x74, 0x7c, 0x41,
-    0x4f, 0x10, 0x20, 0x62, 0x6e, 0x30, 0x73, 0x7d, 0x51, 0x5f, 0x40, 0x72, 0x7e, 0x61, 0x6f, 0x50, 0x71, 0x7f, 0x60, 0x70};
-
-struct PlaneCodes {                     // pixel distance -> distance code for one image width
-    int width; uint32_t near_dist[120];
-    explicit PlaneCodes(int w) : width(w)
-    {
-        for (int i = 0; i < 120; i++) {
-            const int dy = kCodeToPlane[i] >> 4, dx = 8 - (kCodeToPlane[i] & 15);
-            const long long d = (long long)dy * w + dx;
-            near_dist[i] = d >= 1 ? (uint32_t)d : 0u;       // (a decoder clamps codes that point forward to distance 1; never chosen here)
-        }
-    }
-    uint32_t code_of(uint32_t dist) const
-    {
-        if (dist <= 7u * (uint32_t)width + 8u)
-            for (int i = 0; i < 120; i++) if (near_dist[i] == dist) return (uint32_t)i + 1u;
-        return dist + 120u;
-    }
-};
-
-struct PrefixCode { std::vector<uint8_t> len; std::vector<uint16_t> code; int used = 0; };
-
-void make_code(const std::vector<uint32_t> &freq, PrefixCode &pc, dfl::HuffScratch &S)
+void vp8l_make_code(const std::vector<uint32_t> &freq, PrefixCode &pc, Vp8lHuffScratch &S)
 {
     const int n = (int)freq.size();
-    if (n < 1 || n > dfl::MAXSYM) return;
+    if (n < 1 || n > VP8L_NGREEN) return;
     pc.len.assign(n, 0); pc.code.assign(n, 0); pc.used = 0;
     for (int i = 0; i < n; i++) pc.used += freq[i] != 0;
     dfl::huff_lengths(freq.data(), n, 15, pc.len.data(), S);
     dfl::canon_codes(pc.len.data(), n, pc.code.data());
 }
-inline void put_sym(BitsLsb &bw, const PrefixCode &pc, int s) { if (pc.used > 1) bw.put(pc.code[s], pc.len[s]); }   // a one-symbol code takes no bits
 
 // one prefix code in the bitstream (section 6.2.1 / 6.2.2 of the specification)
-void write_code(BitsLsb &bw, const PrefixCode &pc, dfl::HuffScratch &S)
+void vp8l_write_code(BitsLsb &bw, const PrefixCode &pc, Vp8lHuffScratch &S)
 {
     const int n = (int)pc.len.size();
     int s0 = -1, s1 = -1;
@@ -106,12 +55,10 @@ void write_code(BitsLsb &bw, const PrefixCode &pc, dfl::HuffScratch &S)
     for (int i = 0; i < ncodes; i++) bw.put(cl.len[order[i]], 3);
     bw.put(0, 1);                                   // every symbol's length follows (no max_symbol)
     for (const Tk &t : tk) {
-        put_sym(bw, cl, t.sym);
+        vp8l_put_sym(bw, cl, t.sym);
         if (t.sym == 17) bw.put(t.extra, 3); else if (t.sym == 18) bw.put(t.extra, 7);
     }
 }
-
-} // namespace
 
 bool vp8l_alpha_from_tokens(const uint32_t *tok, size_t ntok, int width, int height, std::vector<uint8_t> &alph, int filter)
 {
@@ -132,17 +79,17 @@ bool vp8l_alpha_from_tokens(const uint32_t *tok, size_t ntok, int width, int hei
     }
     if (pos != npix) return false;
     // ---- statistics and codes
-    const PlaneCodes planes(width);
+    Vp8lPlaneCodes planes; vp8l_plane_codes_init(&planes, width);
     std::vector<uint32_t> gf(256 + 24, 0), df(40, 0);
     for (Op &o : ops) {
         if (!o.len) { gf[o.dist]++; continue; }
         int s, nx; uint32_t xv;
-        prefix_of(o.len, s, nx, xv); gf[256 + s]++;
-        prefix_of(planes.code_of(o.dist), s, nx, xv); df[s]++;
+        vp8l_prefix_of(o.len, &s, &nx, &xv); gf[256 + s]++;
+        vp8l_prefix_of(vp8l_plane_code_of(&planes, o.dist), &s, &nx, &xv); df[s]++;
     }
-    dfl::HuffScratch S;
+    static thread_local Vp8lHuffScratch S;
     PrefixCode green, dist, zero;
-    make_code(gf, green, S); make_code(df, dist, S);
+    vp8l_make_code(gf, green, S); vp8l_make_code(df, dist, S);
     zero.len.assign(256, 0); zero.code.assign(256, 0); zero.used = 0;
     // ---- the chunk: header byte (no pre-processing, the caller's prediction filter, lossless compression) + image stream
     alph.clear(); alph.reserve(npix / 8 + 64);
@@ -151,14 +98,14 @@ bool vp8l_alpha_from_tokens(const uint32_t *tok, size_t ntok, int width, int hei
     bw.put(0, 1);                       // no transform
     bw.put(0, 1);                       // no colour cache
     bw.put(0, 1);                       // one prefix-code group
-    write_code(bw, green, S);
-    write_code(bw, zero, S); write_code(bw, zero, S); write_code(bw, zero, S);      // red, blue, alpha: always 0
-    write_code(bw, dist, S);
+    vp8l_write_code(bw, green, S);
+    vp8l_write_code(bw, zero, S); vp8l_write_code(bw, zero, S); vp8l_write_code(bw, zero, S);      // red, blue, alpha: always 0
+    vp8l_write_code(bw, dist, S);
     for (const Op &o : ops) {
-        if (!o.len) { put_sym(bw, green, (int)o.dist); continue; }
+        if (!o.len) { vp8l_put_sym(bw, green, (int)o.dist); continue; }
         int s, nx; uint32_t xv;
-        prefix_of(o.len, s, nx, xv); put_sym(bw, green, 256 + s); bw.put(xv, nx);
-        prefix_of(planes.code_of(o.dist), s, nx, xv); put_sym(bw, dist, s); bw.put(xv, nx);
+        vp8l_prefix_of(o.len, &s, &nx, &xv); vp8l_put_sym(bw, green, 256 + s); bw.put(xv, nx);
+        vp8l_prefix_of(vp8l_plane_code_of(&planes, o.dist), &s, &nx, &xv); vp8l_put_sym(bw, dist, s); bw.put(xv, nx);
     }
     bw.flush();
     return true;

@@ -5,6 +5,7 @@
 // bit reader, canonical prefix codes, LZ77 with the 120 neighbourhood distance codes, colour cache, meta prefix image, the four
 // transforms); the tests pin it against libwebp (Pillow) on lossless files and alpha planes of every flavour libwebp writes.
 #include "vp8l_decode.h"
+#include "vp8l_enc_core.h"
 #include <cstring>
 
 namespace b200 {
@@ -187,56 +188,6 @@ struct Decoder {
     }
 };
 
-inline uint32_t add_px(uint32_t a, uint32_t b)
-{   // per-component sum mod 256
-    const uint32_t ag = (a & 0xFF00FF00u) + (b & 0xFF00FF00u), rb = (a & 0x00FF00FFu) + (b & 0x00FF00FFu);
-    return (ag & 0xFF00FF00u) | (rb & 0x00FF00FFu);
-}
-inline uint32_t avg2(uint32_t a, uint32_t b) { return (((a ^ b) & 0xFEFEFEFEu) >> 1) + (a & b); }
-inline int clip255(int v) { return v < 0 ? 0 : v > 255 ? 255 : v; }
-inline uint32_t select_px(uint32_t T, uint32_t L, uint32_t TL)
-{
-    int s = 0;
-    for (int sh = 0; sh < 32; sh += 8) {
-        const int t = (T >> sh) & 0xFF, l = (L >> sh) & 0xFF, c = (TL >> sh) & 0xFF;
-        const int pb = l - c, pa = t - c;
-        s += (pb < 0 ? -pb : pb) - (pa < 0 ? -pa : pa);
-    }
-    return s <= 0 ? T : L;
-}
-inline uint32_t clamp_add_sub_full(uint32_t a, uint32_t b, uint32_t c)
-{
-    uint32_t o = 0;
-    for (int sh = 0; sh < 32; sh += 8) o |= (uint32_t)clip255((int)((a >> sh) & 0xFF) + (int)((b >> sh) & 0xFF) - (int)((c >> sh) & 0xFF)) << sh;
-    return o;
-}
-inline uint32_t clamp_add_sub_half(uint32_t a, uint32_t b)
-{
-    uint32_t o = 0;
-    for (int sh = 0; sh < 32; sh += 8) { const int x = (a >> sh) & 0xFF, y = (b >> sh) & 0xFF; o |= (uint32_t)clip255(x + (x - y) / 2) << sh; }
-    return o;
-}
-inline uint32_t predict(int mode, const uint32_t *cur /*pixel to fill*/, int w)
-{
-    const uint32_t L = cur[-1], T = cur[-w], TR = cur[-w + 1], TL = cur[-w - 1];
-    switch (mode) {
-        case 1: return L;
-        case 2: return T;
-        case 3: return TR;
-        case 4: return TL;
-        case 5: return avg2(avg2(L, TR), T);
-        case 6: return avg2(L, TL);
-        case 7: return avg2(L, T);
-        case 8: return avg2(TL, T);
-        case 9: return avg2(T, TR);
-        case 10: return avg2(avg2(L, TL), avg2(T, TR));
-        case 11: return select_px(T, L, TL);
-        case 12: return clamp_add_sub_full(L, T, TL);
-        case 13: return clamp_add_sub_half(avg2(L, T), TL);
-        default: return 0xFF000000u;
-    }
-}
-
 struct Transform { int type, bits, xs; std::vector<uint32_t> data; };
 
 } // namespace
@@ -259,7 +210,7 @@ bool vp8l_decode_stream(const uint8_t *data, size_t len, int width, int height, 
         } else if (t.type == 3) {
             const int ncol = (int)d.br.bits(8) + 1;
             if (!d.image(ncol, 1, false, t.data)) return false;
-            for (int i = 1; i < ncol; i++) t.data[i] = add_px(t.data[i], t.data[i - 1]);
+            for (int i = 1; i < ncol; i++) t.data[i] = vp8l_add_px(t.data[i], t.data[i - 1]);
             t.bits = ncol <= 2 ? 3 : ncol <= 4 ? 2 : ncol <= 16 ? 1 : 0;
             t.data.resize(256, 0u);                                   // indices past the table read transparent black
             xs = (xs + (1 << t.bits) - 1) >> t.bits;
@@ -288,14 +239,14 @@ bool vp8l_decode_stream(const uint8_t *data, size_t len, int width, int height, 
             }
         } else if (t.type == 0) {
             const int bw = (w + (1 << t.bits) - 1) >> t.bits;
-            pix[0] = add_px(pix[0], 0xFF000000u);
-            for (int x = 1; x < w; x++) pix[x] = add_px(pix[x], pix[x - 1]);
+            pix[0] = vp8l_add_px(pix[0], 0xFF000000u);
+            for (int x = 1; x < w; x++) pix[x] = vp8l_add_px(pix[x], pix[x - 1]);
             for (int y = 1; y < height; y++) {
                 uint32_t *row = pix.data() + (size_t)y * w;
-                row[0] = add_px(row[0], row[-w]);
+                row[0] = vp8l_add_px(row[0], row[-w]);
                 for (int x = 1; x < w; x++) {
                     const int mode = (int)((t.data[(size_t)(y >> t.bits) * bw + (x >> t.bits)] >> 8) & 0xF);
-                    row[x] = add_px(row[x], predict(mode, row + x, w));
+                    row[x] = vp8l_add_px(row[x], vp8l_predict(mode, row[x - 1], row[x - w], row[x - w + 1], row[x - w - 1]));
                 }
             }
         } else {
@@ -344,7 +295,7 @@ bool webp_alpha_decode(const uint8_t *alph, size_t len, int width, int height, s
             else if (filter == 2) { for (int x = 0; x < width; x++) row[x] = (uint8_t)(prev[x] + row[x]); }
             else {
                 uint8_t top = prev[0], tl = top, left = top;
-                for (int x = 0; x < width; x++) { top = prev[x]; left = (uint8_t)(row[x] + clip255((int)left + top - tl)); tl = top; row[x] = left; }
+                for (int x = 0; x < width; x++) { top = prev[x]; left = (uint8_t)(row[x] + vp8l_clip255((int)left + top - tl)); tl = top; row[x] = left; }
             }
         }
     }

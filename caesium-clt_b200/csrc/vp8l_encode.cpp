@@ -1,0 +1,158 @@
+// vp8l_encode.cpp -- see vp8l_device.h.  The host side of the lossless WebP (VP8L) encoder: it runs the analysis kernels, picks the
+// colour-cache size from their histograms, builds the five prefix codes (dfl_core.h, limit 15), writes the header, the transforms and
+// the code descriptions (vp8l_writer.h, shared with the ALPH coder), and frames what the emission kernel wrote.  Every loop over
+// pixels runs on the device; the host walks tiles (the predictor sub-image) and alphabets only.
+#include <cuda_runtime.h>
+#include <chrono>
+#include <cstdio>
+#include <cstdlib>
+#include <cstring>
+#include <map>
+#include "vp8l_device.h"
+#include "vp8l_kernels.h"
+#include "vp8l_writer.h"
+#include "stream_wait.h"
+#include "launch_timer.h"
+
+namespace b200 {
+
+#define CUV(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return false; } } while (0)
+
+template <typename T> static bool grow(T *&p, size_t &cap, size_t need, bool host, std::string &err)
+{
+    if (need <= cap) return true;
+    if (p) { if (host) cudaFreeHost(p); else cudaFree(p); }
+    p = nullptr; cap = 0;
+    size_t want = 1 << 16; while (want < need) want <<= 1;
+    void *q = nullptr;
+    const cudaError_t e = host ? cudaHostAlloc(&q, want, cudaHostAllocDefault) : cudaMalloc(&q, want);
+    if (e != cudaSuccess) { err = std::string(host ? "cudaHostAlloc: " : "cudaMalloc: ") + cudaGetErrorString(e); return false; }
+    p = (T *)q; cap = want; return true;
+}
+
+Vp8lDevice::~Vp8lDevice()
+{
+    cudaFree(d_arena); cudaFree(d_words); cudaFreeHost(h_in); cudaFreeHost(h_small); cudaFreeHost(h_codes); cudaFreeHost(h_words);
+}
+
+namespace {
+
+// the per-pixel buffers of an n-pixel image carved out of one arena (nullptr base: just the size)
+size_t carve(uint8_t *base, size_t n, int nchunks, int tiles, Vp8lBuffers &B)
+{
+    size_t off = 0;
+    auto take = [&](size_t bytes) { uint8_t *q = base ? base + off : nullptr; off += (bytes + 255) / 256 * 256; return q; };
+    B.planes = take(4 * n);
+    B.argb = (uint32_t *)take(4 * n); B.res = (uint32_t *)take(4 * n); B.best = (uint32_t *)take(4 * n);
+    B.modes = take((size_t)tiles);
+    B.cache_tab = (int *)take(4 * vp8l_cache_table_ints(nchunks));
+    B.hits = take((size_t)(VP8L_NCACHE - 1) * n);
+    B.tok = (uint2 *)take(8 * n); B.cnt = (uint32_t *)take(4 * (size_t)nchunks);
+    B.hist = (uint32_t *)take(sizeof(uint32_t) * VP8L_NCACHE * VP8L_HIST);
+    B.flags = (uint32_t *)take(4);
+    B.codes = (Vp8lCodes *)take(sizeof(Vp8lCodes));
+    B.thread_off = (uint32_t *)take(4 * 256 * (size_t)nchunks);
+    B.chunk_bits = (unsigned long long *)take(8 * (size_t)nchunks); B.chunk_start = (unsigned long long *)take(8 * (size_t)nchunks);
+    B.total = (unsigned long long *)take(8);
+    B.words = nullptr;
+    return off;
+}
+
+void code_of(const std::vector<uint32_t> &freq, PrefixCode &pc, Vp8lHuffScratch &S) { vp8l_make_code(freq, pc, S); }
+PrefixCode zero_code(int n) { PrefixCode pc; pc.len.assign(n, 0); pc.code.assign(n, 0); pc.used = 0; return pc; }
+
+} // namespace
+
+bool Vp8lDevice::encode(const uint8_t *rgb, const uint8_t *alpha, int w, int h, void *stream_, std::vector<uint8_t> &out, std::string &err)
+{
+    cudaStream_t st = (cudaStream_t)stream_;
+    if (w < 1 || h < 1 || w > 16384 || h > 16384) { err = "VP8L dimensions out of range"; return false; }
+    const size_t n = (size_t)w * h;
+    const int nchunks = (int)((n + VP8L_CHUNK - 1) / VP8L_CHUNK);
+    const int tiles_x = (w + VP8L_TILE - 1) >> VP8L_TILE_BITS, tiles_y = (h + VP8L_TILE - 1) >> VP8L_TILE_BITS, tiles = tiles_x * tiles_y;
+    Vp8lBuffers B;
+    const size_t arena = carve(nullptr, n, nchunks, tiles, B);
+    const size_t hist_bytes = sizeof(uint32_t) * VP8L_NCACHE * VP8L_HIST, small = hist_bytes + 16 + (size_t)tiles;
+    if (!grow(d_arena, cap_arena, arena, false, err) || !grow(h_in, cap_hin, 4 * n, true, err) || !grow(h_small, cap_hsmall, small, true, err) ||
+        !grow(h_codes, cap_hcodes, sizeof(Vp8lCodes), true, err)) return false;
+    carve(d_arena, n, nchunks, tiles, B);
+    // ---- analysis: everything that decides the bitstream, for every cache candidate at once
+    memcpy(h_in, rgb, 3 * n);
+    if (alpha) memcpy(h_in + 3 * n, alpha, n);
+    CUV(cudaMemcpyAsync(B.planes, h_in, (alpha ? 4 : 3) * n, cudaMemcpyHostToDevice, st));
+    int rc = launch_vp8l_analyse(B, w, h, alpha ? 1 : 0, st);
+    if (rc) { err = std::string("vp8l kernels: ") + cudaGetErrorString((cudaError_t)rc); return false; }
+    uint32_t *h_hist = (uint32_t *)h_small, *h_flags = (uint32_t *)(h_small + hist_bytes);
+    unsigned long long *h_total = (unsigned long long *)(h_small + hist_bytes + 8);
+    uint8_t *h_modes = h_small + hist_bytes + 16;
+    CUV(cudaMemcpyAsync(h_hist, B.hist, hist_bytes, cudaMemcpyDeviceToHost, st));
+    CUV(cudaMemcpyAsync(h_flags, B.flags, 4, cudaMemcpyDeviceToHost, st));
+    CUV(cudaMemcpyAsync(h_modes, B.modes, (size_t)tiles, cudaMemcpyDeviceToHost, st));
+    const auto t0 = std::chrono::steady_clock::now();
+    CUV(stream_wait(st));
+    const auto t1 = std::chrono::steady_clock::now();
+    last_analyse_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
+    // ---- cache size and codes
+    const int cand = vp8l_choose_cache(h_hist), bits = vp8l_cache_bits(cand);
+    last_cache_bits = bits;
+    const uint32_t *hc = h_hist + (size_t)cand * VP8L_HIST;
+    static thread_local Vp8lHuffScratch S;
+    PrefixCode pc[5];
+    const int base[5] = {0, VP8L_HIST_RED, VP8L_HIST_BLUE, VP8L_HIST_ALPHA, VP8L_HIST_DIST};
+    const int size[5] = {256 + 24 + (bits ? 1 << bits : 0), 256, 256, 256, VP8L_NDIST};
+    for (int k = 0; k < 5; k++) code_of(std::vector<uint32_t>(hc + base[k], hc + base[k] + size[k]), pc[k], S);
+    // ---- header, transforms, predictor sub-image, code descriptions
+    std::vector<uint8_t> hdr;
+    hdr.reserve(4096 + (size_t)tiles);
+    BitsLsb bw(hdr);
+    bw.put(0x2f, 8); bw.put((uint32_t)w - 1, 14); bw.put((uint32_t)h - 1, 14); bw.put(*h_flags & 1u, 1); bw.put(0, 3);
+    bw.put(1, 1); bw.put(2, 2);                                             // subtract-green
+    bw.put(1, 1); bw.put(0, 2); bw.put(VP8L_TILE_BITS - 2, 3);              // predictor, 16x16 tiles
+    {   // the mode image: an entropy-coded image without a cache, the mode in the green channel, literals only
+        std::vector<uint32_t> mf(280, 0);
+        for (int t = 0; t < tiles; t++) mf[h_modes[t]]++;
+        PrefixCode mc; code_of(mf, mc, S);
+        const PrefixCode z256 = zero_code(256), z40 = zero_code(VP8L_NDIST);
+        bw.put(0, 1);
+        vp8l_write_code(bw, mc, S); vp8l_write_code(bw, z256, S); vp8l_write_code(bw, z256, S); vp8l_write_code(bw, z256, S); vp8l_write_code(bw, z40, S);
+        for (int t = 0; t < tiles; t++) vp8l_put_sym(bw, mc, h_modes[t]);
+    }
+    bw.put(0, 1);                                                           // no further transform
+    if (bits) { bw.put(1, 1); bw.put((uint32_t)bits, 4); } else bw.put(0, 1);
+    bw.put(0, 1);                                                           // no meta prefix image
+    for (int k = 0; k < 5; k++) vp8l_write_code(bw, pc[k], S);
+    const unsigned long long bit_base = bw.bits();
+    bw.flush();
+    // ---- the codes go up, the tokens are sized and emitted
+    Vp8lCodes *C = (Vp8lCodes *)h_codes;
+    memset(C, 0, sizeof(Vp8lCodes));
+    for (int k = 0; k < 5; k++)
+        if (pc[k].used > 1) for (int s = 0; s < size[k]; s++) { C->code[base[k] + s] = pc[k].code[s]; C->len[base[k] + s] = pc[k].len[s]; }
+    CUV(cudaMemcpyAsync(B.codes, C, sizeof(Vp8lCodes), cudaMemcpyHostToDevice, st));
+    rc = launch_vp8l_size(B, w, h, cand, bit_base, st);
+    if (rc) { err = std::string("vp8l kernels: ") + cudaGetErrorString((cudaError_t)rc); return false; }
+    CUV(cudaMemcpyAsync(h_total, B.total, 8, cudaMemcpyDeviceToHost, st));
+    CUV(stream_wait(st));
+    const unsigned long long total = *h_total;
+    const size_t words = (size_t)((total + 31) / 32), nbytes = (size_t)((total + 7) / 8);
+    if (!grow(d_words, cap_words, words * 4, false, err) || !grow(h_words, cap_hwords, words * 4, true, err)) return false;
+    B.words = d_words;
+    rc = launch_vp8l_emit(B, w, h, cand, words, st);
+    if (rc) { err = std::string("vp8l kernels: ") + cudaGetErrorString((cudaError_t)rc); return false; }
+    CUV(cudaMemcpyAsync(h_words, d_words, words * 4, cudaMemcpyDeviceToHost, st));
+    CUV(stream_wait(st));
+    // ---- the header bits go into the first bytes, then the RIFF framing
+    uint8_t *payload = h_words;
+    for (size_t i = 0; i < hdr.size(); i++) payload[i] |= hdr[i];
+    const size_t pad = nbytes & 1, riff = 4 + 8 + nbytes + pad;
+    out.resize(8 + riff);
+    uint8_t *o = out.data();
+    auto u32 = [](uint8_t *p, uint32_t v) { for (int i = 0; i < 4; i++) p[i] = (uint8_t)(v >> (8 * i)); };
+    memcpy(o, "RIFF", 4); u32(o + 4, (uint32_t)riff); memcpy(o + 8, "WEBPVP8L", 8); u32(o + 16, (uint32_t)nbytes);
+    memcpy(o + 20, payload, nbytes);
+    if (pad) o[20 + nbytes] = 0;
+    last_code_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t1).count();
+    return true;
+}
+
+} // namespace b200
