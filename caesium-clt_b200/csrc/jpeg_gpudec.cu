@@ -132,16 +132,20 @@ __global__ void __launch_bounds__(64) k_gd_round(const DecImage *__restrict__ im
 
 // Write pass sink: every non-zero coefficient is stored on its own into a buffer that was memset.  (A variant that staged whole
 // blocks in local memory and stored them with 16-byte writes, without the memset, measured slower -- 3,220 vs 3,750 images/s --
-// and was removed.)  The block address moves with a gd::Cursor: no divisions inside the decode loop.
+// and was removed.)  The block address moves with a gd::Cursor: no divisions inside the decode loop.  Every subsequence starts
+// from its true state here, so a stream anomaly met inside a real block (ptr set) is in the stream itself: it is collected and
+// the image goes to the host decoder.
 struct SparseWriteSink {
-    const Walk *walk; int16_t *coefs; uint32_t cur, total; Cursor c; int16_t *ptr;
+    const Walk *walk; int16_t *coefs; uint32_t cur, total; Cursor c; int16_t *ptr; uint32_t anom;
     __device__ __forceinline__ void seek() { c.seek(*walk, cur); ptr = cur < total ? coefs + c.offset(*walk) : nullptr; }
     __device__ __forceinline__ void coef(int k, int v) { if (ptr) ptr[k] = (int16_t)v; }
+    __device__ __forceinline__ void anomaly(uint32_t m) { if (ptr) anom |= m; }
     __device__ __forceinline__ void block_done() { cur++; c.next(*walk); ptr = cur < total ? coefs + c.offset(*walk) : nullptr; }
 };
 
+// marker word per image: bit 0 = a marker inside the segment (un-stuff pass), ANOM_* << 1 = the write pass's stream anomalies
 __global__ void __launch_bounds__(64) k_gd_write(const DecImage *__restrict__ imgs, const uint8_t *__restrict__ stream_all, const DecTables *__restrict__ tabs_all,
-                                                 const DecState *__restrict__ A, const uint32_t *__restrict__ first)
+                                                 const DecState *__restrict__ A, const uint32_t *__restrict__ first, uint32_t *__restrict__ marker)
 {
     __shared__ DecShared sh;
     __shared__ Walk walk;
@@ -154,9 +158,10 @@ __global__ void __launch_bounds__(64) k_gd_write(const DecImage *__restrict__ im
     DecState st;
     if (i == 0) { st.p = 0; st.k = 0; st.b = 0; } else st = A[im.sub_off + i - 1];
     SparseWriteSink sk;
-    sk.walk = &walk; sk.coefs = const_cast<int16_t *>(im.scan.coef); sk.cur = first[im.sub_off + i] - first[im.sub_off]; sk.total = sh.g.total_blocks;
+    sk.walk = &walk; sk.coefs = const_cast<int16_t *>(im.scan.coef); sk.cur = first[im.sub_off + i] - first[im.sub_off]; sk.total = sh.g.total_blocks; sk.anom = 0;
     sk.seek();
     decode_subsequence(stream_all + im.stream_off, sh.g, sh.T, i, st, sk);
+    if (sk.anom) atomicOr(&marker[blockIdx.y], sk.anom << 1);
 }
 
 // ---- DC: gather differences component-major, inclusive scan, subtract the component's base, scatter ------------------
@@ -169,20 +174,14 @@ __device__ __forceinline__ uint32_t dc_slot_index(const ge::Scan &s, uint32_t u,
     *comp_start = start;
     return start + m * s.hs[i] * s.vs[i] + q;
 }
-// Also finishes what the write pass could not: a stream that ends early (truncated file) leaves its last block half written
-// and the following blocks untouched; they are zero-filled here (libjpeg's premature-end behaviour), the buffer is not memset.
-__global__ void k_gd_dc_gather(const DecImage *__restrict__ imgs, int32_t *__restrict__ d, const DecState *__restrict__ A,
-                               const uint32_t *__restrict__ first, const uint32_t *__restrict__ nblk)
+// (a stream that ends before its last block is flagged by the write pass and decoded on the host: nothing to finish here)
+__global__ void k_gd_dc_gather(const DecImage *__restrict__ imgs, int32_t *__restrict__ d)
 {
     const DecImage &im = imgs[blockIdx.y];
     const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
     if (u >= im.g.total_blocks) return;
-    int16_t *blk = const_cast<int16_t *>(ge::locate(im.scan, (int)u).blk);
-    const uint32_t last = im.sub_off + im.g.nsub - 1;
-    const uint32_t done = first[last] - first[im.sub_off] + nblk[last];          // blocks the stream completed
-    if (u >= done) { for (int k = u == done ? (int)A[last].k : 0; k < 64; k++) blk[k] = 0; }
     uint32_t cs;
-    d[im.blk_off + dc_slot_index(im.scan, u, &cs)] = blk[0];
+    d[im.blk_off + dc_slot_index(im.scan, u, &cs)] = ge::locate(im.scan, (int)u).blk[0];
 }
 __global__ void k_gd_dc_scatter(const DecImage *__restrict__ imgs, const int32_t *__restrict__ sum)
 {
@@ -365,16 +364,16 @@ bool GpuDecoder::enqueue(void *stream_, std::string &err)
     }
     rounds_used = nrounds;
     CUD(cudaMemcpyAsync(hF, dF, (size_t)4 * N * nrounds, cudaMemcpyDeviceToHost, st));
-    CUD(cudaMemcpyAsync(h_par + o_mark, dM, (size_t)4 * N, cudaMemcpyDeviceToHost, st));
-    // ---- block counts -> first block of each subsequence -> write -> DC (images that did not converge produce garbage
-    //      that their caller discards)
+    // ---- block counts -> first block of each subsequence -> write -> DC (images that did not converge, or whose stream the
+    //      write pass flagged, produce garbage that their caller discards)
     tb = cap_temp;
     cub::DeviceScan::ExclusiveSum(d_temp, tb, d_nblk, d_first, (int)hw_sub, st);
     LT_MARK("cub_scan");
-    k_gd_write<<<gs, 64, 0, st>>>(dI, d_stream, dT, d_A, d_first);
+    k_gd_write<<<gs, 64, 0, st>>>(dI, d_stream, dT, d_A, d_first, dM);
     LT_MARK("k_gd_write");
+    CUD(cudaMemcpyAsync(h_par + o_mark, dM, (size_t)4 * N, cudaMemcpyDeviceToHost, st));
     const dim3 gb(cdiv((long long)hw_mblk, 128), N);
-    k_gd_dc_gather<<<gb, 128, 0, st>>>(dI, d_dc, d_A, d_first, d_nblk);
+    k_gd_dc_gather<<<gb, 128, 0, st>>>(dI, d_dc);
     LT_MARK("k_gd_dc_gather");
     tb = cap_temp;
     cub::DeviceScan::InclusiveSum(d_temp, tb, d_dc, d_dcs, (int)hw_blk, st);
@@ -393,7 +392,8 @@ void GpuDecoder::finish(std::vector<Item> &items)
     for (int n = 0; n < N && n < (int)items.size(); n++) {
         bool conv = false;
         for (int r = 0; r < rounds_used && !conv; r++) conv = hF[(size_t)r * N + n] == 0;
-        items[n].result = conv && tables_ok[n] && !hM[n] ? OK : NOT_CONVERGED;           // a marker inside the segment: the host decoder's business
+        // a marker inside the segment, or a stream anomaly inside a real block: the host decoder's business
+        items[n].result = conv && tables_ok[n] && !hM[n] ? OK : NOT_CONVERGED;
     }
 }
 

@@ -32,7 +32,8 @@ public:
     enum Result { OK = 0, NOT_CONVERGED = 1, FAILED = 2 };
     struct Item { const JpegReader *rd; const JpegReader::DeviceScan *ds; int16_t *d_coefs; Result result; };
     // Decode every item's scan straight into its d_coefs (device; fully overwritten).  Per item: OK, or NOT_CONVERGED
-    // (the self-synchronisation did not settle within the round budget -- degenerate periodic streams -- the caller
+    // (the self-synchronisation did not settle within the round budget -- degenerate periodic streams -- or the stream is
+    // damaged: a marker inside it, an invalid code, a run past index 63 or an end before the last block; the caller
     // decodes that image on the host instead).  Returns false on a CUDA failure.  Asynchronous work on `stream`, with one
     // short host sync per group of rounds.
     bool decode(std::vector<Item> &items, void *stream, std::string &err);

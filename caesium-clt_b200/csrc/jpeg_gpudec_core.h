@@ -34,8 +34,8 @@ struct DecState { uint32_t p; uint16_t k; uint16_t b; };   // 8 bytes
 GE_HD bool same_state(const DecState &a, const DecState &b) { return a.p == b.p && a.k == b.k && a.b == b.b; }
 
 // 32 bits of the unstuffed stream starting at bit position p (big-endian bit order).  The stream buffer is 4-byte
-// aligned and followed by at least 8 bytes of 0xFF padding, so bits past the end read as 1s (like jdhuff.c's padding)
-// and two aligned word loads always suffice.
+// aligned and followed by at least 8 bytes of 0xFF padding, so bits past the end read as 1s (a real block that needs them
+// is flagged ANOM_END: the host decoder reads 0s there) and two aligned word loads always suffice.
 GE_HD uint32_t load_be32(const uint8_t *__restrict__ s, uint32_t word)
 {
     const uint32_t w = reinterpret_cast<const uint32_t *>(s)[word];
@@ -52,6 +52,10 @@ GE_HD uint32_t peek32(const uint8_t *__restrict__ s, uint32_t /*nbits_total*/, u
     return sh ? (w0 << sh) | (w1 >> (32 - sh)) : w0;
 }
 
+// A bit pattern that is no code of the table decodes as "length NO_CODE_LEN, symbol 0": one bit longer than any real code, so
+// it can never be mistaken for a 16-bit code of symbol 0x00, and it still moves an unsynchronised decoder forward.
+constexpr int NO_CODE_LEN = 17;
+
 // decode one Huffman symbol from the top bits of `bits` (32 valid bits); returns symbol, *len = code length (>= 1)
 GE_HD int decode_symbol(const DecTable &t, uint32_t bits, int *len)
 {
@@ -62,9 +66,28 @@ GE_HD int decode_symbol(const DecTable &t, uint32_t bits, int *len)
         const int c = code16 >> (16 - l);
         if (c <= t.maxcode[l]) { *len = l; return t.vals[(t.valoff[l] + c) & 0xFF]; }
     }
-    *len = 16;                  // invalid code (only reachable while unsynchronised or on corrupt data): skip it
+    *len = NO_CODE_LEN;         // invalid code (reachable while unsynchronised or on corrupt data)
     return 0;
 }
+
+// What the write pass reports about the stream, per image.  Each is something the host decoder (jpeg_host.cpp) handles
+// differently from decode_subsequence, so a real block that meets one must be decoded on the host:
+//   ANOM_CODE  no code of the table (the host refuses the file), or a DC category above 15 (the host reads 16+ bits)
+//   ANOM_RUN   a coefficient run past index 63 (the host ends the block without reading the value's bits)
+//   ANOM_END   the stream ends before the last block does (the host reads 0-bits past the end, the device 1-bits)
+// Symbols decoded from the padding after the last real block are not checked: they are normal on every clean file.
+enum : uint32_t { ANOM_CODE = 1u, ANOM_RUN = 2u, ANOM_END = 4u };
+GE_HD uint32_t symbol_anomaly(int len, int sym, bool dc, int k, uint32_t p_next, uint32_t nbits)
+{
+    return (len == NO_CODE_LEN || (dc && sym > 15) ? ANOM_CODE : 0u) |
+           (!dc && (sym & 15) && k + (sym >> 4) > 63 ? ANOM_RUN : 0u) |
+           (p_next > nbits ? ANOM_END : 0u);
+}
+
+// Only a sink that wants the anomalies defines anomaly(mask); for the others (the round passes' block counters) the call and the
+// mask computation vanish.
+template <class Sink> GE_HD auto report_anomaly(Sink &sk, uint32_t m, int) -> decltype(sk.anomaly(m), void()) { sk.anomaly(m); }
+template <class Sink> GE_HD void report_anomaly(Sink &, uint32_t, long) {}
 
 struct Geometry {               // what the decoder needs to know about the scan
     int blocks_per_mcu;
@@ -82,7 +105,7 @@ struct Geometry {               // what the decoder needs to know about the scan
 // codes put the long codes at the top of the code space, so only a handful of prefixes need a second level (Annex K luminance
 // AC: 5 prefixes, < 300 entries).  Entry format, both levels: (code length << 8) | symbol; first level only: bit 15 set =
 // "second level": bits 11..13 = index bits - 1, bits 0..10 = pool offset.  A bit pattern that is no code at all decodes as
-// (16, 0) -- "skip 16 bits" -- exactly what the canonical jdhuff.c search (decode_symbol above) answers for it.
+// (NO_CODE_LEN, 0), exactly what the canonical jdhuff.c search (decode_symbol above) answers for it.
 constexpr int LOOK_BITS = 9, LOOK_N = 1 << LOOK_BITS, MAX_TABLES = 8, EXT_N = 1536;
 struct DecTables {
     uint16_t look[MAX_TABLES * LOOK_N];     // first level of table slot t at look[t * LOOK_N]
@@ -93,11 +116,11 @@ struct DecTables {
 };
 
 // Build the kernel form from DHT payloads.  dht_bits[kind*4+id] / dht_vals[...] = BITS[17] / HUFFVAL of table (kind, id), null if
-// absent; the scan's table use comes from g.dc_tbl / g.ac_tbl.  Returns false (and leaves a harmless all-invalid table set) when
-// the second-level pool would overflow or a DHT is over-subscribed.
+// absent; the scan's table use comes from g.dc_tbl / g.ac_tbl.  Returns false (and leaves a harmless table set of 16-bit skips)
+// when the second-level pool would overflow or a DHT is over-subscribed.
 inline bool build_dec_tables(const uint8_t *const dht_bits[8], const uint8_t *const dht_vals[8], const Geometry &g, DecTables &T)
 {
-    const uint16_t INVALID = (uint16_t)(16 << 8);
+    const uint16_t INVALID = (uint16_t)(NO_CODE_LEN << 8);
     for (int i = 0; i < MAX_TABLES * LOOK_N; i++) T.look[i] = INVALID;
     for (int i = 0; i < EXT_N; i++) T.ext[i] = INVALID;
     for (int i = 0; i < 20; i++) T.sel[i] = 0;
@@ -146,8 +169,11 @@ inline bool build_dec_tables(const uint8_t *const dht_bits[8], const uint8_t *co
         }
     }
     if (!ok) {
-        for (int i = 0; i < MAX_TABLES * LOOK_N; i++) T.look[i] = INVALID;
-        for (int i = 0; i < EXT_N; i++) T.ext[i] = INVALID;
+        // a refused set is never trusted (T.ok = 0 sends the image to the host decoder): its entries only have to keep the passes
+        // in bounds and moving, so every one is a plain 16-bit skip
+        const uint16_t SKIP = (uint16_t)(16 << 8);
+        for (int i = 0; i < MAX_TABLES * LOOK_N; i++) T.look[i] = SKIP;
+        for (int i = 0; i < EXT_N; i++) T.ext[i] = SKIP;
         T.nlook = 1; T.next = 0; T.ok = 0;
         return false;
     }
@@ -191,7 +217,8 @@ struct Cursor {                 // position of one scan-order unit
 };
 
 // Decode from state `st` until the position leaves subsequence `i` (p >= (i+1)*S) or the stream ends.  Sink receives
-// coef(k, value) for every coefficient (DC as raw difference) and block_done().
+// coef(k, value) for every coefficient (DC as raw difference), block_done(), and -- if it defines anomaly() -- the ANOM_* mask of
+// every symbol and once more when the stream has ended.
 template <class Sink>
 GE_HD DecState decode_subsequence(const uint8_t *__restrict__ stream, const Geometry &g, const DecTables &T, uint32_t i, DecState st, Sink &sk)
 {
@@ -223,12 +250,14 @@ GE_HD DecState decode_subsequence(const uint8_t *__restrict__ stream, const Geom
         const uint32_t ext = s ? (bits << len) >> (32 - s) : 0u;
         const int v = s ? ((int)ext < (1 << (s - 1)) ? (int)ext - (1 << s) + 1 : (int)ext) : 0;
         const bool eob_or_zrl = !dc && s == 0;                                     // AC symbol without a value: ZRL or EOB
+        report_anomaly(sk, symbol_anomaly(len, sym, dc, k, p + (uint32_t)(len + s), g.nbits), 0);  // only the write sink looks
         int kw = k + r; if (kw > 63) kw = 63;                                       // corrupt / unsynchronised run: clamp
         if (!eob_or_zrl) sk.coef(kw, v);
         k = eob_or_zrl ? (r == 15 ? k + 16 : 64) : kw + 1;
         p += (uint32_t)(len + s);
         if (k >= 64) { k = 0; b++; if (b == bpm) b = 0; sk.block_done(); }
     }
+    if (p >= g.nbits) report_anomaly(sk, ANOM_END, 0);         // the stream is over: reported if the sink is still inside a real block
     DecState o; o.p = p; o.k = (uint16_t)k; o.b = (uint16_t)b;
     return o;
 }

@@ -19,13 +19,18 @@ struct WriteSink {             // the device sink's logic: a gd::Cursor stepped 
         if (ptr && ptr != ge::locate(*scan, (int)cur).blk) (*mismatch)++;
     }
     void coef(int k, int v) { if (ptr) ptr[k] = (int16_t)v; }
+    void anomaly(uint32_t m) { if (ptr) anom |= m; }
     void block_done() { cur++; c.next(*walk); set(); }
+    uint32_t anom = 0;
 };
 }
 
-// returns 0 ok, 10 not eligible for the device decoder, 11 no convergence within max_rounds, other = parse error
-extern "C" int emul_gpu_decode(const uint8_t *jpeg, size_t len, int subseq_bits, int max_rounds, int16_t *out, long long out_cap, int *rounds_used)
+// returns 0 ok, 10 not eligible for the device decoder, 11 no convergence within max_rounds, 14 stream anomaly inside a real
+// block (the host decodes the image; *anomalies = the gd::ANOM_* rules that fired), other = parse error
+extern "C" int emul_gpu_decode_checked(const uint8_t *jpeg, size_t len, int subseq_bits, int max_rounds, int16_t *out, long long out_cap,
+                                       int *rounds_used, int *anomalies)
 {
+    if (anomalies) *anomalies = 0;
     std::string err;
     JpegReader rd(jpeg, len);
     if (!rd.read_header(err)) return 1;
@@ -71,19 +76,28 @@ extern "C" int emul_gpu_decode(const uint8_t *jpeg, size_t len, int subseq_bits,
     if (changed) return 11;
     // pass: prefix sum + write
     const gd::Walk walk = gd::make_walk(scan);
-    int mismatch = 0;
+    int mismatch = 0; uint32_t anom = 0;
     std::vector<uint32_t> first(G.nsub); { uint32_t run = 0; for (uint32_t i = 0; i < G.nsub; i++) { first[i] = run; run += nblk[i]; } }
     for (uint32_t i = 0; i < G.nsub; i++) {
         WriteSink sk{&scan, &walk, out, first[i], G.total_blocks, {}, nullptr, &mismatch};
         sk.seek();
         gd::DecState st = i ? A[i - 1] : gd::DecState{0, 0, 0};
         gd::decode_subsequence(stream.data(), G, tabs, i, st, sk);
+        anom |= sk.anom;
     }
     if (mismatch) return 13;
+    if (anomalies) *anomalies = (int)anom;
+    if (anom) return 14;
     // pass: DC prefix sums per component in scan order
     int pred[4] = {0, 0, 0, 0};
     for (uint32_t u = 0; u < G.total_blocks; u++) { ge::BlockRef r = ge::locate(scan, (int)u); int16_t *b = const_cast<int16_t *>(r.blk); pred[r.slot] += b[0]; b[0] = (int16_t)pred[r.slot]; }
     return 0;
+}
+
+// the same without the anomaly report
+extern "C" int emul_gpu_decode(const uint8_t *jpeg, size_t len, int subseq_bits, int max_rounds, int16_t *out, long long out_cap, int *rounds_used)
+{
+    return emul_gpu_decode_checked(jpeg, len, subseq_bits, max_rounds, out, out_cap, rounds_used, nullptr);
 }
 
 // Kernel-form tables against the jdhuff.c reference form: every 16-bit pattern (followed by `tail` bits) through every table the

@@ -37,7 +37,7 @@ def emul_decode(emul, data, total_coefs, subseq=1024, max_rounds=64):
 
 
 @pytest.mark.parametrize("name", BASELINE_INPUTS)
-@pytest.mark.parametrize("subseq", [128, 1024, 4096])
+@pytest.mark.parametrize("subseq", [128, 1024, 2048, 4096])
 def test_parallel_decode_matches_host_decoder(L, emul, golden, name, subseq):
     data = golden(name)
     lay, ref = L.jpeg_decode_coefficients(data)
