@@ -63,9 +63,7 @@ _SYMBOLS = [
     "b200_params_default", "b200_set_entropy_mode", "b200_init", "b200_init_device", "b200_shutdown", "b200_device_count", "b200_version", "b200_free",
     "b200_compress_in_memory", "b200_convert_in_memory", "b200_compress_to_size_in_memory", "b200_compress_batch",
     "b200_sniff_format", "b200_jpeg_decode_coefficients", "b200_jpeg_output_layout", "b200_jpeg_requantize",
-    "b200_jpeg_encode_coefficients", "b200_jpeg_decode_planes", "b200_jpeg_quant_table",
-    "b200_jpeg_batch_create", "b200_jpeg_batch_upload", "b200_jpeg_batch_run", "b200_jpeg_batch_download",
-    "b200_jpeg_batch_time", "b200_jpeg_batch_destroy", "b200_jpeg_encode_coefficients_device",
+    "b200_jpeg_encode_coefficients", "b200_jpeg_decode_planes", "b200_jpeg_quant_table", "b200_jpeg_encode_coefficients_device",
     "b200_png_decode", "b200_png_decode_reduced", "b200_png_filter", "b200_png_lz77", "b200_png_deflate_tokens", "b200_png_level_strategies",
     "b200_webp_encode_rgb", "b200_webp_write_levels", "b200_webp_qindex",
     "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_jpeg_pipe_destroy", "b200_device_jobs", "b200_device_numa_node", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba", "b200_webp_alpha_filter", "b200_webp_d2h_bytes",
@@ -82,8 +80,7 @@ def lib():
             getattr(L, name)  # raises AttributeError if the ABI is incomplete
         for f in ("b200_compress_in_memory", "b200_convert_in_memory", "b200_compress_to_size_in_memory",
                   "b200_jpeg_decode_coefficients", "b200_jpeg_output_layout", "b200_jpeg_requantize",
-                  "b200_jpeg_encode_coefficients", "b200_jpeg_decode_planes", "b200_jpeg_batch_create",
-                  "b200_jpeg_batch_upload", "b200_jpeg_batch_run", "b200_jpeg_batch_download", "b200_jpeg_batch_time",
+                  "b200_jpeg_encode_coefficients", "b200_jpeg_decode_planes",
                   "b200_png_decode", "b200_png_decode_reduced", "b200_png_filter", "b200_png_lz77", "b200_png_deflate_tokens",
                   "b200_webp_encode_rgb", "b200_webp_write_levels", "b200_jpeg_encode_coefficients_device",
                   "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba"):
@@ -92,7 +89,6 @@ def lib():
         L.b200_version.restype = C.c_char_p
         L.b200_sniff_format.restype = C.c_uint32
         L.b200_free.argtypes = [C.c_void_p]
-        L.b200_jpeg_batch_destroy.argtypes = [C.c_void_p]
         L.b200_jpeg_pipe_destroy.argtypes = [C.c_void_p]
         L.b200_device_jobs.restype = C.c_longlong
         _lib = L
@@ -393,45 +389,6 @@ def component_view(layout, coefs, c):
     o = layout.comp_offset[c]
     n = layout.bw[c] * layout.bh[c] * 64
     return coefs[o:o + n].reshape(layout.bh[c], layout.bw[c], 64)
-
-
-class JpegBatch:
-    """Device-resident megabatch of n same-layout images (bench.py's HBM-resident `value`)."""
-
-    def __init__(self, in_layout, out_layout, n):
-        self.h = C.c_void_p()
-        self.in_layout, self.out_layout, self.n = in_layout, out_layout, n
-        _check(lib().b200_jpeg_batch_create(C.byref(in_layout), C.byref(out_layout), int(n), C.byref(self.h)))
-
-    def upload(self, i, coefs):
-        coefs = np.ascontiguousarray(coefs, dtype=np.int16)
-        _check(lib().b200_jpeg_batch_upload(self.h, int(i), coefs.ctypes.data_as(C.c_void_p)))
-
-    def run(self, stream=None):
-        n = C.c_int(0)
-        _check(lib().b200_jpeg_batch_run(self.h, C.c_void_p(stream), C.byref(n)))
-        return n.value
-
-    def download(self, i):
-        out = np.zeros(self.out_layout.total_coefs, dtype=np.int16)
-        _check(lib().b200_jpeg_batch_download(self.h, int(i), out.ctypes.data_as(C.c_void_p)))
-        return out
-
-    def time(self, which=0, iters=10):
-        ms = C.c_float(0)
-        _check(lib().b200_jpeg_batch_time(self.h, int(which), int(iters), C.byref(ms)))
-        return ms.value
-
-    def close(self):
-        if self.h:
-            lib().b200_jpeg_batch_destroy(self.h)
-            self.h = C.c_void_p()
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 class JpegPipe:

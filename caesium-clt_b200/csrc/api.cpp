@@ -1213,43 +1213,6 @@ b200_status b200_jpeg_decode_planes(const b200_jpeg_layout *in_layout, const int
 
 void b200_jpeg_quant_table(int quality, int which, uint16_t out[64]) { jpeg_quant_table(quality, which, out); }
 
-// ---- megabatch --------------------------------------------------------------------------------------------------
-struct b200_jpeg_batch { JpegBatch *b; };
-
-b200_status b200_jpeg_batch_create(const b200_jpeg_layout *in_layout, const b200_jpeg_layout *out_layout, int n, b200_jpeg_batch **batch)
-{
-    if (!in_layout || !out_layout || !batch) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
-    *batch = nullptr;
-    std::string err; JpegGeom gin, gout;
-    if (!geom_from_layout(in_layout, gin, err) || !geom_from_layout(out_layout, gout, err)) return make_status(B200_ERR_INVALID_ARGUMENT, err);
-    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
-    JpegBatch *b = batch_create(gin, gout, n, err);
-    if (!b) return make_status(B200_ERR_CUDA, err);
-    *batch = new b200_jpeg_batch{b};
-    return ok_status();
-}
-b200_status b200_jpeg_batch_upload(b200_jpeg_batch *b, int index, const int16_t *in_coefs)
-{
-    std::string err; if (!b || !in_coefs) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
-    return batch_upload(b->b, index, in_coefs, err) ? ok_status() : make_status(B200_ERR_CUDA, err);
-}
-b200_status b200_jpeg_batch_run(b200_jpeg_batch *b, void *cuda_stream, int *launches)
-{
-    std::string err; if (!b) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
-    return batch_run(b->b, cuda_stream, 0, launches, err) ? ok_status() : make_status(B200_ERR_CUDA, err);
-}
-b200_status b200_jpeg_batch_download(b200_jpeg_batch *b, int index, int16_t *out_coefs)
-{
-    std::string err; if (!b || !out_coefs) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
-    return batch_download(b->b, index, out_coefs, err) ? ok_status() : make_status(B200_ERR_CUDA, err);
-}
-b200_status b200_jpeg_batch_time(b200_jpeg_batch *b, int which, int iters, float *ms_per_run)
-{
-    std::string err; if (!b || !ms_per_run) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
-    return batch_time(b->b, which, iters, ms_per_run, err) ? ok_status() : make_status(B200_ERR_CUDA, err);
-}
-void b200_jpeg_batch_destroy(b200_jpeg_batch *b) { if (b) { batch_destroy(b->b); delete b; } }
-
 // ---- device-resident full path ------------------------------------------------------------------------------------------
 struct b200_jpeg_pipe { JpegPipe *p; };
 b200_status b200_jpeg_pipe_create(const uint8_t *const *in, const size_t *in_len, int n, const b200_params *params, int group, b200_jpeg_pipe **pipe)

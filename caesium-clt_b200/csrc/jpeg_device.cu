@@ -29,7 +29,7 @@ thread_local LaunchTimer *tl_launch_timer = nullptr;
 
 #define CU(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return false; } } while (0)
 
-static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+static constexpr size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 bool plan_image(const JpegGeom &gin, const JpegGeom &gout, ImagePlan &p, std::string &err)
 {
@@ -95,20 +95,17 @@ size_t flatten_work(const WorkLists &wl, CompWork *h)
     return n;
 }
 
-int launch_work(const WorkLists &wl, const CompWork *d, void *stream, int which, int *launches)
+int launch_work(const WorkLists &wl, const CompWork *d, void *stream)
 {
-    int rc = 0, n = 0;
+    int rc = 0;
     const CompWork *p_fused = d, *p_idct = p_fused + wl.fused.size(), *p_c420 = p_idct + wl.idct.size();
     const CompWork *p_up = p_c420 + wl.c420.size(), *p_down = p_up + wl.up.size(), *p_fdct = p_down + wl.down.size();
-    if ((which == 0 || which == 1) && !wl.fused.empty()) { rc = launch_fused_same(p_fused, (int)wl.fused.size(), wl.max_fused, stream); n++; LT_MARK("k_fused_same"); if (rc) return rc; }
-    if ((which == 0 || which == 2) && !wl.idct.empty()) { rc = launch_idct_plane(p_idct, (int)wl.idct.size(), wl.max_idct, stream); n++; LT_MARK("k_idct_plane"); if (rc) return rc; }
-    if ((which == 0 || which == 3) && !wl.c420.empty()) { rc = launch_chroma420_refdct(p_c420, (int)wl.c420.size(), wl.max_c420, stream); n++; LT_MARK("k_chroma420_refdct"); if (rc) return rc; }
-    if (which == 0 || which == 3) {
-        if (!wl.up.empty()) { rc = launch_upsample(p_up, (int)wl.up.size(), wl.max_up_w, wl.max_up_h, stream); n++; if (rc) return rc; }
-        if (!wl.down.empty()) { rc = launch_downsample(p_down, (int)wl.down.size(), wl.max_dn_w, wl.max_dn_h, stream); n++; if (rc) return rc; }
-        if (!wl.fdct.empty()) { rc = launch_fdct_plane(p_fdct, (int)wl.fdct.size(), wl.max_fdct, stream); n++; if (rc) return rc; }
-    }
-    if (launches) *launches = n;
+    if (!wl.fused.empty()) { rc = launch_fused_same(p_fused, (int)wl.fused.size(), wl.max_fused, stream); LT_MARK("k_fused_same"); if (rc) return rc; }
+    if (!wl.idct.empty()) { rc = launch_idct_plane(p_idct, (int)wl.idct.size(), wl.max_idct, stream); LT_MARK("k_idct_plane"); if (rc) return rc; }
+    if (!wl.c420.empty()) { rc = launch_chroma420_refdct(p_c420, (int)wl.c420.size(), wl.max_c420, stream); LT_MARK("k_chroma420_refdct"); if (rc) return rc; }
+    if (!wl.up.empty()) { rc = launch_upsample(p_up, (int)wl.up.size(), wl.max_up_w, wl.max_up_h, stream); if (rc) return rc; }
+    if (!wl.down.empty()) { rc = launch_downsample(p_down, (int)wl.down.size(), wl.max_dn_w, wl.max_dn_h, stream); if (rc) return rc; }
+    if (!wl.fdct.empty()) { rc = launch_fdct_plane(p_fdct, (int)wl.fdct.size(), wl.max_fdct, stream); if (rc) return rc; }
     return 0;
 }
 
@@ -263,16 +260,43 @@ bool Slot::ensure(size_t in_bytes, size_t out_bytes, size_t scratch_bytes, size_
            grow_host(h_par, par_cap, par_bytes, err) && grow_dev(d_par, d_par_cap, par_bytes, err);
 }
 
-// parameter block layout: QuantDev q[4] | uint16 dq[4][64] | CompWork work[...]
-static const size_t PAR_Q = 0, PAR_DQ = sizeof(QuantDev) * 4, PAR_WORK = PAR_DQ + sizeof(uint16_t) * 256;
-static size_t par_bytes_for(size_t nwork) { return PAR_WORK + nwork * sizeof(CompWork); }
+// Parameter block of a transform over K images, each part 256-byte aligned:
+//   QuantDev q[4] (per output table) | uint16 dq[K][4][64] (per image and input component, zigzag) | CompWork work[]
+// The resize leg appends its axis tables after the work descriptors.
+static constexpr size_t par_dq_off = align_up(sizeof(QuantDev) * 4, 256);
+static size_t par_work_off(int K) { return par_dq_off + align_up(sizeof(uint16_t) * 256 * K, 256); }
 
-static void fill_tables(uint8_t *h_par, const JpegGeom &gin, const JpegGeom *gout)
+static void put_quant(Slot *s, const JpegGeom &gout)
 {
-    QuantDev *q = reinterpret_cast<QuantDev *>(h_par + PAR_Q);
-    uint16_t *dq = reinterpret_cast<uint16_t *>(h_par + PAR_DQ);
-    if (gout) for (int t = 0; t < 4; t++) if (gout->qt_present[t]) make_quant_dev(gout->qt[t], &q[t]);
+    QuantDev *q = reinterpret_cast<QuantDev *>(s->h_par);
+    for (int t = 0; t < 4; t++) if (gout.qt_present[t]) make_quant_dev(gout.qt[t], &q[t]);
+}
+static const QuantDev *dev_quant(const Slot *s) { return reinterpret_cast<const QuantDev *>(s->d_par); }
+// image k's dequantisation tables into the pinned block; returns where the kernels read them
+static const uint16_t *put_dequant(Slot *s, int k, const JpegGeom &gin)
+{
+    uint16_t *dq = reinterpret_cast<uint16_t *>(s->h_par + par_dq_off) + 256 * k;
     for (int c = 0; c < gin.ncomp; c++) memcpy(dq + 64 * c, gin.qt[gin.tq[c]], 128);
+    return reinterpret_cast<const uint16_t *>(s->d_par + par_dq_off) + 256 * k;
+}
+
+// Quantiser constants, per-image dequantisation tables and the work descriptors of the K images of L into the slot's pinned
+// parameter block.  wl receives the work lists, par_bytes the size of the block, work_off the offset of the descriptors.
+static bool fill_transform_params(Slot *s, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, WorkLists &wl,
+                                  size_t &par_bytes, size_t &work_off, std::string &err)
+{
+    put_quant(s, gout);
+    wl.clear();
+    for (int k = 0; k < L.K; k++) {
+        const JpegGeom &gin = *gins[k];
+        ImagePlan plan;
+        if (!plan_image(gin, gout, plan, err)) return false;
+        append_image_work(gin, gout, plan, L.coefs(*s, k, true), L.coefs(*s, k, false), s->d_scratch + L.scratch_stride * k,
+                          put_dequant(s, k, gin), dev_quant(s), wl);
+    }
+    work_off = par_work_off(L.K);
+    par_bytes = work_off + flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + work_off)) * sizeof(CompWork);
+    return true;
 }
 
 bool slot_transform(Slot *s, const JpegGeom &gin, const JpegGeom &gout, std::string &err, bool download, bool upload)
@@ -280,16 +304,16 @@ bool slot_transform(Slot *s, const JpegGeom &gin, const JpegGeom &gout, std::str
     ImagePlan plan;
     if (!plan_image(gin, gout, plan, err)) return false;
     cudaStream_t st = (cudaStream_t)s->stream;
-    const size_t pbytes = par_bytes_for(4 * 6);
-    if (!s->ensure(plan.in_bytes, plan.out_bytes, plan.scratch_bytes(), pbytes, err)) return false;
-    fill_tables(s->h_par, gin, &gout);
-    WorkLists wl;
-    append_image_work(gin, gout, plan, s->d_in, s->d_out, s->d_scratch,
-                      reinterpret_cast<const uint16_t *>(s->d_par + PAR_DQ), reinterpret_cast<const QuantDev *>(s->d_par + PAR_Q), wl);
-    size_t nw = flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + PAR_WORK));
-    CU(cudaMemcpyAsync(s->d_par, s->h_par, par_bytes_for(nw), cudaMemcpyHostToDevice, st));
+    if (!s->ensure(plan.in_bytes, plan.out_bytes, plan.scratch_bytes(), par_work_off(1) + sizeof(CompWork) * 4 * 6, err)) return false;
+    // a megabatch of one over the slot's own buffers (no strides needed); the work lists are local because s->group_wl and
+    // the group_* sizes belong to the slot's last megabatch and feed the signature of its captured launch sequence
+    GroupLayout L; L.K = 1;
+    const JpegGeom *gins = &gin;
+    WorkLists wl; size_t pbytes = 0, work_off = 0;
+    if (!fill_transform_params(s, &gins, gout, L, wl, pbytes, work_off, err)) return false;
+    CU(cudaMemcpyAsync(s->d_par, s->h_par, pbytes, cudaMemcpyHostToDevice, st));
     if (upload) CU(cudaMemcpyAsync(s->d_in, s->h_in, plan.in_bytes, cudaMemcpyHostToDevice, st));
-    int rc = launch_work(wl, reinterpret_cast<const CompWork *>(s->d_par + PAR_WORK), st, 0, nullptr);
+    int rc = launch_work(wl, reinterpret_cast<const CompWork *>(s->d_par + work_off), st);
     if (rc) { err = std::string("kernel launch: ") + cudaGetErrorString((cudaError_t)rc); return false; }
     if (!download) return true;          // the coefficients stay in HBM for the device entropy encoder
     CU(cudaMemcpyAsync(s->h_out, s->d_out, plan.out_bytes, cudaMemcpyDeviceToHost, st));
@@ -299,44 +323,28 @@ bool slot_transform(Slot *s, const JpegGeom &gin, const JpegGeom &gout, std::str
 
 // ---- megabatch: K same-shaped images per launch sequence (b200_compress_batch) -------------------------------------
 // Buffers of image k live at d_in + k * in_stride etc.; the input coefficients are already in HBM (device decoder) and
-// the output coefficients stay there (device encoder).  Parameter block: QuantDev q[4] | dq[K][4][64] | CompWork[].
+// the output coefficients stay there (device encoder).
 bool slot_group_layout(Slot *s, const JpegGeom &gin, const JpegGeom &gout, int K, GroupLayout &L, std::string &err)
 {
     ImagePlan plan;
     if (!plan_image(gin, gout, plan, err)) return false;
     L.K = K;
     L.in_stride = align_up(plan.in_bytes, 256); L.out_stride = align_up(plan.out_bytes, 256); L.scratch_stride = align_up(std::max<size_t>(plan.scratch_bytes(), 256), 256);
-    const size_t par = align_up(sizeof(QuantDev) * 4, 256) + align_up(sizeof(uint16_t) * 256 * K, 256) + sizeof(CompWork) * (size_t)K * 4 * 6 + 256;
+    const size_t par = par_work_off(K) + sizeof(CompWork) * (size_t)K * 4 * 6 + 256;
     return s->ensure_device(L.in_stride * K, L.out_stride * K, L.scratch_stride * K, par, err);
 }
 
-// host half: quantiser constants, per-image dequantisation tables and the work descriptors into the slot's pinned parameter block
+// host half: the parameter block into the slot's pinned memory, the work lists into s->group_wl
 bool slot_transform_group_prepare(Slot *s, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, std::string &err)
 {
-    const int K = L.K;
-    const size_t o_q = 0, o_dq = align_up(sizeof(QuantDev) * 4, 256), o_work = o_dq + align_up(sizeof(uint16_t) * 256 * K, 256);
-    QuantDev *q = reinterpret_cast<QuantDev *>(s->h_par + o_q);
-    for (int t = 0; t < 4; t++) if (gout.qt_present[t]) make_quant_dev(gout.qt[t], &q[t]);
-    WorkLists &wl = s->group_wl; wl.clear();
-    for (int k = 0; k < K; k++) {
-        const JpegGeom &gin = *gins[k];
-        ImagePlan plan;
-        if (!plan_image(gin, gout, plan, err)) return false;
-        uint16_t *dq = reinterpret_cast<uint16_t *>(s->h_par + o_dq) + 256 * k;
-        for (int c = 0; c < gin.ncomp; c++) memcpy(dq + 64 * c, gin.qt[gin.tq[c]], 128);
-        append_image_work(gin, gout, plan, L.coefs(*s, k, true), L.coefs(*s, k, false), s->d_scratch + L.scratch_stride * k,
-                          reinterpret_cast<const uint16_t *>(s->d_par + o_dq) + 256 * k, reinterpret_cast<const QuantDev *>(s->d_par + o_q), wl);
-    }
-    const size_t nw = flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + o_work));
-    s->group_par_bytes = o_work + nw * sizeof(CompWork); s->group_work_off = o_work;
-    return true;
+    return fill_transform_params(s, gins, gout, L, s->group_wl, s->group_par_bytes, s->group_work_off, err);
 }
 // stream half: parameter block up, the transform kernels
 bool slot_transform_group_enqueue(Slot *s, std::string &err)
 {
     cudaStream_t st = (cudaStream_t)s->stream;
     CU(cudaMemcpyAsync(s->d_par, s->h_par, s->group_par_bytes, cudaMemcpyHostToDevice, st));
-    int rc = launch_work(s->group_wl, reinterpret_cast<const CompWork *>(s->d_par + s->group_work_off), st, 0, nullptr);
+    int rc = launch_work(s->group_wl, reinterpret_cast<const CompWork *>(s->d_par + s->group_work_off), st);
     if (rc) { err = std::string("kernel launch: ") + cudaGetErrorString((cudaError_t)rc); return false; }
     return true;
 }
@@ -501,17 +509,15 @@ bool slot_decode_planes(Slot *s, const JpegGeom &gin, uint8_t *planes, std::stri
     }
     plan.plane_bytes = off_plane; plan.full_bytes = off_full; plan.dplane_bytes = 0;
     plan.in_bytes = (size_t)gin.total_coefs * 2; plan.out_bytes = 256;
-    const size_t pbytes = par_bytes_for(4 * 6);
-    if (!s->ensure(plan.in_bytes, std::max(plan.out_bytes, plan.full_bytes), plan.scratch_bytes(), pbytes, err)) return false;
-    fill_tables(s->h_par, gin, nullptr);
+    const size_t work_off = par_work_off(1);
+    if (!s->ensure(plan.in_bytes, std::max(plan.out_bytes, plan.full_bytes), plan.scratch_bytes(), work_off + sizeof(CompWork) * 4 * 6, err)) return false;
     WorkLists wl;
-    append_image_work(gin, gout, plan, s->d_in, s->d_out, s->d_scratch,
-                      reinterpret_cast<const uint16_t *>(s->d_par + PAR_DQ), reinterpret_cast<const QuantDev *>(s->d_par + PAR_Q), wl);
+    append_image_work(gin, gout, plan, s->d_in, s->d_out, s->d_scratch, put_dequant(s, 0, gin), dev_quant(s), wl);
     wl.down.clear(); wl.fdct.clear();
-    size_t nw = flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + PAR_WORK));
-    CU(cudaMemcpyAsync(s->d_par, s->h_par, par_bytes_for(nw), cudaMemcpyHostToDevice, st));
+    size_t nw = flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + work_off));
+    CU(cudaMemcpyAsync(s->d_par, s->h_par, work_off + nw * sizeof(CompWork), cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(s->d_in, s->h_in, plan.in_bytes, cudaMemcpyHostToDevice, st));
-    int rc = launch_work(wl, reinterpret_cast<const CompWork *>(s->d_par + PAR_WORK), st, 0, nullptr);
+    int rc = launch_work(wl, reinterpret_cast<const CompWork *>(s->d_par + work_off), st);
     if (rc) { err = std::string("kernel launch: ") + cudaGetErrorString((cudaError_t)rc); return false; }
     uint8_t *h = reinterpret_cast<uint8_t *>(s->h_out);
     for (int c = 0; c < gin.ncomp; c++)
@@ -542,21 +548,20 @@ bool slot_transform_resized(Slot *s, const JpegGeom &gin, const JpegGeom &gout, 
     for (int c = 0; c < nc; c++) { dpl_off[c] = off; off += align_up((size_t)gout.rbw[c] * 8 * gout.rbh[c] * 8, 256); }
     const size_t tmp_off = off; off += align_up((size_t)NH * W * sizeof(float), 256);
     // parameter block: tables | work | axis tables
-    const size_t nwork = (size_t)nc * 4;
-    size_t p_axis = align_up(par_bytes_for(nwork), 256);
-    const size_t lv = p_axis, cv = lv + align_up(sizeof(int) * NH, 256), wv = cv + align_up(sizeof(int) * NH, 256);
+    const size_t work_off = par_work_off(1);
+    const size_t lv = align_up(work_off + sizeof(CompWork) * nc * 4, 256), cv = lv + align_up(sizeof(int) * NH, 256), wv = cv + align_up(sizeof(int) * NH, 256);
     const size_t lh = wv + align_up(sizeof(float) * av.weights.size(), 256), chh = lh + align_up(sizeof(int) * NW, 256), wh = chh + align_up(sizeof(int) * NW, 256);
     const size_t pbytes = wh + align_up(sizeof(float) * ah.weights.size(), 256);
     const size_t in_bytes = (size_t)gin.total_coefs * 2, out_bytes = (size_t)gout.total_coefs * 2;
     if (!s->ensure(in_bytes, out_bytes, off, pbytes, err)) return false;
-    fill_tables(s->h_par, gin, &gout);
+    put_quant(s, gout);
+    const uint16_t *d_dq = put_dequant(s, 0, gin);
+    const QuantDev *d_q = dev_quant(s);
     memcpy(s->h_par + lv, av.left.data(), sizeof(int) * NH); memcpy(s->h_par + cv, av.count.data(), sizeof(int) * NH);
     memcpy(s->h_par + wv, av.weights.data(), sizeof(float) * av.weights.size());
     memcpy(s->h_par + lh, ah.left.data(), sizeof(int) * NW); memcpy(s->h_par + chh, ah.count.data(), sizeof(int) * NW);
     memcpy(s->h_par + wh, ah.weights.data(), sizeof(float) * ah.weights.size());
     WorkLists wl;
-    const uint16_t *d_dq = reinterpret_cast<const uint16_t *>(s->d_par + PAR_DQ);
-    const QuantDev *d_q = reinterpret_cast<const QuantDev *>(s->d_par + PAR_Q);
     for (int c = 0; c < nc; c++) {
         CompWork d; memset(&d, 0, sizeof(d));   // decode side
         d.cin = s->d_in + gin.comp_offset[c]; d.dq = d_dq + 64 * c; d.q = d_q;
@@ -574,11 +579,10 @@ bool slot_transform_resized(Slot *s, const JpegGeom &gin, const JpegGeom &gout, 
         wl.down.push_back(e); wl.max_dn_w = std::max(wl.max_dn_w, e.rbw_out * 8); wl.max_dn_h = std::max(wl.max_dn_h, e.rbh_out * 8);
         wl.fdct.push_back(e); wl.max_fdct = std::max(wl.max_fdct, work_tiles(e.rbw_out, e.rbh_out));
     }
-    size_t nw_ = flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + PAR_WORK));
-    (void)nw_;
+    flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + work_off));
     CU(cudaMemcpyAsync(s->d_par, s->h_par, pbytes, cudaMemcpyHostToDevice, st));
     if (upload && !host_rgb) CU(cudaMemcpyAsync(s->d_in, s->h_in, in_bytes, cudaMemcpyHostToDevice, st));
-    const CompWork *dw = reinterpret_cast<const CompWork *>(s->d_par + PAR_WORK);
+    const CompWork *dw = reinterpret_cast<const CompWork *>(s->d_par + work_off);
     const CompWork *p_idct = dw, *p_up = p_idct + wl.idct.size(), *p_down = p_up + wl.up.size(), *p_fdct = p_down + wl.down.size();
     auto chk = [&](int rc, const char *what) { if (rc) { err = std::string(what) + ": " + cudaGetErrorString((cudaError_t)rc); return false; } return true; };
     uint8_t *full[3] = {s->d_scratch + full_off[0], nc == 3 ? s->d_scratch + full_off[1] : nullptr, nc == 3 ? s->d_scratch + full_off[2] : nullptr};
@@ -609,98 +613,6 @@ bool slot_transform_resized(Slot *s, const JpegGeom &gin, const JpegGeom &gout, 
     CU(cudaMemcpyAsync(s->h_out, s->d_out, out_bytes, cudaMemcpyDeviceToHost, st));
     CU(stream_wait(st));
     return true;
-}
-
-// ================================================================================================================
-// megabatch
-// ================================================================================================================
-JpegBatch *batch_create(const JpegGeom &gin, const JpegGeom &gout, int n, std::string &err)
-{
-    if (g_devs.empty()) { err = "library not initialised (no CUDA device)"; return nullptr; }
-    if (n <= 0) { err = "empty batch"; return nullptr; }
-    auto *b = new JpegBatch();
-    b->dev = 0; b->n = n; b->gin = gin; b->gout = gout;
-    auto fail = [&](const std::string &m) -> JpegBatch * { err = m; batch_destroy(b); return nullptr; };
-    if (!plan_image(gin, gout, b->plan, err)) { batch_destroy(b); return nullptr; }
-    cudaSetDevice(g_devs[0]->ordinal);
-    const size_t in_b = align_up(b->plan.in_bytes, 256), out_b = align_up(b->plan.out_bytes, 256), sc_b = align_up(std::max<size_t>(b->plan.scratch_bytes(), 256), 256);
-    void *p = nullptr;
-    if (cudaMalloc(&p, in_b * n) != cudaSuccess) return fail("cudaMalloc (batch input) failed"); b->d_in = (int16_t *)p;
-    if (cudaMalloc(&p, out_b * n) != cudaSuccess) return fail("cudaMalloc (batch output) failed"); b->d_out = (int16_t *)p;
-    if (cudaMalloc(&p, sc_b * n) != cudaSuccess) return fail("cudaMalloc (batch scratch) failed"); b->d_scratch = (uint8_t *)p;
-    cudaStream_t st; if (cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking) != cudaSuccess) return fail("cudaStreamCreate failed"); b->stream = st;
-    cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1); b->ev0 = e0; b->ev1 = e1;
-    size_t nwork_max = (size_t)n * 4 * 6;
-    size_t pbytes = par_bytes_for(nwork_max);
-    std::vector<uint8_t> hpar(pbytes);
-    if (cudaMalloc(&p, pbytes) != cudaSuccess) return fail("cudaMalloc (batch params) failed"); b->d_par = (uint8_t *)p;
-    fill_tables(hpar.data(), gin, &gout);
-    for (int i = 0; i < n; i++)
-        append_image_work(gin, gout, b->plan, (const int16_t *)((const uint8_t *)b->d_in + in_b * i), (int16_t *)((uint8_t *)b->d_out + out_b * i), b->d_scratch + sc_b * i,
-                          reinterpret_cast<const uint16_t *>(b->d_par + PAR_DQ), reinterpret_cast<const QuantDev *>(b->d_par + PAR_Q), b->wl);
-    size_t nw = flatten_work(b->wl, reinterpret_cast<CompWork *>(hpar.data() + PAR_WORK));
-    if (cudaMemcpy(b->d_par, hpar.data(), par_bytes_for(nw), cudaMemcpyHostToDevice) != cudaSuccess) return fail("cudaMemcpy (batch params) failed");
-    b->d_work = reinterpret_cast<const CompWork *>(b->d_par + PAR_WORK);
-    cudaMemset(b->d_in, 0, in_b * n);
-    return b;
-}
-
-bool batch_upload(JpegBatch *b, int idx, const int16_t *coefs, std::string &err)
-{
-    if (!b || idx < 0 || idx >= b->n) { err = "bad batch index"; return false; }
-    cudaSetDevice(g_devs[0]->ordinal);
-    const size_t in_b = align_up(b->plan.in_bytes, 256);
-    CU(cudaMemcpy((uint8_t *)b->d_in + in_b * idx, coefs, b->plan.in_bytes, cudaMemcpyHostToDevice));
-    return true;
-}
-
-bool batch_run(JpegBatch *b, void *stream, int which, int *launches, std::string &err)
-{
-    if (!b) { err = "null batch"; return false; }
-    cudaSetDevice(g_devs[0]->ordinal);
-    int rc = launch_work(b->wl, b->d_work, stream ? stream : b->stream, which, launches);
-    if (rc) { err = std::string("kernel launch: ") + cudaGetErrorString((cudaError_t)rc); return false; }
-    return true;
-}
-
-bool batch_download(JpegBatch *b, int idx, int16_t *coefs, std::string &err)
-{
-    if (!b || idx < 0 || idx >= b->n) { err = "bad batch index"; return false; }
-    cudaSetDevice(g_devs[0]->ordinal);
-    CU(stream_wait((cudaStream_t)b->stream));
-    CU(cudaDeviceSynchronize());
-    const size_t out_b = align_up(b->plan.out_bytes, 256);
-    CU(cudaMemcpy(coefs, (uint8_t *)b->d_out + out_b * idx, b->plan.out_bytes, cudaMemcpyDeviceToHost));
-    return true;
-}
-
-bool batch_time(JpegBatch *b, int which, int iters, float *ms, std::string &err)
-{
-    if (!b || iters <= 0) { err = "bad arguments"; return false; }
-    cudaSetDevice(g_devs[0]->ordinal);
-    cudaStream_t st = (cudaStream_t)b->stream;
-    CU(stream_wait(st));
-    CU(cudaEventRecord((cudaEvent_t)b->ev0, st));
-    for (int i = 0; i < iters; i++) {
-        int rc = launch_work(b->wl, b->d_work, st, which, nullptr);
-        if (rc) { err = std::string("kernel launch: ") + cudaGetErrorString((cudaError_t)rc); return false; }
-    }
-    CU(cudaEventRecord((cudaEvent_t)b->ev1, st));
-    CU(cudaEventSynchronize((cudaEvent_t)b->ev1));
-    float t = 0; CU(cudaEventElapsedTime(&t, (cudaEvent_t)b->ev0, (cudaEvent_t)b->ev1));
-    *ms = t / iters;
-    return true;
-}
-
-void batch_destroy(JpegBatch *b)
-{
-    if (!b) return;
-    if (!g_devs.empty()) cudaSetDevice(g_devs[0]->ordinal);
-    cudaFree(b->d_in); cudaFree(b->d_out); cudaFree(b->d_scratch); cudaFree(b->d_par);
-    if (b->stream) cudaStreamDestroy((cudaStream_t)b->stream);
-    if (b->ev0) cudaEventDestroy((cudaEvent_t)b->ev0);
-    if (b->ev1) cudaEventDestroy((cudaEvent_t)b->ev1);
-    delete b;
 }
 
 } // namespace b200

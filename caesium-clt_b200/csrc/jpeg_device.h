@@ -1,5 +1,5 @@
 // jpeg_device.h -- device side of the JPEG path: per-GPU slot pools (stream + pinned staging + HBM buffers),
-// work-list construction for the transform kernels, and the device-resident megabatch.
+// work-list construction for the transform kernels, and the megabatch (K same-shaped images per launch sequence).
 #pragma once
 #include <cstdint>
 #include <cstddef>
@@ -37,8 +37,8 @@ void append_image_work(const JpegGeom &gin, const JpegGeom &gout, const ImagePla
                        const uint16_t *d_dq, const QuantDev *d_q, WorkLists &wl);
 // Copy lists into `h_work` (contiguous, order fused|idct|c420|up|down|fdct); returns count.
 size_t flatten_work(const WorkLists &wl, CompWork *h_work);
-// Launch every non-empty list; d_work is the device copy of the flattened array.  which: 0 all, 1 fused, 2 idct, 3 c420(+generic tail).
-int launch_work(const WorkLists &wl, const CompWork *d_work, void *stream, int which, int *launches);
+// Launch every non-empty list; d_work is the device copy of the flattened array.
+int launch_work(const WorkLists &wl, const CompWork *d_work, void *stream);
 
 // ---- device runtime ------------------------------------------------------------------------------------------
 struct Slot {
@@ -126,21 +126,5 @@ bool slot_transform_resized(Slot *s, const JpegGeom &gin, const JpegGeom &gout, 
 bool slot_fetch_planes(Slot *s, uint8_t *const *d_planes, int nplanes, size_t n, uint8_t *host, std::string &err);
 // Same front end, but stop after IDCT + upsample and copy planar full-res samples into `planes` (host).
 bool slot_decode_planes(Slot *s, const JpegGeom &gin, uint8_t *planes, std::string &err);
-
-// ---- device-resident megabatch ---------------------------------------------------------------------------------
-struct JpegBatch {
-    int dev = 0, n = 0;
-    JpegGeom gin, gout; ImagePlan plan;
-    int16_t *d_in = nullptr, *d_out = nullptr; uint8_t *d_scratch = nullptr;
-    uint8_t *d_par = nullptr;
-    WorkLists wl; const CompWork *d_work = nullptr;
-    void *stream = nullptr; void *ev0 = nullptr, *ev1 = nullptr;
-};
-JpegBatch *batch_create(const JpegGeom &gin, const JpegGeom &gout, int n, std::string &err);
-bool batch_upload(JpegBatch *b, int idx, const int16_t *coefs, std::string &err);
-bool batch_run(JpegBatch *b, void *stream, int which, int *launches, std::string &err);
-bool batch_download(JpegBatch *b, int idx, int16_t *coefs, std::string &err);
-bool batch_time(JpegBatch *b, int which, int iters, float *ms, std::string &err);
-void batch_destroy(JpegBatch *b);
 
 } // namespace b200

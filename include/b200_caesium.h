@@ -147,20 +147,6 @@ b200_status b200_jpeg_decode_planes(const b200_jpeg_layout *in_layout, const int
 /* mozjpeg table idx 3 scaled by jpeg_set_quality(q, FALSE); natural order */
 void b200_jpeg_quant_table(int quality, int which, uint16_t out[64]);
 
-/* ---- device-resident megabatch (bench "value": inputs already in HBM) -------------------------- */
-typedef struct b200_jpeg_batch b200_jpeg_batch;
-/* n images that share one layout (the BASELINE megabatch: n x 3840x2160 4:2:0) */
-b200_status b200_jpeg_batch_create(const b200_jpeg_layout *in_layout, const b200_jpeg_layout *out_layout, int n, b200_jpeg_batch **batch);
-b200_status b200_jpeg_batch_upload(b200_jpeg_batch *b, int index, const int16_t *in_coefs);
-/* enqueue the whole hot path for every image of the batch on `cuda_stream` (a cudaStream_t; NULL = the
- * library's own stream); asynchronous.  *launches receives the number of kernels enqueued. */
-b200_status b200_jpeg_batch_run(b200_jpeg_batch *b, void *cuda_stream, int *launches);
-b200_status b200_jpeg_batch_download(b200_jpeg_batch *b, int index, int16_t *out_coefs);
-/* time `iters` back-to-back runs of kernel group `which` (0 = whole path, 1 = fused luma IDCT->FDCT,
- * 2 = chroma IDCT, 3 = chroma resample+FDCT) with CUDA events on the launching stream; ms per run */
-b200_status b200_jpeg_batch_time(b200_jpeg_batch *b, int which, int iters, float *ms_per_run);
-void b200_jpeg_batch_destroy(b200_jpeg_batch *b);
-
 /* ---- device-resident FULL path (bench "value": scan bytes in HBM -> scan bytes in HBM) ------------------
  * n baseline single-scan JPEGs of one shape: parsed and uploaded once at create; every run enqueues Huffman decode ->
  * dequant/IDCT/resample/FDCT/quantise -> Huffman encode (optimal tables, stuffing) for all of them, `group` images per launch

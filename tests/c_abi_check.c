@@ -14,8 +14,7 @@ int main(void)
         (fn)b200_params_default, (fn)b200_init, (fn)b200_init_device, (fn)b200_shutdown, (fn)b200_device_count, (fn)b200_version, (fn)b200_free,
         (fn)b200_set_entropy_mode, (fn)b200_compress_in_memory, (fn)b200_convert_in_memory, (fn)b200_compress_to_size_in_memory, (fn)b200_compress_batch,
         (fn)b200_sniff_format, (fn)b200_jpeg_decode_coefficients, (fn)b200_jpeg_output_layout, (fn)b200_jpeg_requantize, (fn)b200_jpeg_encode_coefficients,
-        (fn)b200_jpeg_encode_coefficients_device, (fn)b200_jpeg_decode_planes, (fn)b200_jpeg_quant_table, (fn)b200_jpeg_batch_create, (fn)b200_jpeg_batch_upload,
-        (fn)b200_jpeg_batch_run, (fn)b200_jpeg_batch_download, (fn)b200_jpeg_batch_time, (fn)b200_jpeg_batch_destroy,
+        (fn)b200_jpeg_encode_coefficients_device, (fn)b200_jpeg_decode_planes, (fn)b200_jpeg_quant_table,
         (fn)b200_png_decode, (fn)b200_png_decode_reduced, (fn)b200_png_filter, (fn)b200_png_lz77, (fn)b200_png_deflate_tokens, (fn)b200_png_level_strategies,
         (fn)b200_webp_encode_rgb, (fn)b200_webp_write_levels, (fn)b200_webp_qindex,
         (fn)b200_jpeg_pipe_create, (fn)b200_jpeg_pipe_run, (fn)b200_jpeg_pipe_finish, (fn)b200_jpeg_pipe_fetch, (fn)b200_jpeg_pipe_kernel_times, (fn)b200_jpeg_pipe_destroy, (fn)b200_device_jobs, (fn)b200_device_numa_node, (fn)b200_png_device_times, (fn)b200_webp_decode, (fn)b200_webp_alpha_chunk, (fn)b200_webp_wrap_alpha, (fn)b200_webp_decode_rgba, (fn)b200_webp_alpha_filter, (fn)b200_webp_d2h_bytes,

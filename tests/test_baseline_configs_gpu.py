@@ -79,6 +79,11 @@ def test_resident_pipe_full_path_matches_oracle(L, O, jpegs_4k, lossless, group)
         assert all(s > 100000 for s in sizes)
     times = pipe.kernel_times(1)
     assert "k_gd_write" in times and "k_geb_emit" in times and (lossless or "k_fused_same" in times)
+    if not lossless:
+        # 4:2:0 -> 4:2:0 transform: fused luma, chroma IDCT, collapsed chroma resample + FDCT, each launched once per megabatch
+        for name in ("k_fused_same", "k_idct_plane", "k_chroma420_refdct"):
+            ms, launches = times[name]
+            assert launches == 1 and ms > 0, (name, times[name])
     pipe.close()
 
 

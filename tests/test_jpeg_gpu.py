@@ -225,28 +225,6 @@ def test_inputs_that_take_the_host_decoder(L, O, kw):
         assert out == O.jpeg_lossy(d, O.params(80, 420, True))
 
 
-def test_megabatch_device_resident(L, O, golden):
-    data = golden("in_420_base_640x480.jpg")
-    lay, co = L.jpeg_decode_coefficients(data)
-    p = _params(L, 80, 420, True)
-    olay = L.jpeg_output_layout(lay, p)
-    b = L.JpegBatch(lay, olay, 5)
-    for i in range(5):
-        b.upload(i, co)
-    n = b.run()
-    assert n == 3
-    ref = L.jpeg_requantize(lay, co, olay)
-    for i in range(5):
-        got = b.download(i)
-        # dummy blocks are filled on the host by the encoder; compare real blocks
-        for c in range(3):
-            a = L.component_view(olay, got, c)[:olay.rbh[c], :olay.rbw[c]]
-            r = L.component_view(olay, ref, c)[:olay.rbh[c], :olay.rbw[c]]
-            assert np.array_equal(a, r)
-    assert b.time(0, 3) > 0
-    b.close()
-
-
 def _oracle_to_size(O, data, ss, prog, max_size, return_smallest=True):
     """libcaesium's quality bisection restated around the oracle's lossy encoder (one full encode per try)."""
     if len(data) <= max_size:

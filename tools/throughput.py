@@ -27,17 +27,9 @@ if __name__ == "__main__":
     for _ in range(2):
         L.compress_batch((work * 4)[:256], p, 32, copy=False)   # and every megabatch worker's slot (buffers are allocated on first use)
     reps = int(os.environ.get("REPS", "4"))
-    burn = None
-    if os.environ.get("TOOL_BURN"):                        # a sustained device-resident transform right before each timed call (clock ramp probe)
-        lay, co = L.jpeg_decode_coefficients(datas[0])
-        burn = L.JpegBatch(lay, L.jpeg_output_layout(lay, p), 32)
-        for i in range(32):
-            burn.upload(i, co)
     for th in threads_list:
         for copy in (False, True):
             for rep in range(reps if not copy else 1):      # the first repetition still grows malloc arenas / page-faults fresh output buffers
-                if burn is not None:
-                    burn.time(0, 200)
                 c0 = os.times()
                 t0 = time.perf_counter()
                 res = L.compress_batch(bi, p, th, copy=copy)
