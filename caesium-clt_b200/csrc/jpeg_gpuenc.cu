@@ -4,11 +4,12 @@
 // 0xFF stuffing) are resolved with prefix scans (CUB DeviceScan -- plumbing, not one of the path's named kernels).
 //
 // Passes (one launch each for ANY number of images x scans; blockIdx.y = scan):
-//   classify -> [max-scan: previous event] [sum-scan: trailing correction bits] -> groups -> histogram -> tables ->
-//   lengths -> [sum-scan: bit offsets] -> scan sizes / buffer layout (on the device) -> zero -> emit -> ffcount -> [sum-scan] ->
+//   classify + inline-symbol histogram -> [max-scan: previous event] [sum-scan: trailing correction bits] -> groups + EOBn
+//   histogram -> tables -> lengths -> [sum-scan: bit offsets] -> scan sizes / buffer layout (on the device) -> zero -> emit -> ffcount -> [sum-scan] ->
 //   layout -> scatter (byte stuffing) | D2H: stuffed scans + DHT payloads.  No host wait in between: see "host orchestration".
 #include <cuda_runtime.h>
 #include <cub/device/device_scan.cuh>
+#include <cuda_pipeline.h>
 #include <algorithm>
 #include <chrono>
 #include <cstring>
@@ -23,18 +24,28 @@ using namespace ge;
 #define CU(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return false; } } while (0)
 
 // ---- kernels ------------------------------------------------------------------------------------------------------
+// EOB groups of the AC scans, and their EOBn symbols into the scan's AC table histogram: a group of c blocks is one symbol
+// (nbits(c) - 1) << 4, so a CTA (one scan: blockIdx.y) counts into 15 shared bins and flushes them once.
 __global__ void k_ge_groups(const Scan *__restrict__ scans, const uint32_t *__restrict__ meta, const int *__restrict__ evkey,
-                            const int *__restrict__ prev, const uint32_t *__restrict__ tsum, uint32_t *__restrict__ gcount)
+                            const int *__restrict__ prev, const uint32_t *__restrict__ tsum, uint32_t *__restrict__ gcount, uint32_t *__restrict__ hist)
 {
+    __shared__ uint32_t eob[16];
     const Scan s = scans[blockIdx.y];
     if (s.mode != MODE_AC_FIRST && s.mode != MODE_AC_REFINE) return;
+    if ((int)(blockIdx.x * blockDim.x) > s.nblocks) return;
+    if (threadIdx.x < 16) eob[threadIdx.x] = 0;
+    __syncthreads();
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b > s.nblocks) return;
-    int pg;
-    if (b < s.nblocks) { if (!meta_event(meta[s.unit_base + b])) return; pg = prev[s.unit_base + b]; }
-    else { const long long last = s.unit_base + s.nblocks - 1; pg = max(prev[last], evkey[last]); }
-    const int pl = pg >= s.unit_base ? (int)(pg - s.unit_base) : -1;
-    assign_groups(meta + s.unit_base, tsum + s.unit_base, s.nblocks, pl, b, gcount + s.unit_base);
+    if (b <= s.nblocks && (b == s.nblocks || meta_event(meta[s.unit_base + b]))) {
+        int pg;
+        if (b < s.nblocks) pg = prev[s.unit_base + b];
+        else { const long long last = s.unit_base + s.nblocks - 1; pg = max(prev[last], evkey[last]); }
+        const int pl = pg >= s.unit_base ? (int)(pg - s.unit_base) : -1;
+        assign_groups(meta + s.unit_base, tsum + s.unit_base, s.nblocks, pl, b, gcount + s.unit_base,
+                      [&](uint32_t c) { atomicAdd(&eob[eob_symbol(c) >> 4], 1u); });
+    }
+    __syncthreads();
+    if (threadIdx.x < 16 && eob[threadIdx.x]) atomicAdd(&hist[((size_t)s.tab_base + 2 + s.tbl[0]) * 256 + (threadIdx.x << 4)], eob[threadIdx.x]);
 }
 
 // jchuff.c jpeg_gen_optimal_table with the two minimum searches spread over a warp (ties resolve to the LARGEST index,
@@ -91,9 +102,9 @@ __global__ void k_ge_tables(const uint32_t *__restrict__ hist, Table *__restrict
         for (int s = 0; s <= 255; s++) if (codesize[s]) T.vals[start[min(codesize[s], 32)]++] = (uint8_t)s;
         T.nvals = p;
         for (int k = 0; k < 17; k++) T.bits[k] = bits[k];
-        for (int s = 0; s < 256; s++) { T.code[s] = 0; T.size[s] = 0; }
+        for (int s = 0; s < 256; s++) T.code_len[s] = 0;
         uint32_t code = 0; int k = 0;
-        for (int l = 1; l <= 16; l++) { for (int n = 0; n < bits[l]; n++, k++) { T.code[T.vals[k]] = code++; T.size[T.vals[k]] = (uint8_t)l; } code <<= 1; }
+        for (int l = 1; l <= 16; l++) { for (int n = 0; n < bits[l]; n++, k++) T.code_len[T.vals[k]] = (code++ << 8) | (uint32_t)l; code <<= 1; }
         DhtOut &D = dht[t];
         D.nvals = p;
         for (int k2 = 0; k2 < 17; k2++) D.bits[k2] = bits[k2];
@@ -144,15 +155,43 @@ __device__ __forceinline__ int unit_of(const Scan &s, const BlockComp &bc, int r
     const int m = (row / bc.vs) * bc.mcux + col / bc.hs, q = bc.q_base + (row % bc.vs) * bc.hs + (col % bc.hs);
     return m * bc.blocks_per_mcu + q;
 }
+// blk = the block in the CTA's shared tile; the DC predecessor of DC / interleaved scans may lie outside the tile and is read
+// from global memory
 __device__ __forceinline__ BlockRef ref_of(const Scan &s, int u, const int16_t *blk)
 {
-    if (s.mode == MODE_SEQ || s.mode == MODE_DC_FIRST || s.ns > 1) return locate(s, u);   // needs the DC predecessor / the slot
-    BlockRef r; r.blk = blk; r.prev = nullptr; r.slot = 0; return r;
+    BlockRef r;
+    if (s.mode == MODE_SEQ || s.mode == MODE_DC_FIRST || s.ns > 1) r = locate(s, u);   // needs the DC predecessor / the slot
+    else { r.prev = nullptr; r.slot = 0; }
+    r.blk = blk;
+    return r;
+}
+
+// A CTA of the block-major passes owns ENC_THREADS consecutive blocks i = row * bw + col of one component: 16 KB of contiguous
+// coefficients, staged in shared memory with coalesced 16-byte loads so that the symbol loops read their scattered non-zero
+// coefficients from the tile instead of with one dependent global load each.  Rows are 144 bytes apart: the 16-byte reads of a
+// quarter warp (eight consecutive blocks at the same offset) then fall on distinct banks.
+constexpr int ENC_THREADS = 128;
+constexpr int TILE_PITCH = 72;                  // int16 per tile row
+typedef int16_t Tile[ENC_THREADS][TILE_PITCH];
+
+// asynchronous copies (cp.async): the 16-byte pieces go to shared memory without passing through registers
+__device__ __forceinline__ void stage_tile(Tile &tile, const BlockComp &bc, int i0, int nblk)
+{
+    const uint4 *src = reinterpret_cast<const uint4 *>(bc.coef + bc.comp_off + (long long)i0 * 64);
+    const int n = min(ENC_THREADS, nblk - i0) * 8;                  // 16-byte pieces, 8 per block
+#pragma unroll
+    for (int k = 0; k < 8; k++) { const int q = threadIdx.x + k * ENC_THREADS; if (q < n) __pipeline_memcpy_async(&tile[q >> 3][(q & 7) * 8], src + q, 16); }
+    __pipeline_commit();
+}
+__device__ __forceinline__ void wait_tile()
+{
+    __pipeline_wait_prior(0);
+    __syncthreads();
 }
 
 // The classify pass builds each block's threshold masks once and leaves them in `masks` (24 bytes per block, indexed
-// comp.mask_base + block); the histogram, length and emit passes read them back instead of re-deriving them from the 128-byte
-// block (the mask construction was a quarter to a third of those passes' instructions).
+// comp.mask_base + block); the length and emit passes read them back instead of re-deriving them from the 128-byte block (the
+// mask construction was a quarter to a third of those passes' instructions).
 __device__ __forceinline__ Masks3 load_masks(const Masks3 *__restrict__ masks, const BlockComp &bc, int i)
 {
     const unsigned long long *q = reinterpret_cast<const unsigned long long *>(masks + bc.mask_base + i);   // 24-byte records
@@ -161,64 +200,77 @@ __device__ __forceinline__ Masks3 load_masks(const Masks3 *__restrict__ masks, c
     return M;
 }
 
-__global__ void k_geb_classify(const BlockComp *__restrict__ comps, const Scan *__restrict__ scans, uint32_t *__restrict__ meta, int *__restrict__ evkey, uint32_t *__restrict__ tail,
-                               Masks3 *__restrict__ masks)
+// Classify + the statistics of the inline symbols (DC differences, run/size symbols, ZRLs: they do not depend on the EOB
+// groups; k_ge_groups adds the EOBn symbols).  Each scan visit of the component uses one table kind (two for a sequential scan)
+// of the component's table, so 256 shared counters per (visit, kind) are enough; a script with more visits than HIST_SLOTS
+// counts the rest straight into global memory.
+constexpr int HIST_SLOTS = 6;
+__global__ void __launch_bounds__(ENC_THREADS) k_geb_classify(const BlockComp *__restrict__ comps, const Scan *__restrict__ scans, uint32_t *__restrict__ meta, int *__restrict__ evkey,
+                                                              uint32_t *__restrict__ tail, Masks3 *__restrict__ masks, uint32_t *__restrict__ hist)
 {
+    __shared__ __align__(16) Tile tile;
+    __shared__ uint32_t h[HIST_SLOTS][256];
+    __shared__ int slot_tab[HIST_SLOTS];        // global table index (tab_base + kind * 2 + tbl) of each counter slot
     const BlockComp bc = comps[blockIdx.y];
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= bc.bw * bc.bh) return;
-    const int row = i / bc.bw, col = i - row * bc.bw;
-    const int16_t *blk = bc.coef + bc.comp_off + ((long long)row * bc.bw + col) * 64;
-    const Masks3 M = make_masks3(blk);
-    masks[bc.mask_base + i] = M;
-    for (int j = 0; j < bc.nscan; j++) {
-        const Scan &s = scans[bc.scan_idx[j]];
-        const int u = unit_of(s, bc, row, col);
-        if (u < 0) continue;
-        const uint32_t m = classify_m(s, M);
-        const long long g = s.unit_base + u;
-        meta[g] = m; evkey[g] = meta_event(m) ? (int)g : -1; tail[g] = (uint32_t)meta_tail(m);
-    }
-}
-
-// 512 blocks per CTA: the 16 KB shared histogram is zeroed and flushed once per CTA (a fifth of the pass at 128)
-constexpr int HIST_THREADS = 512;
-__global__ void __launch_bounds__(HIST_THREADS) k_geb_hist(const BlockComp *__restrict__ comps, const Scan *__restrict__ scans, const uint32_t *__restrict__ gcount, uint32_t *__restrict__ hist, const Masks3 *__restrict__ masks)
-{
-    __shared__ uint32_t h[4][1024];
-    for (int i = threadIdx.x; i < 4096; i += blockDim.x) (&h[0][0])[i] = 0;
-    __syncthreads();
-    const BlockComp bc = comps[blockIdx.y];
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < bc.bw * bc.bh) {
-        const int row = i / bc.bw, col = i - row * bc.bw;
-        const int16_t *blk = bc.coef + bc.comp_off + ((long long)row * bc.bw + col) * 64;
-        const Masks3 M = load_masks(masks, bc, i);
-        for (int j = 0; j < bc.nscan; j++) {
+    const int nblk = bc.bw * bc.bh, i0 = blockIdx.x * ENC_THREADS, i = i0 + threadIdx.x;
+    if (i0 >= nblk) return;
+    stage_tile(tile, bc, i0, nblk);
+    for (int k = threadIdx.x; k < HIST_SLOTS * 256; k += ENC_THREADS) (&h[0][0])[k] = 0;
+    if (threadIdx.x == 0) {
+        for (int j = 0, sb = 0; j < bc.nscan; j++) {
             const Scan &s = scans[bc.scan_idx[j]];
+            int ci = 0;                             // the component's place in the scan (interleaved scans list every component)
+            if (s.ns > 1) for (int q = 0; q < bc.q_base; ci++) q += s.hs[ci] * s.vs[ci];
+            const int k0 = s.mode == MODE_AC_FIRST || s.mode == MODE_AC_REFINE ? 1 : 0, k1 = s.mode == MODE_SEQ ? 1 : k0;
+            for (int kind = k0; kind <= k1; kind++, sb++) if (sb < HIST_SLOTS) slot_tab[sb] = s.tab_base + kind * 2 + s.tbl[ci];
+        }
+    }
+    wait_tile();
+    if (i < nblk) {
+        const int row = i / bc.bw, col = i - row * bc.bw;
+        const int16_t *blk = tile[threadIdx.x];
+        const Masks3 M = make_masks3(blk);
+        masks[bc.mask_base + i] = M;
+        for (int j = 0, sb = 0; j < bc.nscan; j++) {
+            const Scan &s = scans[bc.scan_idx[j]];
+            const int k0 = s.mode == MODE_AC_FIRST || s.mode == MODE_AC_REFINE ? 1 : 0;
             const int u = unit_of(s, bc, row, col);
-            if (u < 0) continue;
-            uint32_t *hj = j < 4 ? h[j] : hist + (size_t)s.tab_base * 256;
-            auto add = [&](int idx) { atomicAdd(&hj[idx], 1u); };
-            HistSink<decltype(add)> sk(add);
-            gen_block_m(s, ref_of(s, u, blk), M, gcount[s.unit_base + u], sk);
+            if (u >= 0) {
+                const uint32_t m = classify_m(s, M);
+                const long long g = s.unit_base + u;
+                meta[g] = m; evkey[g] = meta_event(m) ? (int)g : -1; tail[g] = (uint32_t)meta_tail(m);
+                auto add = [&](int idx) {           // idx = (kind * 2 + tbl) * 256 + symbol
+                    const int sl = sb + (idx >> 9) - k0;
+                    if (sl < HIST_SLOTS) atomicAdd(&h[sl][idx & 255], 1u); else atomicAdd(&hist[(size_t)s.tab_base * 256 + idx], 1u);
+                };
+                HistSink<decltype(add)> sk(add);
+                gen_block_m(s, ref_of(s, u, blk), M, 0, sk);
+            }
+            sb += s.mode == MODE_SEQ ? 2 : 1;
         }
     }
     __syncthreads();
-    for (int j = 0; j < bc.nscan && j < 4; j++) {
-        uint32_t *g = hist + (size_t)scans[bc.scan_idx[j]].tab_base * 256;
-        for (int k = threadIdx.x; k < 1024; k += blockDim.x) if (h[j][k]) atomicAdd(&g[k], h[j][k]);
+    int nslots = 0;
+    for (int j = 0; j < bc.nscan; j++) nslots += scans[bc.scan_idx[j]].mode == MODE_SEQ ? 2 : 1;
+    for (int k = threadIdx.x; k < min(nslots, HIST_SLOTS) * 256; k += ENC_THREADS) {
+        const uint32_t v = (&h[0][0])[k];
+        if (v) atomicAdd(&hist[(size_t)slot_tab[k >> 8] * 256 + (k & 255)], v);
     }
 }
 
-__global__ void k_geb_len(const BlockComp *__restrict__ comps, const Scan *__restrict__ scans, const uint32_t *__restrict__ gcount, const Table *__restrict__ tabs, uint32_t *__restrict__ bitlen, const Masks3 *__restrict__ masks)
+__global__ void __launch_bounds__(ENC_THREADS) k_geb_len(const BlockComp *__restrict__ comps, const Scan *__restrict__ scans, const uint32_t *__restrict__ gcount, const Table *__restrict__ tabs,
+                                                         uint32_t *__restrict__ bitlen, const Masks3 *__restrict__ masks)
 {
+    __shared__ __align__(16) Tile tile;
     const BlockComp bc = comps[blockIdx.y];
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= bc.bw * bc.bh) return;
+    const int nblk = bc.bw * bc.bh, i0 = blockIdx.x * ENC_THREADS, i = i0 + threadIdx.x;
+    if (i0 >= nblk) return;
+    stage_tile(tile, bc, i0, nblk);
+    const Masks3 M = load_masks(masks, bc, min(i, nblk - 1));   // in flight with the tile
+    wait_tile();
+    if (i >= nblk) return;
     const int row = i / bc.bw, col = i - row * bc.bw;
-    const int16_t *blk = bc.coef + bc.comp_off + ((long long)row * bc.bw + col) * 64;
-    const Masks3 M = load_masks(masks, bc, i);
+    const int16_t *blk = tile[threadIdx.x];
     for (int j = 0; j < bc.nscan; j++) {
         const Scan &s = scans[bc.scan_idx[j]];
         const int u = unit_of(s, bc, row, col);
@@ -229,23 +281,28 @@ __global__ void k_geb_len(const BlockComp *__restrict__ comps, const Scan *__res
     }
 }
 
-__global__ void k_geb_emit(const BlockComp *__restrict__ comps, const Scan *__restrict__ scans, const uint32_t *__restrict__ gcount, const Table *__restrict__ tabs,
-                           const uint32_t *__restrict__ bitoff, uint32_t *__restrict__ words, const Masks3 *__restrict__ masks, const ScanOut *__restrict__ so,
-                           const uint32_t *__restrict__ flags)
+__global__ void __launch_bounds__(ENC_THREADS) k_geb_emit(const BlockComp *__restrict__ comps, const Scan *__restrict__ scans, const uint32_t *__restrict__ gcount, const Table *__restrict__ tabs,
+                                                          const uint32_t *__restrict__ bitoff, uint32_t *__restrict__ words, const Masks3 *__restrict__ masks, const ScanOut *__restrict__ so,
+                                                          const uint32_t *__restrict__ flags)
 {
+    __shared__ __align__(16) Tile tile;
     if (flags[0]) return;                   // the bit buffer is too small for this batch: the host re-runs this half with exact sizes
     const BlockComp bc = comps[blockIdx.y];
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= bc.bw * bc.bh) return;
+    const int nblk = bc.bw * bc.bh, i0 = blockIdx.x * ENC_THREADS, i = i0 + threadIdx.x;
+    if (i0 >= nblk) return;
+    stage_tile(tile, bc, i0, nblk);
+    const Masks3 M = load_masks(masks, bc, min(i, nblk - 1));   // in flight with the tile
+    wait_tile();
+    if (i >= nblk) return;
     const int row = i / bc.bw, col = i - row * bc.bw;
-    const int16_t *blk = bc.coef + bc.comp_off + ((long long)row * bc.bw + col) * 64;
-    const Masks3 M = load_masks(masks, bc, i);
+    const int16_t *blk = tile[threadIdx.x];
     auto orw = [&](long long w, uint32_t v) { if (v) atomicOr(&words[w], v); };
+    auto stw = [&](long long w, uint32_t v) { words[w] = v; };
     for (int j = 0; j < bc.nscan; j++) {
         const Scan &s = scans[bc.scan_idx[j]];
         const int u = unit_of(s, bc, row, col);
         if (u < 0) continue;
-        EmitSink<decltype(orw)> sk(tabs + s.tab_base, orw, (long long)so[bc.scan_idx[j]].word_base, (unsigned long long)(bitoff[s.unit_base + u] - bitoff[s.unit_base]));
+        EmitSink<decltype(orw), decltype(stw)> sk(tabs + s.tab_base, orw, stw, (long long)so[bc.scan_idx[j]].word_base, (unsigned long long)(bitoff[s.unit_base + u] - bitoff[s.unit_base]));
         gen_block_m(s, ref_of(s, u, blk), M, gcount[s.unit_base + u], sk);
         sk.finish();
     }
@@ -499,10 +556,10 @@ bool GpuEncoder::enqueue_back(void *stream_, std::string &err)
     cudaStream_t st = (cudaStream_t)stream_;
     const int NS = (int)plan.scans.size(), NC = (int)plan.comps.size();
     uint32_t *h_flags = reinterpret_cast<uint32_t *>(h_small + o_flags);
-    const dim3 gb(cdiv(plan.max_comp_blocks, 128), NC);
+    const dim3 gb(cdiv(plan.max_comp_blocks, ENC_THREADS), NC);
     k_ge_zero<<<dim3(64, NS), 256, 0, st>>>(d_so, d_words);
     LT_MARK("k_ge_zero");
-    k_geb_emit<<<gb, 128, 0, st>>>(d_comps, d_scans, d_gcount, d_tabs, d_bitoff, d_words, d_masks, d_so, d_flags);
+    k_geb_emit<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_scans, d_gcount, d_tabs, d_bitoff, d_words, d_masks, d_so, d_flags);
     LT_MARK("k_geb_emit");
     k_ge_ffcount<<<dim3(32, NS + 1), 128, 0, st>>>(d_so, NS, d_words, d_ffcount, groups_cap, d_flags);
     LT_MARK("k_ge_ffcount");
@@ -534,7 +591,7 @@ bool GpuEncoder::enqueue_front(void *stream_, bool fill_dummy, std::string &err)
     const long long U = plan.total_units;
     int max_units = 0; for (auto &s : plan.scans) max_units = std::max(max_units, s.nblocks);
     launches = 0;
-    const dim3 gb(cdiv(plan.max_comp_blocks, 128), NC);
+    const dim3 gb(cdiv(plan.max_comp_blocks, ENC_THREADS), NC);
     if (fill_dummy) {
         for (int im = 0; im < nimg; im++) for (int cc = 0; cc < g.ncomp; cc++) {
             if (g.rbw[cc] == g.bw[cc] && g.rbh[cc] == g.bh[cc]) continue;
@@ -544,7 +601,9 @@ bool GpuEncoder::enqueue_front(void *stream_, bool fill_dummy, std::string &err)
         }
     }
     const dim3 gu1(cdiv(max_units + 1, 128), NS);
-    k_geb_classify<<<gb, 128, 0, st>>>(d_comps, d_scans, d_meta, d_evkey, d_tail, d_masks);
+    CU(cudaMemsetAsync(d_hist, 0, (size_t)NS * 4 * 256 * 4, st));
+    LT_MARK("memset");
+    k_geb_classify<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_scans, d_meta, d_evkey, d_tail, d_masks, d_hist);
     LT_MARK("k_geb_classify");
     size_t tb = cap_temp;
     cub::DeviceScan::ExclusiveScan(d_temp, tb, d_evkey, d_prev, cub::Max(), -1, (int)U, st);
@@ -554,20 +613,16 @@ bool GpuEncoder::enqueue_front(void *stream_, bool fill_dummy, std::string &err)
     LT_MARK("cub_scan");
     CU(cudaMemsetAsync(d_gcount, 0, U * 4, st));
     LT_MARK("memset");
-    k_ge_groups<<<gu1, 128, 0, st>>>(d_scans, d_meta, d_evkey, d_prev, d_tsum, d_gcount);
+    k_ge_groups<<<gu1, 128, 0, st>>>(d_scans, d_meta, d_evkey, d_prev, d_tsum, d_gcount, d_hist);
     LT_MARK("k_ge_groups");
-    CU(cudaMemsetAsync(d_hist, 0, (size_t)NS * 4 * 256 * 4, st));
-    LT_MARK("memset");
-    k_geb_hist<<<dim3(cdiv(plan.max_comp_blocks, HIST_THREADS), NC), HIST_THREADS, 0, st>>>(d_comps, d_scans, d_gcount, d_hist, d_masks);
-    LT_MARK("k_geb_hist");
     k_ge_tables<<<NS * 4, 32, 0, st>>>(d_hist, d_tabs, d_dht);
     LT_MARK("k_ge_tables");
-    k_geb_len<<<gb, 128, 0, st>>>(d_comps, d_scans, d_gcount, d_tabs, d_bitlen, d_masks);
+    k_geb_len<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_scans, d_gcount, d_tabs, d_bitlen, d_masks);
     LT_MARK("k_geb_len");
     tb = cap_temp;
     cub::DeviceScan::ExclusiveSum(d_temp, tb, d_bitlen, d_bitoff, (int)U, st);
     LT_MARK("cub_scan");
-    launches += 8;
+    launches += 7;
     CU(cudaGetLastError());
     return true;
 }

@@ -50,8 +50,7 @@ struct Scan {
 };
 
 struct Table {                  // derived encoder table + the DHT payload
-    uint32_t code[256];
-    uint8_t size[256];
+    uint32_t code_len[256];     // code << 8 | code length: one load per symbol in the length and emit passes (0: unused)
     uint8_t bits[17];
     uint8_t vals[256];
     int nvals;
@@ -221,14 +220,15 @@ GE_HD void gen_dc(int value_shifted, int pred_shifted, int tbl, Sink &sk)
     sk.sym(0, tbl, nb, nb, (unsigned)temp2);
 }
 
+GE_HD int eob_symbol(unsigned count) { return (nbits_of(count) - 1) << 4; }     // EOBn: AC symbol of a group of `count` blocks
 template <class Sink>
 GE_HD void gen_eob_token(unsigned count, int tbl, Sink &sk)
 {
-    const int nb = nbits_of(count) - 1;
-    sk.sym(1, tbl, nb << 4, nb, count);
+    sk.sym(1, tbl, eob_symbol(count), nbits_of(count) - 1, count);
 }
 
-// group_count: >0 iff this block opens an EOB group (then E_j carries that count)
+// group_count: >0 iff this block opens an EOB group (then E_j carries that count).  The statistics pass runs it with
+// group_count = 0: the inline symbols do not depend on the groups, and the EOBn symbols are counted where the groups are made.
 template <class Sink>
 GE_HD void gen_block_m(const Scan &s, const BlockRef &b, const Masks3 &M, unsigned group_count, Sink &sk)
 {
@@ -311,56 +311,80 @@ struct HistSink {               // add(index) must increment counter [kind*2 + t
 struct LenSink {
     const Table *tabs;          // [kind*2 + tbl]
     unsigned long long bits = 0;
-    GE_HD void sym(int kind, int tbl, int symbol, int nb, unsigned) { bits += tabs[kind * 2 + tbl].size[symbol] + nb; }
+    GE_HD void sym(int kind, int tbl, int symbol, int nb, unsigned) { bits += (tabs[kind * 2 + tbl].code_len[symbol] & 0xFFu) + nb; }
     GE_HD void raw64(int nb, unsigned long long) { bits += nb; }
 };
 
-// MSB-first bit writer into a zero-initialised word buffer; `orw(word_index, value)` must OR atomically on the device
-template <class OrFn>
+GE_HD uint32_t shl_or_zero(uint32_t v, int s)      // v << s for s in [0, 32]
+{
+#if defined(__CUDA_ARCH__)
+    return __funnelshift_lc(0u, v, (unsigned)s);
+#else
+    return s >= 32 ? 0u : v << s;
+#endif
+}
+
+// MSB-first bit writer into a zero-initialised word buffer.  `cur` holds the n < 32 bits of the current word left-aligned
+// (the first word starts with the previous block's n bits as zeros).  Only the first and the last word of a block's range can
+// be shared with a neighbouring block: the first completed word and the one finish() writes go through `orw(word_index,
+// value)`, which must OR atomically on the device; every completed word after the first is the block's own and is stored
+// with `stw`.  A caller that writes the blocks one after another may pass its OR function for both.
+template <class OrFn, class StFn = OrFn>
 struct EmitSink {
     const Table *tabs;
     OrFn orw;
-    long long wpos;             // next word index
-    unsigned long long acc = 0; int n = 0;
-    GE_HD EmitSink(const Table *t, OrFn f, long long word_base, unsigned long long bitoff) : tabs(t), orw(f), wpos(word_base + (long long)(bitoff >> 5)), n((int)(bitoff & 31)) {}
-    GE_HD void put(unsigned code, int len)
+    StFn stw;
+    long long wpos, first;      // next word index, the block's first word
+    uint32_t cur = 0; int n;
+    GE_HD EmitSink(const Table *t, OrFn f, StFn g, long long word_base, unsigned long long bitoff)
+        : tabs(t), orw(f), stw(g), wpos(word_base + (long long)(bitoff >> 5)), first(wpos), n((int)(bitoff & 31)) {}
+    GE_HD EmitSink(const Table *t, OrFn f, long long word_base, unsigned long long bitoff) : EmitSink(t, f, f, word_base, bitoff) {}
+    GE_HD void put(uint32_t code, int len)          // the low len bits of code (len <= 32, nothing above them set)
     {
         if (!len) return;
-        acc = (acc << len) | (code & (len == 32 ? 0xFFFFFFFFu : ((1u << len) - 1u)));
-        n += len;
-        while (n >= 32) { orw(wpos++, (uint32_t)(acc >> (n - 32))); n -= 32; acc &= (n ? ((1ull << n) - 1ull) : 0ull); }
+        const int fill = n + len;
+        if (fill < 32) { cur |= code << (32 - fill); n = fill; return; }
+        const int r = fill - 32;                    // bits of code left over for the next word
+        const uint32_t w = cur | (code >> r);
+        if (wpos == first) orw(wpos, w); else stw(wpos, w);
+        wpos++;
+        cur = shl_or_zero(code, 32 - r); n = r;
     }
     GE_HD void sym(int kind, int tbl, int symbol, int nb, unsigned extra)
     {
         // code and value bits leave as one piece: at most 16 + 16 bits
-        const Table &t = tabs[kind * 2 + tbl];
-        put((t.code[symbol] << nb) | (extra & ((1u << nb) - 1u)), t.size[symbol] + nb);
+        const uint32_t e = tabs[kind * 2 + tbl].code_len[symbol];
+        put(((e >> 8) << nb) | (extra & ((1u << nb) - 1u)), (int)(e & 0xFFu) + nb);
     }
     GE_HD void raw64(int nb, unsigned long long v)
     {
-        if (nb > 32) { put((unsigned)(v >> 32), nb - 32); put((unsigned)v, 32); } else put((unsigned)v, nb);
+        if (nb > 32) { put((unsigned)(v >> 32), nb - 32); put((unsigned)v, 32); } else put((unsigned)v, nb);   // v < 2^nb
     }
-    GE_HD void finish() { if (n > 0) orw(wpos, (uint32_t)(acc << (32 - n))); }
+    GE_HD void finish() { if (n > 0) orw(wpos, cur); }
 };
 
 // ---- EOB groups (pass "groups"): called for every event unit b and once for b == nblocks (end of scan) -------------
 // prev_ev = index of the last event unit before b (-1 if none); meta/tsum are the scan's per-unit arrays (tsum =
-// exclusive prefix sum of trailing correction bits); writes gcount[j] = block count of the group opened at j.
-GE_HD void assign_groups(const uint32_t *meta, const uint32_t *tsum, int nblocks, int prev_ev, int b, uint32_t *gcount)
+// exclusive prefix sum of trailing correction bits); writes gcount[j] = block count of the group opened at j, and calls
+// counted(count) once per group, on the common path and on the overflow replay alike (the caller counts the EOBn symbol).
+struct NoCount { GE_HD void operator()(uint32_t) const {} };
+template <class CountFn = NoCount>
+GE_HD void assign_groups(const uint32_t *meta, const uint32_t *tsum, int nblocks, int prev_ev, int b, uint32_t *gcount, CountFn &&counted = CountFn())
 {
+    auto group = [&](int j, uint32_t c) { gcount[j] = c; counted(c); };
     int gs = prev_ev < 0 ? 0 : (meta_contrib(meta[prev_ev]) ? prev_ev : prev_ev + 1);   // first contributor of the run
     if (gs >= b) return;
     const int count = b - gs;
     const uint32_t tend = b < nblocks ? tsum[b] : tsum[nblocks - 1] + (uint32_t)meta_tail(meta[nblocks - 1]);
     const uint32_t tailbits = tend - tsum[gs];          // modular difference: exact while a run holds < 2^32 bits
-    if (count < EOBRUN_MAX && tailbits <= (uint32_t)CORR_FLUSH) { gcount[gs] = (uint32_t)count; return; }
+    if (count < EOBRUN_MAX && tailbits <= (uint32_t)CORR_FLUSH) { group(gs, (uint32_t)count); return; }
     // rare: the run overflows a counter; replay jcphuff.c's sequential rule over it
     int start = gs, n = 0; unsigned be = 0;
     for (int j = gs; j < b; j++) {
         n++; be += (unsigned)meta_tail(meta[j]);
-        if (n == EOBRUN_MAX || be > (unsigned)CORR_FLUSH) { gcount[start] = (uint32_t)n; start = j + 1; n = 0; be = 0; }
+        if (n == EOBRUN_MAX || be > (unsigned)CORR_FLUSH) { group(start, (uint32_t)n); start = j + 1; n = 0; be = 0; }
     }
-    if (n > 0) gcount[start] = (uint32_t)n;
+    if (n > 0) group(start, (uint32_t)n);
 }
 
 // ---- jchuff.c jpeg_gen_optimal_table + jpeg_make_c_derived_tbl (single-thread form; freq has 256 entries) ------------
@@ -392,9 +416,9 @@ GE_HD void build_table(const uint32_t *freq_in, Table &t, int *codesize /*257*/,
     int p = 0;
     for (int l = 1; l <= 32; l++) for (int s = 0; s <= 255; s++) if (codesize[s] == l) t.vals[p++] = (uint8_t)s;
     t.nvals = p;
-    for (int s = 0; s < 256; s++) { t.code[s] = 0; t.size[s] = 0; }
+    for (int s = 0; s < 256; s++) t.code_len[s] = 0;
     uint32_t code = 0; int k = 0;
-    for (int l = 1; l <= 16; l++) { for (int n = 0; n < t.bits[l]; n++, k++) { t.code[t.vals[k]] = code++; t.size[t.vals[k]] = (uint8_t)l; } code <<= 1; }
+    for (int l = 1; l <= 16; l++) { for (int n = 0; n < t.bits[l]; n++, k++) t.code_len[t.vals[k]] = (code++ << 8) | (uint32_t)l; code <<= 1; }
 }
 
 } // namespace ge
