@@ -67,6 +67,7 @@ _SYMBOLS = [
     "b200_png_decode", "b200_png_decode_reduced", "b200_png_filter", "b200_png_lz77", "b200_png_deflate_tokens", "b200_png_level_strategies",
     "b200_webp_encode_rgb", "b200_webp_write_levels", "b200_webp_qindex",
     "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_jpeg_pipe_destroy", "b200_device_jobs", "b200_device_numa_node", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba", "b200_webp_alpha_filter", "b200_webp_d2h_bytes",
+    "b200_set_png_lossy", "b200_png_quantize",
 ]
 
 
@@ -83,7 +84,7 @@ def lib():
                   "b200_jpeg_encode_coefficients", "b200_jpeg_decode_planes",
                   "b200_png_decode", "b200_png_decode_reduced", "b200_png_filter", "b200_png_lz77", "b200_png_deflate_tokens",
                   "b200_webp_encode_rgb", "b200_webp_write_levels", "b200_jpeg_encode_coefficients_device",
-                  "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba"):
+                  "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba", "b200_png_quantize"):
             getattr(L, f).restype = Status
         L.b200_webp_d2h_bytes.restype = C.c_ulonglong
         L.b200_version.restype = C.c_char_p
@@ -225,6 +226,23 @@ def jpeg_encode_coefficients_device(layout, coefs, progressive=True):
 def set_entropy_mode(mode):
     """1 = device entropy encoder (default), 0 = host encoder."""
     return lib().b200_set_entropy_mode(int(mode))
+
+
+def set_png_lossy(on):
+    """b200_set_png_lossy: lossy PNG (png_optimize = 0) on the device quantiser (True) or refused with code 3 (False, the default)."""
+    return lib().b200_set_png_lossy(int(bool(on)))
+
+
+def png_quantize(rgba, quality):
+    """b200_png_quantize: rgba uint8 [h, w, 4] -> (palette uint8 [n, 4] as R, G, B, A; indices uint8 [h, w])."""
+    rgba = np.ascontiguousarray(rgba, dtype=np.uint8)
+    h, w = rgba.shape[:2]
+    pal = np.zeros((256, 4), np.uint8)
+    idx = np.zeros((h, w), np.uint8)
+    n = C.c_int()
+    _check(lib().b200_png_quantize(rgba.ctypes.data_as(C.c_void_p), w, h, int(quality), pal.ctypes.data_as(C.c_void_p), C.byref(n),
+                                   idx.ctypes.data_as(C.c_void_p)))
+    return pal[:n.value].copy(), idx
 
 
 def jpeg_decode_planes(in_layout, in_coefs):

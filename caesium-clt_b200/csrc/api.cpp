@@ -2,6 +2,7 @@
 // libcaesium's lib.rs performs behind caesium::{compress,convert,compress_to_size}_in_memory
 // (call sites caesium-clt's src/compressor.rs:287-306).  No CPU codec fallback exists anywhere below.
 #include "../../include/b200_caesium.h"
+#include "../../include/b200_caesium_png_lossy.h"
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -24,6 +25,7 @@
 #include "resize_kernels.h"
 #include "png_host.h"
 #include "png_device.h"
+#include "png_quant.h"
 #include "vp8_host.h"
 #include "webp_device.h"
 #include "vp8l_device.h"
@@ -52,6 +54,7 @@ b200_status header_status(const std::string &err) { return make_status(err.compa
 
 int g_forced_device = -1, g_forced_ngpus = 0;
 std::atomic<int> g_entropy_mode{-1};     // -1 unset (env B200_ENTROPY); bit 0 = device entropy encoder, bit 1 = device entropy decoder (default 3)
+std::atomic<int> g_png_lossy{-1};        // -1 unset (env B200_PNG_LOSSY); 1 = lossy PNG on the device's quantiser, 0 = refused (code 3)
 
 // runtime_init is idempotent while initialised, so after b200_shutdown (which frees every slot's device buffers) the next call
 // initialises again: a long-running host can hand the memory of one workload's slots back before starting another
@@ -72,6 +75,16 @@ int entropy_mode()
         g_entropy_mode.store(!e ? 3 : !strcmp(e, "host") ? 0 : !strcmp(e, "gpuenc") ? 1 : !strcmp(e, "gpudec") ? 2 : 3);
     }
     return g_entropy_mode.load();
+}
+
+// lossy PNG (png.optimize == false) on the device: b200_set_png_lossy, else B200_PNG_LOSSY=gpu, read once; off by default
+bool png_lossy()
+{
+    if (g_png_lossy.load() < 0) {
+        const char *e = getenv("B200_PNG_LOSSY");
+        g_png_lossy.store(e && !strcmp(e, "gpu") ? 1 : 0);
+    }
+    return g_png_lossy.load() == 1;
 }
 
 // One slot of one device (prefer_dev < 0: the next device round-robin), held until the lease goes out of scope.  The runtime
@@ -353,19 +366,22 @@ void jpeg_compress_group(const uint8_t *const *in, const size_t *in_len, const s
     tm.lap(5);
 }
 
+b200_status png_lossy_compress(PngInfo &info, const PngIdat &idat, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out);
+
 // ---- PNG (lossless) through the device ---------------------------------------------------------------------------
 // libcaesium png::compress: optimize == true -> png::lossless (oxipng, level = png.optimization_level); otherwise the lossy
 // palette quantiser (imagequant), which is outside this path.  Resizing a PNG goes through the image crate's decoder and is
 // likewise left to the reference.
 b200_status png_compress(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
 {
-    if (!p->png_optimize) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::compress_in_memory)");
+    if (!p->png_optimize && !png_lossy()) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::compress_in_memory)");
     if (p->width || p->height) return make_status(B200_ERR_UNSUPPORTED, "PNG resize is outside the GPU path (route to caesium::compress_in_memory)");
     std::string err;
     PngInfo info; PngIdat idat;
     static const bool verbose = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2;
     const auto t0 = std::chrono::steady_clock::now();
     if (!png_parse_chunks(in, in_len, p->keep_metadata != 0, info, idat, err)) return png_status(err);
+    if (!p->png_optimize) return png_lossy_compress(info, idat, p, prefer_dev, out);
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
     std::vector<uint8_t> z;
     auto t1 = t0;
@@ -397,11 +413,87 @@ b200_status png_compress(const uint8_t *in, size_t in_len, const b200_params *p,
     return ok_status();
 }
 
+// chunks whose meaning depends on the colour type (sBIT, bKGD, hIST) do not survive quantisation, nor does a grey source's ICC
+// profile (iCCP): a grey profile is invalid on the indexed colour output
+void drop_colour_chunks(std::vector<uint8_t> &kept, bool grey_source)
+{
+    std::vector<uint8_t> out;
+    for (size_t i = 0; i + 12 <= kept.size();) {
+        const size_t L = (size_t)kept[i] << 24 | (size_t)kept[i + 1] << 16 | (size_t)kept[i + 2] << 8 | kept[i + 3];
+        if (L > kept.size() - i - 12) break;
+        const char *t = reinterpret_cast<const char *>(kept.data() + i + 4);
+        if (memcmp(t, "sBIT", 4) && memcmp(t, "bKGD", 4) && memcmp(t, "hIST", 4) && (!grey_source || memcmp(t, "iCCP", 4))) out.insert(out.end(), kept.begin() + i, kept.begin() + i + 12 + L);
+        i += 12 + L;
+    }
+    kept.swap(out);
+}
+
+// One lossy PNG try: the quantiser already holds the image (histogram built); palette at `quality`, dithering, indexed coding, file.
+// B200_TRACE=2 prints the per-kernel event times.
+b200_status png_lossy_code(Slot *s, PngInfo info, int quality, int level, std::vector<uint8_t> &out)
+{
+    static const bool verbose = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2;
+    std::string err;
+    std::vector<uint8_t> z;
+    LaunchTimer lt;
+    if (verbose) { lt.begin((cudaStream_t)s->stream); tl_launch_timer = &lt; }
+    const auto t0 = std::chrono::steady_clock::now();
+    const bool ok = s->png_dev()->code_quantized(info, quality < 0 ? 0 : quality > 100 ? 100 : quality, std::min(level, 6), s->stream, z, err);
+    tl_launch_timer = nullptr;
+    if (!ok) return make_status(B200_ERR_CUDA, err);
+    if (verbose) {
+        std::map<std::string, std::pair<double, int>> acc;
+        lt.collect(acc);
+        std::string kt;
+        for (auto &kv : acc) { char b[96]; snprintf(b, sizeof b, " %s=%.4f", kv.first.c_str(), kv.second.first); kt += b; }
+        fprintf(stderr, "[b200 trace] png-lossy %ux%u q%d: %d colours, device %.3f ms (median cut %.3f); kernels ms:%s\n", info.width, info.height, quality,
+                (int)(info.plte.size() / 3), std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(), s->png_dev()->quantiser()->last_cut_ms, kt.c_str());
+    }
+    png_write(info, z, out);
+    return ok_status();
+}
+
+// a parsed PNG's IDAT inflated into the slot's staging buffer, un-filtered, expanded and histogrammed by the quantiser
+b200_status png_lossy_load(Slot *s, PngInfo &info, const PngIdat &idat)
+{
+    std::string err;
+    const bool grey = info.color_type == 0 || info.color_type == 4;
+    drop_colour_chunks(info.kept_before_idat, grey); drop_colour_chunks(info.kept_after_idat, grey);
+    PngDevice *png = s->png_dev();
+    const size_t nin = (info.row_bytes + 1) * (size_t)info.height;
+    size_t cap = 0, got = 0; uint32_t stored_adler = 0;
+    uint8_t *buf = png->input_buffer(nin, cap, err);
+    if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    if (!zlib_inflate_to(idat.p, idat.n, buf, cap, nin, &got, &stored_adler, err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
+    if (got < nin) return make_status(B200_ERR_CORRUPT_INPUT, "IDAT too short");
+    if (!png->load_filtered_lossy(info, got, stored_adler, s->stream, err)) return make_status(png->corrupt ? B200_ERR_CORRUPT_INPUT : B200_ERR_CUDA, err);
+    return ok_status();
+}
+
+// lossy PNG (png.optimize == false, the switch on): palette quantisation with Floyd-Steinberg dithering on the device, then the
+// lossless leg's filter trials, LZ77 and DEFLATE over the indexed image
+b200_status png_lossy_compress(PngInfo &info, const PngIdat &idat, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
+{
+    std::string err;
+    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
+    SlotLease s(prefer_dev);
+    if (!s) return s.failure();
+    const b200_status st = png_lossy_load(s, info, idat);
+    if (st.code) return st;
+    return png_lossy_code(s, info, (int)p->png_quality, (int)p->png_optimization_level, out);
+}
+
 // 8-bit planar samples ([nc][h][w], nc = 1 or 3) and an optional alpha plane -> lossless PNG (K6 filter selection, K7 LZ77) on the
 // slot's PngDevice.  palette: try png_reduce_palette first.
 b200_status png_from_planes(Slot *s, const uint8_t *planes, int nc, const uint8_t *alpha, uint32_t w, uint32_t h, bool palette, const b200_params *p,
                             std::vector<uint8_t> &out, std::string &err)
 {
+    if (!p->png_optimize) {             // lossy PNG (the callers refuse it while the switch is off): the planes go up as they are
+        PngQuant *q = s->png_dev()->quantiser();
+        if (!q->load_planes(planes, nc, alpha, (int)w, (int)h, s->stream, err) || !q->prepare(s->stream, err)) return make_status(B200_ERR_CUDA, err);
+        PngInfo info; info.width = w; info.height = h;
+        return png_lossy_code(s, info, (int)p->png_quality, (int)p->png_optimization_level, out);
+    }
     const size_t n = (size_t)w * h;
     const int ch = nc + (alpha ? 1 : 0);
     std::vector<uint8_t> raw;
@@ -470,7 +562,7 @@ b200_status jpeg_to_webp(const uint8_t *in, size_t in_len, const b200_params *p,
 // the lossless PNG leg (K6 filter selection, K7 LZ77).  A greyscale JPEG becomes a greyscale PNG.
 b200_status jpeg_to_png(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
 {
-    if (!p->png_optimize) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::convert_in_memory)");
+    if (!p->png_optimize && !png_lossy()) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::convert_in_memory)");
     std::string err;
     JpegReader rd(in, in_len);
     if (!rd.read_header(err)) return header_status(err);
@@ -737,7 +829,7 @@ b200_status convert_dispatch(const uint8_t *in, size_t in_len, uint32_t src, uin
     if (src == B200_FMT_WEBP && (fmt == B200_FMT_JPEG || fmt == B200_FMT_PNG)) {
         // WebP source: decoded on the calling thread (vp8_decode.cpp), then the same back ends as a PNG source
         if (fmt == B200_FMT_JPEG && p->jpeg_optimize) return make_status(B200_ERR_UNSUPPORTED, "lossless conversion to JPEG is outside the GPU path (route to caesium::convert_in_memory)");
-        if (fmt == B200_FMT_PNG && !p->png_optimize) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::convert_in_memory)");
+        if (fmt == B200_FMT_PNG && !p->png_optimize && !png_lossy()) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::convert_in_memory)");
         WebpInfo wi; std::vector<uint8_t> rgb, alpha;
         const b200_status s = webp_decode_status(in, in_len, wi, rgb, &alpha);
         if (s.code) return s;
@@ -861,6 +953,7 @@ int b200_device_numa_node(int index) { return index < 0 || index >= runtime_devi
 const char *b200_version(void) { return "b200-caesium 0.1.0 (sm_90a)"; }
 void b200_free(void *p) { free(p); }
 int b200_set_entropy_mode(int mode) { if (mode < 0 || mode > 3) return B200_ERR_INVALID_ARGUMENT; g_entropy_mode.store(mode); return B200_OK; }
+int b200_set_png_lossy(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_png_lossy.store(on); return B200_OK; }
 
 uint32_t b200_sniff_format(const uint8_t *d, size_t n)
 {   // the magic numbers `infer` checks (scan_files.rs:30-40, compressor.rs:259-264)
@@ -1009,6 +1102,29 @@ static b200_status webp_to_size(const uint8_t *in, size_t in_len, b200_params *p
     return bisect_quality(size_at, max_output_size, return_smallest, &params->webp_quality, result);
 }
 
+// PNG (the lossy switch on): the source is decoded, un-filtered, expanded and histogrammed once; every try runs median cut,
+// refinement, dithering and coding at its png_quality
+static b200_status png_to_size(const uint8_t *in, size_t in_len, b200_params *params, size_t max_output_size, bool return_smallest, std::vector<uint8_t> &result)
+{
+    if (!png_lossy()) return make_status(B200_ERR_UNSUPPORTED, "compress_to_size on a PNG bisects the lossy (imagequant) quality, which is outside the GPU path (route to caesium::compress_to_size_in_memory)");
+    if (params->width || params->height) return make_status(B200_ERR_UNSUPPORTED, "PNG resize is outside the GPU path (route to caesium::compress_to_size_in_memory)");
+    std::string err;
+    PngInfo info; PngIdat idat;
+    if (!png_parse_chunks(in, in_len, params->keep_metadata != 0, info, idat, err)) return png_status(err);
+    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
+    SlotLease s(-1);
+    if (!s) return s.failure();
+    const b200_status st = png_lossy_load(s, info, idat);
+    if (st.code) return st;
+    auto size_at = [&](int q, auto want, size_t &sz, std::vector<uint8_t> &cur) -> b200_status {
+        (void)want;
+        const b200_status r = png_lossy_code(s, info, q, (int)params->png_optimization_level, cur);
+        sz = cur.size();
+        return r;
+    };
+    return bisect_quality(size_at, max_output_size, return_smallest, &params->png_quality, result);
+}
+
 b200_status b200_compress_to_size_in_memory(const uint8_t *in, size_t in_len, b200_params *params, size_t max_output_size, uint8_t return_smallest,
                                             uint8_t **out, size_t *out_len)
 {
@@ -1022,7 +1138,7 @@ b200_status b200_compress_to_size_in_memory(const uint8_t *in, size_t in_len, b2
         b200_status s;
         if (fmt == B200_FMT_JPEG) s = jpeg_to_size(in, in_len, params, max_output_size, return_smallest != 0, result);
         else if (fmt == B200_FMT_WEBP) s = webp_to_size(in, in_len, params, max_output_size, return_smallest != 0, result);
-        else if (fmt == B200_FMT_PNG) s = make_status(B200_ERR_UNSUPPORTED, "compress_to_size on a PNG bisects the lossy (imagequant) quality, which is outside the GPU path (route to caesium::compress_to_size_in_memory)");
+        else if (fmt == B200_FMT_PNG) s = png_to_size(in, in_len, params, max_output_size, return_smallest != 0, result);
         else s = make_status(fmt == B200_FMT_UNKNOWN ? B200_ERR_UNKNOWN_FORMAT : B200_ERR_UNSUPPORTED, "compress_to_size for this format is outside the GPU path (route to caesium::compress_to_size_in_memory)");
         return s.code ? s : give(result, out, out_len);
     });
@@ -1426,6 +1542,25 @@ b200_status b200_png_device_times(const uint8_t *in, size_t in_len, int level, i
     if (out.size() + 1 > cap) return make_status(B200_ERR_INVALID_ARGUMENT, "text buffer too small");
     memcpy(text, out.c_str(), out.size() + 1);
     return ok_status();
+}
+
+b200_status b200_png_quantize(const uint8_t *rgba, int width, int height, int quality, uint8_t *palette_rgba, int *npalette, uint8_t *indices)
+{
+    if (!rgba || !palette_rgba || !npalette || !indices || width < 1 || height < 1 || width > 65535 || height > 65535 || quality < 0 || quality > 100)
+        return make_status(B200_ERR_INVALID_ARGUMENT, "invalid argument");
+    std::string err;
+    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
+    return guarded([&] {
+        SlotLease s(-1);
+        if (!s) return s.failure();
+        PngQuant *q = s->png_dev()->quantiser();
+        std::vector<uint32_t> pal;
+        if (!q->load_host(rgba, width, height, s->stream, err) || !q->prepare(s->stream, err) || !q->quantize(quality, s->stream, pal, err) ||
+            !q->fetch_indices(indices, s->stream, err)) return make_status(B200_ERR_CUDA, err);
+        for (size_t k = 0; k < pal.size(); k++) for (int c = 0; c < 4; c++) palette_rgba[4 * k + c] = (uint8_t)(pal[k] >> (8 * c));
+        *npalette = (int)pal.size();
+        return ok_status();
+    });
 }
 
 int b200_png_level_strategies(int level, int *out)

@@ -10,6 +10,7 @@
 #include "png_device.h"
 #include "png_kernels.h"
 #include "png_deflate.h"
+#include "png_quant.h"
 #include <chrono>
 #include <cstdlib>
 #include "stream_wait.h"
@@ -39,7 +40,10 @@ PngDevice::~PngDevice()
     cudaFree(d_raw); cudaFree(d_raw2); cudaFree(d_filt); cudaFree(d_best); cudaFree(d_tok); cudaFree(d_out); cudaFree(d_counts); cudaFree(d_offsets);
     cudaFree(d_hist); cudaFree(d_sums); cudaFree(d_tlog); cudaFree(d_temp); cudaFreeHost(h_small); cudaFreeHost(h_tok); cudaFreeHost(h_raw);
     cudaFree(d_filt_all); cudaFree(d_fin); cudaFree(d_sums_in); cudaFree(d_sync); cudaFree(d_dfl); cudaFree(d_z); cudaFreeHost(h_z);
+    delete quant;
 }
+
+PngQuant *PngDevice::quantiser() { if (!quant) quant = new PngQuant(); return quant; }
 
 // oxipng presets (SURVEY.md §3.4-iii): which row-filter strategies each optimisation level tries
 std::vector<int> png_level_strategies(int level)
@@ -133,7 +137,20 @@ uint8_t *PngDevice::input_buffer(size_t bytes, size_t &cap, std::string &err)
 // (input_buffer()); everything from there to the finished zlib stream runs on the device -- un-filter (wavefront), Adler-32 check of
 // the input, reductions, K6 / K7 per strategy, DEFLATE coding -- except a palette reduction, which (at most 256 colours) goes
 // through the host and the raw-sample entry point below.
-bool PngDevice::compress_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, int level, void *stream_, std::vector<uint8_t> &zlib_stream, int *chosen, std::string &err)
+bool PngDevice::compress_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, int level, void *stream, std::vector<uint8_t> &zlib_stream, int *chosen, std::string &err)
+{
+    return from_filtered(info, nfilt, stored_adler, level, stream, zlib_stream, chosen, err, false);
+}
+
+bool PngDevice::load_filtered_lossy(const PngInfo &info, size_t nfilt, uint32_t stored_adler, void *stream, std::string &err)
+{
+    PngInfo in = info; std::vector<uint8_t> none;
+    return from_filtered(in, nfilt, stored_adler, 0, stream, none, nullptr, err, true);
+}
+
+// lossy: stop after the checks and hand the samples to the quantiser (expand, histogram)
+bool PngDevice::from_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, int level, void *stream_, std::vector<uint8_t> &zlib_stream, int *chosen, std::string &err,
+                              bool lossy)
 {
     cudaStream_t st = (cudaStream_t)stream_;
     corrupt = false;
@@ -150,8 +167,8 @@ bool PngDevice::compress_filtered(PngInfo &info, size_t nfilt, uint32_t stored_a
     if (rc) { err = std::string("png unfilter: ") + cudaGetErrorString((cudaError_t)rc); return false; }
     CUP(cudaMemsetAsync(d_flags, 0, 16, st));
     const bool eight = info.bit_depth == 8 && info.trns.empty();
-    const bool probe_ag = eight && (info.color_type == 2 || info.color_type == 4 || info.color_type == 6);
-    const bool probe_pal = png_palette_candidate(info);
+    const bool probe_ag = !lossy && eight && (info.color_type == 2 || info.color_type == 4 || info.color_type == 6);
+    const bool probe_pal = !lossy && png_palette_candidate(info);
     const size_t npix = (size_t)info.width * info.height;
     if (probe_ag && launch_png_probe(d_raw, npix, info.channels, d_flags, st)) { err = "png probe launch failed"; return false; }
     if (probe_pal && launch_png_colours(d_raw, npix, info.channels, d_set, d_flags, st)) { err = "png palette probe launch failed"; return false; }
@@ -164,6 +181,7 @@ bool PngDevice::compress_filtered(PngInfo &info, size_t nfilt, uint32_t stored_a
     CUP(stream_wait(st)); LT_MARK("host_wait");
     if (h_flags[5]) { err = "bad filter type"; corrupt = true; return false; }
     if (combine_adler(h_sums_in, nin) != stored_adler) { err = "Adler-32 mismatch"; corrupt = true; return false; }
+    if (lossy) return quantiser()->expand(d_raw, info, st, err) && quant->prepare(st, err);
     if (probe_pal && h_flags[2] <= 256) {
         // few colours: oxipng's palette reduction (first-appearance order, tRNS layout, bit packing) runs on the host over the
         // reconstructed samples, and the indexed image takes the raw-sample entry point
@@ -195,6 +213,35 @@ bool PngDevice::compress(PngInfo &info, const std::vector<uint8_t> &raw_in, int 
         CUP(stream_wait(st)); LT_MARK("host_wait");
     }
     return reduce_and_code(info, probe_ag, h_flags, level, stream_, zlib_stream, chosen, err);
+}
+
+bool PngDevice::code_quantized(PngInfo &info, int quality, int level, void *stream_, std::vector<uint8_t> &zlib_stream, std::string &err)
+{
+    cudaStream_t st = (cudaStream_t)stream_;
+    PngQuant *q = quantiser();
+    info.plte.clear(); info.trns.clear();
+    if (q->exact()) {
+        std::vector<uint8_t> raw;
+        if (!q->fetch_rgba(raw, st, err)) return false;
+        info.color_type = 6; info.bit_depth = 8; info.channels = 4; info.bits_per_pixel = 32; info.bpp = 4; info.row_bytes = (size_t)info.width * 4;
+        png_reduce_palette(info, raw);
+        return compress(info, raw, level, stream_, zlib_stream, nullptr, err);
+    }
+    std::vector<uint32_t> pal;
+    if (!q->quantize(quality, st, pal, err)) return false;
+    const int n = (int)pal.size(), depth = png_index_depth(n);
+    info.color_type = 3; info.bit_depth = depth; info.channels = 1; info.bits_per_pixel = depth; info.bpp = 1;
+    info.row_bytes = ((size_t)info.width * depth + 7) / 8;
+    info.plte.resize((size_t)n * 3);
+    int ntrans = 0;
+    for (int k = 0; k < n; k++) {
+        for (int c = 0; c < 3; c++) info.plte[3 * k + c] = (uint8_t)(pal[k] >> (8 * c));
+        if ((pal[k] >> 24) != 255) ntrans = k + 1;
+    }
+    for (int k = 0; k < ntrans; k++) info.trns.push_back((uint8_t)(pal[k] >> 24));
+    const size_t rb = info.row_bytes, nraw = rb * info.height;
+    if (!ensure_buffers(nraw, (size_t)info.height * (rb + 1) + 64, rb, st, err) || !q->pack(d_raw, depth, st, err)) return false;
+    return reduce_and_code(info, false, nullptr, level, stream_, zlib_stream, nullptr, err);
 }
 
 // d_raw holds the reconstructed samples; h_flags the probe results.  Lossless reductions (oxipng reduction::*: opaque alpha, grey

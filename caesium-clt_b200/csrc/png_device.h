@@ -9,6 +9,8 @@
 
 namespace b200 {
 
+struct PngQuant;
+
 // strategies tried per oxipng optimisation level 0..6 (PngStrategy values)
 std::vector<int> png_level_strategies(int level);
 
@@ -32,6 +34,16 @@ struct PngDevice {
     // checksum verification, reductions, K6 / K7 and the DEFLATE coding run on the device.
     uint8_t *input_buffer(size_t bytes, size_t &cap, std::string &err);
     bool compress_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, int level, void *stream, std::vector<uint8_t> &zlib_stream, int *chosen_strategy, std::string &err);
+    // The lossy leg's front end: the same upload, un-filter and checks as compress_filtered, then the samples are expanded to RGBA8
+    // and the quantiser's histogram is built (quantiser(); independent of the quality, so compress_to_size does it once).
+    bool load_filtered_lossy(const PngInfo &info, size_t nfilt, uint32_t stored_adler, void *stream, std::string &err);
+    // The lossy leg's back end over whatever quantiser() holds: palette + dithered indices at `quality`, packed into d_raw as an
+    // indexed image (info becomes colour type 3 with PLTE / tRNS), then the lossless leg's filter trials, LZ77 and DEFLATE.  An
+    // image with at most 256 distinct values is not quantised: it takes the lossless leg's exact palette reduction.
+    bool code_quantized(PngInfo &info, int quality, int level, void *stream, std::vector<uint8_t> &zlib_stream, std::string &err);
+    PngQuant *quantiser();
+    PngQuant *quant = nullptr;
+    bool from_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, int level, void *stream, std::vector<uint8_t> &zlib_stream, int *chosen_strategy, std::string &err, bool lossy);
     bool ensure_buffers(size_t nraw, size_t nmax, size_t rb, void *stream, std::string &err);
     bool reduce_and_code(PngInfo &info, bool probed, const uint32_t *h_flags, int level, void *stream, std::vector<uint8_t> &zlib_stream, int *chosen_strategy, std::string &err);
     // info/raw from png_decode; may rewrite info (colour-type reductions).  Produces the zlib stream of the re-filtered image.

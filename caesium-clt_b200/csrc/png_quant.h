@@ -1,0 +1,46 @@
+// png_quant.h -- the lossy PNG leg's palette quantiser on the device (png_quant.cu; rules in png_quant_core.h).
+#pragma once
+#include <cstdint>
+#include <cstddef>
+#include <string>
+#include <vector>
+#include "png_host.h"
+
+namespace b200 {
+
+// One image at a time: load (host RGBA8 or the un-filtered samples of a PNG already on the device), prepare (histogram, occupied
+// cells, distinct-value count: independent of the quality), then quantize at any number of qualities.  Buffers are high-water
+// allocations kept between calls.
+struct PngQuant {
+    uint32_t *d_rgba = nullptr, *d_cells = nullptr, *d_coords = nullptr, *d_set = nullptr, *d_flags = nullptr, *d_sync = nullptr;
+    unsigned long long *d_count = nullptr, *d_sums = nullptr, *d_box = nullptr, *d_acc = nullptr, *d_keys = nullptr;
+    unsigned long long *d_edge = nullptr;     // dithering: the last row of each 32-row group, four int16 errors per pixel
+    uint8_t *d_label = nullptr, *d_cand = nullptr, *d_idx = nullptr, *h_small = nullptr;
+    uint32_t *d_lut = nullptr;
+    uint8_t *d_planes = nullptr; size_t cap_planes = 0;
+    uint16_t *d_ncand = nullptr;
+    void *d_temp = nullptr;
+    size_t cap_rgba = 0, cap_idx = 0, cap_edge = 0, cap_sync = 0, cap_temp = 0;
+    int w = 0, h = 0, ncells = 0, distinct = 0, clear = 0;     // clear: some pixel is fully transparent (palette entry 0 reserved)
+    double last_cut_ms = 0;                   // host-driven median cut of the last quantize() (tracing)
+    ~PngQuant();
+
+    bool load_host(const uint8_t *rgba, int width, int height, void *stream, std::string &err);
+    // host planes [nc][h][w] (nc = 1 grey or 3 RGB) and an optional alpha plane, interleaved to RGBA8 on the device
+    bool load_planes(const uint8_t *planes, int nc, const uint8_t *alpha, int width, int height, void *stream, std::string &err);
+    // d_raw: height * row_bytes un-filtered samples of any PNG colour type / depth (16 bits: high byte; tRNS / palette expanded)
+    bool expand(const uint8_t *d_raw, const PngInfo &info, void *stream, std::string &err);
+    bool prepare(void *stream, std::string &err);
+    bool exact() const { return distinct <= 256; }
+    // palette (RGBA words, R in the low byte) and the indices (left in d_idx)
+    bool quantize(int quality, void *stream, std::vector<uint32_t> &palette, std::string &err);
+    bool fetch_indices(uint8_t *idx, void *stream, std::string &err);
+    bool fetch_rgba(std::vector<uint8_t> &rgba, void *stream, std::string &err);
+    // indices -> rows of `depth`-bit samples (MSB first, padded to bytes) at d_dst
+    bool pack(uint8_t *d_dst, int depth, void *stream, std::string &err);
+};
+
+// bits per index of a palette of n entries (PNG allows 1, 2, 4, 8)
+inline int png_index_depth(int n) { return n <= 2 ? 1 : n <= 4 ? 2 : n <= 16 ? 4 : 8; }
+
+} // namespace b200

@@ -64,9 +64,36 @@ def main():
             ref = b.getvalue()
             out["webp"].append({"input": name, "quality": q, "ours_bytes": len(ours), "libwebp_bytes": len(ref), "bytes_ratio_ours_over_libwebp": round(len(ours) / len(ref), 4),
                                 "ours_psnr": round(psnr(decode_rgb(ours), rgb), 3), "libwebp_psnr": round(psnr(decode_rgb(ref), rgb), 3)})
+    # lossy PNG (opt-in device quantiser, full-strength Floyd-Steinberg): colours and RGBA PSNR of the quantiser's palette applied to
+    # its indices, next to Pillow's median cut -- dithered with Floyd-Steinberg (its palette applied again with dithering on:
+    # Image.quantize ignores `dither` unless a palette is given) and, as Image.quantize(256, MEDIANCUT) returns it, undithered.
+    # Pillow here has no libimagequant, so imagequant (the reference's quantiser) cannot be compared.  blur_mae: mean absolute error
+    # after a 5x5 box blur, the low-frequency error (banding) that dithering removes and PSNR does not see.
+    from oracle.png_quant import png_quantize
+
+    def blur_mae(a, b, k=5):
+        d = a.astype(np.float64) - b.astype(np.float64)
+        c = np.cumsum(np.cumsum(np.pad(d, ((1, 0), (1, 0), (0, 0))), 0), 1)
+        return float(np.abs((c[k:, k:] - c[:-k, k:] - c[k:, :-k] + c[:-k, :-k]) / (k * k)).mean())
+
+    out["png_lossy"] = []
+    for i in range(3):
+        rgb = synth_rgb(1920, 1280, i)
+        rgba = np.concatenate([rgb, np.full(rgb.shape[:2] + (1,), 255, np.uint8)], axis=2)
+        im = Image.fromarray(rgb)
+        mc = im.quantize(256, method=Image.Quantize.MEDIANCUT)
+        pil = {"dithered": np.asarray(im.quantize(palette=mc, dither=Image.Dither.FLOYDSTEINBERG).convert("RGBA")), "undithered": np.asarray(mc.convert("RGBA"))}
+        for q in (40, 80, 100):
+            pal, idx = png_quantize(rgba, q)
+            row = {"input": f"synthetic 1920x1280 seed {i}", "quality": q, "ours_colours": len(pal), "ours_psnr_rgba": round(psnr(pal[idx], rgba), 3),
+                   "ours_blur_mae": round(blur_mae(pal[idx], rgba), 3)}
+            for k, v in pil.items():
+                row[f"pillow_mediancut_256_{k}_psnr_rgba"] = round(psnr(v, rgba), 3)
+                row[f"pillow_mediancut_256_{k}_blur_mae"] = round(blur_mae(v, rgba), 3)
+            out["png_lossy"].append(row)
     with open(os.path.join(ROOT, "profiles", "quality.json"), "w") as f:
         json.dump(out, f, indent=1)
-    for r in out["jpeg"] + out["webp"]:
+    for r in out["jpeg"] + out["webp"] + out["png_lossy"]:
         print(r)
 
 
