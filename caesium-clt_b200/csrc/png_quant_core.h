@@ -7,12 +7,16 @@
  *                 one colour (0, 0, 0, 0); distances are squared integer differences over the four channels; ties go to the
  *                 lower palette index
  *   histogram     2^20 cells of 5 bits per premultiplied channel; a cell holds its pixel count and the exact 64-bit sums of its
- *                 pixels, and stands for its rounded mean (the cell's representative) in median cut and refinement
+ *                 pixels, and stands for its rounded mean (the cell's representative) in median cut and refinement; every
+ *                 rounded mean here rounds halves up
  *   median cut    boxes are ranges of cell coordinates; the splittable box with the largest weighted SSE of its representatives
- *                 is split on its highest-variance axis (among axes with two or more occupied coordinates) at the weighted
- *                 median; stop at PQ_MAX_COLOURS boxes (one fewer with the reserved entry), when the total SSE is at most
- *                 pq_target_mse[quality] * (pixels that are not fully transparent), or when
- *                 no box can be split; an entry is the mean of the box's pixels
+ *                 (ties to the lower box) is split on its highest-variance axis (among axes with two or more occupied
+ *                 coordinates; ties to the lower axis, R G B A) at the weighted median (the first coordinate t at which twice
+ *                 the pixels up to t reach the box's, at most the last occupied coordinate minus one); an axis's SSE is
+ *                 s2 - floor(s1^2 / n) over the box's pixel count n and the weighted sums s1, s2 of its representatives, and the
+ *                 axis comparison uses that integer; stop at PQ_MAX_COLOURS boxes (one fewer with the reserved entry), when the
+ *                 total SSE is at most pq_target_mse[quality] * (pixels that are not fully transparent), or when no box can be
+ *                 split; an entry is the rounded mean of the box's pixels, un-premultiplied with rounding
  *   refinement    PQ_REFINE_PASSES weighted k-means passes over the occupied cells; entries left without pixels are dropped
  *                 (the others keep their order)
  *   order         the reserved transparent entry, then entries that are not opaque, then the opaque ones, each group in
@@ -21,7 +25,8 @@
  *                 entry 0 = (0, 0, 0, 0) for them, they take it without a search and neither take nor pass dithering error, and no
  *                 other pixel may take it -- so a transparent area stays transparent and an opaque source keeps opaque entries
  *   dithering     Floyd-Steinberg at full strength (7, 3, 5, 1 sixteenths) in raster order on the premultiplied values; the
- *                 incoming error is rounded to whole units and the target clamped to 0..255 (which bounds every error to +-255)
+ *                 incoming error is rounded to whole units, halves away from zero, and the target clamped to 0..255 (which
+ *                 bounds every error to +-255)
  *   exact path    a source with at most 256 distinct RGBA values is not quantised: its palette is those values in pq_exact_key
  *                 order (the PNG writer then takes the lossless leg's exact palette reduction) */
 #ifndef PNG_QUANT_CORE_H
