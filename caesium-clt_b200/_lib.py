@@ -67,7 +67,7 @@ _SYMBOLS = [
     "b200_png_decode", "b200_png_decode_reduced", "b200_png_filter", "b200_png_lz77", "b200_png_deflate_tokens", "b200_png_level_strategies",
     "b200_webp_encode_rgb", "b200_webp_write_levels", "b200_webp_qindex",
     "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_jpeg_pipe_destroy", "b200_device_jobs", "b200_device_numa_node", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba", "b200_webp_alpha_filter", "b200_webp_d2h_bytes",
-    "b200_set_png_lossy", "b200_png_quantize",
+    "b200_set_png_lossy", "b200_png_quantize", "b200_set_jpeg_trellis",
 ]
 
 
@@ -231,6 +231,12 @@ def set_entropy_mode(mode):
 def set_png_lossy(on):
     """b200_set_png_lossy: lossy PNG (png_optimize = 0) on the device quantiser (True) or refused with code 3 (False, the default)."""
     return lib().b200_set_png_lossy(int(bool(on)))
+
+
+def set_jpeg_trellis(on):
+    """b200_set_jpeg_trellis: trellis (rate-distortion) quantisation of lossy JPEG output (1) or plain quantisation (0, the default).
+    Any other value is refused with B200_ERR_INVALID_ARGUMENT."""
+    return lib().b200_set_jpeg_trellis(int(on))
 
 
 def png_quantize(rgba, quality):

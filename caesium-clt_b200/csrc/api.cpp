@@ -3,6 +3,7 @@
 // (call sites caesium-clt's src/compressor.rs:287-306).  No CPU codec fallback exists anywhere below.
 #include "../../include/b200_caesium.h"
 #include "../../include/b200_caesium_png_lossy.h"
+#include "../../include/b200_caesium_jpeg_trellis.h"
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -954,6 +955,7 @@ const char *b200_version(void) { return "b200-caesium 0.1.0 (sm_90a)"; }
 void b200_free(void *p) { free(p); }
 int b200_set_entropy_mode(int mode) { if (mode < 0 || mode > 3) return B200_ERR_INVALID_ARGUMENT; g_entropy_mode.store(mode); return B200_OK; }
 int b200_set_png_lossy(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_png_lossy.store(on); return B200_OK; }
+int b200_set_jpeg_trellis(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; set_jpeg_trellis(on == 1); return B200_OK; }
 
 uint32_t b200_sniff_format(const uint8_t *d, size_t n)
 {   // the magic numbers `infer` checks (scan_files.rs:30-40, compressor.rs:259-264)

@@ -91,7 +91,7 @@ void append_image_work(const JpegGeom &gin, const JpegGeom &gout, const ImagePla
 size_t flatten_work(const WorkLists &wl, CompWork *h)
 {
     size_t n = 0;
-    for (const auto *v : {&wl.fused, &wl.idct, &wl.c420, &wl.up, &wl.down, &wl.fdct}) { if (!v->empty()) memcpy(h + n, v->data(), v->size() * sizeof(CompWork)); n += v->size(); }
+    for (const auto *v : {&wl.fused, &wl.idct, &wl.c420, &wl.up, &wl.down, &wl.fdct, &wl.trel}) { if (!v->empty()) memcpy(h + n, v->data(), v->size() * sizeof(CompWork)); n += v->size(); }
     return n;
 }
 
@@ -100,14 +100,37 @@ int launch_work(const WorkLists &wl, const CompWork *d, void *stream)
     int rc = 0;
     const CompWork *p_fused = d, *p_idct = p_fused + wl.fused.size(), *p_c420 = p_idct + wl.idct.size();
     const CompWork *p_up = p_c420 + wl.c420.size(), *p_down = p_up + wl.up.size(), *p_fdct = p_down + wl.down.size();
-    if (!wl.fused.empty()) { rc = launch_fused_same(p_fused, (int)wl.fused.size(), wl.max_fused, stream); LT_MARK("k_fused_same"); if (rc) return rc; }
+    const CompWork *p_trel = p_fdct + wl.fdct.size();
+    const bool raw = !wl.trel.empty();
+    if (!wl.fused.empty()) { rc = launch_fused_same(p_fused, (int)wl.fused.size(), wl.max_fused, stream, raw); LT_MARK("k_fused_same"); if (rc) return rc; }
     if (!wl.idct.empty()) { rc = launch_idct_plane(p_idct, (int)wl.idct.size(), wl.max_idct, stream); LT_MARK("k_idct_plane"); if (rc) return rc; }
-    if (!wl.c420.empty()) { rc = launch_chroma420_refdct(p_c420, (int)wl.c420.size(), wl.max_c420, stream); LT_MARK("k_chroma420_refdct"); if (rc) return rc; }
+    if (!wl.c420.empty()) { rc = launch_chroma420_refdct(p_c420, (int)wl.c420.size(), wl.max_c420, stream, raw); LT_MARK("k_chroma420_refdct"); if (rc) return rc; }
     if (!wl.up.empty()) { rc = launch_upsample(p_up, (int)wl.up.size(), wl.max_up_w, wl.max_up_h, stream); if (rc) return rc; }
     if (!wl.down.empty()) { rc = launch_downsample(p_down, (int)wl.down.size(), wl.max_dn_w, wl.max_dn_h, stream); if (rc) return rc; }
-    if (!wl.fdct.empty()) { rc = launch_fdct_plane(p_fdct, (int)wl.fdct.size(), wl.max_fdct, stream); if (rc) return rc; }
+    if (!wl.fdct.empty()) { rc = launch_fdct_plane(p_fdct, (int)wl.fdct.size(), wl.max_fdct, stream, raw); if (rc) return rc; }
+    if (raw) { rc = launch_jpeg_trellis(p_trel, (int)wl.trel.size(), wl.max_trel, wl.trel_q, wl.trel_t, stream); LT_MARK("k_jpeg_trellis"); if (rc) return rc; }
     return 0;
 }
+
+// every output-side item of wl (the ones an FDCT kernel writes) into its trellis list
+static void add_trellis_work(WorkLists &wl)
+{
+    for (const auto *v : {&wl.fused, &wl.c420, &wl.fdct})
+        for (const CompWork &w : *v) { wl.trel.push_back(w); wl.max_trel = std::max(wl.max_trel, w.rbw_out * w.rbh_out); }
+}
+
+namespace {
+std::atomic<int> g_jpeg_trellis{-1};     // -1 unset (env B200_JPEG_TRELLIS); 1 = trellis quantisation, 0 = plain
+}
+bool jpeg_trellis()
+{
+    if (g_jpeg_trellis.load() < 0) {
+        const char *e = getenv("B200_JPEG_TRELLIS");
+        g_jpeg_trellis.store(e && !strcmp(e, "1") ? 1 : 0);
+    }
+    return g_jpeg_trellis.load() == 1;
+}
+void set_jpeg_trellis(bool on) { g_jpeg_trellis.store(on ? 1 : 0); }
 
 // ================================================================================================================
 // runtime: devices and slots
@@ -262,9 +285,22 @@ bool Slot::ensure(size_t in_bytes, size_t out_bytes, size_t scratch_bytes, size_
 
 // Parameter block of a transform over K images, each part 256-byte aligned:
 //   QuantDev q[4] (per output table) | uint16 dq[K][4][64] (per image and input component, zigzag) | CompWork work[]
-// The resize leg appends its axis tables after the work descriptors.
+// The resize leg appends its axis tables after the work descriptors.  With trellis quantisation on, JtTable[4] (beside q[4],
+// per output table) comes last.
 static constexpr size_t par_dq_off = align_up(sizeof(QuantDev) * 4, 256);
 static size_t par_work_off(int K) { return par_dq_off + align_up(sizeof(uint16_t) * 256 * K, 256); }
+static constexpr size_t par_trellis_bytes = 256 + sizeof(JtTable) * 4;      // alignment + the tables
+// the trellis tables of gout at the 256-aligned end `end` of the block; returns the new end
+static size_t put_trellis(Slot *s, const JpegGeom &gout, size_t end, WorkLists &wl)
+{
+    const size_t off = align_up(end, 256);
+    JtTable *t = reinterpret_cast<JtTable *>(s->h_par + off);
+    for (int i = 0; i < 4; i++) if (gout.qt_present[i]) jt_make_table(gout.qt[i], i != 0, &t[i]);
+    add_trellis_work(wl);
+    wl.trel_q = reinterpret_cast<const QuantDev *>(s->d_par);
+    wl.trel_t = reinterpret_cast<const JtTable *>(s->d_par + off);
+    return off + sizeof(JtTable) * 4;
+}
 
 static void put_quant(Slot *s, const JpegGeom &gout)
 {
@@ -282,7 +318,7 @@ static const uint16_t *put_dequant(Slot *s, int k, const JpegGeom &gin)
 
 // Quantiser constants, per-image dequantisation tables and the work descriptors of the K images of L into the slot's pinned
 // parameter block.  wl receives the work lists, par_bytes the size of the block, work_off the offset of the descriptors.
-static bool fill_transform_params(Slot *s, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, WorkLists &wl,
+static bool fill_transform_params(Slot *s, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, bool trellis, WorkLists &wl,
                                   size_t &par_bytes, size_t &work_off, std::string &err)
 {
     put_quant(s, gout);
@@ -295,7 +331,10 @@ static bool fill_transform_params(Slot *s, const JpegGeom *const *gins, const Jp
                           put_dequant(s, k, gin), dev_quant(s), wl);
     }
     work_off = par_work_off(L.K);
-    par_bytes = work_off + flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + work_off)) * sizeof(CompWork);
+    if (!trellis) { par_bytes = work_off + flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + work_off)) * sizeof(CompWork); return true; }
+    const size_t end = work_off + (wl.total() + wl.fused.size() + wl.c420.size() + wl.fdct.size()) * sizeof(CompWork);
+    par_bytes = put_trellis(s, gout, end, wl);
+    flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + work_off));
     return true;
 }
 
@@ -304,13 +343,13 @@ bool slot_transform(Slot *s, const JpegGeom &gin, const JpegGeom &gout, std::str
     ImagePlan plan;
     if (!plan_image(gin, gout, plan, err)) return false;
     cudaStream_t st = (cudaStream_t)s->stream;
-    if (!s->ensure(plan.in_bytes, plan.out_bytes, plan.scratch_bytes(), par_work_off(1) + sizeof(CompWork) * 4 * 6, err)) return false;
+    if (!s->ensure(plan.in_bytes, plan.out_bytes, plan.scratch_bytes(), par_work_off(1) + sizeof(CompWork) * 4 * 7 + par_trellis_bytes, err)) return false;
     // a megabatch of one over the slot's own buffers (no strides needed); the work lists are local because s->group_wl and
     // the group_* sizes belong to the slot's last megabatch and feed the signature of its captured launch sequence
     GroupLayout L; L.K = 1;
     const JpegGeom *gins = &gin;
     WorkLists wl; size_t pbytes = 0, work_off = 0;
-    if (!fill_transform_params(s, &gins, gout, L, wl, pbytes, work_off, err)) return false;
+    if (!fill_transform_params(s, &gins, gout, L, jpeg_trellis(), wl, pbytes, work_off, err)) return false;
     CU(cudaMemcpyAsync(s->d_par, s->h_par, pbytes, cudaMemcpyHostToDevice, st));
     if (upload) CU(cudaMemcpyAsync(s->d_in, s->h_in, plan.in_bytes, cudaMemcpyHostToDevice, st));
     int rc = launch_work(wl, reinterpret_cast<const CompWork *>(s->d_par + work_off), st);
@@ -330,14 +369,14 @@ bool slot_group_layout(Slot *s, const JpegGeom &gin, const JpegGeom &gout, int K
     if (!plan_image(gin, gout, plan, err)) return false;
     L.K = K;
     L.in_stride = align_up(plan.in_bytes, 256); L.out_stride = align_up(plan.out_bytes, 256); L.scratch_stride = align_up(std::max<size_t>(plan.scratch_bytes(), 256), 256);
-    const size_t par = par_work_off(K) + sizeof(CompWork) * (size_t)K * 4 * 6 + 256;
+    const size_t par = par_work_off(K) + sizeof(CompWork) * (size_t)K * 4 * 7 + 256 + par_trellis_bytes;
     return s->ensure_device(L.in_stride * K, L.out_stride * K, L.scratch_stride * K, par, err);
 }
 
 // host half: the parameter block into the slot's pinned memory, the work lists into s->group_wl
-bool slot_transform_group_prepare(Slot *s, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, std::string &err)
+bool slot_transform_group_prepare(Slot *s, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, bool trellis, std::string &err)
 {
-    return fill_transform_params(s, gins, gout, L, s->group_wl, s->group_par_bytes, s->group_work_off, err);
+    return fill_transform_params(s, gins, gout, L, trellis, s->group_wl, s->group_par_bytes, s->group_work_off, err);
 }
 // stream half: parameter block up, the transform kernels
 bool slot_transform_group_enqueue(Slot *s, std::string &err)
@@ -348,9 +387,9 @@ bool slot_transform_group_enqueue(Slot *s, std::string &err)
     if (rc) { err = std::string("kernel launch: ") + cudaGetErrorString((cudaError_t)rc); return false; }
     return true;
 }
-bool slot_transform_group(Slot *s, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, std::string &err)
+bool slot_transform_group(Slot *s, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, bool trellis, std::string &err)
 {
-    return slot_transform_group_prepare(s, gins, gout, L, err) && slot_transform_group_enqueue(s, err);
+    return slot_transform_group_prepare(s, gins, gout, L, trellis, err) && slot_transform_group_enqueue(s, err);
 }
 
 // (Measured and dropped: issuing the decode passes on a highest-priority stream so that their small latency-bound grids cut in
@@ -409,7 +448,7 @@ bool slot_run_group(Slot *s, std::vector<GpuDecoder::Item> &items, const JpegGeo
     const auto t0 = std::chrono::steady_clock::now();
     // ---- host half of all three stages (pinned staging, descriptors, plans); nothing touches the stream yet
     if (!s->decoder()->prepare(items, st, err)) return false;
-    if (!lossless && !slot_transform_group_prepare(s, gins, gout, L, err)) return false;
+    if (!lossless && !slot_transform_group_prepare(s, gins, gout, L, jpeg_trellis(), err)) return false;
     std::vector<int16_t *> bases((size_t)L.K);
     for (int k = 0; k < L.K; k++) bases[k] = L.coefs(*s, k, lossless);
     // a re-encode at lower quality (or a transcode with optimal tables) does not grow: the inputs' entropy-coded size sizes the output buffers
@@ -422,6 +461,7 @@ bool slot_run_group(Slot *s, std::vector<GpuDecoder::Item> &items, const JpegGeo
     if (graphs_enabled() && !s->graphs_broken) {
         unsigned long long sig = s->dec->signature() * 1099511628211ull ^ s->enc->signature();
         sig = (sig ^ (unsigned long long)(uintptr_t)s->d_par ^ ((unsigned long long)s->group_par_bytes << 20) ^ (lossless ? 0x9e3779b97f4a7c15ull : 0)) * 1099511628211ull + (unsigned long long)L.K;
+        if (!lossless && !s->group_wl.trel.empty()) sig = (sig ^ 0xc2b2ae3d27d4eb4full) * 1099511628211ull;     // the trellis pass is part of the sequence
         if (!s->graph_front || s->graph_sig != sig) {
             drop_graphs(s);
             std::string gerr;
@@ -549,9 +589,11 @@ bool slot_transform_resized(Slot *s, const JpegGeom &gin, const JpegGeom &gout, 
     const size_t tmp_off = off; off += align_up((size_t)NH * W * sizeof(float), 256);
     // parameter block: tables | work | axis tables
     const size_t work_off = par_work_off(1);
-    const size_t lv = align_up(work_off + sizeof(CompWork) * nc * 4, 256), cv = lv + align_up(sizeof(int) * NH, 256), wv = cv + align_up(sizeof(int) * NH, 256);
+    const size_t lv = align_up(work_off + sizeof(CompWork) * nc * 5, 256), cv = lv + align_up(sizeof(int) * NH, 256), wv = cv + align_up(sizeof(int) * NH, 256);
     const size_t lh = wv + align_up(sizeof(float) * av.weights.size(), 256), chh = lh + align_up(sizeof(int) * NW, 256), wh = chh + align_up(sizeof(int) * NW, 256);
-    const size_t pbytes = wh + align_up(sizeof(float) * ah.weights.size(), 256);
+    const size_t axes_end = wh + align_up(sizeof(float) * ah.weights.size(), 256);
+    const bool trellis = !rgb_out && jpeg_trellis();
+    const size_t pbytes = axes_end + (trellis ? par_trellis_bytes : 0);
     const size_t in_bytes = (size_t)gin.total_coefs * 2, out_bytes = (size_t)gout.total_coefs * 2;
     if (!s->ensure(in_bytes, out_bytes, off, pbytes, err)) return false;
     put_quant(s, gout);
@@ -579,11 +621,13 @@ bool slot_transform_resized(Slot *s, const JpegGeom &gin, const JpegGeom &gout, 
         wl.down.push_back(e); wl.max_dn_w = std::max(wl.max_dn_w, e.rbw_out * 8); wl.max_dn_h = std::max(wl.max_dn_h, e.rbh_out * 8);
         wl.fdct.push_back(e); wl.max_fdct = std::max(wl.max_fdct, work_tiles(e.rbw_out, e.rbh_out));
     }
+    if (trellis) put_trellis(s, gout, axes_end, wl);
     flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + work_off));
     CU(cudaMemcpyAsync(s->d_par, s->h_par, pbytes, cudaMemcpyHostToDevice, st));
     if (upload && !host_rgb) CU(cudaMemcpyAsync(s->d_in, s->h_in, in_bytes, cudaMemcpyHostToDevice, st));
     const CompWork *dw = reinterpret_cast<const CompWork *>(s->d_par + work_off);
     const CompWork *p_idct = dw, *p_up = p_idct + wl.idct.size(), *p_down = p_up + wl.up.size(), *p_fdct = p_down + wl.down.size();
+    const CompWork *p_trel = p_fdct + wl.fdct.size();
     auto chk = [&](int rc, const char *what) { if (rc) { err = std::string(what) + ": " + cudaGetErrorString((cudaError_t)rc); return false; } return true; };
     uint8_t *full[3] = {s->d_scratch + full_off[0], nc == 3 ? s->d_scratch + full_off[1] : nullptr, nc == 3 ? s->d_scratch + full_off[2] : nullptr};
     uint8_t *rz[3] = {s->d_scratch + rz_off[0], nc == 3 ? s->d_scratch + rz_off[1] : nullptr, nc == 3 ? s->d_scratch + rz_off[2] : nullptr};
@@ -608,7 +652,12 @@ bool slot_transform_resized(Slot *s, const JpegGeom &gin, const JpegGeom &gout, 
     if (rgb_out) { rgb_out[0] = rz[0]; rgb_out[1] = nc == 3 ? rz[1] : rz[0]; rgb_out[2] = nc == 3 ? rz[2] : rz[0]; return true; }
     if (nc == 3 && !chk(launch_rgb_to_ycc(rz[0], rz[1], rz[2], (size_t)NW * NH, st), "rgb_to_ycc")) return false;
     if (!chk(launch_downsample(p_down, nc, wl.max_dn_w, wl.max_dn_h, st), "downsample")) return false;
-    if (!chk(launch_fdct_plane(p_fdct, nc, wl.max_fdct, st), "fdct")) return false;
+    if (!chk(launch_fdct_plane(p_fdct, nc, wl.max_fdct, st, trellis), "fdct")) return false;
+    if (trellis) {
+        const int rc = launch_jpeg_trellis(p_trel, nc, wl.max_trel, wl.trel_q, wl.trel_t, st);
+        LT_MARK("k_jpeg_trellis");
+        if (!chk(rc, "trellis")) return false;
+    }
     if (!download) return true;
     CU(cudaMemcpyAsync(s->h_out, s->d_out, out_bytes, cudaMemcpyDeviceToHost, st));
     CU(stream_wait(st));

@@ -24,21 +24,29 @@ struct ImagePlan {
 };
 bool plan_image(const JpegGeom &gin, const JpegGeom &gout, ImagePlan &plan, std::string &err);
 
-// Work lists for one launch group (any number of images).
+// Work lists for one launch group (any number of images).  A non-empty trel list (every output-side item, see add_trellis_work)
+// makes the FDCT kernels store raw DCT output and k_jpeg_trellis quantise it, with the JtTable array trel_t beside QuantDev trel_q.
 struct WorkLists {
-    std::vector<CompWork> fused, idct, c420, up, down, fdct;
-    int max_fused = 0, max_idct = 0, max_c420 = 0, max_fdct = 0, max_up_w = 0, max_up_h = 0, max_dn_w = 0, max_dn_h = 0;
-    size_t total() const { return fused.size() + idct.size() + c420.size() + up.size() + down.size() + fdct.size(); }
-    void clear() { fused.clear(); idct.clear(); c420.clear(); up.clear(); down.clear(); fdct.clear(); max_fused = max_idct = max_c420 = max_fdct = max_up_w = max_up_h = max_dn_w = max_dn_h = 0; }
+    std::vector<CompWork> fused, idct, c420, up, down, fdct, trel;
+    int max_fused = 0, max_idct = 0, max_c420 = 0, max_fdct = 0, max_up_w = 0, max_up_h = 0, max_dn_w = 0, max_dn_h = 0, max_trel = 0;
+    const QuantDev *trel_q = nullptr; const JtTable *trel_t = nullptr;
+    size_t total() const { return fused.size() + idct.size() + c420.size() + up.size() + down.size() + fdct.size() + trel.size(); }
+    void clear() { fused.clear(); idct.clear(); c420.clear(); up.clear(); down.clear(); fdct.clear(); trel.clear(); max_fused = max_idct = max_c420 = max_fdct = max_up_w = max_up_h = max_dn_w = max_dn_h = max_trel = 0; trel_q = nullptr; trel_t = nullptr; }
 };
 // Append one image's work.  d_dq: device uint16[4][64] (per input component, zigzag); d_q: device QuantDev[4] (per output slot).
 void append_image_work(const JpegGeom &gin, const JpegGeom &gout, const ImagePlan &plan,
                        const int16_t *d_in, int16_t *d_out, uint8_t *d_scratch,
                        const uint16_t *d_dq, const QuantDev *d_q, WorkLists &wl);
-// Copy lists into `h_work` (contiguous, order fused|idct|c420|up|down|fdct); returns count.
+// Copy lists into `h_work` (contiguous, order fused|idct|c420|up|down|fdct|trel); returns count.
 size_t flatten_work(const WorkLists &wl, CompWork *h_work);
 // Launch every non-empty list; d_work is the device copy of the flattened array.
 int launch_work(const WorkLists &wl, const CompWork *d_work, void *stream);
+
+// Trellis quantisation of lossy JPEG output (jpeg_trellis_core.h): the process-wide switch b200_set_jpeg_trellis sets; while never
+// set, B200_JPEG_TRELLIS=1 turns it on (read once).  Off by default.  The transforms read it when they build their work lists; the
+// resident pipe reads it once, at create.
+bool jpeg_trellis();
+void set_jpeg_trellis(bool on);
 
 // ---- device runtime ------------------------------------------------------------------------------------------
 struct Slot {
@@ -107,7 +115,7 @@ inline bool same_shape(const JpegGeom &a, const JpegGeom &b)
 // items[k].result says which images the device decoder settled
 bool slot_run_group(Slot *s, std::vector<GpuDecoder::Item> &items, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, bool progressive,
                     bool lossless, std::string &err);
-bool slot_transform_group(Slot *s, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, std::string &err);
+bool slot_transform_group(Slot *s, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, bool trellis, std::string &err);
 // H2D of s->h_out into s->d_out (entry point that encodes caller-supplied coefficients on the device)
 bool slot_upload_out_coefs(Slot *s, size_t bytes, std::string &err);
 // Entropy-code the output coefficients sitting in s->d_out on the device; result in s->enc->results

@@ -12,6 +12,7 @@
 #include <cuda_runtime.h>
 #include <cstdint>
 #include "jpeg_kernels.h"
+#include "jpeg_trellis_core.h"
 
 namespace b200 {
 
@@ -222,11 +223,24 @@ __device__ __forceinline__ void quant_zigzag(const int (&v)[64], const Tables &t
 {
     if (t.any_shift) quant_zigzag_t<true>(v, t, r); else quant_zigzag_t<false>(v, t, r);     // block-uniform branch
 }
+// RAW: the unquantised DCT output (|v| <= 2^13 for 8-bit samples) as zigzag int16, for k_jpeg_trellis to quantise in place
+template <bool RAW>
+__device__ __forceinline__ void store_zigzag(const int (&v)[64], const Tables &t, int4 (&r)[8])
+{
+    if (!RAW) { quant_zigzag(v, t, r); return; }
+    uint32_t ow[32];
+#define X(k, n) if ((k) & 1) ow[(k) >> 1] |= (uint32_t)v[n] << 16; else ow[(k) >> 1] = (uint32_t)v[n] & 0xFFFFu;
+    ZZ_LIST(X)
+#undef X
+#pragma unroll
+    for (int j = 0; j < 8; j++) r[j] = make_int4((int)ow[4 * j], (int)ow[4 * j + 1], (int)ow[4 * j + 2], (int)ow[4 * j + 3]);
+}
 
 // ------------------------------------------------------------------------------------------------------------
 // K1->K5 fused: components whose sample grid is unchanged between decode and encode (luma always; chroma too when
 // neither side subsamples).  coefficients in -> coefficients out, 6 algorithmic bytes... per sample 4 B.
 // ------------------------------------------------------------------------------------------------------------
+template <bool RAW>
 __global__ void __launch_bounds__(THREADS, 2) k_fused_same(const CompWork *__restrict__ work)
 {
     __shared__ Tables tab;
@@ -257,7 +271,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_fused_same(const CompWork *__res
             for (int x = 0; x < 8; x++) if (y >= vr) v[8 * y + x] = v[8 * (y - 1) + x];
     }
     fdct_block(v);
-    quant_zigzag(v, tab, r);
+    store_zigzag<RAW>(v, tab, r);
     warp_store_blocks(reinterpret_cast<int4 *>(w.cout) + ((size_t)t.by * w.bw_out + t.bx0) * 8, t.nvalid, st, lane, r);
 }
 
@@ -325,6 +339,7 @@ __device__ __noinline__ void chroma420_edge_block(const CompWork &w, int bx, int
     }
 }
 
+template <bool RAW>
 __global__ void __launch_bounds__(THREADS, 2) k_chroma420_refdct(const CompWork *__restrict__ work)
 {
     __shared__ Tables tab;
@@ -395,7 +410,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_chroma420_refdct(const CompWork 
     __syncwarp();
     fdct_block(v);
     int4 r[8];
-    quant_zigzag(v, tab, r);
+    store_zigzag<RAW>(v, tab, r);
     warp_store_blocks(reinterpret_cast<int4 *>(w.cout) + ((size_t)t.by * w.bw_out + t.bx0) * 8, t.nvalid, stage + warp * STAGE_INT4_PER_WARP, lane, r);
 }
 
@@ -443,6 +458,7 @@ __global__ void k_downsample(const CompWork *__restrict__ work)
     w.dplane[(size_t)y * pw + x] = (uint8_t)v;
 }
 
+template <bool RAW>
 __global__ void __launch_bounds__(THREADS) k_fdct_plane(const CompWork *__restrict__ work)
 {   // K5: padded component plane -> quantised zigzag coefficients
     __shared__ Tables tab;
@@ -464,8 +480,40 @@ __global__ void __launch_bounds__(THREADS) k_fdct_plane(const CompWork *__restri
     }
     fdct_block(v);
     int4 r[8];
-    quant_zigzag(v, tab, r);
+    store_zigzag<RAW>(v, tab, r);
     warp_store_blocks(reinterpret_cast<int4 *>(w.cout) + ((size_t)t.by * w.bw_out + t.bx0) * 8, t.nvalid, stage + (threadIdx.x >> 5) * STAGE_INT4_PER_WARP, lane, r);
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Trellis quantisation (jpeg_trellis_core.h) of the raw DCT output the RAW transform kernels left in cout, in place, real blocks
+// only.  One thread per block.  The programme's per-position arrays live in shared memory as [position][thread], so the 64
+// threads of a CTA touch one 8-byte word (G) or one byte (pos, pred, size) each at whatever position they have reached: G stays
+// conflict-free (bank = thread), and registers stay free of dynamically indexed arrays that would spill to local memory.
+// 64 x (8 + 3) B x 64 threads = 44 KB + the table: under the 48 KB static limit.  The block is read from and written back to
+// global memory in place (each thread owns its 128 B; the reads of one position across a warp hit L1).
+// ------------------------------------------------------------------------------------------------------------
+constexpr int TRELLIS_THREADS = 64;
+__global__ void __launch_bounds__(TRELLIS_THREADS) k_jpeg_trellis(const CompWork *__restrict__ work, const QuantDev *qbase, const JtTable *__restrict__ tables)
+{
+    __shared__ long long G[64 * TRELLIS_THREADS];
+    __shared__ uint8_t pos[64 * TRELLIS_THREADS], pred[64 * TRELLIS_THREADS], size[64 * TRELLIS_THREADS];
+    __shared__ JtTable tab;
+    const CompWork w = work[blockIdx.y];
+    const int nblk = w.rbw_out * w.rbh_out;
+    if ((int)blockIdx.x * TRELLIS_THREADS >= nblk) return;
+    {
+        const JtTable *src = tables + (w.q - qbase);
+        const uint32_t *s4 = reinterpret_cast<const uint32_t *>(src);
+        uint32_t *d4 = reinterpret_cast<uint32_t *>(&tab);
+        for (int i = threadIdx.x; i < (int)(sizeof(JtTable) / 4); i += TRELLIS_THREADS) d4[i] = s4[i];
+    }
+    __syncthreads();
+    const int i = blockIdx.x * TRELLIS_THREADS + threadIdx.x;
+    if (i >= nblk) return;
+    const int by = i / w.rbw_out, bx = i - by * w.rbw_out;
+    int16_t *blk = w.cout + ((size_t)by * w.bw_out + bx) * 64;
+    const int t = threadIdx.x;
+    jt_trellis_block(blk, &tab, blk, G + t, pos + t, pred + t, size + t, TRELLIS_THREADS);
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -473,11 +521,12 @@ __global__ void __launch_bounds__(THREADS) k_fdct_plane(const CompWork *__restri
 // ------------------------------------------------------------------------------------------------------------
 static inline int cdiv(int a, int b) { return (a + b - 1) / b; }
 
-int launch_fused_same(const CompWork *work, int n, int max_tiles, void *stream)
+int launch_fused_same(const CompWork *work, int n, int max_tiles, void *stream, bool raw)
 {
     if (n <= 0 || max_tiles <= 0) return 0;
     dim3 grid(cdiv(max_tiles, WARPS_PER_CTA), n);
-    k_fused_same<<<grid, THREADS, 0, (cudaStream_t)stream>>>(work);
+    if (raw) k_fused_same<true><<<grid, THREADS, 0, (cudaStream_t)stream>>>(work);
+    else k_fused_same<false><<<grid, THREADS, 0, (cudaStream_t)stream>>>(work);
     return (int)cudaGetLastError();
 }
 int launch_idct_plane(const CompWork *work, int n, int max_tiles, void *stream)
@@ -487,11 +536,12 @@ int launch_idct_plane(const CompWork *work, int n, int max_tiles, void *stream)
     k_idct_plane<<<grid, THREADS, 0, (cudaStream_t)stream>>>(work);
     return (int)cudaGetLastError();
 }
-int launch_chroma420_refdct(const CompWork *work, int n, int max_tiles, void *stream)
+int launch_chroma420_refdct(const CompWork *work, int n, int max_tiles, void *stream, bool raw)
 {
     if (n <= 0 || max_tiles <= 0) return 0;
     dim3 grid(cdiv(max_tiles, WARPS_PER_CTA), n);
-    k_chroma420_refdct<<<grid, THREADS, 0, (cudaStream_t)stream>>>(work);
+    if (raw) k_chroma420_refdct<true><<<grid, THREADS, 0, (cudaStream_t)stream>>>(work);
+    else k_chroma420_refdct<false><<<grid, THREADS, 0, (cudaStream_t)stream>>>(work);
     return (int)cudaGetLastError();
 }
 int launch_upsample(const CompWork *work, int n, int max_w, int max_h, void *stream)
@@ -508,11 +558,19 @@ int launch_downsample(const CompWork *work, int n, int max_w, int max_h, void *s
     k_downsample<<<grid, blk, 0, (cudaStream_t)stream>>>(work);
     return (int)cudaGetLastError();
 }
-int launch_fdct_plane(const CompWork *work, int n, int max_tiles, void *stream)
+int launch_fdct_plane(const CompWork *work, int n, int max_tiles, void *stream, bool raw)
 {
     if (n <= 0 || max_tiles <= 0) return 0;
     dim3 grid(cdiv(max_tiles, WARPS_PER_CTA), n);
-    k_fdct_plane<<<grid, THREADS, 0, (cudaStream_t)stream>>>(work);
+    if (raw) k_fdct_plane<true><<<grid, THREADS, 0, (cudaStream_t)stream>>>(work);
+    else k_fdct_plane<false><<<grid, THREADS, 0, (cudaStream_t)stream>>>(work);
+    return (int)cudaGetLastError();
+}
+int launch_jpeg_trellis(const CompWork *work, int n, int max_blocks, const QuantDev *qbase, const JtTable *tables, void *stream)
+{
+    if (n <= 0 || max_blocks <= 0) return 0;
+    dim3 grid(cdiv(max_blocks, TRELLIS_THREADS), n);
+    k_jpeg_trellis<<<grid, TRELLIS_THREADS, 0, (cudaStream_t)stream>>>(work, qbase, tables);
     return (int)cudaGetLastError();
 }
 int launch_memset_warm(void *p, size_t n, void *stream)

@@ -4,6 +4,7 @@
 #pragma once
 #include <cstdint>
 #include <cstddef>
+#include "jpeg_trellis_core.h"
 
 namespace b200 {
 
@@ -83,12 +84,16 @@ inline int work_tiles(int rbw, int rbh) { return ((rbw + 31) / 32) * rbh; }   //
 // Launchers.  `work` is a DEVICE array of n descriptors; max_tiles = max over the n items of
 // work_tiles(real blocks across, down) for the grid the kernel iterates (sizes grid.x).  All asynchronous on `stream` (cudaStream_t).
 // Return cudaError_t as int.
-int launch_fused_same(const CompWork *work, int n, int max_tiles, void *stream);       // IDCT -> FDCT+quant, same geometry
+// raw = true: the FDCT kernels store the unquantised zigzag DCT output instead, for launch_jpeg_trellis to quantise.
+int launch_fused_same(const CompWork *work, int n, int max_tiles, void *stream, bool raw = false);       // IDCT -> FDCT+quant, same geometry
 int launch_idct_plane(const CompWork *work, int n, int max_tiles, void *stream);       // IDCT -> u8 plane
-int launch_chroma420_refdct(const CompWork *work, int n, int max_tiles, void *stream); // h2v2 fancy up o h2v2 box down o FDCT+quant
+int launch_chroma420_refdct(const CompWork *work, int n, int max_tiles, void *stream, bool raw = false); // h2v2 fancy up o h2v2 box down o FDCT+quant
 int launch_upsample(const CompWork *work, int n, int max_w, int max_h, void *stream);   // plane -> full
 int launch_downsample(const CompWork *work, int n, int max_w, int max_h, void *stream); // full -> dplane
-int launch_fdct_plane(const CompWork *work, int n, int max_tiles, void *stream);       // dplane -> coefficients
+int launch_fdct_plane(const CompWork *work, int n, int max_tiles, void *stream, bool raw = false);       // dplane -> coefficients
+// trellis quantisation in place of the raw coefficients of the real blocks of n items (max_blocks = max rbw_out * rbh_out);
+// item i uses tables[w.q - qbase], the JtTable beside its QuantDev
+int launch_jpeg_trellis(const CompWork *work, int n, int max_blocks, const QuantDev *qbase, const JtTable *tables, void *stream);
 int launch_memset_warm(void *p, size_t n, void *stream);
 
 } // namespace b200

@@ -31,7 +31,7 @@ struct PipeGroup {
 
 struct JpegPipe {
     int n = 0, K = 0, dev = 0;
-    bool lossless = false, progressive = true;
+    bool lossless = false, progressive = true, trellis = false;
     JpegGeom gout;
     JpegWriteOptions wo;
     std::vector<std::unique_ptr<JpegReader>> rd;
@@ -56,7 +56,7 @@ JpegPipe *pipe_create(const uint8_t *const *in, const size_t *in_len, int n, con
 {
     if (n <= 0 || K <= 0) { err = "empty pipe"; return nullptr; }
     std::unique_ptr<JpegPipe> P(new JpegPipe());
-    P->n = n; P->K = K; P->lossless = p->jpeg_optimize != 0; P->progressive = p->jpeg_progressive != 0;
+    P->n = n; P->K = K; P->lossless = p->jpeg_optimize != 0; P->progressive = p->jpeg_progressive != 0; P->trellis = !P->lossless && jpeg_trellis();
     P->wo = write_options(p); P->wo.copy_jfif = P->lossless;
     P->rd.resize((size_t)n); P->ds.resize((size_t)n);
     for (int i = 0; i < n; i++) {
@@ -104,7 +104,7 @@ static bool enqueue_group(JpegPipe *P, PipeGroup &G, int which, int *launches, s
     Slot *s = &G.slot;
     int n = 0;
     if (which == 0 || which == 1) { if (!s->dec->enqueue(s->stream, err)) return false; n += s->dec->launches; }
-    if (!P->lossless && (which == 0 || which == 2)) { if (!slot_transform_group(s, G.gins.data(), P->gout, G.L, err)) return false; n += 3; }
+    if (!P->lossless && (which == 0 || which == 2)) { if (!slot_transform_group(s, G.gins.data(), P->gout, G.L, P->trellis, err)) return false; n += P->trellis ? 4 : 3; }
     if (which == 0 || which == 3) { if (!s->enc->enqueue(s->stream, true, err)) return false; n += s->enc->launches; }
     if (launches) *launches += n;
     return true;

@@ -3,7 +3,8 @@ writes the same bytes as the CUDA path -- that equality is what the GPU tests as
 quality number, standard tables, optimised Huffman, progressive) and, for the WebP leg, libwebp (Pillow) at equal -q.
 The reference (libcaesium -> mozjpeg with trellis quantisation, deringing and scan optimisation) is expected to produce
 SMALLER files than ours at equal -q; libjpeg-turbo, its parent without those three, is the closest stand-in that exists here.
-CPU only.  Writes profiles/quality.json.  usage: python tools/quality_report.py"""
+CPU only.  Writes profiles/quality.json.  usage: python tools/quality_report.py [jpeg_trellis]
+(with `jpeg_trellis`, only that section is recomputed and the others are kept as they are)"""
 import io
 import json
 import os
@@ -91,11 +92,50 @@ def main():
                 row[f"pillow_mediancut_256_{k}_psnr_rgba"] = round(psnr(v, rgba), 3)
                 row[f"pillow_mediancut_256_{k}_blur_mae"] = round(blur_mae(v, rgba), 3)
             out["png_lossy"].append(row)
+    out["jpeg_trellis"] = jpeg_trellis()
     with open(os.path.join(ROOT, "profiles", "quality.json"), "w") as f:
         json.dump(out, f, indent=1)
-    for r in out["jpeg"] + out["webp"] + out["png_lossy"]:
+    for r in out["jpeg"] + out["webp"] + out["png_lossy"] + out["jpeg_trellis"]["rows"]:
         print(r)
 
 
+def jpeg_trellis():
+    """Trellis quantisation (b200_set_jpeg_trellis; the oracle writes the device's bytes) against plain quantisation: bytes and RGB
+    PSNR against the source's decoded pixels at q 50..90 (auto subsampling, progressive), and the BD-rate (bytes at equal PSNR) per
+    image.  The lambda constants were tuned on 1280x720 images of the same synthetic generator; j0 and j1 are held out."""
+    from oracle import jpeg_trellis as T
+    from test_jpeg_trellis_host import bd_rate
+    srcs = [(f"synthetic 3840x2160 seed {i} (q90 4:2:0 source)", synth_jpeg(3840, 2160, i)) for i in range(3)]
+    srcs += [(f"reference samples/{n}", open(os.path.join(ROOT, "tests", "golden", "reference_samples", n), "rb").read()) for n in ("j0.JPG", "j1.jpg")]
+    rows, bd = [], {}
+    for name, data in srcs:
+        truth = decode_rgb(data)
+        curve = {False: ([], []), True: ([], [])}
+        for q in (50, 60, 70, 80, 90):
+            row = {"input": name, "quality": q}
+            for t in (False, True):
+                out = T.jpeg_lossy(data, O.params(q, 0, True), trellis=t)
+                p = psnr(decode_rgb(out), truth)
+                curve[t][0].append(len(out)); curve[t][1].append(p)
+                k = "trellis" if t else "plain"
+                row[f"{k}_bytes"], row[f"{k}_psnr"] = len(out), round(p, 3)
+            row["bytes_ratio_trellis_over_plain"] = round(row["trellis_bytes"] / row["plain_bytes"], 4)
+            rows.append(row)
+        bd[name] = round(float(bd_rate(curve[False][0], curve[False][1], curve[True][0], curve[True][1])), 3)
+    return {"what": "trellis vs plain quantisation, this pipeline (oracle == device); PSNR of RGB against the pixels the source decodes to; "
+                    "bd_rate_percent: Bjontegaard delta of bytes at equal PSNR over q 50-90 (negative = trellis smaller)",
+            "rows": rows, "bd_rate_percent": bd}
+
+
 if __name__ == "__main__":
-    main()
+    if sys.argv[1:] == ["jpeg_trellis"]:
+        O.lib()
+        path = os.path.join(ROOT, "profiles", "quality.json")
+        with open(path) as f:
+            rep = json.load(f)
+        rep["jpeg_trellis"] = jpeg_trellis()
+        with open(path, "w") as f:
+            json.dump(rep, f, indent=1)
+        print(json.dumps(rep["jpeg_trellis"]["bd_rate_percent"]))
+    else:
+        main()
