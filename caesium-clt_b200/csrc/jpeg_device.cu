@@ -27,8 +27,6 @@ namespace b200 {
 
 thread_local LaunchTimer *tl_launch_timer = nullptr;
 
-#define CU(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return false; } } while (0)
-
 static constexpr size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 
 bool plan_image(const JpegGeom &gin, const JpegGeom &gout, ImagePlan &p, std::string &err)
@@ -201,15 +199,15 @@ Slot::~Slot()
 {
     if (stream) cudaStreamDestroy((cudaStream_t)stream);
     drop_graphs(this);
-    cudaFreeHost(h_in); cudaFreeHost(h_out); cudaFree(d_in); cudaFree(d_out); cudaFree(d_scratch); cudaFreeHost(h_par); cudaFree(d_par);
-    delete enc; delete dec; delete png; delete webp; delete vp8l;
 }
 
-GpuEncoder *Slot::encoder() { if (!enc) enc = new GpuEncoder(); return enc; }
-GpuDecoder *Slot::decoder() { if (!dec) dec = new GpuDecoder(); return dec; }
-PngDevice *Slot::png_dev() { if (!png) png = new PngDevice(); return png; }
-WebpDevice *Slot::webp_dev() { if (!webp) webp = new WebpDevice(); return webp; }
-Vp8lDevice *Slot::vp8l_dev() { if (!vp8l) vp8l = new Vp8lDevice(); return vp8l; }
+Slot::Slot() = default;
+
+GpuEncoder *Slot::encoder() { if (!enc) enc.reset(new GpuEncoder()); return enc.get(); }
+GpuDecoder *Slot::decoder() { if (!dec) dec.reset(new GpuDecoder()); return dec.get(); }
+PngDevice *Slot::png_dev() { if (!png) png.reset(new PngDevice()); return png.get(); }
+WebpDevice *Slot::webp_dev() { if (!webp) webp.reset(new WebpDevice()); return webp.get(); }
+Vp8lDevice *Slot::vp8l_dev() { if (!vp8l) vp8l.reset(new Vp8lDevice()); return vp8l.get(); }
 
 int runtime_device_count() { std::lock_guard<std::mutex> lk(g_mu); return g_inited ? (int)g_devs.size() : 0; }
 long long runtime_device_jobs(int i) { return g_devs.empty() || i < 0 || i >= (int)g_devs.size() ? 0 : g_devs[(size_t)i]->jobs.load(); }
@@ -245,42 +243,17 @@ void slot_release(Slot *s)
     d->cv.notify_one();
 }
 
-template <typename T> static bool grow_host(T *&p, size_t &cap, size_t need, std::string &err)
-{
-    if (need <= cap) return true;
-    if (p) cudaFreeHost(p);
-    p = nullptr; cap = 0;
-    size_t want = align_up(need + need / 8, 1 << 16);
-    void *q = nullptr;
-    cudaError_t e = cudaHostAlloc(&q, want, cudaHostAllocDefault);
-    if (e != cudaSuccess) { err = std::string("cudaHostAlloc: ") + cudaGetErrorString(e); return false; }
-    p = (T *)q; cap = want; return true;
-}
-template <typename T> static bool grow_dev(T *&p, size_t &cap, size_t need, std::string &err)
-{
-    if (need <= cap) return true;
-    if (p) cudaFree(p);
-    p = nullptr; cap = 0;
-    size_t want = align_up(need + need / 8, 1 << 16);
-    void *q = nullptr;
-    cudaError_t e = cudaMalloc(&q, want);
-    if (e != cudaSuccess) { err = std::string("cudaMalloc: ") + cudaGetErrorString(e); return false; }
-    p = (T *)q; cap = want; return true;
-}
-
 bool Slot::ensure_device(size_t in_bytes, size_t out_bytes, size_t scratch_bytes, size_t par_bytes, std::string &err)
 {   // megabatch path: coefficients never visit the host, so only the HBM side (and the small parameter block) grows
-    return grow_dev(d_in, d_in_cap, in_bytes, err) && grow_dev(d_out, d_out_cap, out_bytes, err) &&
-           grow_dev(d_scratch, d_scratch_cap, std::max<size_t>(scratch_bytes, 256), err) &&
-           grow_host(h_par, par_cap, par_bytes, err) && grow_dev(d_par, d_par_cap, par_bytes, err);
+    return d_in.reserve(in_bytes, Grow::Slot, err, &generation) && d_out.reserve(out_bytes, Grow::Slot, err, &generation) &&
+           d_scratch.reserve(std::max<size_t>(scratch_bytes, 256), Grow::Slot, err, &generation) &&
+           h_par.reserve(par_bytes, Grow::Slot, err, &generation) && d_par.reserve(par_bytes, Grow::Slot, err, &generation);
 }
 
 bool Slot::ensure(size_t in_bytes, size_t out_bytes, size_t scratch_bytes, size_t par_bytes, std::string &err)
 {
-    return grow_host(h_in, h_in_cap, in_bytes, err) && grow_host(h_out, h_out_cap, out_bytes, err) &&
-           grow_dev(d_in, d_in_cap, in_bytes, err) && grow_dev(d_out, d_out_cap, out_bytes, err) &&
-           grow_dev(d_scratch, d_scratch_cap, std::max<size_t>(scratch_bytes, 256), err) &&
-           grow_host(h_par, par_cap, par_bytes, err) && grow_dev(d_par, d_par_cap, par_bytes, err);
+    return h_in.reserve(in_bytes, Grow::Slot, err) && h_out.reserve(out_bytes, Grow::Slot, err) &&
+           ensure_device(in_bytes, out_bytes, scratch_bytes, par_bytes, err);
 }
 
 // Parameter block of a transform over K images, each part 256-byte aligned:
@@ -297,17 +270,17 @@ static size_t put_trellis(Slot *s, const JpegGeom &gout, size_t end, WorkLists &
     JtTable *t = reinterpret_cast<JtTable *>(s->h_par + off);
     for (int i = 0; i < 4; i++) if (gout.qt_present[i]) jt_make_table(gout.qt[i], i != 0, &t[i]);
     add_trellis_work(wl);
-    wl.trel_q = reinterpret_cast<const QuantDev *>(s->d_par);
+    wl.trel_q = reinterpret_cast<const QuantDev *>(s->d_par.get());
     wl.trel_t = reinterpret_cast<const JtTable *>(s->d_par + off);
     return off + sizeof(JtTable) * 4;
 }
 
 static void put_quant(Slot *s, const JpegGeom &gout)
 {
-    QuantDev *q = reinterpret_cast<QuantDev *>(s->h_par);
+    QuantDev *q = reinterpret_cast<QuantDev *>(s->h_par.get());
     for (int t = 0; t < 4; t++) if (gout.qt_present[t]) make_quant_dev(gout.qt[t], &q[t]);
 }
-static const QuantDev *dev_quant(const Slot *s) { return reinterpret_cast<const QuantDev *>(s->d_par); }
+static const QuantDev *dev_quant(const Slot *s) { return reinterpret_cast<const QuantDev *>(s->d_par.get()); }
 // image k's dequantisation tables into the pinned block; returns where the kernels read them
 static const uint16_t *put_dequant(Slot *s, int k, const JpegGeom &gin)
 {
@@ -352,8 +325,8 @@ bool slot_transform(Slot *s, const JpegGeom &gin, const JpegGeom &gout, std::str
     if (!fill_transform_params(s, &gins, gout, L, jpeg_trellis(), wl, pbytes, work_off, err)) return false;
     CU(cudaMemcpyAsync(s->d_par, s->h_par, pbytes, cudaMemcpyHostToDevice, st));
     if (upload) CU(cudaMemcpyAsync(s->d_in, s->h_in, plan.in_bytes, cudaMemcpyHostToDevice, st));
-    int rc = launch_work(wl, reinterpret_cast<const CompWork *>(s->d_par + work_off), st);
-    if (rc) { err = std::string("kernel launch: ") + cudaGetErrorString((cudaError_t)rc); return false; }
+    const int rc = launch_work(wl, reinterpret_cast<const CompWork *>(s->d_par + work_off), st);
+    if (!launch_ok(rc, "kernel launch", err)) return false;
     if (!download) return true;          // the coefficients stay in HBM for the device entropy encoder
     CU(cudaMemcpyAsync(s->h_out, s->d_out, plan.out_bytes, cudaMemcpyDeviceToHost, st));
     CU(stream_wait(st));
@@ -383,8 +356,8 @@ bool slot_transform_group_enqueue(Slot *s, std::string &err)
 {
     cudaStream_t st = (cudaStream_t)s->stream;
     CU(cudaMemcpyAsync(s->d_par, s->h_par, s->group_par_bytes, cudaMemcpyHostToDevice, st));
-    int rc = launch_work(s->group_wl, reinterpret_cast<const CompWork *>(s->d_par + s->group_work_off), st);
-    if (rc) { err = std::string("kernel launch: ") + cudaGetErrorString((cudaError_t)rc); return false; }
+    const int rc = launch_work(s->group_wl, reinterpret_cast<const CompWork *>(s->d_par + s->group_work_off), st);
+    if (!launch_ok(rc, "kernel launch", err)) return false;
     return true;
 }
 bool slot_transform_group(Slot *s, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, bool trellis, std::string &err)
@@ -460,7 +433,7 @@ bool slot_run_group(Slot *s, std::vector<GpuDecoder::Item> &items, const JpegGeo
     bool launched = false;
     if (graphs_enabled() && !s->graphs_broken) {
         unsigned long long sig = s->dec->signature() * 1099511628211ull ^ s->enc->signature();
-        sig = (sig ^ (unsigned long long)(uintptr_t)s->d_par ^ ((unsigned long long)s->group_par_bytes << 20) ^ (lossless ? 0x9e3779b97f4a7c15ull : 0)) * 1099511628211ull + (unsigned long long)L.K;
+        sig = (sig ^ s->generation ^ ((unsigned long long)s->group_par_bytes << 20) ^ (lossless ? 0x9e3779b97f4a7c15ull : 0)) * 1099511628211ull + (unsigned long long)L.K;
         if (!lossless && !s->group_wl.trel.empty()) sig = (sig ^ 0xc2b2ae3d27d4eb4full) * 1099511628211ull;     // the trellis pass is part of the sequence
         if (!s->graph_front || s->graph_sig != sig) {
             drop_graphs(s);
@@ -557,9 +530,9 @@ bool slot_decode_planes(Slot *s, const JpegGeom &gin, uint8_t *planes, std::stri
     size_t nw = flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + work_off));
     CU(cudaMemcpyAsync(s->d_par, s->h_par, work_off + nw * sizeof(CompWork), cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(s->d_in, s->h_in, plan.in_bytes, cudaMemcpyHostToDevice, st));
-    int rc = launch_work(wl, reinterpret_cast<const CompWork *>(s->d_par + work_off), st);
-    if (rc) { err = std::string("kernel launch: ") + cudaGetErrorString((cudaError_t)rc); return false; }
-    uint8_t *h = reinterpret_cast<uint8_t *>(s->h_out);
+    const int rc = launch_work(wl, reinterpret_cast<const CompWork *>(s->d_par + work_off), st);
+    if (!launch_ok(rc, "kernel launch", err)) return false;
+    uint8_t *h = reinterpret_cast<uint8_t *>(s->h_out.get());
     for (int c = 0; c < gin.ncomp; c++)
         CU(cudaMemcpyAsync(h + (size_t)c * gin.width * gin.height, s->d_scratch + plan.plane_bytes + plan.full_off[c], (size_t)gin.width * gin.height, cudaMemcpyDeviceToHost, st));
     CU(stream_wait(st));
@@ -628,15 +601,14 @@ bool slot_transform_resized(Slot *s, const JpegGeom &gin, const JpegGeom &gout, 
     const CompWork *dw = reinterpret_cast<const CompWork *>(s->d_par + work_off);
     const CompWork *p_idct = dw, *p_up = p_idct + wl.idct.size(), *p_down = p_up + wl.up.size(), *p_fdct = p_down + wl.down.size();
     const CompWork *p_trel = p_fdct + wl.fdct.size();
-    auto chk = [&](int rc, const char *what) { if (rc) { err = std::string(what) + ": " + cudaGetErrorString((cudaError_t)rc); return false; } return true; };
     uint8_t *full[3] = {s->d_scratch + full_off[0], nc == 3 ? s->d_scratch + full_off[1] : nullptr, nc == 3 ? s->d_scratch + full_off[2] : nullptr};
     uint8_t *rz[3] = {s->d_scratch + rz_off[0], nc == 3 ? s->d_scratch + rz_off[1] : nullptr, nc == 3 ? s->d_scratch + rz_off[2] : nullptr};
     if (host_rgb) {   // samples that never were a JPEG (PNG source): planar RGB (or one grey plane) straight into the full-resolution planes
         for (int c = 0; c < nc; c++) CU(cudaMemcpyAsync(full[c], host_rgb + (size_t)c * W * H, (size_t)W * H, cudaMemcpyHostToDevice, st));
     } else {
-        if (!chk(launch_idct_plane(p_idct, nc, wl.max_idct, st), "idct")) return false;
-        if (!chk(launch_upsample(p_up, nc, W, H, st), "upsample")) return false;
-        if (nc == 3 && !chk(launch_ycc_to_rgb(full[0], full[1], full[2], (size_t)W * H, st), "ycc_to_rgb")) return false;
+        if (!launch_ok(launch_idct_plane(p_idct, nc, wl.max_idct, st), "idct", err)) return false;
+        if (!launch_ok(launch_upsample(p_up, nc, W, H, st), "upsample", err)) return false;
+        if (nc == 3 && !launch_ok(launch_ycc_to_rgb(full[0], full[1], full[2], (size_t)W * H, st), "ycc_to_rgb", err)) return false;
     }
     float *tmp = reinterpret_cast<float *>(s->d_scratch + tmp_off);
     for (int c = 0; c < nc; c++) {
@@ -644,19 +616,19 @@ bool slot_transform_resized(Slot *s, const JpegGeom &gin, const JpegGeom &gout, 
             CU(cudaMemcpyAsync(rz[c], full[c], (size_t)W * H, cudaMemcpyDeviceToDevice, st));
             continue;
         }
-        if (!chk(launch_resize_v(full[c], W, H, W, tmp, NH, reinterpret_cast<const int *>(s->d_par + lv), reinterpret_cast<const int *>(s->d_par + cv),
-                                 reinterpret_cast<const float *>(s->d_par + wv), av.cap, st), "resize_v")) return false;
-        if (!chk(launch_resize_h(tmp, W, rz[c], NW, NH, NW, reinterpret_cast<const int *>(s->d_par + lh), reinterpret_cast<const int *>(s->d_par + chh),
-                                 reinterpret_cast<const float *>(s->d_par + wh), ah.cap, st), "resize_h")) return false;
+        if (!launch_ok(launch_resize_v(full[c], W, H, W, tmp, NH, reinterpret_cast<const int *>(s->d_par + lv), reinterpret_cast<const int *>(s->d_par + cv),
+                                 reinterpret_cast<const float *>(s->d_par + wv), av.cap, st), "resize_v", err)) return false;
+        if (!launch_ok(launch_resize_h(tmp, W, rz[c], NW, NH, NW, reinterpret_cast<const int *>(s->d_par + lh), reinterpret_cast<const int *>(s->d_par + chh),
+                                 reinterpret_cast<const float *>(s->d_par + wh), ah.cap, st), "resize_h", err)) return false;
     }
     if (rgb_out) { rgb_out[0] = rz[0]; rgb_out[1] = nc == 3 ? rz[1] : rz[0]; rgb_out[2] = nc == 3 ? rz[2] : rz[0]; return true; }
-    if (nc == 3 && !chk(launch_rgb_to_ycc(rz[0], rz[1], rz[2], (size_t)NW * NH, st), "rgb_to_ycc")) return false;
-    if (!chk(launch_downsample(p_down, nc, wl.max_dn_w, wl.max_dn_h, st), "downsample")) return false;
-    if (!chk(launch_fdct_plane(p_fdct, nc, wl.max_fdct, st, trellis), "fdct")) return false;
+    if (nc == 3 && !launch_ok(launch_rgb_to_ycc(rz[0], rz[1], rz[2], (size_t)NW * NH, st), "rgb_to_ycc", err)) return false;
+    if (!launch_ok(launch_downsample(p_down, nc, wl.max_dn_w, wl.max_dn_h, st), "downsample", err)) return false;
+    if (!launch_ok(launch_fdct_plane(p_fdct, nc, wl.max_fdct, st, trellis), "fdct", err)) return false;
     if (trellis) {
         const int rc = launch_jpeg_trellis(p_trel, nc, wl.max_trel, wl.trel_q, wl.trel_t, st);
         LT_MARK("k_jpeg_trellis");
-        if (!chk(rc, "trellis")) return false;
+        if (!launch_ok(rc, "trellis", err)) return false;
     }
     if (!download) return true;
     CU(cudaMemcpyAsync(s->h_out, s->d_out, out_bytes, cudaMemcpyDeviceToHost, st));

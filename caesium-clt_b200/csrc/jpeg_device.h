@@ -3,8 +3,10 @@
 #pragma once
 #include <cstdint>
 #include <cstddef>
+#include <memory>
 #include <string>
 #include <vector>
+#include "dev_buffer.h"
 #include "jpeg_host.h"
 #include "jpeg_kernels.h"
 #include "jpeg_gpudec.h"
@@ -49,18 +51,22 @@ bool jpeg_trellis();
 void set_jpeg_trellis(bool on);
 
 // ---- device runtime ------------------------------------------------------------------------------------------
+struct PngDevice;
+struct WebpDevice;
+struct Vp8lDevice;
 struct Slot {
     int dev = 0;
     void *stream = nullptr;
-    int16_t *h_in = nullptr, *h_out = nullptr; size_t h_in_cap = 0, h_out_cap = 0;       // pinned
-    int16_t *d_in = nullptr, *d_out = nullptr; size_t d_in_cap = 0, d_out_cap = 0;
-    uint8_t *d_scratch = nullptr; size_t d_scratch_cap = 0;
-    uint8_t *h_par = nullptr, *d_par = nullptr; size_t par_cap = 0, d_par_cap = 0;      // parameter block
-    class GpuEncoder *enc = nullptr;                                                     // device entropy encoder (lazy)
-    class GpuDecoder *dec = nullptr;                                                     // device entropy decoder (lazy)
-    struct PngDevice *png = nullptr;                                                     // lossless PNG state (lazy, png_device.cu)
-    struct WebpDevice *webp = nullptr;                                                   // WebP / VP8 state (lazy, webp_device.cu)
-    struct Vp8lDevice *vp8l = nullptr;                                                   // lossless WebP / VP8L state (lazy, vp8l_encode.cpp)
+    PinnedBuffer<int16_t> h_in, h_out;
+    DeviceBuffer<int16_t> d_in, d_out;
+    DeviceBuffer<uint8_t> d_scratch;
+    PinnedBuffer<uint8_t> h_par; DeviceBuffer<uint8_t> d_par;                           // parameter block
+    unsigned long long generation = 0;                                                   // bumped when d_in, d_out, d_scratch, h_par or d_par move
+    std::unique_ptr<GpuEncoder> enc;                                                     // device entropy encoder (lazy)
+    std::unique_ptr<GpuDecoder> dec;                                                     // device entropy decoder (lazy)
+    std::unique_ptr<PngDevice> png;                                                      // lossless PNG state (lazy, png_device.cu)
+    std::unique_ptr<WebpDevice> webp;                                                    // WebP / VP8 state (lazy, webp_device.cu)
+    std::unique_ptr<Vp8lDevice> vp8l;                                                    // lossless WebP / VP8L state (lazy, vp8l_encode.cpp)
     // megabatch path: transform work lists of the current megabatch, and the captured launch sequence (two CUDA graphs, see
     // slot_run_group) with the signature it was captured for
     WorkLists group_wl; size_t group_par_bytes = 0, group_work_off = 0;
@@ -73,10 +79,10 @@ struct Slot {
     PngDevice *png_dev();
     WebpDevice *webp_dev();
     Vp8lDevice *vp8l_dev();
-    Slot() = default;
+    Slot();
     Slot(const Slot &) = delete;
     Slot &operator=(const Slot &) = delete;
-    ~Slot();        // destroys the stream and frees every buffer; the caller has made the slot's device current and its stream idle
+    ~Slot();        // destroys the stream and the graphs, then the members free every buffer; the caller has made the slot's device current and its stream idle
 };
 
 int  runtime_init(int n_gpus, int only_device, std::string &err);   // returns device count (>0) or 0 with err
@@ -100,7 +106,7 @@ struct GroupLayout {
     // image k's coefficients: its input in s.d_in, or its output in s.d_out
     int16_t *coefs(const Slot &s, int k, bool input) const
     {
-        return reinterpret_cast<int16_t *>(reinterpret_cast<uint8_t *>(input ? s.d_in : s.d_out) + (input ? in_stride : out_stride) * k);
+        return reinterpret_cast<int16_t *>(reinterpret_cast<uint8_t *>((input ? s.d_in : s.d_out).get()) + (input ? in_stride : out_stride) * k);
     }
 };
 bool slot_group_layout(Slot *s, const JpegGeom &gin, const JpegGeom &gout, int K, GroupLayout &L, std::string &err);   // sizes + ensure()

@@ -19,8 +19,6 @@ namespace b200 {
 
 using namespace gd;
 
-#define CUD(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return false; } } while (0)
-
 // ---- un-stuffing: drop the 0x00 that follows every 0xFF -----------------------------------------------------------------
 __global__ void k_gd_unstuff_count(const DecImage *__restrict__ imgs, const uint8_t *__restrict__ raw_all, uint32_t *__restrict__ cnt, uint32_t *__restrict__ marker)
 {
@@ -198,28 +196,6 @@ __global__ void k_gd_dc_scatter(const DecImage *__restrict__ imgs, const int32_t
 // ---- host ---------------------------------------------------------------------------------------------------------------------
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
-static thread_local unsigned long long *tl_generation = nullptr;       // bumped on every reallocation (captured graphs hold the old pointers)
-template <typename T> static bool growd(T *&p, size_t &cap, size_t need, bool host, std::string &err)
-{
-    if (need <= cap) return true;
-    if (tl_generation) ++*tl_generation;
-    if (p) { if (host) cudaFreeHost(p); else cudaFree(p); }
-    p = nullptr; cap = 0;
-    // sizes here depend on image CONTENT (bytes of entropy-coded data); round up to a power of two with headroom so a
-    // slot stops reallocating after its first image of a given class (cudaFree / cudaHostAlloc stall every stream)
-    size_t want = 1 << 16; while (want < need + need / 2) want <<= 1;
-    void *q = nullptr;
-    cudaError_t e = host ? cudaHostAlloc(&q, want, cudaHostAllocDefault) : cudaMalloc(&q, want);
-    if (e != cudaSuccess) { err = std::string(host ? "cudaHostAlloc: " : "cudaMalloc: ") + cudaGetErrorString(e); return false; }
-    p = (T *)q; cap = want; return true;
-}
-
-GpuDecoder::~GpuDecoder()
-{
-    cudaFreeHost(h_raw); cudaFree(d_raw); cudaFree(d_stream); cudaFree(d_cnt); cudaFree(d_off); cudaFree(d_A); cudaFree(d_chgA); cudaFree(d_chgB);
-    cudaFree(d_nblk); cudaFree(d_first); cudaFree(d_dc); cudaFree(d_dcs); cudaFree(d_par); cudaFreeHost(h_par); cudaFree(d_temp);
-}
-
 // prepare(): per-image descriptors, buffers, Huffman tables; entropy-coded bytes and parameters staged in pinned memory and
 // their H2D copies enqueued.  enqueue(): every pass, no host wait -- a fixed number of synchronisation rounds (rounds whose image
 // has already settled leave at once), the per-round "something changed" flags copied back at the end.  finish(): after the
@@ -230,7 +206,6 @@ bool GpuDecoder::prepare(std::vector<Item> &items, void *stream_, std::string &e
     const int N = (int)items.size();
     nitems = N;
     if (N == 0) return true;
-    tl_generation = &generation;
     // ---- per-image descriptors
     imgs.assign((size_t)N, DecImage());
     coef_ptrs.resize((size_t)N); coef_bytes.resize((size_t)N);
@@ -275,18 +250,19 @@ bool GpuDecoder::prepare(std::vector<Item> &items, void *stream_, std::string &e
     o_img = 0; o_tab = align_up(sizeof(DecImage) * N, 256); o_flag = o_tab + align_up(sizeof(DecTables) * N, 256);
     o_mark = o_flag + align_up((size_t)4 * N * (MAX_ROUNDS + 2), 256);
     par_bytes = o_mark + align_up((size_t)4 * N, 256);
-    if (!growd(h_raw, cap_hraw, hw_raw + 64, true, err) || !growd(d_raw, cap_raw, hw_raw + 64, false, err) || !growd(d_stream, cap_stream, hw_stream + 64, false, err) ||
-        !growd(d_cnt, cap_cnt, hw_grp * 4 + 4, false, err) || !growd(d_off, cap_off, hw_grp * 4 + 4, false, err) ||
-        !growd(d_A, cap_A, hw_sub * sizeof(DecState), false, err) ||
-        !growd(d_chgA, cap_chgA, hw_sub, false, err) || !growd(d_chgB, cap_chgB, (size_t)2 * N * cdiv((long long)hw_msub, 64) + 64, false, err) ||
-        !growd(d_nblk, cap_nblk, hw_sub * 4, false, err) || !growd(d_first, cap_first, hw_sub * 4, false, err) ||
-        !growd(d_dc, cap_dc, hw_blk * 4, false, err) || !growd(d_dcs, cap_dcs, hw_blk * 4, false, err) ||
-        !growd(d_par, cap_par, par_bytes, false, err) || !growd(h_par, cap_hpar, par_bytes, true, err)) return false;
+    // sizes here depend on image CONTENT (bytes of entropy-coded data): Grow::Pow2Half rounds up to a power of two with headroom so a
+    // slot stops reallocating after its first image of a given class (cudaFree / cudaHostAlloc stall every stream)
+    auto grow = [&](auto &buf, size_t need) { return buf.reserve(need, Grow::Pow2Half, err, &generation); };
+    if (!grow(h_raw, hw_raw + 64) || !grow(d_raw, hw_raw + 64) || !grow(d_stream, hw_stream + 64) ||
+        !grow(d_cnt, hw_grp * 4 + 4) || !grow(d_off, hw_grp * 4 + 4) || !grow(d_A, hw_sub * sizeof(DecState)) ||
+        !grow(d_chgA, hw_sub) || !grow(d_chgB, (size_t)2 * N * cdiv((long long)hw_msub, 64) + 64) ||
+        !grow(d_nblk, hw_sub * 4) || !grow(d_first, hw_sub * 4) || !grow(d_dc, hw_blk * 4) || !grow(d_dcs, hw_blk * 4) ||
+        !grow(d_par, par_bytes) || !grow(h_par, par_bytes)) return false;
     size_t t1 = 0, t2 = 0, t3 = 0;
-    cub::DeviceScan::ExclusiveSum((void *)nullptr, t1, d_cnt, d_off, (int)hw_grp, st);
-    cub::DeviceScan::ExclusiveSum((void *)nullptr, t2, d_nblk, d_first, (int)hw_sub, st);
-    cub::DeviceScan::InclusiveSum((void *)nullptr, t3, d_dc, d_dcs, (int)hw_blk, st);
-    if (!growd(d_temp, cap_temp, std::max(t1, std::max(t2, t3)) + 256, false, err)) return false;
+    cub::DeviceScan::ExclusiveSum((void *)nullptr, t1, d_cnt.get(), d_off.get(), (int)hw_grp, st);
+    cub::DeviceScan::ExclusiveSum((void *)nullptr, t2, d_nblk.get(), d_first.get(), (int)hw_sub, st);
+    cub::DeviceScan::InclusiveSum((void *)nullptr, t3, d_dc.get(), d_dcs.get(), (int)hw_blk, st);
+    if (!grow(d_temp, std::max(t1, std::max(t2, t3)) + 256)) return false;
     // ---- parameters + raw bytes
     DecTables *ht = reinterpret_cast<DecTables *>(h_par + o_tab);
     tables_ok.assign((size_t)N, 1);
@@ -301,7 +277,6 @@ bool GpuDecoder::prepare(std::vector<Item> &items, void *stream_, std::string &e
     }
     memcpy(h_par + o_img, imgs.data(), sizeof(DecImage) * N);
     memset(h_par + o_flag, 0, (size_t)4 * N * (MAX_ROUNDS + 2));
-    tl_generation = nullptr;
     return true;
 }
 
@@ -311,8 +286,8 @@ bool GpuDecoder::upload(void *stream_, std::string &err)
 {
     cudaStream_t st = (cudaStream_t)stream_;
     if (nitems == 0) return true;
-    CUD(cudaMemcpyAsync(d_par, h_par, o_flag, cudaMemcpyHostToDevice, st));
-    CUD(cudaMemcpyAsync(d_raw, h_raw, hw_raw, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_par, h_par, o_flag, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_raw, h_raw, hw_raw, cudaMemcpyHostToDevice, st));
     return true;
 }
 
@@ -337,22 +312,22 @@ bool GpuDecoder::enqueue(void *stream_, std::string &err)
     const DecTables *dT = reinterpret_cast<const DecTables *>(d_par + o_tab);
     uint32_t *dF = reinterpret_cast<uint32_t *>(d_par + o_flag), *dM = reinterpret_cast<uint32_t *>(d_par + o_mark);
     uint32_t *hF = reinterpret_cast<uint32_t *>(h_par + o_flag);
-    CUD(cudaMemsetAsync(dF, 0, (o_mark - o_flag) + (size_t)4 * N, st));                 // round flags + marker flags
+    CU(cudaMemsetAsync(dF, 0, (o_mark - o_flag) + (size_t)4 * N, st));                 // round flags + marker flags
     LT_MARK("memset");
     // ---- unstuff
     const dim3 gg(cdiv((long long)hw_mgrp, 128), N);
     k_gd_unstuff_count<<<gg, 128, 0, st>>>(dI, d_raw, d_cnt, dM);
     LT_MARK("k_gd_unstuff_count");
-    size_t tb = cap_temp;
-    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_cnt, d_off, (int)hw_grp, st);
+    size_t tb = d_temp.capacity();
+    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_cnt.get(), d_off.get(), (int)hw_grp, st);
     LT_MARK("cub_scan");
     k_gd_unstuff_scatter<<<gg, 128, 0, st>>>(dIw, d_raw, d_off, d_cnt, d_stream);
     LT_MARK("k_gd_unstuff_scatter");
-    for (int n = 0; n < N; n++) CUD(cudaMemsetAsync(coef_ptrs[n], 0, coef_bytes[n], st));
+    for (int n = 0; n < N; n++) CU(cudaMemsetAsync(coef_ptrs[n], 0, coef_bytes[n], st));
     // ---- rounds
     const dim3 gs(cdiv((long long)hw_msub, 64), N);
     const size_t ncta = (size_t)N * gs.x;                    // dirty flags: two buffers of one byte per CTA, by round parity
-    CUD(cudaMemsetAsync(d_chgB, 0, 2 * ncta, st));
+    CU(cudaMemsetAsync(d_chgB, 0, 2 * ncta, st));
     LT_MARK("memset");
     k_gd_round0<<<gs, 64, 0, st>>>(dI, d_stream, dT, d_A, d_chgA, d_nblk);
     LT_MARK("k_gd_round0");
@@ -363,24 +338,24 @@ bool GpuDecoder::enqueue(void *stream_, std::string &err)
         LT_MARK("k_gd_round");
     }
     rounds_used = nrounds;
-    CUD(cudaMemcpyAsync(hF, dF, (size_t)4 * N * nrounds, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(hF, dF, (size_t)4 * N * nrounds, cudaMemcpyDeviceToHost, st));
     // ---- block counts -> first block of each subsequence -> write -> DC (images that did not converge, or whose stream the
     //      write pass flagged, produce garbage that their caller discards)
-    tb = cap_temp;
-    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_nblk, d_first, (int)hw_sub, st);
+    tb = d_temp.capacity();
+    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_nblk.get(), d_first.get(), (int)hw_sub, st);
     LT_MARK("cub_scan");
     k_gd_write<<<gs, 64, 0, st>>>(dI, d_stream, dT, d_A, d_first, dM);
     LT_MARK("k_gd_write");
-    CUD(cudaMemcpyAsync(h_par + o_mark, dM, (size_t)4 * N, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(h_par + o_mark, dM, (size_t)4 * N, cudaMemcpyDeviceToHost, st));
     const dim3 gb(cdiv((long long)hw_mblk, 128), N);
     k_gd_dc_gather<<<gb, 128, 0, st>>>(dI, d_dc);
     LT_MARK("k_gd_dc_gather");
-    tb = cap_temp;
-    cub::DeviceScan::InclusiveSum(d_temp, tb, d_dc, d_dcs, (int)hw_blk, st);
+    tb = d_temp.capacity();
+    cub::DeviceScan::InclusiveSum(d_temp, tb, d_dc.get(), d_dcs.get(), (int)hw_blk, st);
     LT_MARK("cub_scan");
     k_gd_dc_scatter<<<gb, 128, 0, st>>>(dI, d_dcs);
     LT_MARK("k_gd_dc_scatter");
-    CUD(cudaGetLastError());
+    CU(cudaGetLastError());
     launches = 10 + nrounds;
     return true;
 }
@@ -401,7 +376,7 @@ bool GpuDecoder::decode(std::vector<Item> &items, void *stream_, std::string &er
 {
     if (items.empty()) return true;
     if (!prepare(items, stream_, err) || !upload(stream_, err) || !enqueue(stream_, err)) return false;
-    CUD(stream_wait((cudaStream_t)stream_));
+    CU(stream_wait((cudaStream_t)stream_));
     finish(items);
     return true;
 }

@@ -5,6 +5,7 @@
 #include <cstddef>
 #include <string>
 #include <vector>
+#include "dev_buffer.h"
 #include "jpeg_gpudec_core.h"
 #include "jpeg_host.h"
 
@@ -26,7 +27,6 @@ struct DecImage {               // one image of a decode batch (device-visible)
 class GpuDecoder {
 public:
     GpuDecoder() = default;
-    ~GpuDecoder();
     GpuDecoder(const GpuDecoder &) = delete;
     GpuDecoder &operator=(const GpuDecoder &) = delete;
     enum Result { OK = 0, NOT_CONVERGED = 1, FAILED = 2 };
@@ -58,17 +58,17 @@ private:
     std::vector<DecImage> imgs; std::vector<int16_t *> coef_ptrs; std::vector<size_t> coef_bytes; std::vector<char> tables_ok;
     size_t raw_total = 0, o_img = 0, o_tab = 0, o_flag = 0, o_mark = 0, par_bytes = 0;
     size_t hw_raw = 0, hw_stream = 0, hw_grp = 0, hw_sub = 0, hw_blk = 0, hw_mgrp = 0, hw_msub = 0, hw_mblk = 0; int hw_n = 0;
-    unsigned long long generation = 0;
+    unsigned long long generation = 0;          // bumped by every reallocation: captured graphs hold the old addresses
     uint32_t grp_total = 0, sub_total = 0, blk_total = 0, max_grp = 0, max_sub = 0, max_blk = 0;
-    uint8_t *h_raw = nullptr; size_t cap_hraw = 0;          // pinned staging of the entropy-coded segments
-    uint8_t *d_raw = nullptr, *d_stream = nullptr; size_t cap_raw = 0, cap_stream = 0;
-    uint32_t *d_cnt = nullptr, *d_off = nullptr; size_t cap_cnt = 0, cap_off = 0;
-    gd::DecState *d_A = nullptr; size_t cap_A = 0;                             // exit state per subsequence (updated in place)
-    uint8_t *d_chgA = nullptr, *d_chgB = nullptr; size_t cap_chgA = 0, cap_chgB = 0;   // epoch of the last change per subsequence; dirty flags per CTA (x2)
-    uint32_t *d_nblk = nullptr, *d_first = nullptr; size_t cap_nblk = 0, cap_first = 0;
-    int32_t *d_dc = nullptr, *d_dcs = nullptr; size_t cap_dc = 0, cap_dcs = 0;
-    uint8_t *d_par = nullptr, *h_par = nullptr; size_t cap_par = 0, cap_hpar = 0;   // DecImage[] | DecTables[] | round flags
-    uint8_t *d_temp = nullptr; size_t cap_temp = 0;
+    PinnedBuffer<uint8_t> h_raw;                        // staging of the entropy-coded segments
+    DeviceBuffer<uint8_t> d_raw, d_stream;
+    DeviceBuffer<uint32_t> d_cnt, d_off;
+    DeviceBuffer<gd::DecState> d_A;                     // exit state per subsequence (updated in place)
+    DeviceBuffer<uint8_t> d_chgA, d_chgB;               // epoch of the last change per subsequence; dirty flags per CTA (x2)
+    DeviceBuffer<uint32_t> d_nblk, d_first;
+    DeviceBuffer<int32_t> d_dc, d_dcs;
+    DeviceBuffer<uint8_t> d_par; PinnedBuffer<uint8_t> h_par;   // DecImage[] | DecTables[] | round flags
+    DeviceBuffer<uint8_t> d_temp;
 };
 
 } // namespace b200

@@ -21,8 +21,6 @@ namespace b200 {
 
 using namespace ge;
 
-#define CU(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return false; } } while (0)
-
 // ---- kernels ------------------------------------------------------------------------------------------------------
 // EOB groups of the AC scans, and their EOBn symbols into the scan's AC table histogram: a group of c blocks is one symbol
 // (nbits(c) - 1) << 4, so a CTA (one scan: blockIdx.y) counts into 15 shared bins and flushes them once.
@@ -398,32 +396,13 @@ __global__ void k_ge_fill_dummy(int16_t *__restrict__ coef, long long comp_off, 
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 static inline int cdiv(long long a, long long b) { return (int)((a + b - 1) / b); }
 
-static thread_local unsigned long long *tl_enc_generation = nullptr;   // bumped on every reallocation (captured graphs hold the old pointers)
-template <typename T> static bool grow(T *&p, size_t &cap, size_t need, bool host, std::string &err)
-{
-    if (need <= cap) return true;
-    if (tl_enc_generation) ++*tl_enc_generation;
-    if (p) { if (host) cudaFreeHost(p); else cudaFree(p); }
-    p = nullptr; cap = 0;
-    // several sizes depend on image CONTENT (bytes of entropy-coded output); round up to a power of two with headroom so
-    // a slot stops reallocating after its first image of a given class (cudaFree / cudaHostAlloc stall every stream)
-    size_t want = 1 << 16; while (want < need + need / 2) want <<= 1;
-    void *q = nullptr;
-    cudaError_t e = host ? cudaHostAlloc(&q, want, cudaHostAllocDefault) : cudaMalloc(&q, want);
-    if (e != cudaSuccess) { err = std::string(host ? "cudaHostAlloc: " : "cudaMalloc: ") + cudaGetErrorString(e); return false; }
-    p = (T *)q; cap = want; return true;
-}
-
 GpuEncoder::~GpuEncoder()
 {
-    cudaFree(d_scans); cudaFree(d_comps); cudaFree(d_meta); cudaFree(d_evkey); cudaFree(d_prev); cudaFree(d_tail); cudaFree(d_tsum); cudaFree(d_gcount);
-    cudaFree(d_bitlen); cudaFree(d_bitoff); cudaFree(d_hist); cudaFree(d_tabs); cudaFree(d_dht); cudaFree(d_total); cudaFree(d_so);
-    cudaFree(d_words); cudaFree(d_masks); cudaFree(d_ffcount); cudaFree(d_ffoff); cudaFree(d_outoff); cudaFree(d_outlen); cudaFree(d_out); cudaFree(d_temp);
-    cudaFree(d_flags);
-    cudaFreeHost(h_small); cudaFreeHost(h_out);
     if (ev_sizes) cudaEventDestroy((cudaEvent_t)ev_sizes);
 }
 
+// Sizes here depend on image CONTENT (bytes of entropy-coded output): Grow::Pow2Half rounds up to a power of two with headroom so a
+// slot stops reallocating after its first image of a given class (cudaFree / cudaHostAlloc stall every stream).
 bool GpuEncoder::size_back_buffers(size_t image_bytes, std::string &err)
 {   // everything whose size follows the OUTPUT: bit buffer, 16-byte group arrays, stuffed bytes
     const int NS = (int)plan.scans.size();
@@ -436,16 +415,11 @@ bool GpuEncoder::size_back_buffers(size_t image_bytes, std::string &err)
     words_cap = (uint32_t)std::min<size_t>((size_t)nimg * (image_bytes / 4 + 1) + 2 * (size_t)NS + 64, 0xFFFFFF00u);
     groups_cap = (uint32_t)((size_t)words_cap / 4 + NS + 1);
     out_stride = align_up(image_bytes + image_bytes / 8 + 1024, 256);
-    tl_enc_generation = &generation;
-    size_t c;
-    c = cap_words; if (!grow(d_words, c, (size_t)words_cap * 4 + 64, false, err)) return false; cap_words = c;
-    c = cap_ff[0]; if (!grow(d_ffcount, c, (size_t)groups_cap * 4 + 4, false, err)) return false; cap_ff[0] = c;
-    c = cap_ff[1]; if (!grow(d_ffoff, c, (size_t)groups_cap * 4 + 4, false, err)) return false; cap_ff[1] = c;
-    c = cap_out; if (!grow(d_out, c, out_stride * nimg, false, err)) return false; cap_out = c;
-    size_t tb3 = 0; cub::DeviceScan::ExclusiveSum((void *)nullptr, tb3, d_ffcount, d_ffoff, (int)groups_cap, (cudaStream_t)0);
-    c = cap_temp; if (tb3 + 256 > c) { if (!grow(d_temp, c, tb3 + 256, false, err)) return false; cap_temp = c; }
-    tl_enc_generation = nullptr;
-    return true;
+    auto grow = [&](auto &buf, size_t need) { return buf.reserve(need, Grow::Pow2Half, err, &generation); };
+    if (!grow(d_words, (size_t)words_cap * 4 + 64) || !grow(d_ffcount, (size_t)groups_cap * 4 + 4) || !grow(d_ffoff, (size_t)groups_cap * 4 + 4) ||
+        !grow(d_out, out_stride * nimg)) return false;
+    size_t tb3 = 0; cub::DeviceScan::ExclusiveSum((void *)nullptr, tb3, d_ffcount.get(), d_ffoff.get(), (int)groups_cap, (cudaStream_t)0);
+    return grow(d_temp, tb3 + 256);
 }
 
 bool GpuEncoder::prepare(const JpegGeom &g, bool progressive, int16_t *const *d_coefs, int nimages, void *stream_, size_t out_bytes_hint, std::string &err)
@@ -460,40 +434,26 @@ bool GpuEncoder::prepare(const JpegGeom &g, bool progressive, int16_t *const *d_
     const long long U = plan.total_units;
     if (U >= (1ll << 31)) { err = "batch too large for the entropy encoder"; return false; }
     overflow = false;
-    tl_enc_generation = &generation;
     for (auto &sc_ : plan.scans) if (!masks_cover(sc_.mode, sc_.Al)) { err = "scan script outside the device encoder's mask range"; overflow = true; return false; }
     if (!ev_sizes) { cudaEvent_t e; CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming | (stream_wait_mode() == 0 ? 0 : cudaEventBlockingSync))); ev_sizes = e; }
     // ---- buffers whose size follows the INPUT
-    size_t c;
-    c = cap_scans; if (!grow(d_scans, c, NS * sizeof(Scan), false, err)) return false; cap_scans = c;
+    auto grow = [&](auto &buf, size_t need) { return buf.reserve(need, Grow::Pow2Half, err, &generation); };
     const int NC = (int)plan.comps.size();
-    c = cap_comps; if (!grow(d_comps, c, NC * sizeof(BlockComp), false, err)) return false; cap_comps = c;
-    c = cap_u[0]; if (!grow(d_meta, c, U * 4, false, err)) return false; cap_u[0] = c;
-    c = cap_u[1]; if (!grow(d_evkey, c, U * 4, false, err)) return false; cap_u[1] = c;
-    c = cap_u[2]; if (!grow(d_prev, c, U * 4, false, err)) return false; cap_u[2] = c;
-    c = cap_u[3]; if (!grow(d_tail, c, U * 4, false, err)) return false; cap_u[3] = c;
-    c = cap_u[4]; if (!grow(d_tsum, c, U * 4, false, err)) return false; cap_u[4] = c;
-    c = cap_u[5]; if (!grow(d_gcount, c, U * 4, false, err)) return false; cap_u[5] = c;
-    c = cap_u[6]; if (!grow(d_bitlen, c, U * 4, false, err)) return false; cap_u[6] = c;
-    c = cap_u[7]; if (!grow(d_bitoff, c, U * 4, false, err)) return false; cap_u[7] = c;
-    c = cap_hist; if (!grow(d_hist, c, (size_t)NS * 4 * 256 * 4, false, err)) return false; cap_hist = c;
-    c = cap_tabs; if (!grow(d_tabs, c, (size_t)NS * 4 * sizeof(Table), false, err)) return false; cap_tabs = c;
-    c = cap_dht; if (!grow(d_dht, c, (size_t)NS * 4 * sizeof(DhtOut), false, err)) return false; cap_dht = c;
-    c = cap_total; if (!grow(d_total, c, (size_t)NS * 4, false, err)) return false; cap_total = c;
-    c = cap_so; if (!grow(d_so, c, (size_t)NS * sizeof(ScanOut), false, err)) return false; cap_so = c;
-    c = cap_oo; if (!grow(d_outoff, c, (size_t)NS * 4, false, err)) return false; cap_oo = c;
-    c = cap_ol; if (!grow(d_outlen, c, (size_t)NS * 4, false, err)) return false; cap_ol = c;
-    c = cap_flags; if (!grow(d_flags, c, 64, false, err)) return false; cap_flags = c;
-    c = cap_masks; if (!grow(d_masks, c, (size_t)plan.total_comp_blocks * sizeof(Masks3), false, err)) return false; cap_masks = c;
+    if (!grow(d_scans, NS * sizeof(Scan)) || !grow(d_comps, NC * sizeof(BlockComp)) ||
+        !grow(d_meta, U * 4) || !grow(d_evkey, U * 4) || !grow(d_prev, U * 4) || !grow(d_tail, U * 4) || !grow(d_tsum, U * 4) ||
+        !grow(d_gcount, U * 4) || !grow(d_bitlen, U * 4) || !grow(d_bitoff, U * 4) ||
+        !grow(d_hist, (size_t)NS * 4 * 256 * 4) || !grow(d_tabs, (size_t)NS * 4 * sizeof(Table)) || !grow(d_dht, (size_t)NS * 4 * sizeof(DhtOut)) ||
+        !grow(d_total, (size_t)NS * 4) || !grow(d_so, (size_t)NS * sizeof(ScanOut)) || !grow(d_outoff, (size_t)NS * 4) || !grow(d_outlen, (size_t)NS * 4) ||
+        !grow(d_flags, 64) || !grow(d_masks, (size_t)plan.total_comp_blocks * sizeof(Masks3))) return false;
     o_scans = 0; o_total = o_scans + align_up((size_t)NS * sizeof(Scan), 256); o_outlen = o_total + align_up((size_t)NS * 4, 256);
     o_dht = o_outlen + align_up((size_t)NS * 4, 256); o_comps = o_dht + align_up((size_t)NS * 4 * sizeof(DhtOut), 256);
     o_flags = o_comps + align_up((size_t)NC * sizeof(BlockComp), 256);
     const size_t small_bytes = o_flags + 256;
-    c = cap_small; if (!grow(h_small, c, small_bytes, true, err)) return false; cap_small = c;
+    if (!grow(h_small, small_bytes)) return false;
     size_t tb1 = 0, tb2 = 0;
-    cub::DeviceScan::ExclusiveScan((void *)nullptr, tb1, d_evkey, d_prev, cub::Max(), -1, (int)U, st);
-    cub::DeviceScan::ExclusiveSum((void *)nullptr, tb2, d_tail, d_tsum, (int)U, st);
-    c = cap_temp; if (!grow(d_temp, c, std::max(tb1, tb2) + 256, false, err)) return false; cap_temp = c;
+    cub::DeviceScan::ExclusiveScan((void *)nullptr, tb1, d_evkey.get(), d_prev.get(), cub::Max(), -1, (int)U, st);
+    cub::DeviceScan::ExclusiveSum((void *)nullptr, tb2, d_tail.get(), d_tsum.get(), (int)U, st);
+    if (!grow(d_temp, std::max(tb1, tb2) + 256)) return false;
     // ---- buffers whose size follows the OUTPUT: estimate now, exact on a retry.  A re-encode at lower quality does not grow, so
     // the caller's hint is the input's entropy-coded size; without a hint a third of the coefficient bytes (~ 1 byte / pixel).
     const size_t coef_bytes = (size_t)g.total_coefs * 2;
@@ -501,7 +461,6 @@ bool GpuEncoder::prepare(const JpegGeom &g, bool progressive, int16_t *const *d_
     size_t est = out_bytes_hint ? out_bytes_hint / nimages + out_bytes_hint / nimages / 4 : coef_bytes / 3;
     est = std::max(est, learned_image_bytes + learned_image_bytes / 8) + 8192;
     est = std::min(est, coef_bytes * 2 + (size_t)plan.scans_per_image * 64 + 8192);      // worst case: 128 B per block and scan... bounded by the retry anyway
-    tl_enc_generation = nullptr;
     if (!size_back_buffers(est, err)) return false;
     memcpy(h_small + o_scans, plan.scans.data(), NS * sizeof(Scan));
     memcpy(h_small + o_comps, plan.comps.data(), NC * sizeof(BlockComp));
@@ -563,8 +522,8 @@ bool GpuEncoder::enqueue_back(void *stream_, std::string &err)
     LT_MARK("k_geb_emit");
     k_ge_ffcount<<<dim3(32, NS + 1), 128, 0, st>>>(d_so, NS, d_words, d_ffcount, groups_cap, d_flags);
     LT_MARK("k_ge_ffcount");
-    size_t tb = cap_temp;
-    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_ffcount, d_ffoff, (int)groups_cap, st);
+    size_t tb = d_temp.capacity();
+    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_ffcount.get(), d_ffoff.get(), (int)groups_cap, st);
     LT_MARK("cub_scan");
     k_ge_layout<<<cdiv(nimg, 64), 64, 0, st>>>(d_so, plan.scans_per_image, nimg, d_ffcount, d_ffoff, d_outoff, d_outlen, (uint32_t)out_stride, d_flags);
     LT_MARK("k_ge_layout");
@@ -605,11 +564,11 @@ bool GpuEncoder::enqueue_front(void *stream_, bool fill_dummy, std::string &err)
     LT_MARK("memset");
     k_geb_classify<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_scans, d_meta, d_evkey, d_tail, d_masks, d_hist);
     LT_MARK("k_geb_classify");
-    size_t tb = cap_temp;
-    cub::DeviceScan::ExclusiveScan(d_temp, tb, d_evkey, d_prev, cub::Max(), -1, (int)U, st);
+    size_t tb = d_temp.capacity();
+    cub::DeviceScan::ExclusiveScan(d_temp, tb, d_evkey.get(), d_prev.get(), cub::Max(), -1, (int)U, st);
     LT_MARK("cub_scan");
-    tb = cap_temp;
-    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_tail, d_tsum, (int)U, st);
+    tb = d_temp.capacity();
+    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_tail.get(), d_tsum.get(), (int)U, st);
     LT_MARK("cub_scan");
     CU(cudaMemsetAsync(d_gcount, 0, U * 4, st));
     LT_MARK("memset");
@@ -619,8 +578,8 @@ bool GpuEncoder::enqueue_front(void *stream_, bool fill_dummy, std::string &err)
     LT_MARK("k_ge_tables");
     k_geb_len<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_scans, d_gcount, d_tabs, d_bitlen, d_masks);
     LT_MARK("k_geb_len");
-    tb = cap_temp;
-    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_bitlen, d_bitoff, (int)U, st);
+    tb = d_temp.capacity();
+    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_bitlen.get(), d_bitoff.get(), (int)U, st);
     LT_MARK("cub_scan");
     launches += 7;
     CU(cudaGetLastError());
@@ -651,7 +610,7 @@ bool GpuEncoder::finish(void *stream_, bool fetch, std::string &err)
         }
         if (fetch) {
             copy_bytes = std::min(out_stride, align_up(img_max + img_max / 8 + 256, 256));
-            size_t c = cap_hout; if (!grow(h_out, c, copy_bytes * nimg, true, err)) return false; cap_hout = c;
+            if (!h_out.reserve(copy_bytes * nimg, Grow::Pow2Half, err, &generation)) return false;
             for (int im = 0; im < nimg; im++) CU(cudaMemcpyAsync(h_out + (size_t)im * copy_bytes, d_out + (size_t)im * out_stride, copy_bytes, cudaMemcpyDeviceToHost, st));
             CU(cudaGetLastError());
             const auto tw1 = std::chrono::steady_clock::now();
@@ -670,7 +629,7 @@ bool GpuEncoder::finish(void *stream_, bool fetch, std::string &err)
             bool shortc = false;
             for (int im = 0; im < nimg && !shortc; im++) { size_t tot = 0; for (int k = 0; k < spi; k++) tot += h_outlen[im * spi + k]; shortc = tot > copy_bytes; }
             if (shortc) {
-                size_t c = cap_hout; if (!grow(h_out, c, out_stride * nimg, true, err)) return false; cap_hout = c;
+                if (!h_out.reserve(out_stride * nimg, Grow::Pow2Half, err, &generation)) return false;
                 copy_bytes = out_stride;
                 for (int j = 0; j < nimg; j++) CU(cudaMemcpyAsync(h_out + (size_t)j * copy_bytes, d_out + (size_t)j * out_stride, copy_bytes, cudaMemcpyDeviceToHost, st));
                 CU(stream_wait(st));

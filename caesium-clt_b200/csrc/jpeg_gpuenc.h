@@ -4,6 +4,7 @@
 #include <cstddef>
 #include <string>
 #include <vector>
+#include "dev_buffer.h"
 #include "jpeg_gpuenc_plan.h"
 
 namespace b200 {
@@ -45,33 +46,33 @@ public:
     int launches = 0;
 private:
     bool size_back_buffers(size_t image_bytes, std::string &err);
-    unsigned long long generation = 0; int cap_nimg = 0;
+    unsigned long long generation = 0;      // bumped by every reallocation: captured graphs hold the old addresses
+    int cap_nimg = 0;
     int nimg = 0;
     JpegGeom geom; bool prog = false;
     std::vector<int16_t *> coef_bases;
     void *ev_sizes = nullptr;
     uint32_t words_cap = 0, groups_cap = 0;
     size_t est_image_bytes = 0, learned_image_bytes = 0, learned_for = 0;
-    uint32_t *d_flags = nullptr; size_t cap_flags = 0;
+    DeviceBuffer<uint32_t> d_flags;
     size_t o_scans = 0, o_total = 0, o_outlen = 0, o_dht = 0, o_comps = 0, o_flags = 0;
-    ge::Scan *d_scans = nullptr; size_t cap_scans = 0;
-    BlockComp *d_comps = nullptr; size_t cap_comps = 0;
-    uint32_t *d_meta = nullptr, *d_tail = nullptr, *d_tsum = nullptr, *d_gcount = nullptr, *d_bitlen = nullptr, *d_bitoff = nullptr;
-    int *d_evkey = nullptr, *d_prev = nullptr;
-    size_t cap_u[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    uint32_t *d_hist = nullptr; size_t cap_hist = 0;
-    ge::Table *d_tabs = nullptr; size_t cap_tabs = 0;
-    DhtOut *d_dht = nullptr; size_t cap_dht = 0;
-    uint32_t *d_total = nullptr; size_t cap_total = 0;
-    ScanOut *d_so = nullptr; size_t cap_so = 0;
-    uint32_t *d_words = nullptr; size_t cap_words = 0;
-    ge::Masks3 *d_masks = nullptr; size_t cap_masks = 0;       // threshold masks per block, written by the classify pass
-    uint32_t *d_ffcount = nullptr, *d_ffoff = nullptr; size_t cap_ff[2] = {0, 0};
-    uint32_t *d_outoff = nullptr, *d_outlen = nullptr; size_t cap_oo = 0, cap_ol = 0;
-    uint8_t *d_out = nullptr; size_t cap_out = 0;
-    uint8_t *d_temp = nullptr; size_t cap_temp = 0;
-    uint8_t *h_small = nullptr; size_t cap_small = 0;
-    uint8_t *h_out = nullptr; size_t cap_hout = 0;
+    DeviceBuffer<ge::Scan> d_scans;
+    DeviceBuffer<BlockComp> d_comps;
+    DeviceBuffer<uint32_t> d_meta, d_tail, d_tsum, d_gcount, d_bitlen, d_bitoff;
+    DeviceBuffer<int> d_evkey, d_prev;
+    DeviceBuffer<uint32_t> d_hist;
+    DeviceBuffer<ge::Table> d_tabs;
+    DeviceBuffer<DhtOut> d_dht;
+    DeviceBuffer<uint32_t> d_total;
+    DeviceBuffer<ScanOut> d_so;
+    DeviceBuffer<uint32_t> d_words;
+    DeviceBuffer<ge::Masks3> d_masks;                   // threshold masks per block, written by the classify pass
+    DeviceBuffer<uint32_t> d_ffcount, d_ffoff;
+    DeviceBuffer<uint32_t> d_outoff, d_outlen;
+    DeviceBuffer<uint8_t> d_out;
+    DeviceBuffer<uint8_t> d_temp;
+    PinnedBuffer<uint8_t> h_small;
+    PinnedBuffer<uint8_t> h_out;
     size_t out_stride = 0, copy_bytes = 0;
 };
 

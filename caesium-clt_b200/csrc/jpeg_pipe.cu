@@ -17,8 +17,6 @@
 
 namespace b200 {
 
-#define CUP(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return false; } } while (0)
-
 struct PipeGroup {
     Slot slot;                                  // private buffers + stream (not from the runtime's pool)
     cudaEvent_t done = nullptr;
@@ -116,13 +114,13 @@ bool pipe_run(JpegPipe *P, void *stream_, int which, int *launches, std::string 
     cudaSetDevice(runtime_device_ordinal(P->dev));
     if (launches) *launches = 0;
     P->finished = false;
-    CUP(cudaEventRecord(P->fork, caller));
+    CU(cudaEventRecord(P->fork, caller));
     for (auto &G : P->groups) {
         cudaStream_t st = (cudaStream_t)G->slot.stream;
-        CUP(cudaStreamWaitEvent(st, P->fork, 0));
+        CU(cudaStreamWaitEvent(st, P->fork, 0));
         if (!enqueue_group(P, *G, which, launches, err)) return false;
-        CUP(cudaEventRecord(G->done, st));
-        CUP(cudaStreamWaitEvent(caller, G->done, 0));
+        CU(cudaEventRecord(G->done, st));
+        CU(cudaStreamWaitEvent(caller, G->done, 0));
     }
     return true;
 }
@@ -133,7 +131,7 @@ bool pipe_finish(JpegPipe *P, size_t *out_sizes, int *not_settled, int *enc_retr
     int bad = 0, retries = 0;
     for (auto &G : P->groups) {
         Slot *s = &G->slot;
-        CUP(cudaStreamSynchronize((cudaStream_t)s->stream));
+        CU(cudaStreamSynchronize((cudaStream_t)s->stream));
         const int r0 = s->enc->retries;
         if (!s->enc->finish(s->stream, false, err)) return false;
         retries += s->enc->retries - r0;
@@ -170,7 +168,7 @@ bool pipe_kernel_times(JpegPipe *P, int iters, std::map<std::string, std::pair<d
     cudaSetDevice(runtime_device_ordinal(P->dev));
     PipeGroup &G = *P->groups[0];
     cudaStream_t st = (cudaStream_t)G.slot.stream;
-    CUP(cudaDeviceSynchronize());
+    CU(cudaDeviceSynchronize());
     std::map<std::string, std::pair<double, int>> acc;
     for (int it = 0; it < iters; it++) {
         LaunchTimer lt; lt.begin(st);
@@ -178,7 +176,7 @@ bool pipe_kernel_times(JpegPipe *P, int iters, std::map<std::string, std::pair<d
         const bool ok = enqueue_group(P, G, 0, nullptr, err);
         tl_launch_timer = nullptr;
         if (!ok) return false;
-        CUP(cudaStreamSynchronize(st));
+        CU(cudaStreamSynchronize(st));
         lt.collect(acc);
     }
     out.clear();

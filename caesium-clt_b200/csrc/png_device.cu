@@ -18,32 +18,16 @@
 
 namespace b200 {
 
-#define CUP(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return false; } } while (0)
-
 static const int kChunk = 4096;
 static const int kBlockTokens = 1 << 16;            // tokens per DEFLATE block (deflate_tokens' default)
 
-template <typename T> static bool growp(T *&p, size_t &cap, size_t need, bool host, std::string &err)
-{
-    if (need <= cap) return true;
-    if (p) { if (host) cudaFreeHost(p); else cudaFree(p); }
-    p = nullptr; cap = 0;
-    size_t want = 1 << 16; while (want < need + need / 4) want <<= 1;
-    void *q = nullptr;
-    cudaError_t e = host ? cudaHostAlloc(&q, want, cudaHostAllocDefault) : cudaMalloc(&q, want);
-    if (e != cudaSuccess) { err = std::string(host ? "cudaHostAlloc: " : "cudaMalloc: ") + cudaGetErrorString(e); return false; }
-    p = (T *)q; cap = want; return true;
-}
+// growable buffers: the smallest power of two >= 64 KiB and >= need + need / 4
+template <class B> static bool grow(B &buf, size_t need, std::string &err) { return buf.reserve(need, Grow::Pow2Quarter, err); }
 
-PngDevice::~PngDevice()
-{
-    cudaFree(d_raw); cudaFree(d_raw2); cudaFree(d_filt); cudaFree(d_best); cudaFree(d_tok); cudaFree(d_out); cudaFree(d_counts); cudaFree(d_offsets);
-    cudaFree(d_hist); cudaFree(d_sums); cudaFree(d_tlog); cudaFree(d_temp); cudaFreeHost(h_small); cudaFreeHost(h_tok); cudaFreeHost(h_raw);
-    cudaFree(d_filt_all); cudaFree(d_fin); cudaFree(d_sums_in); cudaFree(d_sync); cudaFree(d_dfl); cudaFree(d_z); cudaFreeHost(h_z);
-    delete quant;
-}
+PngDevice::PngDevice() = default;
+PngDevice::~PngDevice() = default;
 
-PngQuant *PngDevice::quantiser() { if (!quant) quant = new PngQuant(); return quant; }
+PngQuant *PngDevice::quantiser() { if (!quant) quant.reset(new PngQuant()); return quant.get(); }
 
 // oxipng presets (SURVEY.md §3.4-iii): which row-filter strategies each optimisation level tries
 std::vector<int> png_level_strategies(int level)
@@ -81,10 +65,10 @@ bool PngDevice::run_strategy(int strategy, int h, int rb, int bpp, void *stream_
     int rc = do_filter ? launch_png_filter(d_raw, filt, h, rb, bpp, strategy, d_tlog, st) : 0;
     if (!rc) rc = launch_png_match(filt, d_best, n, bpp, rb + 1, st);
     if (!rc && with_hash) rc = launch_png_hashmatch(filt, d_best, n, d_hist + 2048, st);
-    if (rc) { err = std::string("png kernels: ") + cudaGetErrorString((cudaError_t)rc); return false; }
-    CUP(cudaMemsetAsync(d_hist, 0, 316 * 4, st));
+    if (!launch_ok(rc, "png kernels", err)) return false;
+    CU(cudaMemsetAsync(d_hist, 0, 316 * 4, st));
     rc = launch_png_parse(d_best, filt, n, kChunk, d_tok, d_counts, d_hist, st);
-    if (rc) { err = std::string("png parse: ") + cudaGetErrorString((cudaError_t)rc); return false; }
+    if (!launch_ok(rc, "png parse", err)) return false;
     return true;
 }
 
@@ -100,18 +84,18 @@ bool PngDevice::ensure_buffers(size_t nraw, size_t nmax, size_t rb, void *stream
     const size_t nchunks_max = (nmax + kChunk - 1) / kChunk;
     z_cap = nmax + nmax / 32 + ((nmax >> 16) + 2) * 512 + 4096;                 // the zlib payload: Huffman-coded literals cannot exceed ~8.1 bits each
     z_cap = (z_cap + 255) / 256 * 256;
-    if (!growp(d_raw, cap_raw, nraw + 64, false, err) || !growp(d_raw2, cap_raw2, nraw + 64, false, err) ||
-        !growp(d_filt, cap_filt, nmax + 64, false, err) || !growp(d_best, cap_best, nmax * 4, false, err) || !growp(d_tok, cap_tok, nmax * 4, false, err) ||
-        !growp(d_out, cap_out, nmax * 4, false, err) || !growp(d_counts, cap_counts, nchunks_max * 4 + 4, false, err) || !growp(d_offsets, cap_offsets, nchunks_max * 4 + 4, false, err) ||
-        !growp(d_hist, cap_hist, 316 * 4 * 16, false, err) || !growp(d_sums, cap_sums, ((nmax + 4095) / 4096) * 16 + 16, false, err) ||
-        !growp(d_sums_in, cap_sums_in, ((nmax + 4095) / 4096) * 16 + 16, false, err) ||
-        !growp(d_tlog, cap_tlog, (rb + 8) * 4, false, err) || !growp(h_small, cap_small, 1 << 16, true, err) ||
-        !growp(d_sync, cap_sync, ((nraw / std::max<size_t>(rb, 1) + 31) / 32 + 16) * 4 + 2048 * 4 + 64, false, err) ||
-        !growp(d_dfl, cap_dfl, png_deflate_scratch_bytes(nmax, kBlockTokens), false, err) || !growp(d_z, cap_z, z_cap + 64, false, err) ||
-        !growp(h_z, cap_hz, z_cap + ((nmax + 4095) / 4096) * 32 + 256, true, err)) return false;
-    size_t tb = 0; cub::DeviceScan::ExclusiveSum((void *)nullptr, tb, d_counts, d_offsets, (int)nchunks_max, st);
-    if (!growp(d_temp, cap_temp, tb + 256, false, err)) return false;
-    if (tlog_n < rb + 2) { std::vector<uint32_t> t(rb + 2); png_make_tlog(t.data(), rb + 1); CUP(cudaMemcpyAsync(d_tlog, t.data(), (rb + 2) * 4, cudaMemcpyHostToDevice, st)); CUP(stream_wait(st)); tlog_n = rb + 2; }
+    if (!grow(d_raw, nraw + 64, err) || !grow(d_raw2, nraw + 64, err) ||
+        !grow(d_filt, nmax + 64, err) || !grow(d_best, nmax * 4, err) || !grow(d_tok, nmax * 4, err) ||
+        !grow(d_out, nmax * 4, err) || !grow(d_counts, nchunks_max * 4 + 4, err) || !grow(d_offsets, nchunks_max * 4 + 4, err) ||
+        !grow(d_hist, 316 * 4 * 16, err) || !grow(d_sums, ((nmax + 4095) / 4096) * 16 + 16, err) ||
+        !grow(d_sums_in, ((nmax + 4095) / 4096) * 16 + 16, err) ||
+        !grow(d_tlog, (rb + 8) * 4, err) || !grow(h_small, 1 << 16, err) ||
+        !grow(d_sync, ((nraw / std::max<size_t>(rb, 1) + 31) / 32 + 16) * 4 + 2048 * 4 + 64, err) ||
+        !grow(d_dfl, png_deflate_scratch_bytes(nmax, kBlockTokens), err) || !grow(d_z, z_cap + 64, err) ||
+        !grow(h_z, z_cap + ((nmax + 4095) / 4096) * 32 + 256, err)) return false;
+    size_t tb = 0; cub::DeviceScan::ExclusiveSum((void *)nullptr, tb, d_counts.get(), d_offsets.get(), (int)nchunks_max, st);
+    if (!grow(d_temp, tb + 256, err)) return false;
+    if (tlog_n < rb + 2) { std::vector<uint32_t> t(rb + 2); png_make_tlog(t.data(), rb + 1); CU(cudaMemcpyAsync(d_tlog, t.data(), (rb + 2) * 4, cudaMemcpyHostToDevice, st)); CU(stream_wait(st)); tlog_n = rb + 2; }
     return true;
 }
 
@@ -128,8 +112,8 @@ static uint32_t combine_adler(const unsigned long long *sums, size_t n)
 
 uint8_t *PngDevice::input_buffer(size_t bytes, size_t &cap, std::string &err)
 {
-    if (!growp(h_raw, cap_hraw, bytes + 4096 + 64, true, err)) return nullptr;
-    cap = cap_hraw;
+    if (!grow(h_raw, bytes + 4096 + 64, err)) return nullptr;
+    cap = h_raw.capacity();
     return h_raw;
 }
 
@@ -158,27 +142,27 @@ bool PngDevice::from_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler
     const size_t nraw = (size_t)h * rb, nin = (size_t)h * (rb + 1);
     if (nfilt < nin) { err = "IDAT too short"; corrupt = true; return false; }
     const size_t nmax = nin + 64;
-    if (!ensure_buffers(nraw, nmax, rb, st, err) || !growp(d_fin, cap_fin, nmax + 64, false, err)) return false;
-    CUP(cudaMemcpyAsync(d_fin, h_raw, nin, cudaMemcpyHostToDevice, st)); LT_MARK("h2d");
+    if (!ensure_buffers(nraw, nmax, rb, st, err) || !grow(d_fin, nmax + 64, err)) return false;
+    CU(cudaMemcpyAsync(d_fin, h_raw, nin, cudaMemcpyHostToDevice, st)); LT_MARK("h2d");
     int rc = launch_png_adler(d_fin, nin, d_sums_in, st);
     uint32_t *d_un = d_sync, *d_flags = d_hist;
     uint32_t *d_set = reinterpret_cast<uint32_t *>(((uintptr_t)(d_sync + ((size_t)(h + 31) / 32 + 8)) + 7) & ~(uintptr_t)7);
     if (!rc) rc = launch_png_unfilter(d_fin, d_raw, h, (int)rb, bpp, d_un, st);
-    if (rc) { err = std::string("png unfilter: ") + cudaGetErrorString((cudaError_t)rc); return false; }
-    CUP(cudaMemsetAsync(d_flags, 0, 16, st));
+    if (!launch_ok(rc, "png unfilter", err)) return false;
+    CU(cudaMemsetAsync(d_flags, 0, 16, st));
     const bool eight = info.bit_depth == 8 && info.trns.empty();
     const bool probe_ag = !lossy && eight && (info.color_type == 2 || info.color_type == 4 || info.color_type == 6);
     const bool probe_pal = !lossy && png_palette_candidate(info);
     const size_t npix = (size_t)info.width * info.height;
     if (probe_ag && launch_png_probe(d_raw, npix, info.channels, d_flags, st)) { err = "png probe launch failed"; return false; }
     if (probe_pal && launch_png_colours(d_raw, npix, info.channels, d_set, d_flags, st)) { err = "png palette probe launch failed"; return false; }
-    uint32_t *h_flags = reinterpret_cast<uint32_t *>(h_small);
-    unsigned long long *h_sums_in = reinterpret_cast<unsigned long long *>(h_z);
+    uint32_t *h_flags = reinterpret_cast<uint32_t *>(h_small.get());
+    unsigned long long *h_sums_in = reinterpret_cast<unsigned long long *>(h_z.get());
     const size_t npieces_in = (nin + 4095) / 4096;
-    CUP(cudaMemcpyAsync(h_flags, d_flags, 16, cudaMemcpyDeviceToHost, st));
-    CUP(cudaMemcpyAsync(h_flags + 4, d_un, 8, cudaMemcpyDeviceToHost, st));
-    CUP(cudaMemcpyAsync(h_sums_in, d_sums_in, npieces_in * 16, cudaMemcpyDeviceToHost, st));
-    CUP(stream_wait(st)); LT_MARK("host_wait");
+    CU(cudaMemcpyAsync(h_flags, d_flags, 16, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(h_flags + 4, d_un, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(h_sums_in, d_sums_in, npieces_in * 16, cudaMemcpyDeviceToHost, st));
+    CU(stream_wait(st)); LT_MARK("host_wait");
     if (h_flags[5]) { err = "bad filter type"; corrupt = true; return false; }
     if (combine_adler(h_sums_in, nin) != stored_adler) { err = "Adler-32 mismatch"; corrupt = true; return false; }
     if (lossy) return quantiser()->expand(d_raw, info, st, err) && quant->prepare(st, err);
@@ -186,7 +170,7 @@ bool PngDevice::from_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler
         // few colours: oxipng's palette reduction (first-appearance order, tRNS layout, bit packing) runs on the host over the
         // reconstructed samples, and the indexed image takes the raw-sample entry point
         std::vector<uint8_t> raw(nraw);
-        CUP(cudaMemcpy(raw.data(), d_raw, nraw, cudaMemcpyDeviceToHost));
+        CU(cudaMemcpy(raw.data(), d_raw, nraw, cudaMemcpyDeviceToHost));
         if (png_reduce_palette(info, raw)) return compress(info, raw, level, stream_, zlib_stream, chosen, err);
     }
     return reduce_and_code(info, probe_ag, h_flags, level, stream_, zlib_stream, chosen, err);
@@ -202,15 +186,15 @@ bool PngDevice::compress(PngInfo &info, const std::vector<uint8_t> &raw_in, int 
     size_t cap = 0;
     if (!ensure_buffers(nraw, nmax, rb, st, err) || !input_buffer(nraw, cap, err)) return false;
     memcpy(h_raw, raw_in.data(), nraw);
-    CUP(cudaMemcpyAsync(d_raw, h_raw, nraw, cudaMemcpyHostToDevice, st));
-    uint32_t *h_flags = reinterpret_cast<uint32_t *>(h_small);
+    CU(cudaMemcpyAsync(d_raw, h_raw, nraw, cudaMemcpyHostToDevice, st));
+    uint32_t *h_flags = reinterpret_cast<uint32_t *>(h_small.get());
     const bool probe_ag = info.bit_depth == 8 && info.trns.empty() && (info.color_type == 2 || info.color_type == 4 || info.color_type == 6);
     if (probe_ag) {
         uint32_t *d_flags = d_hist;
-        CUP(cudaMemsetAsync(d_flags, 0, 16, st));
+        CU(cudaMemsetAsync(d_flags, 0, 16, st));
         if (launch_png_probe(d_raw, (size_t)info.width * info.height, info.channels, d_flags, st)) { err = "png probe launch failed"; return false; }
-        CUP(cudaMemcpyAsync(h_flags, d_flags, 16, cudaMemcpyDeviceToHost, st));
-        CUP(stream_wait(st)); LT_MARK("host_wait");
+        CU(cudaMemcpyAsync(h_flags, d_flags, 16, cudaMemcpyDeviceToHost, st));
+        CU(stream_wait(st)); LT_MARK("host_wait");
     }
     return reduce_and_code(info, probe_ag, h_flags, level, stream_, zlib_stream, chosen, err);
 }
@@ -260,7 +244,7 @@ bool PngDevice::reduce_and_code(PngInfo &info, bool probed, const uint32_t *h_fl
             for (int c = 0; c < ncolor; c++) if (!to_grey || c == 0) mask |= 1 << c;
             if (has_alpha && !drop_alpha) mask |= 1 << (ch - 1);
             if (launch_png_repack(d_raw, d_raw2, npix, ch, mask, st)) { err = "png repack launch failed"; return false; }
-            std::swap(d_raw, d_raw2); std::swap(cap_raw, cap_raw2);
+            d_raw.swap(d_raw2);
             const bool grey = to_grey || !is_rgb, alpha = has_alpha && !drop_alpha;
             info.color_type = grey ? (alpha ? 4 : 0) : (alpha ? 6 : 2);
             info.channels = (grey ? 1 : 3) + (alpha ? 1 : 0);
@@ -276,12 +260,12 @@ bool PngDevice::reduce_and_code(PngInfo &info, bool probed, const uint32_t *h_fl
     const size_t fstride = (n + 64 + 255) / 256 * 256;
     if (strategies.size() > 1) {
         // every trial keeps its filtered stream (K6 is not repeated for the winner)
-        if (!growp(d_filt_all, cap_filt_all, fstride * strategies.size() + 64, false, err)) return false;
+        if (!grow(d_filt_all, fstride * strategies.size() + 64, err)) return false;
         for (size_t k = 0; k < strategies.size(); k++) {
             if (!run_strategy(strategies[k], h, (int)rb, bpp, st, err, d_filt_all + k * fstride, true, false)) return false;
-            CUP(cudaMemcpyAsync(h_small + 1024 + k * 316 * 4, d_hist, 316 * 4, cudaMemcpyDeviceToHost, st));
+            CU(cudaMemcpyAsync(h_small + 1024 + k * 316 * 4, d_hist, 316 * 4, cudaMemcpyDeviceToHost, st));
         }
-        CUP(stream_wait(st)); LT_MARK("host_wait");
+        CU(stream_wait(st)); LT_MARK("host_wait");
         for (size_t k = 0; k < strategies.size(); k++) {
             const double bits = estimate_bits(reinterpret_cast<const uint32_t *>(h_small + 1024 + k * 316 * 4));
             if (best_bits < 0 || bits < best_bits) { best_bits = bits; best_s = strategies[k]; best_k = k; }
@@ -292,11 +276,11 @@ bool PngDevice::reduce_and_code(PngInfo &info, bool probed, const uint32_t *h_fl
     //      stream, DEFLATE coding -- all on the device
     uint8_t *const wfilt = strategies.size() > 1 ? d_filt_all + best_k * fstride : d_filt;
     if (!run_strategy(best_s, h, (int)rb, bpp, st, err, wfilt, strategies.size() <= 1, true)) return false;
-    size_t tb = cap_temp;
-    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_counts, d_offsets, (int)nchunks, st); LT_MARK("cub_scan");
+    size_t tb = d_temp.capacity();
+    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_counts.get(), d_offsets.get(), (int)nchunks, st); LT_MARK("cub_scan");
     int rc = launch_png_compact(d_tok, d_counts, d_offsets, nchunks, kChunk, d_out, st);
     if (!rc) rc = launch_png_adler(wfilt, n, d_sums, st);
-    if (rc) { err = std::string("png compact/adler: ") + cudaGetErrorString((cudaError_t)rc); return false; }
+    if (!launch_ok(rc, "png compact/adler", err)) return false;
     unsigned long long *d_total = reinterpret_cast<unsigned long long *>(d_hist + 1024);          // [0] payload bits, [1] tokens
     uint32_t *d_ntok = d_hist + 1032;
     k_png_ntok<<<1, 32, 0, st>>>(d_counts, d_offsets, nchunks, d_ntok);
@@ -305,15 +289,15 @@ bool PngDevice::reduce_and_code(PngInfo &info, bool probed, const uint32_t *h_fl
     const size_t npieces = (n + 4095) / 4096;
     unsigned long long *h_sums = reinterpret_cast<unsigned long long *>(h_z + z_cap + 64);
     if (!host_huffman) {
-        rc = launch_png_deflate(d_out, d_ntok, n, kBlockTokens, d_dfl, reinterpret_cast<uint32_t *>(d_z), z_cap, d_total, st);
-        if (rc) { err = std::string("png deflate: ") + cudaGetErrorString((cudaError_t)rc); return false; }
-        CUP(cudaMemcpyAsync(h_total, d_total, 16, cudaMemcpyDeviceToHost, st));
-        CUP(cudaMemcpyAsync(h_sums, d_sums, npieces * 16, cudaMemcpyDeviceToHost, st));
-        CUP(stream_wait(st)); LT_MARK("host_wait");
+        rc = launch_png_deflate(d_out, d_ntok, n, kBlockTokens, d_dfl, reinterpret_cast<uint32_t *>(d_z.get()), z_cap, d_total, st);
+        if (!launch_ok(rc, "png deflate", err)) return false;
+        CU(cudaMemcpyAsync(h_total, d_total, 16, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(h_sums, d_sums, npieces * 16, cudaMemcpyDeviceToHost, st));
+        CU(stream_wait(st)); LT_MARK("host_wait");
         const size_t zbytes = (size_t)((h_total[0] + 7) / 8);
         if (zbytes + 8 <= z_cap) {
-            CUP(cudaMemcpyAsync(h_z, d_z, zbytes, cudaMemcpyDeviceToHost, st)); LT_MARK("d2h");
-            CUP(stream_wait(st)); LT_MARK("host_wait");
+            CU(cudaMemcpyAsync(h_z, d_z, zbytes, cudaMemcpyDeviceToHost, st)); LT_MARK("d2h");
+            CU(stream_wait(st)); LT_MARK("host_wait");
             const uint32_t adler = combine_adler(h_sums, n);
             zlib_stream.resize(zbytes + 4);
             memcpy(zlib_stream.data(), h_z, zbytes);
@@ -324,15 +308,15 @@ bool PngDevice::reduce_and_code(PngInfo &info, bool probed, const uint32_t *h_fl
         }
         // does not fit the device buffer (cannot happen for Huffman-coded literals; kept as a guard): the host codes the tokens
     } else {
-        CUP(cudaMemcpyAsync(h_total + 1, d_ntok, 4, cudaMemcpyDeviceToHost, st));
-        CUP(cudaMemcpyAsync(h_sums, d_sums, npieces * 16, cudaMemcpyDeviceToHost, st));
-        CUP(stream_wait(st)); LT_MARK("host_wait");
+        CU(cudaMemcpyAsync(h_total + 1, d_ntok, 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(h_sums, d_sums, npieces * 16, cudaMemcpyDeviceToHost, st));
+        CU(stream_wait(st)); LT_MARK("host_wait");
         h_total[1] &= 0xFFFFFFFFull;
     }
     const size_t ntok = (size_t)h_total[1];
-    if (!growp(h_tok, cap_htok, (n + 64) * 4 + 64, true, err)) return false;
-    CUP(cudaMemcpyAsync(h_tok, d_out, ntok * 4, cudaMemcpyDeviceToHost, st));
-    CUP(stream_wait(st)); LT_MARK("host_wait");
+    if (!grow(h_tok, (n + 64) * 4 + 64, err)) return false;
+    CU(cudaMemcpyAsync(h_tok, d_out, ntok * 4, cudaMemcpyDeviceToHost, st));
+    CU(stream_wait(st)); LT_MARK("host_wait");
     const auto td = std::chrono::steady_clock::now();
     deflate_tokens(h_tok, ntok, combine_adler(h_sums, n), zlib_stream);
     last_deflate_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - td).count();
@@ -346,81 +330,71 @@ bool PngDevice::plane_tokens(const uint8_t *plane, size_t n, int stride, void *s
     cudaStream_t st = (cudaStream_t)stream_;
     if (!n || stride < 1) { err = "empty plane"; return false; }
     if (!ensure_buffers(n, n, (size_t)stride, st, err)) return false;
-    if (!growp(h_raw, cap_hraw, n + 4096 + 64, true, err) || !growp(h_tok, cap_htok, (n + 64) * 4 + 64, true, err)) return false;
+    if (!grow(h_raw, n + 4096 + 64, err) || !grow(h_tok, (n + 64) * 4 + 64, err)) return false;
     memcpy(h_raw, plane, n);
-    CUP(cudaMemcpyAsync(d_filt, h_raw, n, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_filt, h_raw, n, cudaMemcpyHostToDevice, st));
     const size_t nchunks = (n + kChunk - 1) / kChunk;
     int rc = launch_png_match(d_filt, d_best, n, 1, stride, st);
     if (!rc) rc = launch_png_hashmatch(d_filt, d_best, n, d_hist + 2048, st);
-    if (rc) { err = std::string("png kernels: ") + cudaGetErrorString((cudaError_t)rc); return false; }
-    CUP(cudaMemsetAsync(d_hist, 0, 316 * 4, st));
+    if (!launch_ok(rc, "png kernels", err)) return false;
+    CU(cudaMemsetAsync(d_hist, 0, 316 * 4, st));
     rc = launch_png_parse(d_best, d_filt, n, kChunk, d_tok, d_counts, d_hist, st);
-    if (rc) { err = std::string("png parse: ") + cudaGetErrorString((cudaError_t)rc); return false; }
-    size_t tb = cap_temp;
-    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_counts, d_offsets, (int)nchunks, st);
+    if (!launch_ok(rc, "png parse", err)) return false;
+    size_t tb = d_temp.capacity();
+    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_counts.get(), d_offsets.get(), (int)nchunks, st);
     rc = launch_png_compact(d_tok, d_counts, d_offsets, nchunks, kChunk, d_out, st);
-    if (rc) { err = std::string("png compact: ") + cudaGetErrorString((cudaError_t)rc); return false; }
+    if (!launch_ok(rc, "png compact", err)) return false;
     uint32_t *d_ntok = d_hist + 1032;
     k_png_ntok<<<1, 32, 0, st>>>(d_counts, d_offsets, nchunks, d_ntok);
     uint32_t *h_n = reinterpret_cast<uint32_t *>(h_small + 64);
-    CUP(cudaMemcpyAsync(h_n, d_ntok, 4, cudaMemcpyDeviceToHost, st));
-    CUP(stream_wait(st));
+    CU(cudaMemcpyAsync(h_n, d_ntok, 4, cudaMemcpyDeviceToHost, st));
+    CU(stream_wait(st));
     const size_t ntok = *h_n;
     if (ntok > n) { err = "token count out of range"; return false; }
-    CUP(cudaMemcpyAsync(h_tok, d_out, ntok * 4, cudaMemcpyDeviceToHost, st));
-    CUP(stream_wait(st));
-    tokens.assign(h_tok, h_tok + ntok);
+    CU(cudaMemcpyAsync(h_tok, d_out, ntok * 4, cudaMemcpyDeviceToHost, st));
+    CU(stream_wait(st));
+    tokens.assign(h_tok.get(), h_tok + ntok);
     return true;
 }
 
 // ---- stage entry points (b200_png_filter / b200_png_lz77): plain allocate-run-free, used by the parity tests ----------------
 bool png_stage_filter(const uint8_t *raw, int h, int rb, int bpp, int strategy, uint8_t *filtered, std::string &err)
 {
-    uint8_t *d_raw = nullptr, *d_filt = nullptr; uint32_t *d_tlog = nullptr;
+    DeviceBuffer<uint8_t> d_raw, d_filt; DeviceBuffer<uint32_t> d_tlog;
     const size_t nraw = (size_t)h * rb, n = (size_t)h * (rb + 1);
-    bool ok = false;
-    do {
-        if (cudaMalloc(&d_raw, nraw + 64) != cudaSuccess || cudaMalloc(&d_filt, n + 64) != cudaSuccess || cudaMalloc(&d_tlog, ((size_t)rb + 8) * 4) != cudaSuccess) { err = "cudaMalloc failed"; break; }
-        std::vector<uint32_t> t(rb + 2); png_make_tlog(t.data(), rb + 1);
-        cudaMemcpy(d_tlog, t.data(), t.size() * 4, cudaMemcpyHostToDevice);
-        cudaMemcpy(d_raw, raw, nraw, cudaMemcpyHostToDevice);
-        if (launch_png_filter(d_raw, d_filt, h, rb, bpp, strategy, d_tlog, nullptr)) { err = "png filter launch failed"; break; }
-        cudaError_t e = cudaMemcpy(filtered, d_filt, n, cudaMemcpyDeviceToHost);
-        if (e != cudaSuccess) { err = std::string("png filter: ") + cudaGetErrorString(e); break; }
-        ok = true;
-    } while (0);
-    cudaFree(d_raw); cudaFree(d_filt); cudaFree(d_tlog);
-    return ok;
+    if (!d_raw.reserve(nraw + 64, Grow::Exact, err) || !d_filt.reserve(n + 64, Grow::Exact, err) || !d_tlog.reserve(((size_t)rb + 8) * 4, Grow::Exact, err)) return false;
+    std::vector<uint32_t> t(rb + 2); png_make_tlog(t.data(), rb + 1);
+    cudaMemcpy(d_tlog, t.data(), t.size() * 4, cudaMemcpyHostToDevice);
+    cudaMemcpy(d_raw, raw, nraw, cudaMemcpyHostToDevice);
+    if (launch_png_filter(d_raw, d_filt, h, rb, bpp, strategy, d_tlog, nullptr)) { err = "png filter launch failed"; return false; }
+    cudaError_t e = cudaMemcpy(filtered, d_filt, n, cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) { err = std::string("png filter: ") + cudaGetErrorString(e); return false; }
+    return true;
 }
 
 bool png_stage_lz77(const uint8_t *filtered, size_t n, int bpp, int stride, std::vector<uint32_t> &tokens, uint32_t *hist, std::string &err)
 {
-    uint8_t *d_filt = nullptr, *d_temp = nullptr; uint32_t *d_best = nullptr, *d_tok = nullptr, *d_out = nullptr, *d_counts = nullptr, *d_offsets = nullptr, *d_hist = nullptr;
+    DeviceBuffer<uint8_t> d_filt, d_temp; DeviceBuffer<uint32_t> d_best, d_tok, d_out, d_counts, d_offsets, d_hist;
     const size_t nchunks = (n + kChunk - 1) / kChunk;
-    bool ok = false;
-    do {
-        size_t tb = 0; cub::DeviceScan::ExclusiveSum((void *)nullptr, tb, d_counts, d_offsets, (int)nchunks);
-        if (cudaMalloc(&d_filt, n + 64) != cudaSuccess || cudaMalloc(&d_best, n * 4 + 64) != cudaSuccess || cudaMalloc(&d_tok, n * 4 + 64) != cudaSuccess ||
-            cudaMalloc(&d_out, n * 4 + 64) != cudaSuccess || cudaMalloc(&d_counts, nchunks * 4 + 4) != cudaSuccess || cudaMalloc(&d_offsets, nchunks * 4 + 4) != cudaSuccess ||
-            cudaMalloc(&d_hist, (320 + 544) * 4) != cudaSuccess || cudaMalloc(&d_temp, tb + 256) != cudaSuccess) { err = "cudaMalloc failed"; break; }
-        cudaMemset(d_filt + n, 0, 64);
-        cudaMemcpy(d_filt, filtered, n, cudaMemcpyHostToDevice);
-        cudaMemset(d_hist, 0, 316 * 4);
-        if (launch_png_match(d_filt, d_best, n, bpp, stride, nullptr) || launch_png_hashmatch(d_filt, d_best, n, d_hist + 320, nullptr) || launch_png_parse(d_best, d_filt, n, kChunk, d_tok, d_counts, d_hist, nullptr)) { err = "png lz77 launch failed"; break; }
-        cub::DeviceScan::ExclusiveSum(d_temp, tb, d_counts, d_offsets, (int)nchunks);
-        if (launch_png_compact(d_tok, d_counts, d_offsets, nchunks, kChunk, d_out, nullptr)) { err = "png compact launch failed"; break; }
-        uint32_t last[2];
-        cudaMemcpy(&last[0], d_offsets + (nchunks - 1), 4, cudaMemcpyDeviceToHost);
-        cudaError_t e = cudaMemcpy(&last[1], d_counts + (nchunks - 1), 4, cudaMemcpyDeviceToHost);
-        if (e != cudaSuccess) { err = std::string("png lz77: ") + cudaGetErrorString(e); break; }
-        tokens.resize((size_t)last[0] + last[1]);
-        cudaMemcpy(tokens.data(), d_out, tokens.size() * 4, cudaMemcpyDeviceToHost);
-        e = cudaMemcpy(hist, d_hist, 316 * 4, cudaMemcpyDeviceToHost);
-        if (e != cudaSuccess) { err = std::string("png lz77: ") + cudaGetErrorString(e); break; }
-        ok = true;
-    } while (0);
-    cudaFree(d_filt); cudaFree(d_best); cudaFree(d_tok); cudaFree(d_out); cudaFree(d_counts); cudaFree(d_offsets); cudaFree(d_hist); cudaFree(d_temp);
-    return ok;
+    size_t tb = 0; cub::DeviceScan::ExclusiveSum((void *)nullptr, tb, d_counts.get(), d_offsets.get(), (int)nchunks);
+    if (!d_filt.reserve(n + 64, Grow::Exact, err) || !d_best.reserve(n * 4 + 64, Grow::Exact, err) || !d_tok.reserve(n * 4 + 64, Grow::Exact, err) ||
+        !d_out.reserve(n * 4 + 64, Grow::Exact, err) || !d_counts.reserve(nchunks * 4 + 4, Grow::Exact, err) || !d_offsets.reserve(nchunks * 4 + 4, Grow::Exact, err) ||
+        !d_hist.reserve((320 + 544) * 4, Grow::Exact, err) || !d_temp.reserve(tb + 256, Grow::Exact, err)) return false;
+    cudaMemset(d_filt + n, 0, 64);
+    cudaMemcpy(d_filt, filtered, n, cudaMemcpyHostToDevice);
+    cudaMemset(d_hist, 0, 316 * 4);
+    if (launch_png_match(d_filt, d_best, n, bpp, stride, nullptr) || launch_png_hashmatch(d_filt, d_best, n, d_hist + 320, nullptr) || launch_png_parse(d_best, d_filt, n, kChunk, d_tok, d_counts, d_hist, nullptr)) { err = "png lz77 launch failed"; return false; }
+    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_counts.get(), d_offsets.get(), (int)nchunks);
+    if (launch_png_compact(d_tok, d_counts, d_offsets, nchunks, kChunk, d_out, nullptr)) { err = "png compact launch failed"; return false; }
+    uint32_t last[2];
+    cudaMemcpy(&last[0], d_offsets + (nchunks - 1), 4, cudaMemcpyDeviceToHost);
+    cudaError_t e = cudaMemcpy(&last[1], d_counts + (nchunks - 1), 4, cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) { err = std::string("png lz77: ") + cudaGetErrorString(e); return false; }
+    tokens.resize((size_t)last[0] + last[1]);
+    cudaMemcpy(tokens.data(), d_out, tokens.size() * 4, cudaMemcpyDeviceToHost);
+    e = cudaMemcpy(hist, d_hist, 316 * 4, cudaMemcpyDeviceToHost);
+    if (e != cudaSuccess) { err = std::string("png lz77: ") + cudaGetErrorString(e); return false; }
+    return true;
 }
 
 } // namespace b200

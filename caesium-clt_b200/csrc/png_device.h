@@ -3,8 +3,10 @@
 #include <cstdint>
 #include <cstddef>
 #include <cmath>
+#include <memory>
 #include <string>
 #include <vector>
+#include "dev_buffer.h"
 #include "png_host.h"
 
 namespace b200 {
@@ -15,18 +17,17 @@ struct PngQuant;
 std::vector<int> png_level_strategies(int level);
 
 struct PngDevice {
-    uint8_t *d_raw = nullptr, *d_raw2 = nullptr, *d_filt = nullptr, *d_temp = nullptr;
-    uint32_t *d_best = nullptr, *d_tok = nullptr, *d_out = nullptr, *d_counts = nullptr, *d_offsets = nullptr, *d_hist = nullptr, *d_tlog = nullptr;
-    unsigned long long *d_sums = nullptr;
-    uint8_t *h_small = nullptr, *h_raw = nullptr;
-    uint32_t *h_tok = nullptr;
-    size_t cap_raw = 0, cap_raw2 = 0, cap_filt = 0, cap_best = 0, cap_tok = 0, cap_out = 0, cap_counts = 0, cap_offsets = 0, cap_hist = 0, cap_sums = 0,
-           cap_tlog = 0, cap_temp = 0, cap_small = 0, cap_htok = 0, cap_hraw = 0;
-    uint8_t *d_fin = nullptr, *d_dfl = nullptr, *d_z = nullptr, *h_z = nullptr; uint32_t *d_sync = nullptr; unsigned long long *d_sums_in = nullptr;
-    size_t cap_fin = 0, cap_dfl = 0, cap_z = 0, cap_hz = 0, cap_sync = 0, cap_sums_in = 0, z_cap = 0;
+    DeviceBuffer<uint8_t> d_raw, d_raw2, d_filt, d_temp;
+    DeviceBuffer<uint32_t> d_best, d_tok, d_out, d_counts, d_offsets, d_hist, d_tlog;
+    DeviceBuffer<unsigned long long> d_sums;
+    PinnedBuffer<uint8_t> h_small, h_raw;
+    PinnedBuffer<uint32_t> h_tok;
+    DeviceBuffer<uint8_t> d_fin, d_dfl, d_z; PinnedBuffer<uint8_t> h_z; DeviceBuffer<uint32_t> d_sync; DeviceBuffer<unsigned long long> d_sums_in;
+    size_t z_cap = 0;
     bool corrupt = false;                                // the last failure was the INPUT's fault (bad filter byte, Adler-32 mismatch)
     size_t tlog_n = 0;
     double last_deflate_ms = 0;                          // host Huffman/bit-packing time of the last compress() (tracing)
+    PngDevice();
     ~PngDevice();
 
     // The lossless path: the caller inflates the IDAT stream into input_buffer() (pinned, `bytes` = height * (row_bytes + 1); the
@@ -42,7 +43,7 @@ struct PngDevice {
     // image with at most 256 distinct values is not quantised: it takes the lossless leg's exact palette reduction.
     bool code_quantized(PngInfo &info, int quality, int level, void *stream, std::vector<uint8_t> &zlib_stream, std::string &err);
     PngQuant *quantiser();
-    PngQuant *quant = nullptr;
+    std::unique_ptr<PngQuant> quant;
     bool from_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, int level, void *stream, std::vector<uint8_t> &zlib_stream, int *chosen_strategy, std::string &err, bool lossy);
     bool ensure_buffers(size_t nraw, size_t nmax, size_t rb, void *stream, std::string &err);
     bool reduce_and_code(PngInfo &info, bool probed, const uint32_t *h_flags, int level, void *stream, std::vector<uint8_t> &zlib_stream, int *chosen_strategy, std::string &err);
@@ -52,7 +53,7 @@ struct PngDevice {
     bool run_strategy(int strategy, int h, int rb, int bpp, void *stream, std::string &err, uint8_t *filt = nullptr, bool do_filter = true, bool with_hash = true);
     // K7 over a byte plane on the host (bpp 1, stride = width) -> compacted LZ77 tokens on the host
     bool plane_tokens(const uint8_t *plane, size_t n, int stride, void *stream, std::vector<uint32_t> &tokens, std::string &err);
-    uint8_t *d_filt_all = nullptr; size_t cap_filt_all = 0;          // the trials' filtered streams, one after another
+    DeviceBuffer<uint8_t> d_filt_all;                   // the trials' filtered streams, one after another
 };
 
 // allocate-run-free stage helpers behind b200_png_filter / b200_png_lz77 (current device)

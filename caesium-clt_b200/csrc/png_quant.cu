@@ -17,28 +17,13 @@
 
 namespace b200 {
 
-#define CUP(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return false; } } while (0)
-#define KCHECK(name) do { LT_MARK(name); cudaError_t e_ = cudaGetLastError(); if (e_ != cudaSuccess) { err = std::string(name) + ": " + cudaGetErrorString(e_); return false; } } while (0)
+#define KCHECK(name) do { LT_MARK(name); if (!launch_ok(cudaGetLastError(), name, err)) return false; } while (0)
 
 static const int kSmall = 32 * 1024;          // pinned readback buffer
 
-template <typename T> static bool grow(T *&p, size_t &cap, size_t need, std::string &err)
-{
-    if (need <= cap) return true;
-    cudaFree(p); p = nullptr; cap = 0;
-    size_t want = 1 << 16; while (want < need + need / 4) want <<= 1;
-    void *q = nullptr;
-    const cudaError_t e = cudaMalloc(&q, want);
-    if (e != cudaSuccess) { err = std::string("cudaMalloc: ") + cudaGetErrorString(e); return false; }
-    p = (T *)q; cap = want; return true;
-}
-
-PngQuant::~PngQuant()
-{
-    cudaFree(d_rgba); cudaFree(d_cells); cudaFree(d_coords); cudaFree(d_set); cudaFree(d_flags); cudaFree(d_sync); cudaFree(d_count); cudaFree(d_sums);
-    cudaFree(d_box); cudaFree(d_acc); cudaFree(d_keys); cudaFree(d_edge); cudaFree(d_label); cudaFree(d_cand); cudaFree(d_idx); cudaFree(d_lut);
-    cudaFree(d_ncand); cudaFree(d_temp); cudaFree(d_planes); cudaFreeHost(h_small);
-}
+// image-sized buffers: the smallest power of two >= 64 KiB and >= need + need / 4; the rest are allocated at their exact size
+template <class B> static bool grow(B &buf, size_t need, std::string &err) { return buf.reserve(need, Grow::Pow2Quarter, err); }
+template <class B> static bool fixed(B &buf, size_t bytes, std::string &err) { return buf.reserve(bytes, Grow::Exact, err); }
 
 // ---- kernels -------------------------------------------------------------------------------------------------------------------
 // any PNG colour type / bit depth -> RGBA8 (16 bits: the high byte; sub-byte grey scaled to 8 bits; palette and tRNS through lut;
@@ -322,8 +307,8 @@ bool PngQuant::load_host(const uint8_t *rgba, int width, int height, void *strea
 {
     w = width; h = height;
     const size_t n = (size_t)w * h * 4;
-    if (!grow(d_rgba, cap_rgba, n + 64, err)) return false;
-    CUP(cudaMemcpyAsync(d_rgba, rgba, n, cudaMemcpyHostToDevice, (cudaStream_t)stream));
+    if (!grow(d_rgba, n + 64, err)) return false;
+    CU(cudaMemcpyAsync(d_rgba, rgba, n, cudaMemcpyHostToDevice, (cudaStream_t)stream));
     return true;
 }
 
@@ -332,9 +317,9 @@ bool PngQuant::load_planes(const uint8_t *planes, int nc, const uint8_t *alpha, 
     cudaStream_t st = (cudaStream_t)stream;
     w = width; h = height;
     const size_t n = (size_t)w * h;
-    if (!grow(d_rgba, cap_rgba, n * 4 + 64, err) || !grow(d_planes, cap_planes, n * (nc + 1) + 64, err)) return false;
-    CUP(cudaMemcpyAsync(d_planes, planes, n * nc, cudaMemcpyHostToDevice, st));
-    if (alpha) CUP(cudaMemcpyAsync(d_planes + n * nc, alpha, n, cudaMemcpyHostToDevice, st));
+    if (!grow(d_rgba, n * 4 + 64, err) || !grow(d_planes, n * (nc + 1) + 64, err)) return false;
+    CU(cudaMemcpyAsync(d_planes, planes, n * nc, cudaMemcpyHostToDevice, st));
+    if (alpha) CU(cudaMemcpyAsync(d_planes + n * nc, alpha, n, cudaMemcpyHostToDevice, st));
     k_pq_planes<<<grid_for(n, 256), 256, 0, st>>>(d_planes, n, nc, alpha ? 1 : 0, d_rgba);
     KCHECK("k_pq_planes");
     return true;
@@ -345,25 +330,24 @@ bool PngQuant::expand(const uint8_t *d_raw, const PngInfo &info, void *stream_, 
     cudaStream_t st = (cudaStream_t)stream_;
     w = (int)info.width; h = (int)info.height;
     const size_t npix = (size_t)w * h;
-    if (!grow(d_rgba, cap_rgba, npix * 4 + 64, err)) return false;
-    if (!d_lut) CUP(cudaMalloc(&d_lut, 256 * 4));
-    if (!h_small) CUP(cudaHostAlloc(&h_small, kSmall, cudaHostAllocDefault));
+    if (!grow(d_rgba, npix * 4 + 64, err)) return false;
+    if (!fixed(d_lut, 256 * 4, err) || !fixed(h_small, kSmall, err)) return false;
     int has_key = 0, key[3] = {0, 0, 0};
     const int ct = info.color_type;
     if (ct == 3) {
-        uint32_t *lut = reinterpret_cast<uint32_t *>(h_small);
+        uint32_t *lut = reinterpret_cast<uint32_t *>(h_small.get());
         for (int i = 0; i < 256; i++) {
             uint32_t r = 0, g = 0, b = 0;
             if ((size_t)(3 * i + 2) < info.plte.size()) { r = info.plte[3 * i]; g = info.plte[3 * i + 1]; b = info.plte[3 * i + 2]; }
             const uint32_t a = (size_t)i < info.trns.size() ? info.trns[i] : 255;
             lut[i] = r | g << 8 | b << 16 | a << 24;
         }
-        CUP(cudaMemcpyAsync(d_lut, lut, 1024, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(d_lut, lut, 1024, cudaMemcpyHostToDevice, st));
     } else if (ct == 0 && info.trns.size() >= 2) { has_key = 1; key[0] = info.trns[0] << 8 | info.trns[1]; }
     else if (ct == 2 && info.trns.size() >= 6) { has_key = 1; for (int c = 0; c < 3; c++) key[c] = info.trns[2 * c] << 8 | info.trns[2 * c + 1]; }
     k_pq_expand<<<grid_for(npix, 256), 256, 0, st>>>(d_raw, info.row_bytes, w, h, ct, info.bit_depth, d_lut, has_key, key[0], key[1], key[2], d_rgba);
     KCHECK("k_pq_expand");
-    if (ct == 3) CUP(stream_wait(st));          // the lut staging buffer is reused by the next readback
+    if (ct == 3) CU(stream_wait(st));          // the lut staging buffer is reused by the next readback
     return true;
 }
 
@@ -371,31 +355,27 @@ bool PngQuant::prepare(void *stream_, std::string &err)
 {
     cudaStream_t st = (cudaStream_t)stream_;
     const size_t npix = (size_t)w * h;
-    if (!d_count) {
-        CUP(cudaMalloc(&d_count, (size_t)PQ_NCELLS * 8)); CUP(cudaMalloc(&d_sums, (size_t)PQ_NCELLS * 32)); CUP(cudaMalloc(&d_cells, (size_t)PQ_NCELLS * 4 + 64));
-        CUP(cudaMalloc(&d_label, PQ_NCELLS)); CUP(cudaMalloc(&d_box, 2 * PQ_BOX_WORDS * 8)); CUP(cudaMalloc(&d_acc, PQ_MAX_COLOURS * 5 * 8));
-        CUP(cudaMalloc(&d_coords, PQ_MAX_COLOURS * 4)); CUP(cudaMalloc(&d_keys, 256 * 8)); CUP(cudaMalloc(&d_set, 2048 * 4)); CUP(cudaMalloc(&d_flags, 64));
-        CUP(cudaMalloc(&d_cand, (size_t)PQ_GRID * 256)); CUP(cudaMalloc(&d_ncand, (size_t)PQ_GRID * 2));
-        if (!h_small) CUP(cudaHostAlloc(&h_small, kSmall, cudaHostAllocDefault));
-        size_t tb = 0;
-        cub::DeviceSelect::If(nullptr, tb, thrust::counting_iterator<uint32_t>(0), d_cells, d_flags, PQ_NCELLS, PqOccupied{d_count}, st);
-        if (!grow(d_temp, cap_temp, tb + 256, err)) return false;
-    }
-    if (!grow(d_idx, cap_idx, npix + 64, err)) return false;
-    CUP(cudaMemsetAsync(d_count, 0, (size_t)PQ_NCELLS * 8, st));
-    CUP(cudaMemsetAsync(d_sums, 0, (size_t)PQ_NCELLS * 32, st));
-    CUP(cudaMemsetAsync(d_flags, 0, 64, st));
+    if (!fixed(d_count, (size_t)PQ_NCELLS * 8, err) || !fixed(d_sums, (size_t)PQ_NCELLS * 32, err) || !fixed(d_cells, (size_t)PQ_NCELLS * 4 + 64, err) ||
+        !fixed(d_label, PQ_NCELLS, err) || !fixed(d_box, 2 * PQ_BOX_WORDS * 8, err) || !fixed(d_acc, PQ_MAX_COLOURS * 5 * 8, err) ||
+        !fixed(d_coords, PQ_MAX_COLOURS * 4, err) || !fixed(d_keys, 256 * 8, err) || !fixed(d_set, 2048 * 4, err) || !fixed(d_flags, 64, err) ||
+        !fixed(d_cand, (size_t)PQ_GRID * 256, err) || !fixed(d_ncand, (size_t)PQ_GRID * 2, err) || !fixed(h_small, kSmall, err)) return false;
+    size_t tb = 0;
+    cub::DeviceSelect::If(nullptr, tb, thrust::counting_iterator<uint32_t>(0), d_cells.get(), d_flags.get(), PQ_NCELLS, PqOccupied{d_count}, st);
+    if (!grow(d_temp, tb + 256, err) || !grow(d_idx, npix + 64, err)) return false;
+    CU(cudaMemsetAsync(d_count, 0, (size_t)PQ_NCELLS * 8, st));
+    CU(cudaMemsetAsync(d_sums, 0, (size_t)PQ_NCELLS * 32, st));
+    CU(cudaMemsetAsync(d_flags, 0, 64, st));
     k_pq_hist<<<grid_for(npix, 256), 256, 0, st>>>(d_rgba, npix, d_count, d_sums, d_flags + 8);
     KCHECK("k_pq_hist");
-    size_t tb = cap_temp;
-    cudaError_t e = cub::DeviceSelect::If(d_temp, tb, thrust::counting_iterator<uint32_t>(0), d_cells, d_flags, PQ_NCELLS, PqOccupied{d_count}, st);
+    tb = d_temp.capacity();
+    cudaError_t e = cub::DeviceSelect::If(d_temp, tb, thrust::counting_iterator<uint32_t>(0), d_cells.get(), d_flags.get(), PQ_NCELLS, PqOccupied{d_count}, st);
     if (e != cudaSuccess) { err = std::string("cub select: ") + cudaGetErrorString(e); return false; }
     LT_MARK("cub_select");
     // the distinct-value probe of the lossless leg over the RGBA samples (flags[2], saturating above 256)
-    if (launch_png_colours(reinterpret_cast<const uint8_t *>(d_rgba), npix, 4, d_set, d_flags + 4, st)) { err = "png colours launch failed"; return false; }
-    CUP(cudaMemcpyAsync(h_small, d_flags, 48, cudaMemcpyDeviceToHost, st));
-    CUP(stream_wait(st)); LT_MARK("host_wait");
-    const uint32_t *f = reinterpret_cast<const uint32_t *>(h_small);
+    if (launch_png_colours(reinterpret_cast<const uint8_t *>(d_rgba.get()), npix, 4, d_set, d_flags + 4, st)) { err = "png colours launch failed"; return false; }
+    CU(cudaMemcpyAsync(h_small, d_flags, 48, cudaMemcpyDeviceToHost, st));
+    CU(stream_wait(st)); LT_MARK("host_wait");
+    const uint32_t *f = reinterpret_cast<const uint32_t *>(h_small.get());
     ncells = (int)f[0]; distinct = (int)f[6]; clear = (int)f[8];
     last_cut_ms = 0;
     return true;
@@ -427,25 +407,25 @@ bool PngQuant::quantize(int quality, void *stream_, std::vector<uint32_t> &palet
     palette.clear();
     if (exact()) {
         // the distinct values from the probe's set (keys 1 << 32 | value), sorted by pq_exact_key
-        CUP(cudaMemcpyAsync(h_small, d_set, 1024 * 8, cudaMemcpyDeviceToHost, st));
-        CUP(stream_wait(st)); LT_MARK("host_wait");
-        const unsigned long long *set = reinterpret_cast<const unsigned long long *>(h_small);
+        CU(cudaMemcpyAsync(h_small, d_set, 1024 * 8, cudaMemcpyDeviceToHost, st));
+        CU(stream_wait(st)); LT_MARK("host_wait");
+        const unsigned long long *set = reinterpret_cast<const unsigned long long *>(h_small.get());
         std::vector<unsigned long long> keys;
         for (int i = 0; i < 1024; i++) if (set[i]) keys.push_back(pq_exact_key((uint32_t)set[i]));
         std::sort(keys.begin(), keys.end());
         for (unsigned long long k : keys) palette.push_back((uint32_t)k);
-        CUP(cudaMemcpyAsync(d_keys, keys.data(), keys.size() * 8, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(d_keys, keys.data(), keys.size() * 8, cudaMemcpyHostToDevice, st));
         k_pq_exact<<<grid_for(npix, 256), 256, 0, st>>>(d_rgba, npix, d_keys, (int)keys.size(), d_idx);
         KCHECK("k_pq_exact");
         return true;
     }
     if (!ncells) {              // every pixel fully transparent: the reserved entry alone
         palette.assign(1, 0u);
-        CUP(cudaMemsetAsync(d_idx, 0, npix, st));
+        CU(cudaMemsetAsync(d_idx, 0, npix, st));
         return true;
     }
     const auto t0 = std::chrono::steady_clock::now();
-    CUP(cudaMemsetAsync(d_label, 0, (size_t)ncells, st));
+    CU(cudaMemsetAsync(d_label, 0, (size_t)ncells, st));
     SplitCtx ctx{this, st, &err};
     std::vector<PqBox> boxes(PQ_MAX_COLOURS);
     const int nb = pq_median_cut(&ctx, split_cb, quality, PQ_MAX_COLOURS - clear, boxes.data());
@@ -453,18 +433,18 @@ bool PngQuant::quantize(int quality, void *stream_, std::vector<uint32_t> &palet
     last_cut_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     // box means, then the refinement passes
     uint32_t ent[PQ_MAX_COLOURS], coords[PQ_MAX_COLOURS];
-    unsigned long long *acc = reinterpret_cast<unsigned long long *>(h_small);
+    unsigned long long *acc = reinterpret_cast<unsigned long long *>(h_small.get());
     int n = nb;
     for (int pass = 0; pass <= PQ_REFINE_PASSES; pass++) {
         if (pass) {
             for (int k = 0; k < n; k++) coords[k] = pq_entry_coords(ent[k]);
-            CUP(cudaMemcpyAsync(d_coords, coords, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+            CU(cudaMemcpyAsync(d_coords, coords, (size_t)n * 4, cudaMemcpyHostToDevice, st));
         }
-        CUP(cudaMemsetAsync(d_acc, 0, PQ_MAX_COLOURS * 5 * 8, st));
-        k_pq_accum<<<grid_for((size_t)ncells, 256), 256, 0, st>>>(d_cells, ncells, d_count, d_sums, d_label, pass ? d_coords : nullptr, n, d_acc);
+        CU(cudaMemsetAsync(d_acc, 0, PQ_MAX_COLOURS * 5 * 8, st));
+        k_pq_accum<<<grid_for((size_t)ncells, 256), 256, 0, st>>>(d_cells, ncells, d_count, d_sums, d_label, pass ? d_coords.get() : nullptr, n, d_acc);
         KCHECK(pass ? "k_pq_refine" : "k_pq_box_means");
-        CUP(cudaMemcpyAsync(acc, d_acc, (size_t)n * 5 * 8, cudaMemcpyDeviceToHost, st));
-        CUP(stream_wait(st)); LT_MARK("host_wait");
+        CU(cudaMemcpyAsync(acc, d_acc, (size_t)n * 5 * 8, cudaMemcpyDeviceToHost, st));
+        CU(stream_wait(st)); LT_MARK("host_wait");
         n = pq_entries_from_sums(acc, n, ent);
     }
     pq_order(ent, n);
@@ -472,12 +452,12 @@ bool PngQuant::quantize(int quality, void *stream_, std::vector<uint32_t> &palet
     for (int k = 0; k < n; k++) coords[k] = pq_entry_coords(ent[k]);
     palette.assign((size_t)clear, 0u);
     palette.insert(palette.end(), ent, ent + n);
-    CUP(cudaMemcpyAsync(d_coords, coords, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(d_coords, coords, (size_t)n * 4, cudaMemcpyHostToDevice, st));
     k_pq_cands<<<PQ_GRID, 256, 0, st>>>(d_coords, n, d_cand, d_ncand);
     KCHECK("k_pq_cands");
     const int groups = (h + 31) / 32;
-    if (!grow(d_edge, cap_edge, (size_t)groups * w * 8 + 64, err) || !grow(d_sync, cap_sync, (size_t)(groups + 2) * 4, err)) return false;
-    CUP(cudaMemsetAsync(d_sync, 0, (size_t)(groups + 2) * 4, st));
+    if (!grow(d_edge, (size_t)groups * w * 8 + 64, err) || !grow(d_sync, (size_t)(groups + 2) * 4, err)) return false;
+    CU(cudaMemsetAsync(d_sync, 0, (size_t)(groups + 2) * 4, st));
     k_pq_dither<<<groups, 32, 0, st>>>(d_rgba, w, h, d_coords, n, d_cand, d_ncand, clear, d_idx, d_edge, d_sync, d_sync + 2);
     KCHECK("k_pq_dither");
     return true;
@@ -485,16 +465,16 @@ bool PngQuant::quantize(int quality, void *stream_, std::vector<uint32_t> &palet
 
 bool PngQuant::fetch_indices(uint8_t *idx, void *stream, std::string &err)
 {
-    CUP(cudaMemcpyAsync(idx, d_idx, (size_t)w * h, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-    CUP(stream_wait((cudaStream_t)stream));
+    CU(cudaMemcpyAsync(idx, d_idx, (size_t)w * h, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+    CU(stream_wait((cudaStream_t)stream));
     return true;
 }
 
 bool PngQuant::fetch_rgba(std::vector<uint8_t> &rgba, void *stream, std::string &err)
 {
     rgba.resize((size_t)w * h * 4);
-    CUP(cudaMemcpyAsync(rgba.data(), d_rgba, rgba.size(), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
-    CUP(stream_wait((cudaStream_t)stream));
+    CU(cudaMemcpyAsync(rgba.data(), d_rgba, rgba.size(), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+    CU(stream_wait((cudaStream_t)stream));
     return true;
 }
 

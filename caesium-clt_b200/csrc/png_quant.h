@@ -4,6 +4,7 @@
 #include <cstddef>
 #include <string>
 #include <vector>
+#include "dev_buffer.h"
 #include "png_host.h"
 
 namespace b200 {
@@ -12,18 +13,18 @@ namespace b200 {
 // cells, distinct-value count: independent of the quality), then quantize at any number of qualities.  Buffers are high-water
 // allocations kept between calls.
 struct PngQuant {
-    uint32_t *d_rgba = nullptr, *d_cells = nullptr, *d_coords = nullptr, *d_set = nullptr, *d_flags = nullptr, *d_sync = nullptr;
-    unsigned long long *d_count = nullptr, *d_sums = nullptr, *d_box = nullptr, *d_acc = nullptr, *d_keys = nullptr;
-    unsigned long long *d_edge = nullptr;     // dithering: the last row of each 32-row group, four int16 errors per pixel
-    uint8_t *d_label = nullptr, *d_cand = nullptr, *d_idx = nullptr, *h_small = nullptr;
-    uint32_t *d_lut = nullptr;
-    uint8_t *d_planes = nullptr; size_t cap_planes = 0;
-    uint16_t *d_ncand = nullptr;
-    void *d_temp = nullptr;
-    size_t cap_rgba = 0, cap_idx = 0, cap_edge = 0, cap_sync = 0, cap_temp = 0;
+    // growable, image-sized
+    DeviceBuffer<uint32_t> d_rgba, d_sync;
+    DeviceBuffer<unsigned long long> d_edge;     // dithering: the last row of each 32-row group, four int16 errors per pixel
+    DeviceBuffer<uint8_t> d_idx, d_planes, d_temp;
+    // fixed-size
+    DeviceBuffer<uint32_t> d_cells, d_coords, d_set, d_flags, d_lut;
+    DeviceBuffer<unsigned long long> d_count, d_sums, d_box, d_acc, d_keys;
+    DeviceBuffer<uint8_t> d_label, d_cand;
+    DeviceBuffer<uint16_t> d_ncand;
+    PinnedBuffer<uint8_t> h_small;
     int w = 0, h = 0, ncells = 0, distinct = 0, clear = 0;     // clear: some pixel is fully transparent (palette entry 0 reserved)
     double last_cut_ms = 0;                   // host-driven median cut of the last quantize() (tracing)
-    ~PngQuant();
 
     bool load_host(const uint8_t *rgba, int width, int height, void *stream, std::string &err);
     // host planes [nc][h][w] (nc = 1 grey or 3 RGB) and an optional alpha plane, interleaved to RGBA8 on the device

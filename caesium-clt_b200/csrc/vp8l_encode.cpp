@@ -16,24 +16,8 @@
 
 namespace b200 {
 
-#define CUV(expr) do { cudaError_t e_ = (expr); if (e_ != cudaSuccess) { err = std::string(#expr) + ": " + cudaGetErrorString(e_); return false; } } while (0)
-
-template <typename T> static bool grow(T *&p, size_t &cap, size_t need, bool host, std::string &err)
-{
-    if (need <= cap) return true;
-    if (p) { if (host) cudaFreeHost(p); else cudaFree(p); }
-    p = nullptr; cap = 0;
-    size_t want = 1 << 16; while (want < need) want <<= 1;
-    void *q = nullptr;
-    const cudaError_t e = host ? cudaHostAlloc(&q, want, cudaHostAllocDefault) : cudaMalloc(&q, want);
-    if (e != cudaSuccess) { err = std::string(host ? "cudaHostAlloc: " : "cudaMalloc: ") + cudaGetErrorString(e); return false; }
-    p = (T *)q; cap = want; return true;
-}
-
-Vp8lDevice::~Vp8lDevice()
-{
-    cudaFree(d_arena); cudaFree(d_words); cudaFreeHost(h_in); cudaFreeHost(h_small); cudaFreeHost(h_codes); cudaFreeHost(h_words);
-}
+// the smallest power of two >= 64 KiB and >= need
+template <class B> static bool grow(B &buf, size_t need, std::string &err) { return buf.reserve(need, Grow::Pow2, err); }
 
 namespace {
 
@@ -73,23 +57,23 @@ bool Vp8lDevice::encode(const uint8_t *rgb, const uint8_t *alpha, int w, int h, 
     Vp8lBuffers B;
     const size_t arena = carve(nullptr, n, nchunks, tiles, B);
     const size_t hist_bytes = sizeof(uint32_t) * VP8L_NCACHE * VP8L_HIST, small = hist_bytes + 16 + (size_t)tiles;
-    if (!grow(d_arena, cap_arena, arena, false, err) || !grow(h_in, cap_hin, 4 * n, true, err) || !grow(h_small, cap_hsmall, small, true, err) ||
-        !grow(h_codes, cap_hcodes, sizeof(Vp8lCodes), true, err)) return false;
+    if (!grow(d_arena, arena, err) || !grow(h_in, 4 * n, err) || !grow(h_small, small, err) ||
+        !grow(h_codes, sizeof(Vp8lCodes), err)) return false;
     carve(d_arena, n, nchunks, tiles, B);
     // ---- analysis: everything that decides the bitstream, for every cache candidate at once
     memcpy(h_in, rgb, 3 * n);
     if (alpha) memcpy(h_in + 3 * n, alpha, n);
-    CUV(cudaMemcpyAsync(B.planes, h_in, (alpha ? 4 : 3) * n, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(B.planes, h_in, (alpha ? 4 : 3) * n, cudaMemcpyHostToDevice, st));
     int rc = launch_vp8l_analyse(B, w, h, alpha ? 1 : 0, st);
-    if (rc) { err = std::string("vp8l kernels: ") + cudaGetErrorString((cudaError_t)rc); return false; }
-    uint32_t *h_hist = (uint32_t *)h_small, *h_flags = (uint32_t *)(h_small + hist_bytes);
+    if (!launch_ok(rc, "vp8l kernels", err)) return false;
+    uint32_t *h_hist = (uint32_t *)h_small.get(), *h_flags = (uint32_t *)(h_small + hist_bytes);
     unsigned long long *h_total = (unsigned long long *)(h_small + hist_bytes + 8);
     uint8_t *h_modes = h_small + hist_bytes + 16;
-    CUV(cudaMemcpyAsync(h_hist, B.hist, hist_bytes, cudaMemcpyDeviceToHost, st));
-    CUV(cudaMemcpyAsync(h_flags, B.flags, 4, cudaMemcpyDeviceToHost, st));
-    CUV(cudaMemcpyAsync(h_modes, B.modes, (size_t)tiles, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(h_hist, B.hist, hist_bytes, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(h_flags, B.flags, 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(h_modes, B.modes, (size_t)tiles, cudaMemcpyDeviceToHost, st));
     const auto t0 = std::chrono::steady_clock::now();
-    CUV(stream_wait(st));
+    CU(stream_wait(st));
     const auto t1 = std::chrono::steady_clock::now();
     last_analyse_ms = std::chrono::duration<double, std::milli>(t1 - t0).count();
     // ---- cache size and codes
@@ -124,23 +108,23 @@ bool Vp8lDevice::encode(const uint8_t *rgb, const uint8_t *alpha, int w, int h, 
     const unsigned long long bit_base = bw.bits();
     bw.flush();
     // ---- the codes go up, the tokens are sized and emitted
-    Vp8lCodes *C = (Vp8lCodes *)h_codes;
+    Vp8lCodes *C = (Vp8lCodes *)h_codes.get();
     memset(C, 0, sizeof(Vp8lCodes));
     for (int k = 0; k < 5; k++)
         if (pc[k].used > 1) for (int s = 0; s < size[k]; s++) { C->code[base[k] + s] = pc[k].code[s]; C->len[base[k] + s] = pc[k].len[s]; }
-    CUV(cudaMemcpyAsync(B.codes, C, sizeof(Vp8lCodes), cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(B.codes, C, sizeof(Vp8lCodes), cudaMemcpyHostToDevice, st));
     rc = launch_vp8l_size(B, w, h, cand, bit_base, st);
-    if (rc) { err = std::string("vp8l kernels: ") + cudaGetErrorString((cudaError_t)rc); return false; }
-    CUV(cudaMemcpyAsync(h_total, B.total, 8, cudaMemcpyDeviceToHost, st));
-    CUV(stream_wait(st));
+    if (!launch_ok(rc, "vp8l kernels", err)) return false;
+    CU(cudaMemcpyAsync(h_total, B.total, 8, cudaMemcpyDeviceToHost, st));
+    CU(stream_wait(st));
     const unsigned long long total = *h_total;
     const size_t words = (size_t)((total + 31) / 32), nbytes = (size_t)((total + 7) / 8);
-    if (!grow(d_words, cap_words, words * 4, false, err) || !grow(h_words, cap_hwords, words * 4, true, err)) return false;
+    if (!grow(d_words, words * 4, err) || !grow(h_words, words * 4, err)) return false;
     B.words = d_words;
     rc = launch_vp8l_emit(B, w, h, cand, words, st);
-    if (rc) { err = std::string("vp8l kernels: ") + cudaGetErrorString((cudaError_t)rc); return false; }
-    CUV(cudaMemcpyAsync(h_words, d_words, words * 4, cudaMemcpyDeviceToHost, st));
-    CUV(stream_wait(st));
+    if (!launch_ok(rc, "vp8l kernels", err)) return false;
+    CU(cudaMemcpyAsync(h_words, d_words, words * 4, cudaMemcpyDeviceToHost, st));
+    CU(stream_wait(st));
     // ---- the header bits go into the first bytes, then the RIFF framing
     uint8_t *payload = h_words;
     for (size_t i = 0; i < hdr.size(); i++) payload[i] |= hdr[i];

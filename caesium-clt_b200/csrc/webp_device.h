@@ -4,6 +4,7 @@
 #include <cstddef>
 #include <string>
 #include <vector>
+#include "dev_buffer.h"
 
 namespace b200 {
 
@@ -11,19 +12,18 @@ namespace b200 {
 unsigned long long webp_d2h_bytes_total();
 
 struct WebpDevice {
-    uint8_t *d_planes = nullptr; size_t cap_planes = 0;        // Y,U,V source + RY,RU,RV reconstruction, macroblock-padded
-    uint8_t *d_rgb = nullptr; size_t cap_rgb = 0;              // staging for callers whose RGB starts on the host
-    int16_t *d_levels = nullptr; size_t cap_levels = 0;
-    uint8_t *d_modes = nullptr; size_t cap_modes = 0;
-    int *d_progress = nullptr; size_t cap_progress = 0;
-    uint8_t *h_out = nullptr; size_t cap_hout = 0;             // pinned: levels | modes
-    uint8_t *h_rgb = nullptr; size_t cap_hrgb = 0;             // pinned staging for host RGB
-    uint32_t *d_tokwork = nullptr; size_t cap_tokwork = 0;     // mask | counts | offsets | tallies
-    void *d_toktemp = nullptr; size_t cap_toktemp = 0;         // scan scratch
-    uint16_t *d_tokens = nullptr; size_t cap_tokens = 0;       // the frame's decision records
-    uint8_t *h_tokens = nullptr; size_t cap_htokens = 0;       // pinned: records
+    DeviceBuffer<uint8_t> d_planes;         // Y,U,V source + RY,RU,RV reconstruction, macroblock-padded
+    DeviceBuffer<uint8_t> d_rgb;            // staging for callers whose RGB starts on the host
+    DeviceBuffer<int16_t> d_levels;
+    DeviceBuffer<uint8_t> d_modes;
+    DeviceBuffer<int> d_progress;
+    PinnedBuffer<uint8_t> h_out;            // levels | modes
+    PinnedBuffer<uint8_t> h_rgb;            // staging for host RGB
+    DeviceBuffer<uint32_t> d_tokwork;       // mask | counts | offsets | tallies
+    DeviceBuffer<uint8_t> d_toktemp;        // scan scratch
+    DeviceBuffer<uint16_t> d_tokens;        // the frame's decision records
+    PinnedBuffer<uint8_t> h_tokens;         // records
     double last_wait_ms = 0, last_code_ms = 0;                 // tracing: wait for the kernels + D2H, host boolean coder of the last encode
-    ~WebpDevice();
     // d_r/d_g/d_b: device planes (pitch w).  Produces the .webp file; optionally also hands back the levels/modes (tests).
     bool encode_planes(const uint8_t *d_r, const uint8_t *d_g, const uint8_t *d_b, int w, int h, int quality, void *stream,
                        std::vector<uint8_t> &out, std::string &err, int16_t *levels_out = nullptr, uint8_t *modes_out = nullptr);
