@@ -67,7 +67,7 @@ _SYMBOLS = [
     "b200_png_decode", "b200_png_decode_reduced", "b200_png_filter", "b200_png_lz77", "b200_png_deflate_tokens", "b200_png_level_strategies",
     "b200_webp_encode_rgb", "b200_webp_write_levels", "b200_webp_qindex",
     "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_jpeg_pipe_destroy", "b200_device_jobs", "b200_device_numa_node", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba", "b200_webp_alpha_filter", "b200_webp_d2h_bytes",
-    "b200_set_png_lossy", "b200_png_quantize", "b200_set_jpeg_trellis",
+    "b200_set_png_lossy", "b200_png_quantize", "b200_set_jpeg_trellis", "b200_set_gif", "b200_gif_decode", "b200_gif_lzw",
 ]
 
 
@@ -84,7 +84,8 @@ def lib():
                   "b200_jpeg_encode_coefficients", "b200_jpeg_decode_planes",
                   "b200_png_decode", "b200_png_decode_reduced", "b200_png_filter", "b200_png_lz77", "b200_png_deflate_tokens",
                   "b200_webp_encode_rgb", "b200_webp_write_levels", "b200_jpeg_encode_coefficients_device",
-                  "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba", "b200_png_quantize"):
+                  "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba", "b200_png_quantize",
+                  "b200_gif_decode", "b200_gif_lzw"):
             getattr(L, f).restype = Status
         L.b200_webp_d2h_bytes.restype = C.c_ulonglong
         L.b200_version.restype = C.c_char_p
@@ -249,6 +250,32 @@ def png_quantize(rgba, quality):
     _check(lib().b200_png_quantize(rgba.ctypes.data_as(C.c_void_p), w, h, int(quality), pal.ctypes.data_as(C.c_void_p), C.byref(n),
                                    idx.ctypes.data_as(C.c_void_p)))
     return pal[:n.value].copy(), idx
+
+
+def set_gif(on):
+    """b200_set_gif: GIF sources re-encoded on the device (True) or refused with code 3 (False, the default)."""
+    return lib().b200_set_gif(int(bool(on)))
+
+
+def gif_decode(data):
+    """b200_gif_decode (host): -> (canvases uint8 [n, h, w, 4], delays list, loop or None)."""
+    w, h, n, loop = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+    px, dl = C.POINTER(C.c_uint8)(), C.POINTER(C.c_int)()
+    _check(lib().b200_gif_decode(data, C.c_size_t(len(data)), C.byref(w), C.byref(h), C.byref(n), C.byref(loop), C.byref(px), C.byref(dl)))
+    size = n.value * h.value * w.value * 4
+    canv = np.frombuffer(C.string_at(px, size), np.uint8).reshape(n.value, h.value, w.value, 4).copy()
+    delays = list(np.frombuffer(C.string_at(dl, 4 * n.value), np.int32))
+    lib().b200_free(px)
+    lib().b200_free(dl)
+    return canv, [int(x) for x in delays], (None if loop.value < 0 else loop.value)
+
+
+def gif_lzw(indices, min_code_size):
+    """b200_gif_lzw (device): indices uint8 [n] -> GIF image data as sub-blocks with the terminator."""
+    idx = np.ascontiguousarray(indices, dtype=np.uint8).reshape(-1)
+    outp, outl = C.c_void_p(), C.c_size_t()
+    _check(lib().b200_gif_lzw(idx.ctypes.data_as(C.c_void_p), C.c_size_t(idx.size), int(min_code_size), C.byref(outp), C.byref(outl)))
+    return _take(outp, outl)
 
 
 def jpeg_decode_planes(in_layout, in_coefs):

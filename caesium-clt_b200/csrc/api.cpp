@@ -4,6 +4,7 @@
 #include "../../include/b200_caesium.h"
 #include "../../include/b200_caesium_png_lossy.h"
 #include "../../include/b200_caesium_jpeg_trellis.h"
+#include "../../include/b200_caesium_gif.h"
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -32,6 +33,8 @@
 #include "vp8l_device.h"
 #include "vp8_decode.h"
 #include "vp8l_alpha.h"
+#include "gif_host.h"
+#include "gif_device.h"
 #include "jpeg_pipe.h"
 #include "topology.h"
 #include "launch_timer.h"
@@ -56,6 +59,7 @@ b200_status header_status(const std::string &err) { return make_status(err.compa
 int g_forced_device = -1, g_forced_ngpus = 0;
 std::atomic<int> g_entropy_mode{-1};     // -1 unset (env B200_ENTROPY); bit 0 = device entropy encoder, bit 1 = device entropy decoder (default 3)
 std::atomic<int> g_png_lossy{-1};        // -1 unset (env B200_PNG_LOSSY); 1 = lossy PNG on the device's quantiser, 0 = refused (code 3)
+std::atomic<int> g_gif{-1};              // -1 unset (env B200_GIF); 1 = GIF re-encoded on the device, 0 = refused (code 3)
 
 // runtime_init is idempotent while initialised, so after b200_shutdown (which frees every slot's device buffers) the next call
 // initialises again: a long-running host can hand the memory of one workload's slots back before starting another
@@ -86,6 +90,16 @@ bool png_lossy()
         g_png_lossy.store(e && !strcmp(e, "gpu") ? 1 : 0);
     }
     return g_png_lossy.load() == 1;
+}
+
+// GIF sources on the device: b200_set_gif, else B200_GIF=gpu, read once; off by default
+bool gif_on()
+{
+    if (g_gif.load() < 0) {
+        const char *e = getenv("B200_GIF");
+        g_gif.store(e && !strcmp(e, "gpu") ? 1 : 0);
+    }
+    return g_gif.load() == 1;
 }
 
 // One slot of one device (prefer_dev < 0: the next device round-robin), held until the lease goes out of scope.  The runtime
@@ -848,13 +862,38 @@ b200_status convert_dispatch(const uint8_t *in, size_t in_len, uint32_t src, uin
     return make_status(B200_ERR_UNSUPPORTED, "conversion from this format is outside the GPU path (route to caesium::convert_in_memory)");
 }
 
+// GIF (the switch on): decoded frame by frame on the calling thread, every composited canvas re-encoded on the device (palette
+// quantiser at gif_quality, segmented LZW); the container is written here.  B200_TRACE=2 prints host decode against device time.
+b200_status gif_compress(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
+{
+    if (!gif_on()) return make_status(B200_ERR_UNSUPPORTED, "GIF is outside the GPU path (route to caesium::compress_in_memory)");
+    if (p->width || p->height) return make_status(B200_ERR_UNSUPPORTED, "GIF resize is outside the GPU path (route to caesium::compress_in_memory)");
+    static const bool verbose = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2;
+    std::string err;
+    GifReader rd;
+    if (!rd.open(in, in_len, err)) return make_status(rd.unsupported ? B200_ERR_UNSUPPORTED : B200_ERR_CORRUPT_INPUT, err);
+    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
+    SlotLease s(prefer_dev);
+    if (!s) return s.failure();
+    const auto t0 = std::chrono::steady_clock::now();
+    bool corrupt = false;
+    const int q = (int)std::min<uint32_t>(p->gif_quality, 100);
+    if (!s->gif_dev()->encode(rd, *s->png_dev()->quantiser(), q, s->stream, out, corrupt, err)) return make_status(corrupt ? B200_ERR_CORRUPT_INPUT : B200_ERR_CUDA, err);
+    if (verbose) {
+        const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+        fprintf(stderr, "[b200 trace] gif %dx%d, %d frames q%d: host decode %.1f ms, device and container %.1f ms\n", rd.width, rd.height, rd.frames, q,
+                s->gif_dev()->decode_ms, ms - s->gif_dev()->decode_ms);
+    }
+    return ok_status();
+}
+
 b200_status compress_dispatch(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
 {
     switch (b200_sniff_format(in, in_len)) {
         case B200_FMT_JPEG: return jpeg_compress(in, in_len, p, prefer_dev, out);
         case B200_FMT_PNG: return png_compress(in, in_len, p, prefer_dev, out);
         case B200_FMT_WEBP: return webp_compress(in, in_len, p, prefer_dev, out);
-        case B200_FMT_GIF: return make_status(B200_ERR_UNSUPPORTED, "GIF is outside the GPU path (route to caesium::compress_in_memory)");
+        case B200_FMT_GIF: return gif_compress(in, in_len, p, prefer_dev, out);
         case B200_FMT_TIFF: return make_status(B200_ERR_UNSUPPORTED, "TIFF is outside the GPU path (route to caesium::compress_in_memory)");
         default: return make_status(B200_ERR_UNKNOWN_FORMAT, "Unknown file type");
     }
@@ -955,6 +994,7 @@ const char *b200_version(void) { return "b200-caesium 0.1.0 (sm_90a)"; }
 void b200_free(void *p) { free(p); }
 int b200_set_entropy_mode(int mode) { if (mode < 0 || mode > 3) return B200_ERR_INVALID_ARGUMENT; g_entropy_mode.store(mode); return B200_OK; }
 int b200_set_png_lossy(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_png_lossy.store(on); return B200_OK; }
+int b200_set_gif(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_gif.store(on); return B200_OK; }
 int b200_set_jpeg_trellis(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; set_jpeg_trellis(on == 1); return B200_OK; }
 
 uint32_t b200_sniff_format(const uint8_t *d, size_t n)
@@ -1562,6 +1602,50 @@ b200_status b200_png_quantize(const uint8_t *rgba, int width, int height, int qu
         for (size_t k = 0; k < pal.size(); k++) for (int c = 0; c < 4; c++) palette_rgba[4 * k + c] = (uint8_t)(pal[k] >> (8 * c));
         *npalette = (int)pal.size();
         return ok_status();
+    });
+}
+
+b200_status b200_gif_decode(const uint8_t *in, size_t in_len, int *width, int *height, int *nframes, int *loop, uint8_t **rgba, int **delays)
+{
+    if (!in || !width || !height || !nframes || !loop || !rgba || !delays) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
+    *rgba = nullptr; *delays = nullptr;
+    return guarded([&] {
+        std::string err;
+        GifReader rd;
+        if (!rd.open(in, in_len, err)) return make_status(rd.unsupported ? B200_ERR_UNSUPPORTED : B200_ERR_CORRUPT_INPUT, err);
+        const size_t npix = (size_t)rd.width * rd.height;
+        std::vector<uint32_t> px(npix * (size_t)rd.frames);
+        std::vector<int> dl((size_t)rd.frames);
+        for (int f = 0; f < rd.frames; f++)
+            if (!rd.next(px.data() + npix * f, dl[(size_t)f], err)) return make_status(B200_ERR_CORRUPT_INPUT, err.empty() ? "GIF frame missing" : err);
+        size_t n = 0;
+        std::vector<uint8_t> bytes(px.size() * 4);
+        memcpy(bytes.data(), px.data(), bytes.size());
+        b200_status s = give(dl, delays, &n);
+        if (s.code) return s;
+        s = give(bytes, rgba, &n);
+        if (s.code) { free(*delays); *delays = nullptr; return s; }
+        *width = rd.width; *height = rd.height; *nframes = rd.frames; *loop = rd.loop;
+        return s;
+    });
+}
+
+b200_status b200_gif_lzw(const uint8_t *indices, size_t n, int min_code_size, uint8_t **out, size_t *out_len)
+{
+    if (!indices || !out || !out_len || min_code_size < 2 || min_code_size > 8) return make_status(B200_ERR_INVALID_ARGUMENT, "invalid argument");
+    *out = nullptr; *out_len = 0;
+    for (size_t i = 0; i < n; i++) if (indices[i] >> min_code_size) return make_status(B200_ERR_INVALID_ARGUMENT, "index not below 2^min_code_size");
+    std::string err;
+    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
+    return guarded([&] {
+        SlotLease s(-1);
+        if (!s) return s.failure();
+        DeviceBuffer<uint8_t> d_idx;
+        std::vector<uint8_t> v;
+        if (!d_idx.reserve(n + 1, Grow::Exact, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+        if (cudaMemcpyAsync(d_idx, indices, n, cudaMemcpyHostToDevice, (cudaStream_t)s->stream) != cudaSuccess || !s->gif_dev()->lzw(d_idx, n, min_code_size, s->stream, v, err))
+            return make_status(B200_ERR_CUDA, err.empty() ? "upload failed" : err);
+        return give(v, out, out_len);
     });
 }
 

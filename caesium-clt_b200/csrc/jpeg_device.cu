@@ -20,6 +20,7 @@
 #include "png_device.h"
 #include "webp_device.h"
 #include "vp8l_device.h"
+#include "gif_device.h"
 #include "stream_wait.h"
 #include "launch_timer.h"
 
@@ -208,6 +209,7 @@ GpuDecoder *Slot::decoder() { if (!dec) dec.reset(new GpuDecoder()); return dec.
 PngDevice *Slot::png_dev() { if (!png) png.reset(new PngDevice()); return png.get(); }
 WebpDevice *Slot::webp_dev() { if (!webp) webp.reset(new WebpDevice()); return webp.get(); }
 Vp8lDevice *Slot::vp8l_dev() { if (!vp8l) vp8l.reset(new Vp8lDevice()); return vp8l.get(); }
+GifDevice *Slot::gif_dev() { if (!gif) gif.reset(new GifDevice()); return gif.get(); }
 
 int runtime_device_count() { std::lock_guard<std::mutex> lk(g_mu); return g_inited ? (int)g_devs.size() : 0; }
 long long runtime_device_jobs(int i) { return g_devs.empty() || i < 0 || i >= (int)g_devs.size() ? 0 : g_devs[(size_t)i]->jobs.load(); }

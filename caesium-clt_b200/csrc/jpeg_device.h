@@ -54,6 +54,7 @@ void set_jpeg_trellis(bool on);
 struct PngDevice;
 struct WebpDevice;
 struct Vp8lDevice;
+struct GifDevice;
 struct Slot {
     int dev = 0;
     void *stream = nullptr;
@@ -67,6 +68,7 @@ struct Slot {
     std::unique_ptr<PngDevice> png;                                                      // lossless PNG state (lazy, png_device.cu)
     std::unique_ptr<WebpDevice> webp;                                                    // WebP / VP8 state (lazy, webp_device.cu)
     std::unique_ptr<Vp8lDevice> vp8l;                                                    // lossless WebP / VP8L state (lazy, vp8l_encode.cpp)
+    std::unique_ptr<GifDevice> gif;                                                      // GIF state (lazy, gif_device.cu)
     // megabatch path: transform work lists of the current megabatch, and the captured launch sequence (two CUDA graphs, see
     // slot_run_group) with the signature it was captured for
     WorkLists group_wl; size_t group_par_bytes = 0, group_work_off = 0;
@@ -79,6 +81,7 @@ struct Slot {
     PngDevice *png_dev();
     WebpDevice *webp_dev();
     Vp8lDevice *vp8l_dev();
+    GifDevice *gif_dev();
     Slot();
     Slot(const Slot &) = delete;
     Slot &operator=(const Slot &) = delete;

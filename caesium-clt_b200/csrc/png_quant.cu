@@ -312,6 +312,12 @@ bool PngQuant::load_host(const uint8_t *rgba, int width, int height, void *strea
     return true;
 }
 
+uint32_t *PngQuant::rgba_for(int width, int height, std::string &err)
+{
+    w = width; h = height;
+    return grow(d_rgba, (size_t)w * h * 4 + 64, err) ? d_rgba.get() : nullptr;
+}
+
 bool PngQuant::load_planes(const uint8_t *planes, int nc, const uint8_t *alpha, int width, int height, void *stream, std::string &err)
 {
     cudaStream_t st = (cudaStream_t)stream;
@@ -400,12 +406,12 @@ int split_cb(void *ctx_, int b, int axis, int t, int k, PqBox *sb, PqBox *sk)
 }
 } // namespace
 
-bool PngQuant::quantize(int quality, void *stream_, std::vector<uint32_t> &palette, std::string &err)
+bool PngQuant::quantize(int quality, void *stream_, std::vector<uint32_t> &palette, std::string &err, bool allow_exact)
 {
     cudaStream_t st = (cudaStream_t)stream_;
     const size_t npix = (size_t)w * h;
     palette.clear();
-    if (exact()) {
+    if (allow_exact && exact()) {
         // the distinct values from the probe's set (keys 1 << 32 | value), sorted by pq_exact_key
         CU(cudaMemcpyAsync(h_small, d_set, 1024 * 8, cudaMemcpyDeviceToHost, st));
         CU(stream_wait(st)); LT_MARK("host_wait");

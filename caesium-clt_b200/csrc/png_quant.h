@@ -31,10 +31,13 @@ struct PngQuant {
     bool load_planes(const uint8_t *planes, int nc, const uint8_t *alpha, int width, int height, void *stream, std::string &err);
     // d_raw: height * row_bytes un-filtered samples of any PNG colour type / depth (16 bits: high byte; tRNS / palette expanded)
     bool expand(const uint8_t *d_raw, const PngInfo &info, void *stream, std::string &err);
+    // room for a width x height RGBA8 image written in place by the caller's kernels (d_rgba), or null with err
+    uint32_t *rgba_for(int width, int height, std::string &err);
     bool prepare(void *stream, std::string &err);
     bool exact() const { return distinct <= 256; }
-    // palette (RGBA words, R in the low byte) and the indices (left in d_idx)
-    bool quantize(int quality, void *stream, std::vector<uint32_t> &palette, std::string &err);
+    // palette (RGBA words, R in the low byte) and the indices (left in d_idx).  allow_exact = false quantises an image with at most
+    // 256 distinct values too, so that the quality still applies to it.
+    bool quantize(int quality, void *stream, std::vector<uint32_t> &palette, std::string &err, bool allow_exact = true);
     bool fetch_indices(uint8_t *idx, void *stream, std::string &err);
     bool fetch_rgba(std::vector<uint8_t> &rgba, void *stream, std::string &err);
     // indices -> rows of `depth`-bit samples (MSB first, padded to bytes) at d_dst
