@@ -56,6 +56,18 @@ b200_status make_status(int code, const std::string &msg)
 // a header the reader refused: RGB-coded sources are "recognised but not on this path" (code 3), everything else is corrupt input
 b200_status header_status(const std::string &err) { return make_status(err.compare(0, 9, "RGB-coded") == 0 ? B200_ERR_UNSUPPORTED : B200_ERR_CORRUPT_INPUT, err); }
 
+// Every leg that decodes a JPEG to samples (lossy compress, resize, conversion, compress-to-size) upsamples each component by
+// hmax / hs x vmax / vs.  A factor that does not divide the largest one has no such ratio: libjpeg refuses the file the same
+// way (jdsample.c, JERR_FRACT_SAMPLE_NOT_IMPL).  Each such leg asks this right after the header, before it reserves or launches
+// anything, so that they all answer alike.  The coefficient-domain transcode (jpeg_optimize) has no upsampling and takes these files.
+bool fractional_sampling(const JpegGeom &g)
+{
+    for (int c = 0; c < g.ncomp; c++)
+        if (g.hmax % g.hs[c] || g.vmax % g.vs[c]) return true;
+    return false;
+}
+const char *const kFractional = "fractional sampling ratio unsupported (upsampling needs factors that divide the largest ones)";
+
 int g_forced_device = -1, g_forced_ngpus = 0;
 std::atomic<int> g_entropy_mode{-1};     // -1 unset (env B200_ENTROPY); bit 0 = device entropy encoder, bit 1 = device entropy decoder (default 3)
 std::atomic<int> g_png_lossy{-1};        // -1 unset (env B200_PNG_LOSSY); 1 = lossy PNG on the device's quantiser, 0 = refused (code 3)
@@ -295,6 +307,7 @@ b200_status jpeg_compress(const uint8_t *in, size_t in_len, const b200_params *p
         if (!jpeg_write(gin, coefs.data(), wo, &rd.meta(), out, err)) return make_status(B200_ERR_INVALID_ARGUMENT, err);
         return ok_status();
     }
+    if (fractional_sampling(gin)) return make_status(B200_ERR_UNSUPPORTED, kFractional);
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
     JpegGeom gout;
     if (!jpeg_output_geom(gin, (int)p->jpeg_quality, (int)p->jpeg_chroma_subsampling, gout, err)) return make_status(B200_ERR_INVALID_ARGUMENT, err);
@@ -547,6 +560,7 @@ b200_status jpeg_to_webp(const uint8_t *in, size_t in_len, const b200_params *p,
     JpegReader rd(in, in_len);
     if (!rd.read_header(err)) return header_status(err);
     const JpegGeom &gin = rd.geom();
+    if (fractional_sampling(gin)) return make_status(B200_ERR_UNSUPPORTED, kFractional);
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
     uint32_t nw, nh;
     b200_status st = target_size((uint32_t)gin.width, (uint32_t)gin.height, p, 16383, nw, nh, "invalid target dimensions for WebP");
@@ -582,6 +596,7 @@ b200_status jpeg_to_png(const uint8_t *in, size_t in_len, const b200_params *p, 
     JpegReader rd(in, in_len);
     if (!rd.read_header(err)) return header_status(err);
     const JpegGeom &gin = rd.geom();
+    if (fractional_sampling(gin)) return make_status(B200_ERR_UNSUPPORTED, kFractional);
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
     uint32_t nw, nh;
     b200_status st = target_size((uint32_t)gin.width, (uint32_t)gin.height, p, 65535, nw, nh, "invalid target dimensions");
@@ -935,6 +950,7 @@ static b200_status jpeg_to_size(const uint8_t *in, size_t in_len, b200_params *p
     JpegReader rd(in, in_len);
     if (!rd.read_header(err)) return header_status(err);
     const JpegGeom &gin = rd.geom();
+    if (fractional_sampling(gin)) return make_status(B200_ERR_UNSUPPORTED, kFractional);
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
     if (params->width || params->height || (entropy_mode() & 1) == 0) {
         // resize, or the host-entropy mode: every try is a whole compress call (the resized planes are not kept between tries)

@@ -253,6 +253,7 @@ bool JpegReader::decode_scan(const uint8_t *seg, size_t sl, const uint8_t *ecs, 
         td[k] = seg[2 + 2 * k] >> 4; ta[k] = seg[2 + 2 * k] & 15;
         if (td[k] > 3 || ta[k] > 3) { err = "bad table selector"; return false; }
     }
+    if (mcu_blocks(ns, ci) > 10) { err = "corrupt JPEG data: more than 10 blocks in an interleaved MCU"; return false; }
     int Ss = seg[1 + 2 * ns], Se = seg[2 + 2 * ns], Ah = seg[3 + 2 * ns] >> 4, Al = seg[3 + 2 * ns] & 15;
     const bool prog = g.progressive;
     if (!prog) { Ss = 0; Se = 63; Ah = Al = 0; }
@@ -400,6 +401,7 @@ bool JpegReader::device_decodable(DeviceScan &ds, bool scan_on_device)
         ds.td[k] = seg[2 + 2 * k] >> 4; ds.ta[k] = seg[2 + 2 * k] & 15;
         if (ds.td[k] > 3 || ds.ta[k] > 3 || !dc_[ds.td[k]].present || !ac_[ds.ta[k]].present) return false;
     }
+    if (mcu_blocks(ds.ns, ds.ci) > 10) return false;           // corrupt: decode_scan refuses it with the reason
     for (int c = 0; c < g_.ncomp; c++) if (!g_.qt_present[g_.tq[c]]) return false;
     ds.ecs_begin = pos_ + 2 + L;
     ds.stuffed = 0; ds.verified = !scan_on_device;

@@ -68,6 +68,15 @@ public:
 private:
     bool parse_segment(unsigned marker, const uint8_t *seg, size_t sl, std::string &err);
     bool decode_scan(const uint8_t *seg, size_t sl, const uint8_t *ecs, const uint8_t **next, int16_t *coefs, std::string &err);
+    // blocks in one MCU of a scan over components ci[0..ns): libjpeg (jdinput.c per_scan_setup) refuses an interleaved scan whose
+    // MCU holds more than 10 (D_MAX_BLOCKS_IN_MCU); a single-component scan's MCU is one block whatever the factors
+    int mcu_blocks(int ns, const int *ci) const
+    {
+        if (ns == 1) return 1;
+        int n = 0;
+        for (int k = 0; k < ns; k++) n += g_.hs[ci[k]] * g_.vs[ci[k]];
+        return n;
+    }
     const uint8_t *d_; size_t n_; size_t pos_ = 0;
     JpegGeom g_; JpegMeta m_;
     Huff dc_[4], ac_[4];

@@ -546,6 +546,11 @@ int orc_jpeg_read(const uint8_t *d, size_t len, orc_jpeg *j, char err[256])
                 s.ci[k] = ci; s.td[k] = seg[2 + 2 * k] >> 4; s.ta[k] = seg[2 + 2 * k] & 15;
                 if (s.td[k] > 3 || s.ta[k] > 3) { SETERR("bad table selector"); goto done; }
             }
+            if (s.ns > 1) { /* jdinput.c per_scan_setup: an interleaved MCU holds at most D_MAX_BLOCKS_IN_MCU (10) blocks */
+                int blocks = 0;
+                for (int k = 0; k < s.ns; k++) blocks += j->hs[s.ci[k]] * j->vs[s.ci[k]];
+                if (blocks > 10) { SETERR("bad MCU size: %d blocks in an interleaved MCU", blocks); goto done; }
+            }
             s.Ss = seg[1 + 2 * s.ns]; s.Se = seg[2 + 2 * s.ns]; s.Ah = seg[3 + 2 * s.ns] >> 4; s.Al = seg[3 + 2 * s.ns] & 15;
             if (!j->progressive) { s.Ss = 0; s.Se = 63; s.Ah = s.Al = 0; }
             else if (s.Ss > s.Se || s.Se > 63 || (s.Ss == 0 && s.Se != 0) || (s.Ss > 0 && s.ns != 1) || s.Al > 13) { SETERR("bad progressive scan parameters"); goto done; }
