@@ -68,6 +68,7 @@ _SYMBOLS = [
     "b200_webp_encode_rgb", "b200_webp_write_levels", "b200_webp_qindex",
     "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_jpeg_pipe_destroy", "b200_device_jobs", "b200_device_numa_node", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba", "b200_webp_alpha_filter", "b200_webp_d2h_bytes",
     "b200_set_png_lossy", "b200_png_quantize", "b200_set_jpeg_trellis", "b200_set_gif", "b200_gif_decode", "b200_gif_lzw",
+    "b200_set_png_resize", "b200_png_resize_samples",
 ]
 
 
@@ -85,7 +86,7 @@ def lib():
                   "b200_png_decode", "b200_png_decode_reduced", "b200_png_filter", "b200_png_lz77", "b200_png_deflate_tokens",
                   "b200_webp_encode_rgb", "b200_webp_write_levels", "b200_jpeg_encode_coefficients_device",
                   "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba", "b200_png_quantize",
-                  "b200_gif_decode", "b200_gif_lzw"):
+                  "b200_gif_decode", "b200_gif_lzw", "b200_png_resize_samples"):
             getattr(L, f).restype = Status
         L.b200_webp_d2h_bytes.restype = C.c_ulonglong
         L.b200_version.restype = C.c_char_p
@@ -232,6 +233,11 @@ def set_entropy_mode(mode):
 def set_png_lossy(on):
     """b200_set_png_lossy: lossy PNG (png_optimize = 0) on the device quantiser (True) or refused with code 3 (False, the default)."""
     return lib().b200_set_png_lossy(int(bool(on)))
+
+
+def set_png_resize(on):
+    """b200_set_png_resize: PNG -> PNG with width / height resized on the device (True) or refused with code 3 (False, the default)."""
+    return lib().b200_set_png_resize(int(bool(on)))
 
 
 def set_jpeg_trellis(on):
@@ -489,3 +495,15 @@ class JpegPipe:
             self.close()
         except Exception:
             pass
+
+
+def png_resize_samples(data, width=0, height=0):
+    """b200_png_resize_samples (device): -> (PngInfo of the decoded type at the target size, rows uint8 [height, row_bytes] in PNG
+    byte order).  width / height as in Params; both 0 = the expanded image at the source's size."""
+    info, raw = PngInfo(), C.POINTER(C.c_uint8)()
+    buf = (C.c_uint8 * len(data)).from_buffer_copy(data)
+    _check(lib().b200_png_resize_samples(buf, C.c_size_t(len(data)), C.c_uint32(width), C.c_uint32(height), C.byref(info), C.byref(raw)))
+    n = info.height * info.row_bytes
+    arr = np.frombuffer(C.string_at(raw, n), dtype=np.uint8).reshape(info.height, info.row_bytes).copy()
+    lib().b200_free(raw)
+    return info, arr

@@ -5,6 +5,7 @@
 #include "../../include/b200_caesium_png_lossy.h"
 #include "../../include/b200_caesium_jpeg_trellis.h"
 #include "../../include/b200_caesium_gif.h"
+#include "../../include/b200_caesium_png_resize.h"
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -72,6 +73,7 @@ int g_forced_device = -1, g_forced_ngpus = 0;
 std::atomic<int> g_entropy_mode{-1};     // -1 unset (env B200_ENTROPY); bit 0 = device entropy encoder, bit 1 = device entropy decoder (default 3)
 std::atomic<int> g_png_lossy{-1};        // -1 unset (env B200_PNG_LOSSY); 1 = lossy PNG on the device's quantiser, 0 = refused (code 3)
 std::atomic<int> g_gif{-1};              // -1 unset (env B200_GIF); 1 = GIF re-encoded on the device, 0 = refused (code 3)
+std::atomic<int> g_png_resize{-1};       // -1 unset (env B200_PNG_RESIZE); 1 = PNG -> PNG with width / height on the device, 0 = refused (code 3)
 
 // runtime_init is idempotent while initialised, so after b200_shutdown (which frees every slot's device buffers) the next call
 // initialises again: a long-running host can hand the memory of one workload's slots back before starting another
@@ -102,6 +104,16 @@ bool png_lossy()
         g_png_lossy.store(e && !strcmp(e, "gpu") ? 1 : 0);
     }
     return g_png_lossy.load() == 1;
+}
+
+// PNG -> PNG with a target size on the device: b200_set_png_resize, else B200_PNG_RESIZE=gpu, read once; off by default
+bool png_resize()
+{
+    if (g_png_resize.load() < 0) {
+        const char *e = getenv("B200_PNG_RESIZE");
+        g_png_resize.store(e && !strcmp(e, "gpu") ? 1 : 0);
+    }
+    return g_png_resize.load() == 1;
 }
 
 // GIF sources on the device: b200_set_gif, else B200_GIF=gpu, read once; off by default
@@ -394,26 +406,47 @@ void jpeg_compress_group(const uint8_t *const *in, const size_t *in_len, const s
     tm.lap(5);
 }
 
-b200_status png_lossy_compress(PngInfo &info, const PngIdat &idat, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out);
+b200_status png_lossy_compress(PngInfo &info, const PngIdat &idat, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out, uint32_t nw, uint32_t nh);
+
+// a failed PngDevice call: the input's fault (code 4); with a resize, a failed allocation is out of memory (code 7); else a CUDA error
+b200_status png_device_status(const PngDevice *png, bool resize, const std::string &err)
+{
+    if (png->corrupt) return make_status(B200_ERR_CORRUPT_INPUT, err);
+    if (resize && (!err.compare(0, 11, "cudaMalloc:") || !err.compare(0, 14, "cudaHostAlloc:"))) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    return make_status(B200_ERR_CUDA, err);
+}
+
+// With width / height set (the resize switch on), the PNG leg resizes before coding: PngDevice expands the samples to the image crate's
+// decoded type and resamples them with K3 between the un-filter and the back end.  target_size gives nw x nh (0 x 0 = no resize).
+b200_status png_target(const PngInfo &info, const b200_params *p, uint32_t &nw, uint32_t &nh)
+{
+    nw = nh = 0;
+    if (!p->width && !p->height) return ok_status();
+    return target_size(info.width, info.height, p, 65535, nw, nh, "invalid target dimensions");
+}
 
 // ---- PNG (lossless) through the device ---------------------------------------------------------------------------
 // libcaesium png::compress: optimize == true -> png::lossless (oxipng, level = png.optimization_level); otherwise the lossy
-// palette quantiser (imagequant), which is outside this path.  Resizing a PNG goes through the image crate's decoder and is
-// likewise left to the reference.
+// palette quantiser (imagequant) when the lossy switch is on.  Resizing (width / height) runs on the device when the resize switch is on.
 b200_status png_compress(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
 {
     if (!p->png_optimize && !png_lossy()) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::compress_in_memory)");
-    if (p->width || p->height) return make_status(B200_ERR_UNSUPPORTED, "PNG resize is outside the GPU path (route to caesium::compress_in_memory)");
+    if ((p->width || p->height) && !png_resize()) return make_status(B200_ERR_UNSUPPORTED, "PNG resize is outside the GPU path (route to caesium::compress_in_memory)");
     std::string err;
     PngInfo info; PngIdat idat;
     static const bool verbose = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2;
     const auto t0 = std::chrono::steady_clock::now();
     if (!png_parse_chunks(in, in_len, p->keep_metadata != 0, info, idat, err)) return png_status(err);
-    if (!p->png_optimize) return png_lossy_compress(info, idat, p, prefer_dev, out);
+    uint32_t nw, nh;
+    const b200_status tst = png_target(info, p, nw, nh);
+    if (tst.code) return tst;
+    if (!p->png_optimize) return png_lossy_compress(info, idat, p, prefer_dev, out, nw, nh);
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
     std::vector<uint8_t> z;
     auto t1 = t0;
     double deflate_ms = 0;
+    const uint32_t sw = info.width, sh = info.height;
+    std::map<std::string, std::pair<double, int>> ev;      // B200_TRACE=2: device event times of the stages
     {   // the slot goes back before the container is written
         SlotLease s(prefer_dev);
         if (!s) return s.failure();
@@ -427,8 +460,12 @@ b200_status png_compress(const uint8_t *in, size_t in_len, const b200_params *p,
         if (!zlib_inflate_to(idat.p, idat.n, buf, cap, nin, &got, &stored_adler, err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
         if (got < nin) return make_status(B200_ERR_CORRUPT_INPUT, "IDAT too short");
         t1 = std::chrono::steady_clock::now();
-        if (!png->compress_filtered(info, got, stored_adler, std::min((int)p->png_optimization_level, 6), s->stream, z, nullptr, err))
-            return make_status(png->corrupt ? B200_ERR_CORRUPT_INPUT : B200_ERR_CUDA, err);
+        LaunchTimer lt;
+        if (verbose) { lt.begin((cudaStream_t)s->stream); tl_launch_timer = &lt; }
+        const bool ok = png->compress_filtered(info, got, stored_adler, std::min((int)p->png_optimization_level, 6), s->stream, z, nullptr, err, nw, nh);
+        tl_launch_timer = nullptr;
+        if (verbose) { cudaStreamSynchronize((cudaStream_t)s->stream); lt.collect(ev); }
+        if (!ok) return png_device_status(png, nw != 0, err);
         deflate_ms = png->last_deflate_ms;
     }
     const auto t3 = std::chrono::steady_clock::now();
@@ -437,6 +474,10 @@ b200_status png_compress(const uint8_t *in, size_t in_len, const b200_params *p,
         auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
         fprintf(stderr, "[b200 trace] png %ux%u: parse + inflate %.1f ms, device (un-filter, filter trials, LZ77, DEFLATE coding; host Huffman %.1f) %.1f ms, container %.1f ms\n",
                 info.width, info.height, ms(t0, t1), deflate_ms, ms(t1, t3), ms(t3, std::chrono::steady_clock::now()));
+        auto at = [&](const char *k) { auto it = ev.find(k); return it == ev.end() ? 0.0 : it->second.first; };
+        const double up = at("h2d") + at("png_unfilter"), rz = at("png_resize");
+        fprintf(stderr, "[b200 trace] png stages %ux%u -> %ux%u: parse + inflate %.3f ms, h2d + un-filter %.3f ms, expand + K3 + pack %.3f ms, back end %.3f ms\n",
+                sw, sh, info.width, info.height, ms(t0, t1), up, rz, ms(t1, t3) - up - rz);
     }
     return ok_status();
 }
@@ -481,8 +522,8 @@ b200_status png_lossy_code(Slot *s, PngInfo info, int quality, int level, std::v
     return ok_status();
 }
 
-// a parsed PNG's IDAT inflated into the slot's staging buffer, un-filtered, expanded and histogrammed by the quantiser
-b200_status png_lossy_load(Slot *s, PngInfo &info, const PngIdat &idat)
+// a parsed PNG's IDAT inflated into the slot's staging buffer, un-filtered, (nw, nh > 0: resized,) expanded and histogrammed by the quantiser
+b200_status png_lossy_load(Slot *s, PngInfo &info, const PngIdat &idat, uint32_t nw = 0, uint32_t nh = 0)
 {
     std::string err;
     const bool grey = info.color_type == 0 || info.color_type == 4;
@@ -494,19 +535,19 @@ b200_status png_lossy_load(Slot *s, PngInfo &info, const PngIdat &idat)
     if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
     if (!zlib_inflate_to(idat.p, idat.n, buf, cap, nin, &got, &stored_adler, err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
     if (got < nin) return make_status(B200_ERR_CORRUPT_INPUT, "IDAT too short");
-    if (!png->load_filtered_lossy(info, got, stored_adler, s->stream, err)) return make_status(png->corrupt ? B200_ERR_CORRUPT_INPUT : B200_ERR_CUDA, err);
+    if (!png->load_filtered_lossy(info, got, stored_adler, s->stream, err, nw, nh)) return png_device_status(png, nw != 0, err);
     return ok_status();
 }
 
 // lossy PNG (png.optimize == false, the switch on): palette quantisation with Floyd-Steinberg dithering on the device, then the
 // lossless leg's filter trials, LZ77 and DEFLATE over the indexed image
-b200_status png_lossy_compress(PngInfo &info, const PngIdat &idat, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
+b200_status png_lossy_compress(PngInfo &info, const PngIdat &idat, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out, uint32_t nw, uint32_t nh)
 {
     std::string err;
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
     SlotLease s(prefer_dev);
     if (!s) return s.failure();
-    const b200_status st = png_lossy_load(s, info, idat);
+    const b200_status st = png_lossy_load(s, info, idat, nw, nh);
     if (st.code) return st;
     return png_lossy_code(s, info, (int)p->png_quality, (int)p->png_optimization_level, out);
 }
@@ -1011,6 +1052,7 @@ void b200_free(void *p) { free(p); }
 int b200_set_entropy_mode(int mode) { if (mode < 0 || mode > 3) return B200_ERR_INVALID_ARGUMENT; g_entropy_mode.store(mode); return B200_OK; }
 int b200_set_png_lossy(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_png_lossy.store(on); return B200_OK; }
 int b200_set_gif(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_gif.store(on); return B200_OK; }
+int b200_set_png_resize(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_png_resize.store(on); return B200_OK; }
 int b200_set_jpeg_trellis(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; set_jpeg_trellis(on == 1); return B200_OK; }
 
 uint32_t b200_sniff_format(const uint8_t *d, size_t n)
@@ -1160,19 +1202,22 @@ static b200_status webp_to_size(const uint8_t *in, size_t in_len, b200_params *p
     return bisect_quality(size_at, max_output_size, return_smallest, &params->webp_quality, result);
 }
 
-// PNG (the lossy switch on): the source is decoded, un-filtered, expanded and histogrammed once; every try runs median cut,
+// PNG (the lossy switch on): the source is decoded, un-filtered, (resized,) expanded and histogrammed once; every try runs median cut,
 // refinement, dithering and coding at its png_quality
 static b200_status png_to_size(const uint8_t *in, size_t in_len, b200_params *params, size_t max_output_size, bool return_smallest, std::vector<uint8_t> &result)
 {
     if (!png_lossy()) return make_status(B200_ERR_UNSUPPORTED, "compress_to_size on a PNG bisects the lossy (imagequant) quality, which is outside the GPU path (route to caesium::compress_to_size_in_memory)");
-    if (params->width || params->height) return make_status(B200_ERR_UNSUPPORTED, "PNG resize is outside the GPU path (route to caesium::compress_to_size_in_memory)");
+    if ((params->width || params->height) && !png_resize()) return make_status(B200_ERR_UNSUPPORTED, "PNG resize is outside the GPU path (route to caesium::compress_to_size_in_memory)");
     std::string err;
     PngInfo info; PngIdat idat;
     if (!png_parse_chunks(in, in_len, params->keep_metadata != 0, info, idat, err)) return png_status(err);
+    uint32_t nw, nh;
+    b200_status st = png_target(info, params, nw, nh);
+    if (st.code) return st;
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
     SlotLease s(-1);
     if (!s) return s.failure();
-    const b200_status st = png_lossy_load(s, info, idat);
+    st = png_lossy_load(s, info, idat, nw, nh);
     if (st.code) return st;
     auto size_at = [&](int q, auto want, size_t &sz, std::vector<uint8_t> &cur) -> b200_status {
         (void)want;
@@ -1618,6 +1663,36 @@ b200_status b200_png_quantize(const uint8_t *rgba, int width, int height, int qu
         for (size_t k = 0; k < pal.size(); k++) for (int c = 0; c < 4; c++) palette_rgba[4 * k + c] = (uint8_t)(pal[k] >> (8 * c));
         *npalette = (int)pal.size();
         return ok_status();
+    });
+}
+
+b200_status b200_png_resize_samples(const uint8_t *in, size_t in_len, uint32_t width, uint32_t height, b200_png_info *info, uint8_t **raw)
+{
+    if (!in || !info || !raw) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
+    *raw = nullptr;
+    return guarded([&] {
+        std::string err;
+        PngInfo pi; PngIdat idat;
+        if (!png_parse_chunks(in, in_len, false, pi, idat, err)) return png_status(err);
+        b200_params p; memset(&p, 0, sizeof p); p.width = width; p.height = height;
+        uint32_t nw, nh;                                        // both 0: the expanded image at the source's size
+        const b200_status st = target_size(pi.width, pi.height, &p, 65535, nw, nh, "invalid target dimensions");
+        if (st.code) return st;
+        if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
+        SlotLease s(-1);
+        if (!s) return s.failure();
+        PngDevice *png = s->png_dev();
+        const size_t nin = (pi.row_bytes + 1) * (size_t)pi.height;
+        size_t cap = 0, got = 0; uint32_t stored_adler = 0;
+        uint8_t *buf = png->input_buffer(nin, cap, err);
+        if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+        if (!zlib_inflate_to(idat.p, idat.n, buf, cap, nin, &got, &stored_adler, err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
+        if (got < nin) return make_status(B200_ERR_CORRUPT_INPUT, "IDAT too short");
+        std::vector<uint8_t> r;
+        if (!png->resize_filtered(pi, got, stored_adler, nw, nh, s->stream, r, err)) return png_device_status(png, true, err);
+        info->width = pi.width; info->height = pi.height; info->bit_depth = pi.bit_depth; info->color_type = pi.color_type; info->bpp = pi.bpp; info->row_bytes = pi.row_bytes;
+        size_t n;
+        return give(r, raw, &n);
     });
 }
 

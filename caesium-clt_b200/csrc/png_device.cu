@@ -11,6 +11,8 @@
 #include "png_kernels.h"
 #include "png_deflate.h"
 #include "png_quant.h"
+#include "png_resize.h"
+#include "resize_kernels.h"
 #include <chrono>
 #include <cstdlib>
 #include "stream_wait.h"
@@ -121,20 +123,79 @@ uint8_t *PngDevice::input_buffer(size_t bytes, size_t &cap, std::string &err)
 // (input_buffer()); everything from there to the finished zlib stream runs on the device -- un-filter (wavefront), Adler-32 check of
 // the input, reductions, K6 / K7 per strategy, DEFLATE coding -- except a palette reduction, which (at most 256 colours) goes
 // through the host and the raw-sample entry point below.
-bool PngDevice::compress_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, int level, void *stream, std::vector<uint8_t> &zlib_stream, int *chosen, std::string &err)
+bool PngDevice::compress_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, int level, void *stream, std::vector<uint8_t> &zlib_stream, int *chosen, std::string &err,
+                                  uint32_t nw, uint32_t nh)
 {
-    return from_filtered(info, nfilt, stored_adler, level, stream, zlib_stream, chosen, err, false);
+    return from_filtered(info, nfilt, stored_adler, level, stream, zlib_stream, chosen, err, Tail::Code, nw, nh);
 }
 
-bool PngDevice::load_filtered_lossy(const PngInfo &info, size_t nfilt, uint32_t stored_adler, void *stream, std::string &err)
+bool PngDevice::load_filtered_lossy(PngInfo &info, size_t nfilt, uint32_t stored_adler, void *stream, std::string &err, uint32_t nw, uint32_t nh)
 {
-    PngInfo in = info; std::vector<uint8_t> none;
-    return from_filtered(in, nfilt, stored_adler, 0, stream, none, nullptr, err, true);
+    std::vector<uint8_t> none;
+    return from_filtered(info, nfilt, stored_adler, 0, stream, none, nullptr, err, Tail::Quantise, nw, nh);
 }
 
-// lossy: stop after the checks and hand the samples to the quantiser (expand, histogram)
+bool PngDevice::resize_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, uint32_t nw, uint32_t nh, void *stream_, std::vector<uint8_t> &raw, std::string &err)
+{
+    cudaStream_t st = (cudaStream_t)stream_;
+    std::vector<uint8_t> none;
+    if (!from_filtered(info, nfilt, stored_adler, 0, stream_, none, nullptr, err, Tail::Samples, nw, nh)) return false;
+    raw.resize(info.row_bytes * info.height);
+    CU(cudaMemcpyAsync(raw.data(), d_raw, raw.size(), cudaMemcpyDeviceToHost, st));
+    CU(stream_wait(st));
+    return true;
+}
+
+// Expansion, K3 (skipped at the same size: imageops::resize copies) and packing, all enqueued behind the un-filter: d_raw holds the
+// source's rows on entry and the resized image's rows on exit.  Vertical pass first into f32 planes, then horizontal, every plane
+// of the image in one launch per pass.
+bool PngDevice::resize_raw(const PngInfo &src, const PngInfo &out, void *stream_, std::string &err)
+{
+    cudaStream_t st = (cudaStream_t)stream_;
+    const PngDecodedType t = png_decoded_type(src);
+    const int W = (int)src.width, H = (int)src.height, NW = (int)out.width, NH = (int)out.height, ch = t.channels;
+    const size_t bps = (size_t)t.depth / 8, in_pitch = (size_t)W * H, out_pitch = (size_t)NW * NH;
+    if (!grow(d_planes, ch * in_pitch * bps + 64, err)) return false;
+    if (!launch_ok(launch_png_expand_planes(d_raw, src, png_palette_lut(src), d_planes, st), "png expand", err)) return false;
+    const uint8_t *planes = d_planes;
+    if (NW != W || NH != H) {
+        ResizeAxis av, ah;
+        make_resize_axis(H, NH, av);
+        make_resize_axis(W, NW, ah);
+        auto al = [](size_t b) { return (b + 255) / 256 * 256; };       // left | count | weights of the vertical axis, then of the horizontal one
+        const size_t cv = al(4 * (size_t)NH), wv = cv + al(4 * (size_t)NH), lh = wv + al(4 * av.weights.size());
+        const size_t chh = lh + al(4 * (size_t)NW), wh = chh + al(4 * (size_t)NW), end = wh + al(4 * ah.weights.size());
+        if (!grow(h_axes, end, err) || !grow(d_axes, end, err) || !grow(d_rtmp, ch * (size_t)NH * W * sizeof(float) + 64, err) ||
+            !grow(d_rplanes, ch * out_pitch * bps + 64, err)) return false;
+        memcpy(h_axes, av.left.data(), 4 * (size_t)NH); memcpy(h_axes + cv, av.count.data(), 4 * (size_t)NH);
+        memcpy(h_axes + wv, av.weights.data(), 4 * av.weights.size());
+        memcpy(h_axes + lh, ah.left.data(), 4 * (size_t)NW); memcpy(h_axes + chh, ah.count.data(), 4 * (size_t)NW);
+        memcpy(h_axes + wh, ah.weights.data(), 4 * ah.weights.size());
+        CU(cudaMemcpyAsync(d_axes, h_axes, end, cudaMemcpyHostToDevice, st));
+        const int *ax = reinterpret_cast<const int *>(d_axes.get());
+        const float *axf = reinterpret_cast<const float *>(d_axes.get());
+        int rc;
+        if (t.depth == 16) {
+            rc = launch_resize_v_planes(reinterpret_cast<const uint16_t *>(planes), W, H, W, in_pitch, d_rtmp, NH, (size_t)NH * W, ch, ax, ax + cv / 4, axf + wv / 4, av.cap, st);
+            if (!rc) rc = launch_resize_h_planes(d_rtmp, W, (size_t)NH * W, reinterpret_cast<uint16_t *>(d_rplanes.get()), NW, NH, NW, out_pitch, ch,
+                                                 ax + lh / 4, ax + chh / 4, axf + wh / 4, ah.cap, st);
+        } else {
+            rc = launch_resize_v_planes(planes, W, H, W, in_pitch, d_rtmp, NH, (size_t)NH * W, ch, ax, ax + cv / 4, axf + wv / 4, av.cap, st);
+            if (!rc) rc = launch_resize_h_planes(d_rtmp, W, (size_t)NH * W, d_rplanes.get(), NW, NH, NW, out_pitch, ch, ax + lh / 4, ax + chh / 4, axf + wh / 4, ah.cap, st);
+        }
+        if (!launch_ok(rc, "png resize", err)) return false;
+        planes = d_rplanes;
+    }
+    if (!launch_ok(launch_png_pack_planes(planes, ch, t.depth, NW, NH, d_raw, st), "png pack", err)) return false;
+    LT_MARK("png_resize");
+    return true;
+}
+
+// Tail::Quantise (the lossy leg): stop after the checks and hand the samples to the quantiser (expand, histogram).  Tail::Samples: stop
+// after the checks.  nw, nh > 0: the resize runs between the un-filter and the checks' host wait (a corrupt input's resized samples
+// are discarded) and info describes the resized image from there on.
 bool PngDevice::from_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, int level, void *stream_, std::vector<uint8_t> &zlib_stream, int *chosen, std::string &err,
-                              bool lossy)
+                              Tail tail, uint32_t nw, uint32_t nh)
 {
     cudaStream_t st = (cudaStream_t)stream_;
     corrupt = false;
@@ -143,16 +204,25 @@ bool PngDevice::from_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler
     if (nfilt < nin) { err = "IDAT too short"; corrupt = true; return false; }
     const size_t nmax = nin + 64;
     if (!ensure_buffers(nraw, nmax, rb, st, err) || !grow(d_fin, nmax + 64, err)) return false;
+    const bool resize = nw && nh;
+    const PngInfo src = resize ? info : PngInfo();
+    if (resize) {   // every buffer of the back end for the larger of the two images
+        png_resized_info(info, nw, nh);
+        if (!ensure_buffers(info.row_bytes * info.height, (info.row_bytes + 1) * info.height + 64, info.row_bytes, st, err)) return false;
+    }
     CU(cudaMemcpyAsync(d_fin, h_raw, nin, cudaMemcpyHostToDevice, st)); LT_MARK("h2d");
     int rc = launch_png_adler(d_fin, nin, d_sums_in, st);
     uint32_t *d_un = d_sync, *d_flags = d_hist;
     uint32_t *d_set = reinterpret_cast<uint32_t *>(((uintptr_t)(d_sync + ((size_t)(h + 31) / 32 + 8)) + 7) & ~(uintptr_t)7);
     if (!rc) rc = launch_png_unfilter(d_fin, d_raw, h, (int)rb, bpp, d_un, st);
     if (!launch_ok(rc, "png unfilter", err)) return false;
+    LT_MARK("png_unfilter");
+    if (resize && !resize_raw(src, info, st, err)) return false;
     CU(cudaMemsetAsync(d_flags, 0, 16, st));
+    const bool lossless = tail == Tail::Code;
     const bool eight = info.bit_depth == 8 && info.trns.empty();
-    const bool probe_ag = !lossy && eight && (info.color_type == 2 || info.color_type == 4 || info.color_type == 6);
-    const bool probe_pal = !lossy && png_palette_candidate(info);
+    const bool probe_ag = lossless && eight && (info.color_type == 2 || info.color_type == 4 || info.color_type == 6);
+    const bool probe_pal = lossless && png_palette_candidate(info);
     const size_t npix = (size_t)info.width * info.height;
     if (probe_ag && launch_png_probe(d_raw, npix, info.channels, d_flags, st)) { err = "png probe launch failed"; return false; }
     if (probe_pal && launch_png_colours(d_raw, npix, info.channels, d_set, d_flags, st)) { err = "png palette probe launch failed"; return false; }
@@ -165,12 +235,13 @@ bool PngDevice::from_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler
     CU(stream_wait(st)); LT_MARK("host_wait");
     if (h_flags[5]) { err = "bad filter type"; corrupt = true; return false; }
     if (combine_adler(h_sums_in, nin) != stored_adler) { err = "Adler-32 mismatch"; corrupt = true; return false; }
-    if (lossy) return quantiser()->expand(d_raw, info, st, err) && quant->prepare(st, err);
+    if (tail == Tail::Samples) return true;
+    if (tail == Tail::Quantise) return quantiser()->expand(d_raw, info, st, err) && quant->prepare(st, err);
     if (probe_pal && h_flags[2] <= 256) {
         // few colours: oxipng's palette reduction (first-appearance order, tRNS layout, bit packing) runs on the host over the
         // reconstructed samples, and the indexed image takes the raw-sample entry point
-        std::vector<uint8_t> raw(nraw);
-        CU(cudaMemcpy(raw.data(), d_raw, nraw, cudaMemcpyDeviceToHost));
+        std::vector<uint8_t> raw(info.row_bytes * info.height);
+        CU(cudaMemcpy(raw.data(), d_raw, raw.size(), cudaMemcpyDeviceToHost));
         if (png_reduce_palette(info, raw)) return compress(info, raw, level, stream_, zlib_stream, chosen, err);
     }
     return reduce_and_code(info, probe_ag, h_flags, level, stream_, zlib_stream, chosen, err);

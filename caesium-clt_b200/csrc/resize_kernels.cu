@@ -4,18 +4,22 @@
 // Bit-exact with oracle/resize_oracle.c: tap windows and normalised f32 weights are computed on the host with the
 // same libm calls (resize_host.cpp); the kernels accumulate taps in the same order with separately rounded multiply
 // and add (__fmul_rn/__fadd_rn: no FMA contraction), clamp and round half away from zero.  Vertical pass first into
-// an f32 plane, then horizontal, as imageops::resize does.  Planar u8 channels; HBM-bound streaming kernels.
+// an f32 plane, then horizontal, as imageops::resize does.  Planar u8 or u16 channels; HBM-bound streaming kernels.
 #include <cuda_runtime.h>
 #include <cstdint>
 #include "resize_kernels.h"
 
 namespace b200 {
 
-__global__ void k_resize_v(const uint8_t *__restrict__ in, int w, int stride, float *__restrict__ out, int nh,
+// One launch resamples every plane of an image: blockIdx.z selects the plane, `in_pitch` / `out_pitch` are the planes' sizes in
+// samples.  T = uint8_t or uint16_t; the horizontal pass clamps to T's range before rounding.
+template <class T>
+__global__ void k_resize_v(const T *__restrict__ in, int w, int stride, size_t in_pitch, float *__restrict__ out, int nh, size_t out_pitch,
                            const int *__restrict__ left, const int *__restrict__ count, const float *__restrict__ weights, int cap)
 {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, oy = blockIdx.y;
     if (x >= w || oy >= nh) return;
+    in += blockIdx.z * in_pitch; out += blockIdx.z * out_pitch;
     const int l = left[oy], n = count[oy];
     const float *ws = weights + (size_t)oy * cap;
     float t = 0.0f;
@@ -23,18 +27,20 @@ __global__ void k_resize_v(const uint8_t *__restrict__ in, int w, int stride, fl
     out[(size_t)oy * w + x] = t;
 }
 
-__global__ void k_resize_h(const float *__restrict__ in, int w, uint8_t *__restrict__ out, int nw, int nh, int ostride,
+template <class T>
+__global__ void k_resize_h(const float *__restrict__ in, int w, size_t in_pitch, T *__restrict__ out, int nw, int nh, int ostride, size_t out_pitch,
                            const int *__restrict__ left, const int *__restrict__ count, const float *__restrict__ weights, int cap)
 {
     const int ox = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
     if (ox >= nw || y >= nh) return;
+    in += blockIdx.z * in_pitch; out += blockIdx.z * out_pitch;
     const int l = left[ox], n = count[ox];
     const float *ws = weights + (size_t)ox * cap;
     const float *row = in + (size_t)y * w + l;
     float t = 0.0f;
     for (int i = 0; i < n; i++) t = __fadd_rn(t, __fmul_rn(row[i], __ldg(ws + i)));
-    t = fminf(fmaxf(t, 0.0f), 255.0f);
-    out[(size_t)y * ostride + ox] = (uint8_t)roundf(t);
+    t = fminf(fmaxf(t, 0.0f), sizeof(T) == 1 ? 255.0f : 65535.0f);
+    out[(size_t)y * ostride + ox] = (T)roundf(t);
 }
 
 #define FIXC(x) ((int)((x) * 65536.0 + 0.5))
@@ -67,17 +73,33 @@ static inline int cdiv(size_t a, size_t b) { return (int)((a + b - 1) / b); }
 
 int launch_resize_v(const uint8_t *in, int w, int h, int stride, float *out, int nh, const int *left, const int *count, const float *weights, int cap, void *stream)
 {
-    (void)h;
-    dim3 grid(cdiv((size_t)w, 256), nh);
-    k_resize_v<<<grid, 256, 0, (cudaStream_t)stream>>>(in, w, stride, out, nh, left, count, weights, cap);
-    return (int)cudaGetLastError();
+    return launch_resize_v_planes(in, w, h, stride, 0, out, nh, 0, 1, left, count, weights, cap, stream);
 }
 int launch_resize_h(const float *in, int w, uint8_t *out, int nw, int nh, int ostride, const int *left, const int *count, const float *weights, int cap, void *stream)
 {
-    dim3 grid(cdiv((size_t)nw, 128), nh);
-    k_resize_h<<<grid, 128, 0, (cudaStream_t)stream>>>(in, w, out, nw, nh, ostride, left, count, weights, cap);
+    return launch_resize_h_planes(in, w, 0, out, nw, nh, ostride, 0, 1, left, count, weights, cap, stream);
+}
+template <class T>
+int launch_resize_v_planes(const T *in, int w, int h, int stride, size_t in_pitch, float *out, int nh, size_t out_pitch, int planes,
+                           const int *left, const int *count, const float *weights, int cap, void *stream)
+{
+    (void)h;
+    dim3 grid(cdiv((size_t)w, 256), nh, planes);
+    k_resize_v<T><<<grid, 256, 0, (cudaStream_t)stream>>>(in, w, stride, in_pitch, out, nh, out_pitch, left, count, weights, cap);
     return (int)cudaGetLastError();
 }
+template <class T>
+int launch_resize_h_planes(const float *in, int w, size_t in_pitch, T *out, int nw, int nh, int ostride, size_t out_pitch, int planes,
+                           const int *left, const int *count, const float *weights, int cap, void *stream)
+{
+    dim3 grid(cdiv((size_t)nw, 128), nh, planes);
+    k_resize_h<T><<<grid, 128, 0, (cudaStream_t)stream>>>(in, w, in_pitch, out, nw, nh, ostride, out_pitch, left, count, weights, cap);
+    return (int)cudaGetLastError();
+}
+template int launch_resize_v_planes<uint8_t>(const uint8_t *, int, int, int, size_t, float *, int, size_t, int, const int *, const int *, const float *, int, void *);
+template int launch_resize_v_planes<uint16_t>(const uint16_t *, int, int, int, size_t, float *, int, size_t, int, const int *, const int *, const float *, int, void *);
+template int launch_resize_h_planes<uint8_t>(const float *, int, size_t, uint8_t *, int, int, int, size_t, int, const int *, const int *, const float *, int, void *);
+template int launch_resize_h_planes<uint16_t>(const float *, int, size_t, uint16_t *, int, int, int, size_t, int, const int *, const int *, const float *, int, void *);
 int launch_ycc_to_rgb(uint8_t *p0, uint8_t *p1, uint8_t *p2, size_t n, void *stream)
 {
     k_ycc_to_rgb<<<cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(p0, p1, p2, n);
