@@ -3,7 +3,7 @@
 // Batched: every pass is one launch for all images of the batch (blockIdx.y = image), which is what keeps the launch
 // count per image low when b200_compress_batch packs images into megabatches.
 // Pass order: unstuff (count, scan, scatter) -> round 0 -> rounds (in groups, one host check per group) -> block-count
-// scan -> write -> DC gather / scan / scatter.  Coefficients land directly in the transform kernels' input buffers, so the
+// scan -> write (coefficients and DC differences) -> DC scan / scatter.  Coefficients land directly in the transform kernels' input buffers, so the
 // host never sees them.
 #include <cuda_runtime.h>
 #include <cub/device/device_scan.cuh>
@@ -128,25 +128,60 @@ __global__ void __launch_bounds__(64) k_gd_round(const DecImage *__restrict__ im
     }
 }
 
-// Write pass sink: every non-zero coefficient is stored on its own into a buffer that was memset.  (A variant that staged whole
-// blocks in local memory and stored them with 16-byte writes, without the memset, measured slower -- 3,220 vs 3,750 images/s --
-// and was removed.)  The block address moves with a gd::Cursor: no divisions inside the decode loop.  Every subsequence starts
-// from its true state here, so a stream anomaly met inside a real block (ptr set) is in the stream itself: it is collected and
-// the image goes to the host decoder.
-struct SparseWriteSink {
-    const Walk *walk; int16_t *coefs; uint32_t cur, total; Cursor c; int16_t *ptr; uint32_t anom;
-    __device__ __forceinline__ void seek() { c.seek(*walk, cur); ptr = cur < total ? coefs + c.offset(*walk) : nullptr; }
-    __device__ __forceinline__ void coef(int k, int v) { if (ptr) ptr[k] = (int16_t)v; }
-    __device__ __forceinline__ void anomaly(uint32_t m) { if (ptr) anom |= m; }
-    __device__ __forceinline__ void block_done() { cur++; c.next(*walk); ptr = cur < total ? coefs + c.offset(*walk) : nullptr; }
+// Write pass sink: whole-sector stores.  A block of this layout (int16, zigzag, 128 bytes) is one cache line of four 32-byte
+// sectors, a block's non-zero coefficients arrive in ascending zigzag index, and in gd::decode_owned_blocks every block has one
+// writer.  So the sink holds the block's current sector (16 coefficients) in shared memory, stores it with two 16-byte writes
+// when a coefficient of a later sector arrives, and stores zeros for the sectors in between and behind: every owned block
+// receives exactly eight 16-byte stores whatever its content, and nothing has to be zeroed beforehand.  The staging area is
+// word-major, stage[word][thread]: a thread's eight words live in its own bank, so neither the 2-byte placement nor the flush
+// can conflict.  The lanes of a warp reach their sector changes at unrelated symbols, and a flush run by one lane costs the
+// warp as much as one run by all, so there is ONE flush site in the loop: the end of a block only marks the held block as
+// ended, and its last sectors leave when the next block's DC coefficient arrives (or in finish()), together with the other
+// lanes' mid-block sector changes of that iteration.  With a second flush site at the end of the block the kernel took
+// 0.436 ms per 8-image 4K megabatch, H100 SXM 700 W; see DESIGN.md 4.2 for the figures of the sink this one replaced.
+// The sector that holds the DC coefficient also delivers the block's DC difference to the component-major array the DC prefix
+// sum runs over.  The block address moves with a gd::Cursor: no divisions inside the decode loop.  Every subsequence starts
+// from its true state here, so a stream anomaly met inside a real block (cur < total) is in the stream itself: it is collected
+// and the image goes to the host decoder.
+constexpr int WRITE_THREADS = 64;
+struct SectorWriteSink {
+    const Walk *walk; int16_t *coefs; int32_t *dc; uint32_t *stage;
+    uint32_t cur, total; Cursor c;      // the block the decoder is in (cur >= total: padding after the last real block)
+    int16_t *ptr; int32_t *dcp;         // the held block and where its DC difference goes; null before the first DC and in the padding
+    int sec; bool ended; uint32_t anom; // sector held; the held block is complete (the cursor has moved on)
+    __device__ __forceinline__ void seek() { c.seek(*walk, cur); ptr = nullptr; dcp = nullptr; sec = 0; ended = true; for (int w = 0; w < 8; w++) stage[w * WRITE_THREADS] = 0; }
+    __device__ __forceinline__ void flush_to(int target)
+    {   // sectors sec .. target - 1 leave: the held one from the staging words, the others as zeros
+        uint4 lo = make_uint4(stage[0], stage[WRITE_THREADS], stage[2 * WRITE_THREADS], stage[3 * WRITE_THREADS]);
+        uint4 hi = make_uint4(stage[4 * WRITE_THREADS], stage[5 * WRITE_THREADS], stage[6 * WRITE_THREADS], stage[7 * WRITE_THREADS]);
+        if (sec == 0) *dcp = (int16_t)(lo.x & 0xFFFFu);
+        for (int w = 0; w < 8; w++) stage[w * WRITE_THREADS] = 0;
+        uint4 *out = reinterpret_cast<uint4 *>(ptr) + 2 * sec;
+        for (int s = sec; s < target; s++, out += 2) { out[0] = lo; out[1] = hi; lo = hi = make_uint4(0, 0, 0, 0); }
+    }
+    __device__ __forceinline__ void coef(int k, int v)
+    {
+        const int s = k >> 4;
+        if (ended || s != sec) {
+            if (ptr) flush_to(ended ? 4 : s);
+            if (ended) { ended = false; ptr = cur < total ? coefs + c.offset(*walk) : nullptr; dcp = dc + c.dc_slot(*walk); }
+            sec = s;
+        }
+        if (ptr) reinterpret_cast<int16_t *>(stage + ((k & 15) >> 1) * WRITE_THREADS)[k & 1] = (int16_t)v;
+    }
+    __device__ __forceinline__ void anomaly(uint32_t m) { if (cur < total) anom |= m; }
+    __device__ __forceinline__ void block_done() { cur++; c.next(*walk); ended = true; }
+    __device__ __forceinline__ void finish() { if (ptr) flush_to(4); }      // the last block (cut short only if the stream was: flagged)
 };
 
 // marker word per image: bit 0 = a marker inside the segment (un-stuff pass), ANOM_* << 1 = the write pass's stream anomalies
-__global__ void __launch_bounds__(64) k_gd_write(const DecImage *__restrict__ imgs, const uint8_t *__restrict__ stream_all, const DecTables *__restrict__ tabs_all,
-                                                 const DecState *__restrict__ A, const uint32_t *__restrict__ first, uint32_t *__restrict__ marker)
+__global__ void __launch_bounds__(WRITE_THREADS) k_gd_write(const DecImage *__restrict__ imgs, const uint8_t *__restrict__ stream_all, const DecTables *__restrict__ tabs_all,
+                                                            const DecState *__restrict__ A, const uint32_t *__restrict__ first, int32_t *__restrict__ dc, uint32_t *__restrict__ marker)
 {
     __shared__ DecShared sh;
     __shared__ Walk walk;
+    __shared__ uint32_t stage[8][WRITE_THREADS];
+    static_assert(sizeof(Walk) / 4 <= WRITE_THREADS, "one thread per word stages the Walk");
     const DecImage &im = imgs[blockIdx.y];
     if (blockIdx.x * blockDim.x >= im.g.nsub) return;
     if (threadIdx.x < sizeof(Walk) / 4) reinterpret_cast<uint32_t *>(&walk)[threadIdx.x] = reinterpret_cast<const uint32_t *>(&im.walk)[threadIdx.x];
@@ -155,32 +190,17 @@ __global__ void __launch_bounds__(64) k_gd_write(const DecImage *__restrict__ im
     if (i >= sh.g.nsub) return;
     DecState st;
     if (i == 0) { st.p = 0; st.k = 0; st.b = 0; } else st = A[im.sub_off + i - 1];
-    SparseWriteSink sk;
-    sk.walk = &walk; sk.coefs = const_cast<int16_t *>(im.scan.coef); sk.cur = first[im.sub_off + i] - first[im.sub_off]; sk.total = sh.g.total_blocks; sk.anom = 0;
+    SectorWriteSink sk;
+    sk.walk = &walk; sk.coefs = const_cast<int16_t *>(im.scan.coef); sk.dc = dc + im.blk_off; sk.stage = &stage[0][threadIdx.x];
+    sk.cur = first_owned_block(first[im.sub_off + i] - first[im.sub_off], st); sk.total = sh.g.total_blocks; sk.anom = 0;
     sk.seek();
-    decode_subsequence(stream_all + im.stream_off, sh.g, sh.T, i, st, sk);
+    decode_owned_blocks(stream_all + im.stream_off, sh.g, sh.T, i, st, sk);
+    sk.finish();
     if (sk.anom) atomicOr(&marker[blockIdx.y], sk.anom << 1);
 }
 
-// ---- DC: gather differences component-major, inclusive scan, subtract the component's base, scatter ------------------
-__device__ __forceinline__ uint32_t dc_slot_index(const ge::Scan &s, uint32_t u, uint32_t *comp_start)
-{   // position of scan-order unit u inside the image's component-major difference array
-    if (s.ns == 1) { *comp_start = 0; return u; }
-    const uint32_t m = u / s.blocks_per_mcu; int q = (int)(u - m * s.blocks_per_mcu), i = 0; uint32_t start = 0;
-    const uint32_t mcus = (uint32_t)s.mcux * s.mcuy;
-    while (q >= s.hs[i] * s.vs[i]) { q -= s.hs[i] * s.vs[i]; start += mcus * s.hs[i] * s.vs[i]; i++; }
-    *comp_start = start;
-    return start + m * s.hs[i] * s.vs[i] + q;
-}
+// ---- DC: the write pass left the differences component-major; inclusive scan, subtract the component's base, scatter ------------------
 // (a stream that ends before its last block is flagged by the write pass and decoded on the host: nothing to finish here)
-__global__ void k_gd_dc_gather(const DecImage *__restrict__ imgs, int32_t *__restrict__ d)
-{
-    const DecImage &im = imgs[blockIdx.y];
-    const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
-    if (u >= im.g.total_blocks) return;
-    uint32_t cs;
-    d[im.blk_off + dc_slot_index(im.scan, u, &cs)] = ge::locate(im.scan, (int)u).blk[0];
-}
 __global__ void k_gd_dc_scatter(const DecImage *__restrict__ imgs, const int32_t *__restrict__ sum)
 {
     const DecImage &im = imgs[blockIdx.y];
@@ -236,7 +256,11 @@ bool GpuDecoder::prepare(std::vector<Item> &items, void *stream_, std::string &e
         im.sub_off = sub_total; sub_total += G.nsub;
         im.blk_off = blk_total; blk_total += G.total_blocks;
         max_grp = std::max(max_grp, im.ngrp); max_sub = std::max(max_sub, G.nsub); max_blk = std::max(max_blk, G.total_blocks);
-        coef_ptrs[n] = items[n].d_coefs; coef_bytes[n] = (size_t)g.total_coefs * 2;
+        // The write pass stores every block of the scan whole, so the buffer needs no clearing -- unless the layout has blocks the
+        // scan does not code: a single-component scan codes rbw x rbh blocks into a plane pitched bw, and those padding blocks
+        // would have to read as zero.  JpegReader lays a single-component file out at one block per MCU whatever sampling
+        // factors it declares (bw == rbw), so no file it accepts has them today; the layout is still checked, not assumed.
+        coef_ptrs[n] = items[n].d_coefs; coef_bytes[n] = (long long)G.total_blocks * 64 != g.total_coefs ? (size_t)g.total_coefs * 2 : 0;
     }
     if (raw_total >= (1ull << 31) || stream_total >= (1ull << 31)) { err = "decode batch too large"; return false; }
     // ---- launch-side sizes are HIGH-WATER marks, not this batch's exact sizes: grids, scan lengths and the H2D size of the pass
@@ -323,7 +347,7 @@ bool GpuDecoder::enqueue(void *stream_, std::string &err)
     LT_MARK("cub_scan");
     k_gd_unstuff_scatter<<<gg, 128, 0, st>>>(dIw, d_raw, d_off, d_cnt, d_stream);
     LT_MARK("k_gd_unstuff_scatter");
-    for (int n = 0; n < N; n++) CU(cudaMemsetAsync(coef_ptrs[n], 0, coef_bytes[n], st));
+    for (int n = 0; n < N; n++) if (coef_bytes[n]) CU(cudaMemsetAsync(coef_ptrs[n], 0, coef_bytes[n], st));      // padding blocks only
     // ---- rounds
     const dim3 gs(cdiv((long long)hw_msub, 64), N);
     const size_t ncta = (size_t)N * gs.x;                    // dirty flags: two buffers of one byte per CTA, by round parity
@@ -344,19 +368,17 @@ bool GpuDecoder::enqueue(void *stream_, std::string &err)
     tb = d_temp.capacity();
     cub::DeviceScan::ExclusiveSum(d_temp, tb, d_nblk.get(), d_first.get(), (int)hw_sub, st);
     LT_MARK("cub_scan");
-    k_gd_write<<<gs, 64, 0, st>>>(dI, d_stream, dT, d_A, d_first, dM);
+    k_gd_write<<<gs, WRITE_THREADS, 0, st>>>(dI, d_stream, dT, d_A, d_first, d_dc, dM);
     LT_MARK("k_gd_write");
     CU(cudaMemcpyAsync(h_par + o_mark, dM, (size_t)4 * N, cudaMemcpyDeviceToHost, st));
     const dim3 gb(cdiv((long long)hw_mblk, 128), N);
-    k_gd_dc_gather<<<gb, 128, 0, st>>>(dI, d_dc);
-    LT_MARK("k_gd_dc_gather");
     tb = d_temp.capacity();
     cub::DeviceScan::InclusiveSum(d_temp, tb, d_dc.get(), d_dcs.get(), (int)hw_blk, st);
     LT_MARK("cub_scan");
     k_gd_dc_scatter<<<gb, 128, 0, st>>>(dI, d_dcs);
     LT_MARK("k_gd_dc_scatter");
     CU(cudaGetLastError());
-    launches = 10 + nrounds;
+    launches = 9 + nrounds;
     return true;
 }
 

@@ -31,7 +31,7 @@ public:
     GpuDecoder &operator=(const GpuDecoder &) = delete;
     enum Result { OK = 0, NOT_CONVERGED = 1, FAILED = 2 };
     struct Item { const JpegReader *rd; const JpegReader::DeviceScan *ds; int16_t *d_coefs; Result result; };
-    // Decode every item's scan straight into its d_coefs (device; fully overwritten).  Per item: OK, or NOT_CONVERGED
+    // Decode every item's scan straight into its d_coefs (device; fully overwritten, whatever it held before).  Per item: OK, or NOT_CONVERGED
     // (the self-synchronisation did not settle within the round budget -- degenerate periodic streams -- or the stream is
     // damaged: a marker inside it, an invalid code, a run past index 63 or an end before the last block; the caller
     // decodes that image on the host instead).  Returns false on a CUDA failure.  Asynchronous work on `stream`, with one

@@ -13,7 +13,8 @@
 //             data, so a handful of rounds suffice; streams that do not converge within the round budget (degenerate
 //             periodic content) are handed to the host decoder by the caller.
 //   count   : blocks completed per subsequence -> exclusive prefix sum -> first block index of every subsequence.
-//   write   : thread i decodes once more from its true state, writing coefficients (DC as the raw difference).
+//   write   : thread i decodes once more from its true state and stores the blocks that START in its subsequence, whole
+//             (decode_owned_blocks), with the DC as the raw difference, which it also hands to the dc pass.
 //   dc      : per-component prefix sum over the DC differences in scan order.
 #pragma once
 #include <cstdint>
@@ -189,6 +190,18 @@ GE_HD uint32_t lookup_symbol(const DecTables &T, uint32_t base, uint32_t bits)
     return e;
 }
 
+// position of scan-order unit u inside the image's component-major array of DC differences (the DC prefix sum runs over it);
+// *comp_start = where u's component begins in that array
+GE_HD uint32_t dc_slot_index(const ge::Scan &s, uint32_t u, uint32_t *comp_start)
+{
+    if (s.ns == 1) { *comp_start = 0; return u; }
+    const uint32_t m = u / s.blocks_per_mcu; int q = (int)(u - m * s.blocks_per_mcu), i = 0; uint32_t start = 0;
+    const uint32_t mcus = (uint32_t)s.mcux * s.mcuy;
+    while (q >= s.hs[i] * s.vs[i]) { q -= s.hs[i] * s.vs[i]; start += mcus * s.hs[i] * s.vs[i]; i++; }
+    *comp_start = start;
+    return start + m * s.hs[i] * s.vs[i] + q;
+}
+
 // ---- output addressing without divisions -------------------------------------------------------------------------------------
 // Scan-order unit -> coefficient offset, walked incrementally: the write pass finishes a block every dozen symbols, and
 // ge::locate()'s divisions were half of its instructions.  A non-interleaved scan is the special case "one block per MCU".
@@ -196,16 +209,23 @@ struct Walk {
     int bpm, mcux;              // blocks per MCU, MCUs per row (single-component scan: 1, real blocks per row)
     long long base[10];         // int16 offset of block q of MCU (0, 0)
     int colstep[10], rowstep[10];   // offset step to the next MCU in the row / to the next MCU row
+    // the block's place in the image's component-major array of DC differences: dc_base[q] + MCU index * dc_step[q]
+    uint32_t dc_base[10]; int dc_step[10];
 };
 inline Walk make_walk(const ge::Scan &s)
 {
     Walk w{};
-    if (s.ns == 1) { w.bpm = 1; w.mcux = s.rbw; w.base[0] = s.comp_off[0]; w.colstep[0] = 64; w.rowstep[0] = s.bw[0] * 64; return w; }
+    if (s.ns == 1) { w.bpm = 1; w.mcux = s.rbw; w.base[0] = s.comp_off[0]; w.colstep[0] = 64; w.rowstep[0] = s.bw[0] * 64; w.dc_step[0] = 1; return w; }
     w.bpm = s.blocks_per_mcu; w.mcux = s.mcux;
-    int q = 0;
-    for (int i = 0; i < s.ns; i++) for (int by = 0; by < s.vs[i]; by++) for (int bx = 0; bx < s.hs[i]; bx++, q++) if (q < 10) {
-        w.base[q] = s.comp_off[i] + ((long long)by * s.bw[i] + bx) * 64;
-        w.colstep[q] = s.hs[i] * 64; w.rowstep[q] = s.vs[i] * s.bw[i] * 64;
+    int q = 0; uint32_t comp_start = 0;
+    for (int i = 0; i < s.ns; i++) {
+        const int per_mcu = s.hs[i] * s.vs[i];
+        for (int by = 0; by < s.vs[i]; by++) for (int bx = 0; bx < s.hs[i]; bx++, q++) if (q < 10) {
+            w.base[q] = s.comp_off[i] + ((long long)by * s.bw[i] + bx) * 64;
+            w.colstep[q] = s.hs[i] * 64; w.rowstep[q] = s.vs[i] * s.bw[i] * 64;
+            w.dc_base[q] = comp_start + (uint32_t)(by * s.hs[i] + bx); w.dc_step[q] = per_mcu;
+        }
+        comp_start += (uint32_t)s.mcux * (uint32_t)s.mcuy * (uint32_t)per_mcu;
     }
     return w;
 }
@@ -214,16 +234,27 @@ struct Cursor {                 // position of one scan-order unit
     GE_HD void seek(const Walk &w, uint32_t u) { const uint32_t m = u / (uint32_t)w.bpm; q = (int)(u - m * (uint32_t)w.bpm); my = (int)(m / (uint32_t)w.mcux); mx = (int)(m - (uint32_t)my * (uint32_t)w.mcux); }
     GE_HD void next(const Walk &w) { if (++q == w.bpm) { q = 0; if (++mx == w.mcux) { mx = 0; my++; } } }
     GE_HD long long offset(const Walk &w) const { return w.base[q] + (long long)my * w.rowstep[q] + (long long)mx * w.colstep[q]; }
+    GE_HD uint32_t dc_slot(const Walk &w) const { return w.dc_base[q] + (uint32_t)(my * w.mcux + mx) * (uint32_t)w.dc_step[q]; }
 };
 
 // Decode from state `st` until the position leaves subsequence `i` (p >= (i+1)*S) or the stream ends.  Sink receives
 // coef(k, value) for every coefficient (DC as raw difference), block_done(), and -- if it defines anomaly() -- the ANOM_* mask of
 // every symbol and once more when the stream has ended.
-template <class Sink>
-GE_HD DecState decode_subsequence(const uint8_t *__restrict__ stream, const Geometry &g, const DecTables &T, uint32_t i, DecState st, Sink &sk)
+// OWN = false is the form of the synchronisation rounds.  OWN = true is the write pass, where a block belongs to the subsequence
+// in which its DC symbol starts, so that every block has exactly one writer and can be stored whole:
+//   * a block entered in the middle (st.k != 0, the "head") is the previous thread's: it is decoded for its length only and the
+//     sink hears nothing of it, neither coefficients nor anomalies nor its end;
+//   * the thread then owns every block that starts at p < end and decodes PAST `end` until the last of them is complete (or the
+//     stream is over: g.nbits is the only other bound).  A head that reaches `end` leaves the thread without a block of its own.
+// `st` must be the true state.  The blocks completed inside the subsequence, and so first[] (the index of the block that is
+// current at entry), mean what they mean in the rounds: the sink starts at first_owned_block(first[i], st).
+GE_HD uint32_t first_owned_block(uint32_t first_i, const DecState &st) { return first_i + (st.k != 0 ? 1u : 0u); }
+template <bool OWN, class Sink>
+GE_HD DecState decode_span(const uint8_t *__restrict__ stream, const Geometry &g, const DecTables &T, uint32_t i, DecState st, Sink &sk)
 {
     const uint32_t end = (i + 1) * g.subseq_bits < g.nbits ? (i + 1) * g.subseq_bits : g.nbits;
     uint32_t p = st.p; int k = st.k, b = st.b;
+    bool head = OWN && k != 0;
     // Three-word window over the stream: w0 / w1 hold the words the next 32 bits come from, w2 is fetched one word ahead so
     // the load is off the critical path.  A symbol consumes at most 16 + 15 bits, so the window moves by at most one word.
     uint32_t wi = p >> 5;
@@ -233,7 +264,7 @@ GE_HD DecState decode_subsequence(const uint8_t *__restrict__ stream, const Geom
     // per-symbol table choice is a shift and a mask instead of a dependent shared-memory read in front of the table lookup
     uint32_t sel_dc = 0, sel_ac = 0;
     for (int q = 0; q < bpm && q < 10; q++) { sel_dc |= (uint32_t)(T.sel[2 * q] >> LOOK_BITS) << (3 * q); sel_ac |= (uint32_t)(T.sel[2 * q + 1] >> LOOK_BITS) << (3 * q); }
-    while (p < end) {
+    while (p < end || (OWN && k != 0 && !head && p < g.nbits)) {
         if ((p >> 5) != wi) { wi = p >> 5; w0 = w1; w1 = w2; w2 = load_be32(stream, wi + 2); }
         const uint32_t sh = p & 31;
 #if defined(__CUDA_ARCH__)
@@ -250,16 +281,29 @@ GE_HD DecState decode_subsequence(const uint8_t *__restrict__ stream, const Geom
         const uint32_t ext = s ? (bits << len) >> (32 - s) : 0u;
         const int v = s ? ((int)ext < (1 << (s - 1)) ? (int)ext - (1 << s) + 1 : (int)ext) : 0;
         const bool eob_or_zrl = !dc && s == 0;                                     // AC symbol without a value: ZRL or EOB
-        report_anomaly(sk, symbol_anomaly(len, sym, dc, k, p + (uint32_t)(len + s), g.nbits), 0);  // only the write sink looks
+        if (!head) report_anomaly(sk, symbol_anomaly(len, sym, dc, k, p + (uint32_t)(len + s), g.nbits), 0);  // only the write sink looks
         int kw = k + r; if (kw > 63) kw = 63;                                       // corrupt / unsynchronised run: clamp
-        if (!eob_or_zrl) sk.coef(kw, v);
+        if (!eob_or_zrl && !head) sk.coef(kw, v);
         k = eob_or_zrl ? (r == 15 ? k + 16 : 64) : kw + 1;
         p += (uint32_t)(len + s);
-        if (k >= 64) { k = 0; b++; if (b == bpm) b = 0; sk.block_done(); }
+        if (k >= 64) {
+            k = 0; b++; if (b == bpm) b = 0;
+            if (head) head = false; else sk.block_done();
+        }
     }
     if (p >= g.nbits) report_anomaly(sk, ANOM_END, 0);         // the stream is over: reported if the sink is still inside a real block
     DecState o; o.p = p; o.k = (uint16_t)k; o.b = (uint16_t)b;
     return o;
+}
+template <class Sink>
+GE_HD DecState decode_subsequence(const uint8_t *__restrict__ stream, const Geometry &g, const DecTables &T, uint32_t i, DecState st, Sink &sk)
+{
+    return decode_span<false>(stream, g, T, i, st, sk);
+}
+template <class Sink>
+GE_HD void decode_owned_blocks(const uint8_t *__restrict__ stream, const Geometry &g, const DecTables &T, uint32_t i, DecState st, Sink &sk)
+{
+    decode_span<true>(stream, g, T, i, st, sk);
 }
 
 struct NullSink { uint32_t nblk = 0; GE_HD void coef(int, int) {} GE_HD void block_done() { nblk++; } };
