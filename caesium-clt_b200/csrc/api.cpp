@@ -342,7 +342,12 @@ b200_status jpeg_compress(const uint8_t *in, size_t in_len, const b200_params *p
     const b200_status st = decode_into_slot(s, rd, on_device, err, &tm);
     if (st.code) return st;
     tm.lap(2);
-    if (!(resize ? slot_transform_resized(s, gin, gout, err, !gpu_entropy, !on_device) : slot_transform(s, gin, gout, err, !gpu_entropy, !on_device))) return make_status(B200_ERR_CUDA, err);
+    SamplePlan sp;
+    uint8_t *full[3], *rz[3];
+    const bool ok = resize ? plan_samples(s, gin, gout.width, gout.height, &gout, sp, err) && samples_from_coefs(s, gin, sp, !on_device, true, full, err) &&
+                                 resize_samples(s, full, sp, rz, err) && coefs_from_samples(s, rz, gout, sp, err)
+                           : slot_transform(s, gin, gout, err, false, !on_device);
+    if (!ok || (!gpu_entropy && !slot_download_coefs(s, plan.out_bytes, err))) return make_status(B200_ERR_CUDA, err);
     tm.lap(3);
     if (gpu_entropy) return encode_from_slot(s, gout, wo, &rd.meta(), out, err, &tm);
     jpeg_fill_dummy_blocks(gout, s->h_out);
@@ -583,13 +588,20 @@ b200_status png_from_planes(Slot *s, const uint8_t *planes, int nc, const uint8_
     return ok_status();
 }
 
-// Lanczos3 (K3) of nc host planes [nc][h][w] to [nc][nh][nw], fetched back into dst
+// Lanczos3 (K3) of nc host planes [nc][h][w] to nc device planes of nw x nh on the slot
+bool resize_host_planes(Slot *s, const uint8_t *src, uint32_t w, uint32_t h, uint32_t nw, uint32_t nh, int nc, uint8_t **planes, std::string &err)
+{
+    SamplePlan sp;
+    uint8_t *full[3];
+    return plan_samples(s, planar_geom(w, h, nc), (int)nw, (int)nh, nullptr, sp, err) && samples_from_host(s, src, sp, full, err) && resize_samples(s, full, sp, planes, err);
+}
+
+// the same, fetched back into dst [nc][nh][nw]
 bool resize_to_host(Slot *s, const uint8_t *src, uint32_t w, uint32_t h, uint32_t nw, uint32_t nh, int nc, std::vector<uint8_t> &dst, std::string &err)
 {
-    const JpegGeom gin = planar_geom(w, h, nc);
-    uint8_t *dp[3] = {nullptr, nullptr, nullptr};
+    uint8_t *rz[3];
     dst.resize((size_t)nc * nw * nh);
-    return slot_transform_resized(s, gin, with_size(gin, nw, nh), err, false, false, dp, src) && slot_fetch_planes(s, dp, nc, (size_t)nw * nh, dst.data(), err);
+    return resize_host_planes(s, src, w, h, nw, nh, nc, rz, err) && slot_fetch_planes(s, rz, nc, (size_t)nw * nh, dst.data(), err);
 }
 
 // ---- conversion to WebP (lossy VP8) ----------------------------------------------------------------------------------
@@ -606,20 +618,22 @@ b200_status jpeg_to_webp(const uint8_t *in, size_t in_len, const b200_params *p,
     uint32_t nw, nh;
     b200_status st = target_size((uint32_t)gin.width, (uint32_t)gin.height, p, 16383, nw, nh, "invalid target dimensions for WebP");
     if (st.code) return st;
-    const JpegGeom gout = with_size(gin, nw, nh);
     SlotLease s(prefer_dev);
     if (!s) return s.failure();
     static const bool verbose = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2;
     const auto t0 = std::chrono::steady_clock::now();
-    if (!s->ensure((size_t)gin.total_coefs * 2, (size_t)gout.total_coefs * 2, 0, 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    if (!s->ensure((size_t)gin.total_coefs * 2, 0, 0, 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
     bool on_device;
     if ((st = decode_into_slot(s, rd, on_device, err)).code) return st;
     const auto t1 = std::chrono::steady_clock::now();
-    uint8_t *rgb[3] = {nullptr, nullptr, nullptr};
-    if (!slot_transform_resized(s, gin, gout, err, false, !on_device, rgb)) return make_status(B200_ERR_CUDA, err);
+    SamplePlan sp;
+    uint8_t *full[3], *rgb[3];
+    if (!(plan_samples(s, gin, (int)nw, (int)nh, nullptr, sp, err) && samples_from_coefs(s, gin, sp, !on_device, true, full, err) && resize_samples(s, full, sp, rgb, err)))
+        return make_status(B200_ERR_CUDA, err);
     const auto t2 = std::chrono::steady_clock::now();
     WebpDevice *webp = s->webp_dev();
-    if (!webp->encode_planes(rgb[0], rgb[1], rgb[2], (int)nw, (int)nh, (int)p->webp_quality, s->stream, out, err)) return make_status(B200_ERR_CUDA, err);
+    const int g = gin.ncomp == 3;          // a grey source is its one plane three times
+    if (!webp->encode_planes(rgb[0], rgb[g], rgb[2 * g], (int)nw, (int)nh, (int)p->webp_quality, s->stream, out, err)) return make_status(B200_ERR_CUDA, err);
     if (verbose) {
         auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
         fprintf(stderr, "[b200 trace] jpeg %dx%d -> webp %ux%u: segment walk + entropy decode (device %d) %.1f ms, transform + resize launch %.1f ms, VP8 (wait for the device %.1f ms, boolean coder %.1f ms) %.1f ms\n",
@@ -642,16 +656,17 @@ b200_status jpeg_to_png(const uint8_t *in, size_t in_len, const b200_params *p, 
     uint32_t nw, nh;
     b200_status st = target_size((uint32_t)gin.width, (uint32_t)gin.height, p, 65535, nw, nh, "invalid target dimensions");
     if (st.code) return st;
-    const JpegGeom gout = with_size(gin, nw, nh);
     SlotLease s(prefer_dev);
     if (!s) return s.failure();
-    if (!s->ensure((size_t)gin.total_coefs * 2, (size_t)gout.total_coefs * 2, 0, 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    if (!s->ensure((size_t)gin.total_coefs * 2, 0, 0, 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
     bool on_device;
     if ((st = decode_into_slot(s, rd, on_device, err)).code) return st;
     const int nc = gin.ncomp == 1 ? 1 : 3;
-    uint8_t *rgb[3] = {nullptr, nullptr, nullptr};
+    SamplePlan sp;
+    uint8_t *full[3], *rgb[3];
     std::vector<uint8_t> planes((size_t)nc * nw * nh);
-    if (!slot_transform_resized(s, gin, gout, err, false, !on_device, rgb) || !slot_fetch_planes(s, rgb, nc, (size_t)nw * nh, planes.data(), err))
+    if (!(plan_samples(s, gin, (int)nw, (int)nh, nullptr, sp, err) && samples_from_coefs(s, gin, sp, !on_device, true, full, err) && resize_samples(s, full, sp, rgb, err) &&
+          slot_fetch_planes(s, rgb, nc, (size_t)nw * nh, planes.data(), err)))
         return make_status(B200_ERR_CUDA, err);
     return png_from_planes(s, planes.data(), nc, nullptr, nw, nh, false, p, out, err);
 }
@@ -700,7 +715,10 @@ b200_status planes_to_jpeg(const std::vector<uint8_t> &planes, uint32_t w, uint3
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
     SlotLease s(prefer_dev);
     if (!s) return s.failure();
-    if (!slot_transform_resized(s, gin, gout, err, false, false, nullptr, planes.data())) return make_status(B200_ERR_CUDA, err);
+    SamplePlan sp;
+    uint8_t *full[3], *rz[3];
+    if (!(plan_samples(s, gin, gout.width, gout.height, &gout, sp, err) && samples_from_host(s, planes.data(), sp, full, err) && resize_samples(s, full, sp, rz, err) &&
+          coefs_from_samples(s, rz, gout, sp, err))) return make_status(B200_ERR_CUDA, err);
     return encode_from_slot(s, gout, write_options(p), nullptr, out, err);      // no source metadata: only `progressive` matters
 }
 
@@ -732,10 +750,8 @@ b200_status rgb_to_webp(const std::vector<uint8_t> &rgb, uint32_t w, uint32_t h,
     if (!resize) {
         if (!webp->encode_host_rgb(rgb.data(), (int)nw, (int)nh, (int)p->webp_quality, s->stream, out, err)) return make_status(B200_ERR_CUDA, err);
     } else {   // through the resize leg (K3 Lanczos3) first
-        const JpegGeom gin = planar_geom(w, h, 3);
-        uint8_t *planes[3] = {nullptr, nullptr, nullptr};
-        if (!slot_transform_resized(s, gin, with_size(gin, nw, nh), err, false, false, planes, rgb.data()) ||
-            !webp->encode_planes(planes[0], planes[1], planes[2], (int)nw, (int)nh, (int)p->webp_quality, s->stream, out, err)) return make_status(B200_ERR_CUDA, err);
+        uint8_t *planes[3];
+        if (!resize_host_planes(s, rgb.data(), w, h, nw, nh, 3, planes, err) || !webp->encode_planes(planes[0], planes[1], planes[2], (int)nw, (int)nh, (int)p->webp_quality, s->stream, out, err)) return make_status(B200_ERR_CUDA, err);
     }
     if (!alpha) return ok_status();
     const size_t n = (size_t)nw * nh;
@@ -1189,10 +1205,9 @@ static b200_status webp_to_size(const uint8_t *in, size_t in_len, b200_params *p
     SlotLease s(-1);
     if (!s) return s.failure();
     WebpDevice *webp = s->webp_dev();
-    uint8_t *planes[3] = {nullptr, nullptr, nullptr};
-    const JpegGeom gin = planar_geom((uint32_t)wi.width, (uint32_t)wi.height, 3);
+    uint8_t *planes[3];
     // the (possibly resized) RGB planes stay in the slot's scratch memory for all tries
-    if (!slot_transform_resized(s, gin, with_size(gin, nw, nh), err, false, false, planes, rgb.data())) return make_status(B200_ERR_CUDA, err);
+    if (!resize_host_planes(s, rgb.data(), (uint32_t)wi.width, (uint32_t)wi.height, nw, nh, 3, planes, err)) return make_status(B200_ERR_CUDA, err);
     auto size_at = [&](int q, auto want, size_t &sz, std::vector<uint8_t> &cur) -> b200_status {
         std::string e2; (void)want;
         if (!webp->encode_planes(planes[0], planes[1], planes[2], (int)nw, (int)nh, q, s->stream, cur, e2)) return make_status(B200_ERR_CUDA, e2);
@@ -1426,7 +1441,10 @@ b200_status b200_jpeg_decode_planes(const b200_jpeg_layout *in_layout, const int
     if (!s) return s.failure();
     if (!s->ensure((size_t)gin.total_coefs * 2, 256, 256, 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
     memcpy(s->h_in, in_coefs, (size_t)gin.total_coefs * 2);
-    if (!slot_decode_planes(s, gin, planes, err)) return make_status(B200_ERR_CUDA, err);
+    SamplePlan sp;
+    uint8_t *full[3];
+    if (!(plan_samples(s, gin, gin.width, gin.height, nullptr, sp, err) && samples_from_coefs(s, gin, sp, true, false, full, err) &&
+          slot_fetch_planes(s, full, gin.ncomp, (size_t)gin.width * gin.height, planes, err))) return make_status(B200_ERR_CUDA, err);
     return ok_status();
 }
 

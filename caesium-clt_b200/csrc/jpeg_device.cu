@@ -260,8 +260,8 @@ bool Slot::ensure(size_t in_bytes, size_t out_bytes, size_t scratch_bytes, size_
 
 // Parameter block of a transform over K images, each part 256-byte aligned:
 //   QuantDev q[4] (per output table) | uint16 dq[K][4][64] (per image and input component, zigzag) | CompWork work[]
-// The resize leg appends its axis tables after the work descriptors.  With trellis quantisation on, JtTable[4] (beside q[4],
-// per output table) comes last.
+// With trellis quantisation on, JtTable[4] (beside q[4], per output table) comes last.  The sample stages lay out K = 1 the same way
+// (see SamplePlan).
 static constexpr size_t par_dq_off = align_up(sizeof(QuantDev) * 4, 256);
 static size_t par_work_off(int K) { return par_dq_off + align_up(sizeof(uint16_t) * 256 * K, 256); }
 static constexpr size_t par_trellis_bytes = 256 + sizeof(JtTable) * 4;      // alignment + the tables
@@ -507,135 +507,87 @@ bool slot_fetch_planes(Slot *s, uint8_t *const *d_planes, int nplanes, size_t n,
     return true;
 }
 
-bool slot_decode_planes(Slot *s, const JpegGeom &gin, uint8_t *planes, std::string &err)
+bool plan_samples(Slot *s, const JpegGeom &gin, int nw, int nh, const JpegGeom *gout, SamplePlan &p, std::string &err)
 {
-    // route every component through idct (+ upsample) by planning against a 4:4:4 output of the same size
-    JpegGeom gout = gin;
-    for (int c = 0; c < gin.ncomp; c++) { gout.hs[c] = gout.vs[c] = 1; }
-    gout.finalize();
-    cudaStream_t st = (cudaStream_t)s->stream;
-    ImagePlan plan; plan = ImagePlan();
-    size_t off_plane = 0, off_full = 0;
-    for (int c = 0; c < gin.ncomp; c++) {
-        if (gin.hmax % gin.hs[c] || gin.vmax % gin.vs[c]) { err = "fractional sampling ratio unsupported"; return false; }
-        plan.path[c] = PATH_GENERIC;
-        plan.plane_off[c] = off_plane; off_plane += align_up((size_t)gin.bw[c] * 8 * gin.bh[c] * 8, 256);
-        plan.full_off[c] = off_full; off_full += align_up((size_t)gin.width * gin.height, 256);
+    p = SamplePlan();
+    const int nc = gin.ncomp;
+    if (gout && gout->ncomp != nc) { err = "component count mismatch"; return false; }
+    p.nc = nc; p.w = gin.width; p.h = gin.height; p.nw = nw; p.nh = nh;
+    size_t idct = 0, later = 0;
+    for (int c = 0; c < nc; c++) {
+        if (gin.hmax % gin.hs[c] || gin.vmax % gin.vs[c] || (gout && (gout->hmax % gout->hs[c] || gout->vmax % gout->vs[c]))) { err = "fractional sampling ratio unsupported"; return false; }
+        p.front.path[c] = PATH_GENERIC;
+        p.front.plane_off[c] = idct; idct += align_up((size_t)gin.bw[c] * 8 * gin.bh[c] * 8, 256);
+        p.front.full_off[c] = p.front.full_bytes; p.front.full_bytes += align_up((size_t)gin.width * gin.height, 256);
     }
-    plan.plane_bytes = off_plane; plan.full_bytes = off_full; plan.dplane_bytes = 0;
-    plan.in_bytes = (size_t)gin.total_coefs * 2; plan.out_bytes = 256;
-    const size_t work_off = par_work_off(1);
-    if (!s->ensure(plan.in_bytes, std::max(plan.out_bytes, plan.full_bytes), plan.scratch_bytes(), work_off + sizeof(CompWork) * 4 * 6, err)) return false;
+    for (int c = 0; (nw != p.w || nh != p.h) && c < nc; c++) { p.rz_off[c] = later; later += align_up((size_t)nw * nh, 256); }
+    for (int c = 0; gout && c < nc; c++) { p.dpl_off[c] = later; later += align_up((size_t)gout->rbw[c] * 8 * gout->rbh[c] * 8, 256); }
+    p.front.plane_bytes = std::max(idct, later);
+    p.in_bytes = (size_t)gin.total_coefs * 2; p.out_bytes = gout ? (size_t)gout->total_coefs * 2 : 0;
+    p.scratch_bytes = p.front.scratch_bytes();
+    p.trellis = gout && jpeg_trellis();
+    p.sink_off = par_work_off(1) + sizeof(CompWork) * 2 * nc;                  // front end: idct, up
+    p.par_bytes = !gout ? p.sink_off : p.sink_off + sizeof(CompWork) * 3 * nc + (p.trellis ? par_trellis_bytes : 0);     // down, fdct, trel
+    return s->ensure(p.in_bytes, p.out_bytes, p.scratch_bytes, p.par_bytes, err);
+}
+
+bool samples_from_coefs(Slot *s, const JpegGeom &gin, const SamplePlan &p, bool upload, bool rgb, uint8_t **planes, std::string &err)
+{
+    cudaStream_t st = (cudaStream_t)s->stream;
+    JpegGeom g444 = gin;            // every component through IDCT + upsampling: planned against a 4:4:4 output of the same size
+    for (int c = 0; c < gin.ncomp; c++) g444.hs[c] = g444.vs[c] = 1;
+    g444.finalize();
     WorkLists wl;
-    append_image_work(gin, gout, plan, s->d_in, s->d_out, s->d_scratch, put_dequant(s, 0, gin), dev_quant(s), wl);
+    append_image_work(gin, g444, p.front, s->d_in, s->d_out, s->d_scratch, put_dequant(s, 0, gin), dev_quant(s), wl);
     wl.down.clear(); wl.fdct.clear();
-    size_t nw = flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + work_off));
-    CU(cudaMemcpyAsync(s->d_par, s->h_par, work_off + nw * sizeof(CompWork), cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(s->d_in, s->h_in, plan.in_bytes, cudaMemcpyHostToDevice, st));
-    const int rc = launch_work(wl, reinterpret_cast<const CompWork *>(s->d_par + work_off), st);
-    if (!launch_ok(rc, "kernel launch", err)) return false;
-    uint8_t *h = reinterpret_cast<uint8_t *>(s->h_out.get());
-    for (int c = 0; c < gin.ncomp; c++)
-        CU(cudaMemcpyAsync(h + (size_t)c * gin.width * gin.height, s->d_scratch + plan.plane_bytes + plan.full_off[c], (size_t)gin.width * gin.height, cudaMemcpyDeviceToHost, st));
-    CU(stream_wait(st));
-    memcpy(planes, h, (size_t)gin.ncomp * gin.width * gin.height);
+    const size_t work_off = par_work_off(1), end = work_off + flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + work_off)) * sizeof(CompWork);
+    CU(cudaMemcpyAsync(s->d_par + par_dq_off, s->h_par + par_dq_off, end - par_dq_off, cudaMemcpyHostToDevice, st));
+    if (upload) CU(cudaMemcpyAsync(s->d_in, s->h_in, p.in_bytes, cudaMemcpyHostToDevice, st));
+    if (!launch_ok(launch_work(wl, reinterpret_cast<const CompWork *>(s->d_par + work_off), st), "kernel launch", err)) return false;
+    for (int c = 0; c < p.nc; c++) planes[c] = s->d_scratch + p.front.plane_bytes + p.front.full_off[c];
+    if (rgb && p.nc == 3 && !launch_ok(launch_ycc_to_rgb(planes[0], planes[1], planes[2], (size_t)p.w * p.h, st), "ycc_to_rgb", err)) return false;
     return true;
 }
 
-// ---- resize path: decode -> (YCbCr->RGB) -> Lanczos3 -> (RGB->YCbCr) -> encode side --------------------------------
-bool slot_transform_resized(Slot *s, const JpegGeom &gin, const JpegGeom &gout, std::string &err, bool download, bool upload, uint8_t **rgb_out,
-                            const uint8_t *host_rgb)
+bool samples_from_host(Slot *s, const uint8_t *host, const SamplePlan &p, uint8_t **planes, std::string &err)
 {
-    const int W = gin.width, H = gin.height, NW = gout.width, NH = gout.height, nc = gin.ncomp;
-    if (gout.ncomp != nc) { err = "component count mismatch"; return false; }
-    cudaStream_t st = (cudaStream_t)s->stream;
-    ResizeAxis av, ah;
-    make_resize_axis(H, NH, av);
-    make_resize_axis(W, NW, ah);
-    // scratch layout
-    size_t off = 0, plane_off[4], full_off[4], rz_off[4], dpl_off[4];
-    for (int c = 0; c < nc; c++) {
-        if (gin.hmax % gin.hs[c] || gin.vmax % gin.vs[c] || gout.hmax % gout.hs[c] || gout.vmax % gout.vs[c]) { err = "fractional sampling ratio unsupported"; return false; }
-        plane_off[c] = off; off += align_up((size_t)gin.bw[c] * 8 * gin.bh[c] * 8, 256);
+    const size_t n = (size_t)p.w * p.h;
+    for (int c = 0; c < p.nc; c++) {
+        planes[c] = s->d_scratch + p.front.plane_bytes + p.front.full_off[c];
+        CU(cudaMemcpyAsync(planes[c], host + c * n, n, cudaMemcpyHostToDevice, (cudaStream_t)s->stream));
     }
-    for (int c = 0; c < nc; c++) { full_off[c] = off; off += align_up((size_t)W * H, 256); }
-    for (int c = 0; c < nc; c++) { rz_off[c] = off; off += align_up((size_t)NW * NH, 256); }
-    for (int c = 0; c < nc; c++) { dpl_off[c] = off; off += align_up((size_t)gout.rbw[c] * 8 * gout.rbh[c] * 8, 256); }
-    const size_t tmp_off = off; off += align_up((size_t)NH * W * sizeof(float), 256);
-    // parameter block: tables | work | axis tables
-    const size_t work_off = par_work_off(1);
-    const size_t lv = align_up(work_off + sizeof(CompWork) * nc * 5, 256), cv = lv + align_up(sizeof(int) * NH, 256), wv = cv + align_up(sizeof(int) * NH, 256);
-    const size_t lh = wv + align_up(sizeof(float) * av.weights.size(), 256), chh = lh + align_up(sizeof(int) * NW, 256), wh = chh + align_up(sizeof(int) * NW, 256);
-    const size_t axes_end = wh + align_up(sizeof(float) * ah.weights.size(), 256);
-    const bool trellis = !rgb_out && jpeg_trellis();
-    const size_t pbytes = axes_end + (trellis ? par_trellis_bytes : 0);
-    const size_t in_bytes = (size_t)gin.total_coefs * 2, out_bytes = (size_t)gout.total_coefs * 2;
-    if (!s->ensure(in_bytes, out_bytes, off, pbytes, err)) return false;
+    return true;
+}
+
+bool resize_samples(Slot *s, uint8_t *const *in, const SamplePlan &p, uint8_t **out, std::string &err)
+{
+    const bool same = p.nw == p.w && p.nh == p.h;
+    for (int c = 0; c < p.nc; c++) out[c] = same ? in[c] : s->d_scratch + p.rz_off[c];
+    return s->resampler.run(in, p.w, p.h, out, p.nw, p.nh, p.nc, s->stream, err);
+}
+
+bool coefs_from_samples(Slot *s, uint8_t *const *planes, const JpegGeom &gout, const SamplePlan &p, std::string &err)
+{
+    cudaStream_t st = (cudaStream_t)s->stream;
+    const int nc = gout.ncomp;
+    if (nc == 3 && !launch_ok(launch_rgb_to_ycc(planes[0], planes[1], planes[2], (size_t)gout.width * gout.height, st), "rgb_to_ycc", err)) return false;
     put_quant(s, gout);
-    const uint16_t *d_dq = put_dequant(s, 0, gin);
-    const QuantDev *d_q = dev_quant(s);
-    memcpy(s->h_par + lv, av.left.data(), sizeof(int) * NH); memcpy(s->h_par + cv, av.count.data(), sizeof(int) * NH);
-    memcpy(s->h_par + wv, av.weights.data(), sizeof(float) * av.weights.size());
-    memcpy(s->h_par + lh, ah.left.data(), sizeof(int) * NW); memcpy(s->h_par + chh, ah.count.data(), sizeof(int) * NW);
-    memcpy(s->h_par + wh, ah.weights.data(), sizeof(float) * ah.weights.size());
     WorkLists wl;
     for (int c = 0; c < nc; c++) {
-        CompWork d; memset(&d, 0, sizeof(d));   // decode side
-        d.cin = s->d_in + gin.comp_offset[c]; d.dq = d_dq + 64 * c; d.q = d_q;
-        d.bw_in = gin.bw[c]; d.bh_in = gin.bh[c]; d.rbw_in = gin.rbw[c]; d.rbh_in = gin.rbh[c]; d.cw = gin.cw[c]; d.ch = gin.ch[c];
-        d.W = W; d.H = H; d.pstride = gin.bw[c] * 8; d.fstride = W;
-        d.up_hx = gin.hmax / gin.hs[c]; d.up_vx = gin.vmax / gin.vs[c]; d.dn_hx = d.dn_vx = 1;
-        d.plane = s->d_scratch + plane_off[c]; d.full = s->d_scratch + full_off[c];
-        wl.idct.push_back(d); wl.max_idct = std::max(wl.max_idct, work_tiles(d.rbw_in, d.rbh_in));
-        wl.up.push_back(d); wl.max_up_w = W; wl.max_up_h = H;
-        CompWork e; memset(&e, 0, sizeof(e));   // encode side
-        e.cout = s->d_out + gout.comp_offset[c]; e.dq = d_dq; e.q = d_q + gout.tq[c];
+        CompWork e; memset(&e, 0, sizeof(e));
+        e.cout = s->d_out + gout.comp_offset[c]; e.q = dev_quant(s) + gout.tq[c];
         e.bw_out = gout.bw[c]; e.bh_out = gout.bh[c]; e.rbw_out = gout.rbw[c]; e.rbh_out = gout.rbh[c];
-        e.W = NW; e.H = NH; e.fstride = NW; e.full = s->d_scratch + rz_off[c]; e.dplane = s->d_scratch + dpl_off[c];
+        e.W = gout.width; e.H = gout.height; e.fstride = gout.width; e.full = planes[c]; e.dplane = s->d_scratch + p.dpl_off[c];
         e.dn_hx = gout.hmax / gout.hs[c]; e.dn_vx = gout.vmax / gout.vs[c]; e.up_hx = e.up_vx = 1;
         wl.down.push_back(e); wl.max_dn_w = std::max(wl.max_dn_w, e.rbw_out * 8); wl.max_dn_h = std::max(wl.max_dn_h, e.rbh_out * 8);
         wl.fdct.push_back(e); wl.max_fdct = std::max(wl.max_fdct, work_tiles(e.rbw_out, e.rbh_out));
     }
-    if (trellis) put_trellis(s, gout, axes_end, wl);
-    flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + work_off));
-    CU(cudaMemcpyAsync(s->d_par, s->h_par, pbytes, cudaMemcpyHostToDevice, st));
-    if (upload && !host_rgb) CU(cudaMemcpyAsync(s->d_in, s->h_in, in_bytes, cudaMemcpyHostToDevice, st));
-    const CompWork *dw = reinterpret_cast<const CompWork *>(s->d_par + work_off);
-    const CompWork *p_idct = dw, *p_up = p_idct + wl.idct.size(), *p_down = p_up + wl.up.size(), *p_fdct = p_down + wl.down.size();
-    const CompWork *p_trel = p_fdct + wl.fdct.size();
-    uint8_t *full[3] = {s->d_scratch + full_off[0], nc == 3 ? s->d_scratch + full_off[1] : nullptr, nc == 3 ? s->d_scratch + full_off[2] : nullptr};
-    uint8_t *rz[3] = {s->d_scratch + rz_off[0], nc == 3 ? s->d_scratch + rz_off[1] : nullptr, nc == 3 ? s->d_scratch + rz_off[2] : nullptr};
-    if (host_rgb) {   // samples that never were a JPEG (PNG source): planar RGB (or one grey plane) straight into the full-resolution planes
-        for (int c = 0; c < nc; c++) CU(cudaMemcpyAsync(full[c], host_rgb + (size_t)c * W * H, (size_t)W * H, cudaMemcpyHostToDevice, st));
-    } else {
-        if (!launch_ok(launch_idct_plane(p_idct, nc, wl.max_idct, st), "idct", err)) return false;
-        if (!launch_ok(launch_upsample(p_up, nc, W, H, st), "upsample", err)) return false;
-        if (nc == 3 && !launch_ok(launch_ycc_to_rgb(full[0], full[1], full[2], (size_t)W * H, st), "ycc_to_rgb", err)) return false;
-    }
-    float *tmp = reinterpret_cast<float *>(s->d_scratch + tmp_off);
-    for (int c = 0; c < nc; c++) {
-        if (NW == W && NH == H) {   // imageops::resize copies when the dimensions are unchanged
-            CU(cudaMemcpyAsync(rz[c], full[c], (size_t)W * H, cudaMemcpyDeviceToDevice, st));
-            continue;
-        }
-        if (!launch_ok(launch_resize_v(full[c], W, H, W, tmp, NH, reinterpret_cast<const int *>(s->d_par + lv), reinterpret_cast<const int *>(s->d_par + cv),
-                                 reinterpret_cast<const float *>(s->d_par + wv), av.cap, st), "resize_v", err)) return false;
-        if (!launch_ok(launch_resize_h(tmp, W, rz[c], NW, NH, NW, reinterpret_cast<const int *>(s->d_par + lh), reinterpret_cast<const int *>(s->d_par + chh),
-                                 reinterpret_cast<const float *>(s->d_par + wh), ah.cap, st), "resize_h", err)) return false;
-    }
-    if (rgb_out) { rgb_out[0] = rz[0]; rgb_out[1] = nc == 3 ? rz[1] : rz[0]; rgb_out[2] = nc == 3 ? rz[2] : rz[0]; return true; }
-    if (nc == 3 && !launch_ok(launch_rgb_to_ycc(rz[0], rz[1], rz[2], (size_t)NW * NH, st), "rgb_to_ycc", err)) return false;
-    if (!launch_ok(launch_downsample(p_down, nc, wl.max_dn_w, wl.max_dn_h, st), "downsample", err)) return false;
-    if (!launch_ok(launch_fdct_plane(p_fdct, nc, wl.max_fdct, st, trellis), "fdct", err)) return false;
-    if (trellis) {
-        const int rc = launch_jpeg_trellis(p_trel, nc, wl.max_trel, wl.trel_q, wl.trel_t, st);
-        LT_MARK("k_jpeg_trellis");
-        if (!launch_ok(rc, "trellis", err)) return false;
-    }
-    if (!download) return true;
-    CU(cudaMemcpyAsync(s->h_out, s->d_out, out_bytes, cudaMemcpyDeviceToHost, st));
-    CU(stream_wait(st));
-    return true;
+    const size_t tables_end = p.trellis ? put_trellis(s, gout, p.sink_off + sizeof(CompWork) * 3 * nc, wl) : 0;
+    const size_t works_end = p.sink_off + flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + p.sink_off)) * sizeof(CompWork);
+    const size_t end = p.trellis ? tables_end : works_end;
+    CU(cudaMemcpyAsync(s->d_par, s->h_par, sizeof(QuantDev) * 4, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(s->d_par + p.sink_off, s->h_par + p.sink_off, end - p.sink_off, cudaMemcpyHostToDevice, st));
+    return launch_ok(launch_work(wl, reinterpret_cast<const CompWork *>(s->d_par + p.sink_off), st), "kernel launch", err);
 }
 
 } // namespace b200

@@ -11,6 +11,7 @@
 #include "jpeg_kernels.h"
 #include "jpeg_gpudec.h"
 #include "jpeg_gpuenc.h"
+#include "resize_kernels.h"
 
 namespace b200 {
 
@@ -82,6 +83,7 @@ struct Slot {
     WebpDevice *webp_dev();
     Vp8lDevice *vp8l_dev();
     GifDevice *gif_dev();
+    Resampler resampler{Grow::Slot};                                                     // K3 of the sample stages
     Slot();
     Slot(const Slot &) = delete;
     Slot &operator=(const Slot &) = delete;
@@ -99,7 +101,7 @@ int  runtime_device_ordinal(int dev_index);                         // CUDA ordi
 
 // Run the transform for ONE image whose input coefficients already sit in s->h_in; result lands in s->h_out.
 bool slot_transform(Slot *s, const JpegGeom &gin, const JpegGeom &gout, std::string &err, bool download = true, bool upload = true);
-// D2H of the output coefficients left in HBM by a download=false transform (host-encoder fallback)
+// D2H of the output coefficients left in HBM by a download=false transform or coefs_from_samples (host encoder)
 bool slot_download_coefs(Slot *s, size_t out_bytes, std::string &err);
 // Entropy-decode a baseline single-scan file on the device into s->d_in (0 ok, 1 not converged -> host decode, 2 failed)
 int slot_gpu_decode(Slot *s, const JpegReader &rd, const JpegReader::DeviceScan &ds, std::string &err);
@@ -132,16 +134,40 @@ bool slot_gpu_encode(Slot *s, const JpegGeom &gout, bool progressive, std::strin
 // the same without fetching the stuffed scans (results carry lengths only); slot_gpu_fetch() brings them over afterwards
 bool slot_gpu_encode_sizes(Slot *s, const JpegGeom &gout, bool progressive, std::string &err);
 bool slot_gpu_fetch(Slot *s, std::string &err);
-// Resize path (CSParameters.width/height): gout carries the TARGET dimensions; decode -> RGB -> Lanczos3 -> YCbCr -> encode.
-// rgb_out != nullptr: stop after the resize and hand back the three device planes (R, G, B of the TARGET size, pitch = target
-// width; a greyscale source returns its single plane three times) -- the front end of the format-conversion paths.
-// host_rgb != nullptr: the source is not a JPEG -- planar samples [ncomp][H][W] (RGB, or one grey plane) replace the decode
-// front end; gin then only carries width / height / ncomp with 1x1 sampling.
-bool slot_transform_resized(Slot *s, const JpegGeom &gin, const JpegGeom &gout, std::string &err, bool download = true, bool upload = true,
-                            uint8_t **rgb_out = nullptr, const uint8_t *host_rgb = nullptr);
-// D2H of nplanes device planes of n bytes each (rgb_out of slot_transform_resized) into one host buffer, synchronised
+// D2H of nplanes device planes of n bytes each into one host buffer, synchronised
 bool slot_fetch_planes(Slot *s, uint8_t *const *d_planes, int nplanes, size_t n, uint8_t *host, std::string &err);
-// Same front end, but stop after IDCT + upsample and copy planar full-res samples into `planes` (host).
-bool slot_decode_planes(Slot *s, const JpegGeom &gin, uint8_t *planes, std::string &err);
+
+// ---- sample stages: 8-bit planar samples on the slot, between a decode front end, K3 and the encode back end -------------------
+// A caller chains them: samples_from_coefs or samples_from_host -> resize_samples -> coefs_from_samples (then the device entropy
+// encoder, or slot_download_coefs for the host one), an encoder that reads device planes, or slot_fetch_planes.  Two facts of the
+// slot make plan_samples fix every stage's region of d_scratch and of the parameter block before anything is enqueued:
+// - Buffer::reserve frees the old memory, so a stage that grew a buffer would destroy the previous stage's output in it: nothing
+//   grows between the stages of one chain.
+// - h_par is pinned and goes up with cudaMemcpyAsync, and the stages of one chain do not wait for the stream: a stage that rewrote a
+//   region an earlier stage has queued for upload would corrupt the queued copy.  So each stage writes and uploads only its own
+//   regions (QuantDev q[4] at the start and the sink's work after the front end's), and the trellis tables stay at the end.
+// The resize's tables and intermediate live in the slot's Resampler, which no other stage touches.
+struct SamplePlan {
+    int nc = 0, w = 0, h = 0, nw = 0, nh = 0;
+    bool trellis = false;                     // coefs_from_samples runs the trellis pass (jpeg_trellis() when planned)
+    // d_scratch: front's IDCT planes, then the full-resolution planes.  Every component takes PATH_GENERIC (IDCT + upsample), and
+    // front.plane_bytes also holds the resized planes and the sink's downsampled planes: they are written after the IDCT planes die.
+    ImagePlan front;
+    size_t rz_off[4] = {0}, dpl_off[4] = {0};
+    size_t in_bytes = 0, out_bytes = 0, scratch_bytes = 0, par_bytes = 0;
+    size_t sink_off = 0;                      // the sink's work descriptors in the parameter block, after the front end's
+};
+// The chain from gin's samples (a JPEG's, or planar_geom for host planes) to nw x nh, and on to the coefficients of gout when the chain
+// ends in coefs_from_samples (else gout is null).  Sizes the slot with one ensure().  Fails on fractional sampling ratios.
+bool plan_samples(Slot *s, const JpegGeom &gin, int nw, int nh, const JpegGeom *gout, SamplePlan &p, std::string &err);
+// Dequantisation, IDCT and upsampling of the coefficients in s->d_in (upload: s->h_in goes up first) into full-resolution planes,
+// converted YCbCr -> RGB in place when rgb is set and there are three components.
+bool samples_from_coefs(Slot *s, const JpegGeom &gin, const SamplePlan &p, bool upload, bool rgb, uint8_t **planes, std::string &err);
+// host planes [nc][h][w] into the full-resolution planes
+bool samples_from_host(Slot *s, const uint8_t *host, const SamplePlan &p, uint8_t **planes, std::string &err);
+// K3 of the planes `in` to nw x nh; `out` are the resized planes, or `in` itself at the same size
+bool resize_samples(Slot *s, uint8_t *const *in, const SamplePlan &p, uint8_t **out, std::string &err);
+// RGB -> YCbCr in place (three components), K4 downsampling, K5 FDCT + quantisation (and the trellis pass) into s->d_out
+bool coefs_from_samples(Slot *s, uint8_t *const *planes, const JpegGeom &gout, const SamplePlan &p, std::string &err);
 
 } // namespace b200

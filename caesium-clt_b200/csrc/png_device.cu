@@ -146,44 +146,29 @@ bool PngDevice::resize_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adl
     return true;
 }
 
+// K3 of the ch planes of T at `in` (W x H each, one after another) into `out` (NW x NH each)
+template <class T> static bool resample_planes(Resampler &rs, const uint8_t *in, int W, int H, uint8_t *out, int NW, int NH, int ch, void *stream, std::string &err)
+{
+    const T *src[4]; T *dst[4];
+    for (int c = 0; c < ch; c++) { src[c] = reinterpret_cast<const T *>(in) + (size_t)c * W * H; dst[c] = reinterpret_cast<T *>(out) + (size_t)c * NW * NH; }
+    return rs.run(src, W, H, dst, NW, NH, ch, stream, err);
+}
+
 // Expansion, K3 (skipped at the same size: imageops::resize copies) and packing, all enqueued behind the un-filter: d_raw holds the
-// source's rows on entry and the resized image's rows on exit.  Vertical pass first into f32 planes, then horizontal, every plane
-// of the image in one launch per pass.
+// source's rows on entry and the resized image's rows on exit.
 bool PngDevice::resize_raw(const PngInfo &src, const PngInfo &out, void *stream_, std::string &err)
 {
     cudaStream_t st = (cudaStream_t)stream_;
     const PngDecodedType t = png_decoded_type(src);
     const int W = (int)src.width, H = (int)src.height, NW = (int)out.width, NH = (int)out.height, ch = t.channels;
-    const size_t bps = (size_t)t.depth / 8, in_pitch = (size_t)W * H, out_pitch = (size_t)NW * NH;
-    if (!grow(d_planes, ch * in_pitch * bps + 64, err)) return false;
+    const size_t bps = (size_t)t.depth / 8;
+    if (!grow(d_planes, ch * (size_t)W * H * bps + 64, err)) return false;
     if (!launch_ok(launch_png_expand_planes(d_raw, src, png_palette_lut(src), d_planes, st), "png expand", err)) return false;
     const uint8_t *planes = d_planes;
     if (NW != W || NH != H) {
-        ResizeAxis av, ah;
-        make_resize_axis(H, NH, av);
-        make_resize_axis(W, NW, ah);
-        auto al = [](size_t b) { return (b + 255) / 256 * 256; };       // left | count | weights of the vertical axis, then of the horizontal one
-        const size_t cv = al(4 * (size_t)NH), wv = cv + al(4 * (size_t)NH), lh = wv + al(4 * av.weights.size());
-        const size_t chh = lh + al(4 * (size_t)NW), wh = chh + al(4 * (size_t)NW), end = wh + al(4 * ah.weights.size());
-        if (!grow(h_axes, end, err) || !grow(d_axes, end, err) || !grow(d_rtmp, ch * (size_t)NH * W * sizeof(float) + 64, err) ||
-            !grow(d_rplanes, ch * out_pitch * bps + 64, err)) return false;
-        memcpy(h_axes, av.left.data(), 4 * (size_t)NH); memcpy(h_axes + cv, av.count.data(), 4 * (size_t)NH);
-        memcpy(h_axes + wv, av.weights.data(), 4 * av.weights.size());
-        memcpy(h_axes + lh, ah.left.data(), 4 * (size_t)NW); memcpy(h_axes + chh, ah.count.data(), 4 * (size_t)NW);
-        memcpy(h_axes + wh, ah.weights.data(), 4 * ah.weights.size());
-        CU(cudaMemcpyAsync(d_axes, h_axes, end, cudaMemcpyHostToDevice, st));
-        const int *ax = reinterpret_cast<const int *>(d_axes.get());
-        const float *axf = reinterpret_cast<const float *>(d_axes.get());
-        int rc;
-        if (t.depth == 16) {
-            rc = launch_resize_v_planes(reinterpret_cast<const uint16_t *>(planes), W, H, W, in_pitch, d_rtmp, NH, (size_t)NH * W, ch, ax, ax + cv / 4, axf + wv / 4, av.cap, st);
-            if (!rc) rc = launch_resize_h_planes(d_rtmp, W, (size_t)NH * W, reinterpret_cast<uint16_t *>(d_rplanes.get()), NW, NH, NW, out_pitch, ch,
-                                                 ax + lh / 4, ax + chh / 4, axf + wh / 4, ah.cap, st);
-        } else {
-            rc = launch_resize_v_planes(planes, W, H, W, in_pitch, d_rtmp, NH, (size_t)NH * W, ch, ax, ax + cv / 4, axf + wv / 4, av.cap, st);
-            if (!rc) rc = launch_resize_h_planes(d_rtmp, W, (size_t)NH * W, d_rplanes.get(), NW, NH, NW, out_pitch, ch, ax + lh / 4, ax + chh / 4, axf + wh / 4, ah.cap, st);
-        }
-        if (!launch_ok(rc, "png resize", err)) return false;
+        if (!grow(d_rplanes, ch * (size_t)NW * NH * bps + 64, err)) return false;
+        if (!(t.depth == 16 ? resample_planes<uint16_t>(resampler, d_planes, W, H, d_rplanes, NW, NH, ch, st, err)
+                            : resample_planes<uint8_t>(resampler, d_planes, W, H, d_rplanes, NW, NH, ch, st, err))) return false;
         planes = d_rplanes;
     }
     if (!launch_ok(launch_png_pack_planes(planes, ch, t.depth, NW, NH, d_raw, st), "png pack", err)) return false;

@@ -8,6 +8,7 @@
 #include <vector>
 #include "dev_buffer.h"
 #include "png_host.h"
+#include "resize_kernels.h"
 
 namespace b200 {
 
@@ -65,8 +66,9 @@ struct PngDevice {
     // K7 over a byte plane on the host (bpp 1, stride = width) -> compacted LZ77 tokens on the host
     bool plane_tokens(const uint8_t *plane, size_t n, int stride, void *stream, std::vector<uint32_t> &tokens, std::string &err);
     DeviceBuffer<uint8_t> d_filt_all;                   // the trials' filtered streams, one after another
-    // the resize: source planes, resized planes, the vertical pass's f32 planes, the two axes' tap tables (and their pinned staging)
-    DeviceBuffer<uint8_t> d_planes, d_rplanes, d_axes; DeviceBuffer<float> d_rtmp; PinnedBuffer<uint8_t> h_axes;
+    // the resize: source planes, resized planes, and K3's tables and intermediate
+    DeviceBuffer<uint8_t> d_planes, d_rplanes;
+    Resampler resampler{Grow::Pow2Quarter};
 };
 
 // allocate-run-free stage helpers behind b200_png_filter / b200_png_lz77 (current device)

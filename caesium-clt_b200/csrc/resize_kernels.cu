@@ -7,40 +7,38 @@
 // an f32 plane, then horizontal, as imageops::resize does.  Planar u8 or u16 channels; HBM-bound streaming kernels.
 #include <cuda_runtime.h>
 #include <cstdint>
+#include <cstring>
 #include "resize_kernels.h"
 
 namespace b200 {
 
-// One launch resamples every plane of an image: blockIdx.z selects the plane, `in_pitch` / `out_pitch` are the planes' sizes in
-// samples.  T = uint8_t or uint16_t; the horizontal pass clamps to T's range before rounding.
+// T = uint8_t or uint16_t; the horizontal pass clamps to T's range before rounding.
 template <class T>
-__global__ void k_resize_v(const T *__restrict__ in, int w, int stride, size_t in_pitch, float *__restrict__ out, int nh, size_t out_pitch,
+__global__ void k_resize_v(const T *__restrict__ in, int w, float *__restrict__ out, int nh,
                            const int *__restrict__ left, const int *__restrict__ count, const float *__restrict__ weights, int cap)
 {
     const int x = blockIdx.x * blockDim.x + threadIdx.x, oy = blockIdx.y;
     if (x >= w || oy >= nh) return;
-    in += blockIdx.z * in_pitch; out += blockIdx.z * out_pitch;
     const int l = left[oy], n = count[oy];
     const float *ws = weights + (size_t)oy * cap;
     float t = 0.0f;
-    for (int i = 0; i < n; i++) t = __fadd_rn(t, __fmul_rn((float)in[(size_t)(l + i) * stride + x], __ldg(ws + i)));
+    for (int i = 0; i < n; i++) t = __fadd_rn(t, __fmul_rn((float)in[(size_t)(l + i) * w + x], __ldg(ws + i)));
     out[(size_t)oy * w + x] = t;
 }
 
 template <class T>
-__global__ void k_resize_h(const float *__restrict__ in, int w, size_t in_pitch, T *__restrict__ out, int nw, int nh, int ostride, size_t out_pitch,
+__global__ void k_resize_h(const float *__restrict__ in, int w, T *__restrict__ out, int nw, int nh,
                            const int *__restrict__ left, const int *__restrict__ count, const float *__restrict__ weights, int cap)
 {
     const int ox = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
     if (ox >= nw || y >= nh) return;
-    in += blockIdx.z * in_pitch; out += blockIdx.z * out_pitch;
     const int l = left[ox], n = count[ox];
     const float *ws = weights + (size_t)ox * cap;
     const float *row = in + (size_t)y * w + l;
     float t = 0.0f;
     for (int i = 0; i < n; i++) t = __fadd_rn(t, __fmul_rn(row[i], __ldg(ws + i)));
     t = fminf(fmaxf(t, 0.0f), sizeof(T) == 1 ? 255.0f : 65535.0f);
-    out[(size_t)y * ostride + ox] = (T)roundf(t);
+    out[(size_t)y * nw + ox] = (T)roundf(t);
 }
 
 #define FIXC(x) ((int)((x) * 65536.0 + 0.5))
@@ -71,35 +69,35 @@ __global__ void k_rgb_to_ycc(uint8_t *__restrict__ p0, uint8_t *__restrict__ p1,
 
 static inline int cdiv(size_t a, size_t b) { return (int)((a + b - 1) / b); }
 
-int launch_resize_v(const uint8_t *in, int w, int h, int stride, float *out, int nh, const int *left, const int *count, const float *weights, int cap, void *stream)
-{
-    return launch_resize_v_planes(in, w, h, stride, 0, out, nh, 0, 1, left, count, weights, cap, stream);
-}
-int launch_resize_h(const float *in, int w, uint8_t *out, int nw, int nh, int ostride, const int *left, const int *count, const float *weights, int cap, void *stream)
-{
-    return launch_resize_h_planes(in, w, 0, out, nw, nh, ostride, 0, 1, left, count, weights, cap, stream);
-}
 template <class T>
-int launch_resize_v_planes(const T *in, int w, int h, int stride, size_t in_pitch, float *out, int nh, size_t out_pitch, int planes,
-                           const int *left, const int *count, const float *weights, int cap, void *stream)
+bool Resampler::run(const T *const *in, int w, int h, T *const *out, int nw, int nh, int planes, void *stream, std::string &err)
 {
-    (void)h;
-    dim3 grid(cdiv((size_t)w, 256), nh, planes);
-    k_resize_v<T><<<grid, 256, 0, (cudaStream_t)stream>>>(in, w, stride, in_pitch, out, nh, out_pitch, left, count, weights, cap);
-    return (int)cudaGetLastError();
+    if (nw == w && nh == h) return true;
+    cudaStream_t st = (cudaStream_t)stream;
+    ResizeAxis av, ah;
+    make_resize_axis(h, nh, av);
+    make_resize_axis(w, nw, ah);
+    auto al = [](size_t b) { return (b + 255) / 256 * 256; };
+    const size_t cv = al(4 * (size_t)nh), wv = cv + al(4 * (size_t)nh), lh = wv + al(4 * av.weights.size());
+    const size_t chh = lh + al(4 * (size_t)nw), wh = chh + al(4 * (size_t)nw), end = wh + al(4 * ah.weights.size());
+    if (!h_tab.reserve(end, rule, err) || !d_tab.reserve(end, rule, err) || !d_tmp.reserve((size_t)nh * w * sizeof(float), rule, err)) return false;
+    memcpy(h_tab, av.left.data(), 4 * (size_t)nh); memcpy(h_tab + cv, av.count.data(), 4 * (size_t)nh);
+    memcpy(h_tab + wv, av.weights.data(), 4 * av.weights.size());
+    memcpy(h_tab + lh, ah.left.data(), 4 * (size_t)nw); memcpy(h_tab + chh, ah.count.data(), 4 * (size_t)nw);
+    memcpy(h_tab + wh, ah.weights.data(), 4 * ah.weights.size());
+    CU(cudaMemcpyAsync(d_tab, h_tab, end, cudaMemcpyHostToDevice, st));
+    const int *ax = reinterpret_cast<const int *>(d_tab.get());
+    const float *axf = reinterpret_cast<const float *>(d_tab.get());
+    for (int p = 0; p < planes; p++) {
+        k_resize_v<T><<<dim3(cdiv((size_t)w, 256), nh), 256, 0, st>>>(in[p], w, d_tmp, nh, ax, ax + cv / 4, axf + wv / 4, av.cap);
+        k_resize_h<T><<<dim3(cdiv((size_t)nw, 128), nh), 128, 0, st>>>(d_tmp, w, out[p], nw, nh, ax + lh / 4, ax + chh / 4, axf + wh / 4, ah.cap);
+        if (!launch_ok((int)cudaGetLastError(), "resize", err)) return false;
+    }
+    return true;
 }
-template <class T>
-int launch_resize_h_planes(const float *in, int w, size_t in_pitch, T *out, int nw, int nh, int ostride, size_t out_pitch, int planes,
-                           const int *left, const int *count, const float *weights, int cap, void *stream)
-{
-    dim3 grid(cdiv((size_t)nw, 128), nh, planes);
-    k_resize_h<T><<<grid, 128, 0, (cudaStream_t)stream>>>(in, w, in_pitch, out, nw, nh, ostride, out_pitch, left, count, weights, cap);
-    return (int)cudaGetLastError();
-}
-template int launch_resize_v_planes<uint8_t>(const uint8_t *, int, int, int, size_t, float *, int, size_t, int, const int *, const int *, const float *, int, void *);
-template int launch_resize_v_planes<uint16_t>(const uint16_t *, int, int, int, size_t, float *, int, size_t, int, const int *, const int *, const float *, int, void *);
-template int launch_resize_h_planes<uint8_t>(const float *, int, size_t, uint8_t *, int, int, int, size_t, int, const int *, const int *, const float *, int, void *);
-template int launch_resize_h_planes<uint16_t>(const float *, int, size_t, uint16_t *, int, int, int, size_t, int, const int *, const int *, const float *, int, void *);
+template bool Resampler::run<uint8_t>(const uint8_t *const *, int, int, uint8_t *const *, int, int, int, void *, std::string &);
+template bool Resampler::run<uint16_t>(const uint16_t *const *, int, int, uint16_t *const *, int, int, int, void *, std::string &);
+
 int launch_ycc_to_rgb(uint8_t *p0, uint8_t *p1, uint8_t *p2, size_t n, void *stream)
 {
     k_ycc_to_rgb<<<cdiv(n, 256), 256, 0, (cudaStream_t)stream>>>(p0, p1, p2, n);
