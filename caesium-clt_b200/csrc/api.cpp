@@ -173,7 +173,8 @@ JpegGeom planar_geom(uint32_t w, uint32_t h, int nc)
 JpegGeom with_size(JpegGeom g, uint32_t w, uint32_t h) { g.width = (int)w; g.height = (int)h; g.finalize(); return g; }
 
 // libcaesium resize::resize_image -> compute_dimensions (the source size when neither width nor height is set); source and
-// target must fit the format: both sides at most 65535, the target at most `limit` and not empty
+// target must fit the format: both sides at most 65535, the target at most `limit` (65535 for PNG, kJpegMaxDimension for JPEG,
+// 16383 for WebP) and not empty
 b200_status target_size(uint32_t w, uint32_t h, const b200_params *p, uint32_t limit, uint32_t &nw, uint32_t &nh, const char *msg)
 {
     nw = w; nh = h;
@@ -326,7 +327,7 @@ b200_status jpeg_compress(const uint8_t *in, size_t in_len, const b200_params *p
     const bool resize = p->width || p->height;
     if (resize) {
         uint32_t nw, nh;
-        const b200_status st = target_size((uint32_t)gin.width, (uint32_t)gin.height, p, 65535, nw, nh, "invalid target dimensions");
+        const b200_status st = target_size((uint32_t)gin.width, (uint32_t)gin.height, p, kJpegMaxDimension, nw, nh, "invalid target dimensions");
         if (st.code) return st;
         gout = with_size(gout, nw, nh);
     }
@@ -702,16 +703,13 @@ void png_expand_planar(const PngInfo &info, const std::vector<uint8_t> &raw, boo
 b200_status planes_to_jpeg(const std::vector<uint8_t> &planes, uint32_t w, uint32_t h, int nc, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
 {
     std::string err;
-    if (w > 65535 || h > 65535) return make_status(B200_ERR_INVALID_ARGUMENT, "image too large for JPEG");
+    uint32_t nw, nh;                                // the source's size unless width / height are set
+    const b200_status st = target_size(w, h, p, kJpegMaxDimension, nw, nh, "invalid target dimensions");
+    if (st.code) return st;
     const JpegGeom gin = planar_geom(w, h, nc);
     JpegGeom gout;
     if (!jpeg_output_geom(gin, (int)p->jpeg_quality, (int)p->jpeg_chroma_subsampling, gout, err)) return make_status(B200_ERR_INVALID_ARGUMENT, err);
-    if (p->width || p->height) {
-        uint32_t nw, nh;
-        const b200_status st = target_size(w, h, p, 65535, nw, nh, "invalid target dimensions");
-        if (st.code) return st;
-        gout = with_size(gout, nw, nh);
-    }
+    if (p->width || p->height) gout = with_size(gout, nw, nh);
     if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
     SlotLease s(prefer_dev);
     if (!s) return s.failure();

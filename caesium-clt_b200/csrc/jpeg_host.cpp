@@ -185,6 +185,9 @@ bool JpegReader::parse_segment(unsigned m, const uint8_t *seg, size_t sl, std::s
         g_.progressive = m == 0xC2;
         g_.height = (int)rd16(seg + 1); g_.width = (int)rd16(seg + 3); g_.ncomp = seg[5];
         if (g_.width <= 0 || g_.height <= 0) { err = "empty image"; return false; }
+        if ((uint32_t)g_.width > kJpegMaxDimension || (uint32_t)g_.height > kJpegMaxDimension) {      // jdinput.c initial_setup
+            err = "Maximum supported image dimension is " + std::to_string(kJpegMaxDimension) + " pixels"; return false;
+        }
         if (g_.ncomp != 1 && g_.ncomp != 3) { err = "unsupported component count " + std::to_string(g_.ncomp); return false; }
         if (sl < (size_t)(6 + 3 * g_.ncomp)) { err = "short SOF"; return false; }
         for (int c = 0; c < g_.ncomp; c++) {

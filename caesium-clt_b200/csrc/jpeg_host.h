@@ -11,6 +11,10 @@
 
 namespace b200 {
 
+// libjpeg's JPEG_MAX_DIMENSION (jmorecfg.h): libjpeg-turbo and mozjpeg refuse to read or write a side longer than this, so
+// a JPEG source over it is corrupt input and a JPEG target over it is an invalid size, although the SOF field holds 65535
+constexpr uint32_t kJpegMaxDimension = 65500;
+
 struct JpegGeom {
     int width = 0, height = 0, ncomp = 0;
     bool progressive = false;

@@ -519,6 +519,7 @@ int orc_jpeg_read(const uint8_t *d, size_t len, orc_jpeg *j, char err[256])
             j->progressive = (m == 0xC2);
             j->height = (seg[1] << 8) | seg[2]; j->width = (seg[3] << 8) | seg[4]; j->ncomp = seg[5];
             if (j->width <= 0 || j->height <= 0) { SETERR("empty image"); goto done; }
+            if (j->width > ORC_JPEG_MAX_DIMENSION || j->height > ORC_JPEG_MAX_DIMENSION) { SETERR("Maximum supported image dimension is %d pixels", ORC_JPEG_MAX_DIMENSION); goto done; }
             if (j->ncomp != 1 && j->ncomp != 3) { SETERR("unsupported component count %d", j->ncomp); goto done; }
             if (sl < (size_t)(6 + 3 * j->ncomp)) { SETERR("short SOF"); goto done; }
             for (int c = 0; c < j->ncomp; c++) {
@@ -642,6 +643,7 @@ int orc_jpeg_forward(const uint8_t *const planes[ORC_MAX_COMP], int width, int h
                      const orc_jpeg_params *p, orc_jpeg *o, char err[256])
 {
     memset(o, 0, sizeof(*o));
+    if (width < 1 || height < 1 || width > ORC_JPEG_MAX_DIMENSION || height > ORC_JPEG_MAX_DIMENSION) { SETERR("invalid target dimensions"); return -1; }  /* jcinit.c initial_setup */
     o->width = width; o->height = height; o->ncomp = ncomp; o->progressive = p->progressive;
     int lh = 1, lv = 1;
     if (ncomp == 3) {

@@ -31,6 +31,8 @@ extern "C" {
 #endif
 
 #define ORC_MAX_COMP 4
+/* libjpeg jmorecfg.h JPEG_MAX_DIMENSION: jdinput.c initial_setup refuses a larger SOF, and no larger JPEG is written */
+#define ORC_JPEG_MAX_DIMENSION 65500
 
 typedef struct {
     int width, height, ncomp;

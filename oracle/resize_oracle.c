@@ -124,7 +124,7 @@ int orc_jpeg_lossy_resized(const uint8_t *data, size_t len, const orc_jpeg_param
     memset(&fw, 0, sizeof(fw));
     uint32_t nw, nh;
     orc_compute_dimensions((uint32_t)in.width, (uint32_t)in.height, want_w, want_h, &nw, &nh);
-    if (nw == 0 || nh == 0 || nw > 65535 || nh > 65535) { if (err) strcpy(err, "invalid target dimensions"); orc_jpeg_free(&in); return -1; }
+    if (nw == 0 || nh == 0 || nw > ORC_JPEG_MAX_DIMENSION || nh > ORC_JPEG_MAX_DIMENSION) { if (err) strcpy(err, "invalid target dimensions"); orc_jpeg_free(&in); return -1; }
     size_t n = (size_t)in.width * in.height, m = (size_t)nw * nh;
     uint8_t *src[4] = {0, 0, 0, 0}, *rgb[3] = {0, 0, 0}, *dst[3] = {0, 0, 0}, *ycc[4] = {0, 0, 0, 0};
     for (int c = 0; c < in.ncomp; c++) { src[c] = malloc(n); ycc[c] = malloc(m); }
