@@ -146,24 +146,7 @@ __global__ void k_ge_zero(const ScanOut *__restrict__ so, uint32_t *__restrict__
 }
 
 // ---- block-major passes: one thread per block; the block is read (and its threshold masks built) once per pass and
-// serves every scan that visits it ------------------------------------------------------------------------------------
-__device__ __forceinline__ int unit_of(const Scan &s, const BlockComp &bc, int row, int col)
-{
-    if (s.ns == 1) return (row < bc.rbh && col < bc.rbw) ? row * bc.rbw + col : -1;
-    const int m = (row / bc.vs) * bc.mcux + col / bc.hs, q = bc.q_base + (row % bc.vs) * bc.hs + (col % bc.hs);
-    return m * bc.blocks_per_mcu + q;
-}
-// blk = the block in the CTA's shared tile; the DC predecessor of DC / interleaved scans may lie outside the tile and is read
-// from global memory
-__device__ __forceinline__ BlockRef ref_of(const Scan &s, int u, const int16_t *blk)
-{
-    BlockRef r;
-    if (s.mode == MODE_SEQ || s.mode == MODE_DC_FIRST || s.ns > 1) r = locate(s, u);   // needs the DC predecessor / the slot
-    else { r.prev = nullptr; r.slot = 0; }
-    r.blk = blk;
-    return r;
-}
-
+// serves every scan that visits the block ------------------------------------------------------------------------------------
 // A CTA of the block-major passes owns ENC_THREADS consecutive blocks i = row * bw + col of one component: 16 KB of contiguous
 // coefficients, staged in shared memory with coalesced 16-byte loads so that the symbol loops read their scattered non-zero
 // coefficients from the tile instead of with one dependent global load each.  Rows are 144 bytes apart: the 16-byte reads of a
@@ -187,6 +170,31 @@ __device__ __forceinline__ void wait_tile()
     __syncthreads();
 }
 
+// The component's scan visits go to shared memory once per CTA: the symbol loops index them with the loop counter, which would
+// put a register copy in local memory, and read their fields on every block, which from the descriptors in global memory would
+// be one load each.
+__device__ __forceinline__ void stage_visits(EncVisit *vis, const BlockComp &bc)
+{
+    if ((int)threadIdx.x < bc.nscan) vis[threadIdx.x] = bc.visit[threadIdx.x];
+}
+// block (row, col) in the scan of visit v: blk = the block in the CTA's shared tile; the DC predecessor of a DC-coding scan is
+// read from the tile when it is one of the CTA's blocks, from global memory otherwise
+__device__ __forceinline__ BlockRef ref_of(const EncVisit &v, const BlockComp &bc, const Tile &tile, int i0, int row, int col)
+{
+    BlockRef r;
+    r.blk = tile[threadIdx.x]; r.prev = nullptr; r.slot = 0;
+    if (v.mode == MODE_SEQ || v.mode == MODE_DC_FIRST) {
+        const int p = enc_dc_prev(bc, v.ns, row, col);
+        if (p >= i0 && p < i0 + ENC_THREADS) r.prev = tile[p - i0];
+        else if (p >= 0) r.prev = bc.coef + bc.comp_off + (long long)p * 64;
+    }
+    return r;
+}
+
+// symbol counters / code words of the visit's two table kinds in the on-chip table layout
+template <class T>
+__device__ __forceinline__ KindTabs<T> kind_tabs(T *tab, const EncVisit &v) { return KindTabs<T>{tab + ENC_DC_ENTRY, tab + v.ac_entry}; }
+
 // The classify pass builds each block's threshold masks once and leaves them in `masks` (24 bytes per block, indexed
 // comp.mask_base + block); the length and emit passes read them back instead of re-deriving them from the 128-byte block (the
 // mask construction was a quarter to a third of those passes' instructions).
@@ -199,109 +207,113 @@ __device__ __forceinline__ Masks3 load_masks(const Masks3 *__restrict__ masks, c
 }
 
 // Classify + the statistics of the inline symbols (DC differences, run/size symbols, ZRLs: they do not depend on the EOB
-// groups; k_ge_groups adds the EOBn symbols).  Each scan visit of the component uses one table kind (two for a sequential scan)
-// of the component's table, so 256 shared counters per (visit, kind) are enough; a script with more visits than HIST_SLOTS
-// counts the rest straight into global memory.
-constexpr int HIST_SLOTS = 6;
-__global__ void __launch_bounds__(ENC_THREADS) k_geb_classify(const BlockComp *__restrict__ comps, const Scan *__restrict__ scans, uint32_t *__restrict__ meta, int *__restrict__ evkey,
+// groups; k_ge_groups adds the EOBn symbols), counted into the on-chip table slots of the CTA's visits and flushed once.
+struct SmemHist {
+    KindTabs<uint32_t> h;
+    __device__ void sym(int kind, int, int symbol, int, unsigned) { atomicAdd((kind ? h.ac : h.dc) + symbol, 1u); }
+    __device__ void raw64(int, unsigned long long) {}
+};
+__global__ void __launch_bounds__(ENC_THREADS) k_geb_classify(const BlockComp *__restrict__ comps, uint32_t *__restrict__ meta, int *__restrict__ evkey,
                                                               uint32_t *__restrict__ tail, Masks3 *__restrict__ masks, uint32_t *__restrict__ hist)
 {
     __shared__ __align__(16) Tile tile;
-    __shared__ uint32_t h[HIST_SLOTS][256];
-    __shared__ int slot_tab[HIST_SLOTS];        // global table index (tab_base + kind * 2 + tbl) of each counter slot
-    const BlockComp bc = comps[blockIdx.y];
+    __shared__ uint32_t h[ENC_TAB_ENTRIES];
+    __shared__ EncVisit vis[ENC_MAX_VISITS];
+    const BlockComp &bc = comps[blockIdx.y];
     const int nblk = bc.bw * bc.bh, i0 = blockIdx.x * ENC_THREADS, i = i0 + threadIdx.x;
     if (i0 >= nblk) return;
     stage_tile(tile, bc, i0, nblk);
-    for (int k = threadIdx.x; k < HIST_SLOTS * 256; k += ENC_THREADS) (&h[0][0])[k] = 0;
-    if (threadIdx.x == 0) {
-        for (int j = 0, sb = 0; j < bc.nscan; j++) {
-            const Scan &s = scans[bc.scan_idx[j]];
-            int ci = 0;                             // the component's place in the scan (interleaved scans list every component)
-            if (s.ns > 1) for (int q = 0; q < bc.q_base; ci++) q += s.hs[ci] * s.vs[ci];
-            const int k0 = s.mode == MODE_AC_FIRST || s.mode == MODE_AC_REFINE ? 1 : 0, k1 = s.mode == MODE_SEQ ? 1 : k0;
-            for (int kind = k0; kind <= k1; kind++, sb++) if (sb < HIST_SLOTS) slot_tab[sb] = s.tab_base + kind * 2 + s.tbl[ci];
-        }
-    }
+    for (int k = threadIdx.x; k < ENC_TAB_ENTRIES; k += ENC_THREADS) h[k] = 0;
+    stage_visits(vis, bc);
     wait_tile();
     if (i < nblk) {
         const int row = i / bc.bw, col = i - row * bc.bw;
-        const int16_t *blk = tile[threadIdx.x];
-        const Masks3 M = make_masks3(blk);
+        const Masks3 M = make_masks3(tile[threadIdx.x]);
         masks[bc.mask_base + i] = M;
-        for (int j = 0, sb = 0; j < bc.nscan; j++) {
-            const Scan &s = scans[bc.scan_idx[j]];
-            const int k0 = s.mode == MODE_AC_FIRST || s.mode == MODE_AC_REFINE ? 1 : 0;
-            const int u = unit_of(s, bc, row, col);
-            if (u >= 0) {
-                const uint32_t m = classify_m(s, M);
-                const long long g = s.unit_base + u;
-                meta[g] = m; evkey[g] = meta_event(m) ? (int)g : -1; tail[g] = (uint32_t)meta_tail(m);
-                auto add = [&](int idx) {           // idx = (kind * 2 + tbl) * 256 + symbol
-                    const int sl = sb + (idx >> 9) - k0;
-                    if (sl < HIST_SLOTS) atomicAdd(&h[sl][idx & 255], 1u); else atomicAdd(&hist[(size_t)s.tab_base * 256 + idx], 1u);
-                };
-                HistSink<decltype(add)> sk(add);
-                gen_block_m(s, ref_of(s, u, blk), M, 0, sk);
-            }
-            sb += s.mode == MODE_SEQ ? 2 : 1;
+        for (int j = 0; j < bc.nscan; j++) {
+            const EncVisit &v = vis[j];
+            const int u = enc_unit_of(bc, v.ns, row, col);
+            if (u < 0) continue;
+            const uint32_t m = classify_m(v, M);
+            const int g = v.unit_base + u;
+            meta[g] = m; evkey[g] = meta_event(m) ? g : -1; tail[g] = (uint32_t)meta_tail(m);
+            SmemHist sk{kind_tabs(h, v)};
+            gen_block_m(v, v.tbl, ref_of(v, bc, tile, i0, row, col), M, 0, sk);
         }
     }
     __syncthreads();
-    int nslots = 0;
-    for (int j = 0; j < bc.nscan; j++) nslots += scans[bc.scan_idx[j]].mode == MODE_SEQ ? 2 : 1;
-    for (int k = threadIdx.x; k < min(nslots, HIST_SLOTS) * 256; k += ENC_THREADS) {
-        const uint32_t v = (&h[0][0])[k];
-        if (v) atomicAdd(&hist[(size_t)slot_tab[k >> 8] * 256 + (k & 255)], v);
+    for (int k = threadIdx.x; k < ENC_TAB_ENTRIES; k += ENC_THREADS) {
+        int symbol; const int t = enc_entry_table(bc, k, symbol);
+        if (h[k]) atomicAdd(&hist[(size_t)t * 256 + symbol], h[k]);     // an unused slot counts nothing
     }
 }
 
-__global__ void __launch_bounds__(ENC_THREADS) k_geb_len(const BlockComp *__restrict__ comps, const Scan *__restrict__ scans, const uint32_t *__restrict__ gcount, const Table *__restrict__ tabs,
+// The length and emit passes load the tables of the CTA's visits once (k_ge_tables wrote them): the per-symbol lookup on the
+// symbol's dependent chain is a shared-memory read.  len keeps the code lengths only.
+__global__ void __launch_bounds__(ENC_THREADS) k_geb_len(const BlockComp *__restrict__ comps, const uint32_t *__restrict__ gcount, const Table *__restrict__ tabs,
                                                          uint32_t *__restrict__ bitlen, const Masks3 *__restrict__ masks)
 {
     __shared__ __align__(16) Tile tile;
-    const BlockComp bc = comps[blockIdx.y];
+    __shared__ uint8_t tl[ENC_TAB_ENTRIES];
+    __shared__ EncVisit vis[ENC_MAX_VISITS];
+    const BlockComp &bc = comps[blockIdx.y];
     const int nblk = bc.bw * bc.bh, i0 = blockIdx.x * ENC_THREADS, i = i0 + threadIdx.x;
     if (i0 >= nblk) return;
     stage_tile(tile, bc, i0, nblk);
     const Masks3 M = load_masks(masks, bc, min(i, nblk - 1));   // in flight with the tile
+    stage_visits(vis, bc);
+    for (int k = threadIdx.x; k < ENC_TAB_ENTRIES; k += ENC_THREADS) {
+        int symbol; const int t = enc_entry_table(bc, k, symbol);
+        if (t >= 0) tl[k] = (uint8_t)tabs[t].code_len[symbol];
+    }
     wait_tile();
     if (i >= nblk) return;
     const int row = i / bc.bw, col = i - row * bc.bw;
-    const int16_t *blk = tile[threadIdx.x];
     for (int j = 0; j < bc.nscan; j++) {
-        const Scan &s = scans[bc.scan_idx[j]];
-        const int u = unit_of(s, bc, row, col);
+        const EncVisit &v = vis[j];
+        const int u = enc_unit_of(bc, v.ns, row, col);
         if (u < 0) continue;
-        LenSink sk; sk.tabs = tabs + s.tab_base;
-        gen_block_m(s, ref_of(s, u, blk), M, gcount[s.unit_base + u], sk);
-        bitlen[s.unit_base + u] = (uint32_t)sk.bits;
+        LenSinkT<KindTabs<const uint8_t>> sk{kind_tabs<const uint8_t>(tl, v)};
+        gen_block_m(v, v.tbl, ref_of(v, bc, tile, i0, row, col), M, gcount[v.unit_base + u], sk);
+        bitlen[v.unit_base + u] = (uint32_t)sk.bits;
     }
 }
 
-__global__ void __launch_bounds__(ENC_THREADS) k_geb_emit(const BlockComp *__restrict__ comps, const Scan *__restrict__ scans, const uint32_t *__restrict__ gcount, const Table *__restrict__ tabs,
+__global__ void __launch_bounds__(ENC_THREADS) k_geb_emit(const BlockComp *__restrict__ comps, const uint32_t *__restrict__ gcount, const Table *__restrict__ tabs,
                                                           const uint32_t *__restrict__ bitoff, uint32_t *__restrict__ words, const Masks3 *__restrict__ masks, const ScanOut *__restrict__ so,
                                                           const uint32_t *__restrict__ flags)
 {
     __shared__ __align__(16) Tile tile;
+    __shared__ uint32_t tc[ENC_TAB_ENTRIES];
+    __shared__ EncVisit vis[ENC_MAX_VISITS];
+    __shared__ uint32_t vword[ENC_MAX_VISITS], vbit0[ENC_MAX_VISITS];     // each visit's scan: first word, bit offset of unit 0
     if (flags[0]) return;                   // the bit buffer is too small for this batch: the host re-runs this half with exact sizes
-    const BlockComp bc = comps[blockIdx.y];
+    const BlockComp &bc = comps[blockIdx.y];
     const int nblk = bc.bw * bc.bh, i0 = blockIdx.x * ENC_THREADS, i = i0 + threadIdx.x;
     if (i0 >= nblk) return;
     stage_tile(tile, bc, i0, nblk);
     const Masks3 M = load_masks(masks, bc, min(i, nblk - 1));   // in flight with the tile
+    stage_visits(vis, bc);
+    if ((int)threadIdx.x < bc.nscan) {
+        const EncVisit &v = bc.visit[threadIdx.x];
+        vword[threadIdx.x] = so[v.scan].word_base; vbit0[threadIdx.x] = bitoff[v.unit_base];
+    }
+    for (int k = threadIdx.x; k < ENC_TAB_ENTRIES; k += ENC_THREADS) {
+        int symbol; const int t = enc_entry_table(bc, k, symbol);
+        if (t >= 0) tc[k] = tabs[t].code_len[symbol];
+    }
     wait_tile();
     if (i >= nblk) return;
     const int row = i / bc.bw, col = i - row * bc.bw;
-    const int16_t *blk = tile[threadIdx.x];
     auto orw = [&](long long w, uint32_t v) { if (v) atomicOr(&words[w], v); };
     auto stw = [&](long long w, uint32_t v) { words[w] = v; };
     for (int j = 0; j < bc.nscan; j++) {
-        const Scan &s = scans[bc.scan_idx[j]];
-        const int u = unit_of(s, bc, row, col);
+        const EncVisit &v = vis[j];
+        const int u = enc_unit_of(bc, v.ns, row, col);
         if (u < 0) continue;
-        EmitSink<decltype(orw), decltype(stw)> sk(tabs + s.tab_base, orw, stw, (long long)so[bc.scan_idx[j]].word_base, (unsigned long long)(bitoff[s.unit_base + u] - bitoff[s.unit_base]));
-        gen_block_m(s, ref_of(s, u, blk), M, gcount[s.unit_base + u], sk);
+        EmitSink<decltype(orw), decltype(stw), KindTabs<const uint32_t>> sk(kind_tabs<const uint32_t>(tc, v), orw, stw, (long long)vword[j],
+                                                                            (unsigned long long)(bitoff[v.unit_base + u] - vbit0[j]));
+        gen_block_m(v, v.tbl, ref_of(v, bc, tile, i0, row, col), M, gcount[v.unit_base + u], sk);
         sk.finish();
     }
 }
@@ -435,6 +447,7 @@ bool GpuEncoder::prepare(const JpegGeom &g, bool progressive, int16_t *const *d_
     if (U >= (1ll << 31)) { err = "batch too large for the entropy encoder"; return false; }
     overflow = false;
     for (auto &sc_ : plan.scans) if (!masks_cover(sc_.mode, sc_.Al)) { err = "scan script outside the device encoder's mask range"; overflow = true; return false; }
+    if (!plan.on_chip) { err = "scan script outside the device encoder's on-chip table slots"; overflow = true; return false; }
     if (!ev_sizes) { cudaEvent_t e; CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming | (stream_wait_mode() == 0 ? 0 : cudaEventBlockingSync))); ev_sizes = e; }
     // ---- buffers whose size follows the INPUT
     auto grow = [&](auto &buf, size_t need) { return buf.reserve(need, Grow::Pow2Half, err, &generation); };
@@ -518,7 +531,7 @@ bool GpuEncoder::enqueue_back(void *stream_, std::string &err)
     const dim3 gb(cdiv(plan.max_comp_blocks, ENC_THREADS), NC);
     k_ge_zero<<<dim3(64, NS), 256, 0, st>>>(d_so, d_words);
     LT_MARK("k_ge_zero");
-    k_geb_emit<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_scans, d_gcount, d_tabs, d_bitoff, d_words, d_masks, d_so, d_flags);
+    k_geb_emit<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_gcount, d_tabs, d_bitoff, d_words, d_masks, d_so, d_flags);
     LT_MARK("k_geb_emit");
     k_ge_ffcount<<<dim3(32, NS + 1), 128, 0, st>>>(d_so, NS, d_words, d_ffcount, groups_cap, d_flags);
     LT_MARK("k_ge_ffcount");
@@ -562,7 +575,7 @@ bool GpuEncoder::enqueue_front(void *stream_, bool fill_dummy, std::string &err)
     const dim3 gu1(cdiv(max_units + 1, 128), NS);
     CU(cudaMemsetAsync(d_hist, 0, (size_t)NS * 4 * 256 * 4, st));
     LT_MARK("memset");
-    k_geb_classify<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_scans, d_meta, d_evkey, d_tail, d_masks, d_hist);
+    k_geb_classify<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_meta, d_evkey, d_tail, d_masks, d_hist);
     LT_MARK("k_geb_classify");
     size_t tb = d_temp.capacity();
     cub::DeviceScan::ExclusiveScan(d_temp, tb, d_evkey.get(), d_prev.get(), cub::Max(), -1, (int)U, st);
@@ -576,7 +589,7 @@ bool GpuEncoder::enqueue_front(void *stream_, bool fill_dummy, std::string &err)
     LT_MARK("k_ge_groups");
     k_ge_tables<<<NS * 4, 32, 0, st>>>(d_hist, d_tabs, d_dht);
     LT_MARK("k_ge_tables");
-    k_geb_len<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_scans, d_gcount, d_tabs, d_bitlen, d_masks);
+    k_geb_len<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_gcount, d_tabs, d_bitlen, d_masks);
     LT_MARK("k_geb_len");
     tb = d_temp.capacity();
     cub::DeviceScan::ExclusiveSum(d_temp, tb, d_bitlen.get(), d_bitoff.get(), (int)U, st);

@@ -134,6 +134,8 @@ GE_HD unsigned long long band_mask(int Ss, int Se) { return (Se >= 63 ? ~0ull : 
 // in jpeg_scan_script use Al <= 1 / Al = 0).  One block read serves every scan that visits the block.
 struct Masks3 { unsigned long long m[3]; };
 GE_HD bool masks_cover(int mode, int Al) { return mode == MODE_AC_REFINE ? Al <= 1 : Al <= 2; }
+// M.m[t] by selects: an array indexed with a runtime value would put the masks in local memory on the device
+GE_HD unsigned long long mask_at(const Masks3 &M, int t) { return t == 0 ? M.m[0] : t == 1 ? M.m[1] : M.m[2]; }
 
 // SWAR over the 32 coefficient pairs of a block (two int16 per 32-bit word, little endian): per word |c| of both halves,
 // then for each threshold one add turns "half >= T" into bit 15 / bit 31, which is shifted onto the word's position in a
@@ -187,11 +189,13 @@ inline Masks3 make_masks3_reference(const int16_t *blk)
 }
 
 // ---- classification (pass 0) ------------------------------------------------------------------------------------
-GE_HD uint32_t classify_m(const Scan &s, const Masks3 &M)
+// S: a Scan, or any descriptor with its mode, Ss, Se and Al (the device passes stage one per scan visit on chip)
+template <class S>
+GE_HD uint32_t classify_m(const S &s, const Masks3 &M)
 {
     if (s.mode == MODE_SEQ || s.mode == MODE_DC_FIRST) return meta_pack(true, false, 0);
     const unsigned long long band = band_mask(s.Ss, s.Se);
-    const unsigned long long mA = M.m[s.Al] & band, mB = (s.mode == MODE_AC_REFINE ? M.m[s.Al + 1] : 0ull) & band;
+    const unsigned long long mA = mask_at(M, s.Al) & band, mB = (s.mode == MODE_AC_REFINE ? mask_at(M, s.Al + 1) : 0ull) & band;
     if (s.mode == MODE_AC_FIRST) { const int last = msb64(mA); return meta_pack(last >= 0, last < s.Se, 0); }
     // AC refinement: inline symbols exist iff some coefficient becomes non-zero in this scan (|c| >> Al == 1).  After
     // the last such coefficient every remaining position is either zero (r++) or already non-zero (a pending correction
@@ -229,11 +233,11 @@ GE_HD void gen_eob_token(unsigned count, int tbl, Sink &sk)
 
 // group_count: >0 iff this block opens an EOB group (then E_j carries that count).  The statistics pass runs it with
 // group_count = 0: the inline symbols do not depend on the groups, and the EOBn symbols are counted where the groups are made.
-template <class Sink>
-GE_HD void gen_block_m(const Scan &s, const BlockRef &b, const Masks3 &M, unsigned group_count, Sink &sk)
+// S as for classify_m; tbl = the block's Huffman table id, passed on to the sink.
+template <class S, class Sink>
+GE_HD void gen_block_m(const S &s, int tbl, const BlockRef &b, const Masks3 &M, unsigned group_count, Sink &sk)
 {
     const int16_t *blk = b.blk;
-    const int tbl = s.tbl[b.slot];
     if (s.mode == MODE_DC_FIRST) { gen_dc(blk[0] >> s.Al, b.prev ? (b.prev[0] >> s.Al) : 0, tbl, sk); return; }
     if (s.mode == MODE_SEQ) {
         gen_dc(blk[0], b.prev ? b.prev[0] : 0, tbl, sk);
@@ -250,8 +254,8 @@ GE_HD void gen_block_m(const Scan &s, const BlockRef &b, const Masks3 &M, unsign
         return;
     }
     const unsigned long long band = band_mask(s.Ss, s.Se);
-    const unsigned long long mA = M.m[s.Al] & band;                                              // |c| >= 2^Al
-    const unsigned long long mB = (s.mode == MODE_AC_REFINE ? M.m[s.Al + 1] : 0ull) & band;     // |c| >= 2^(Al+1)
+    const unsigned long long mA = mask_at(M, s.Al) & band;                                              // |c| >= 2^Al
+    const unsigned long long mB = (s.mode == MODE_AC_REFINE ? mask_at(M, s.Al + 1) : 0ull) & band;     // |c| >= 2^(Al+1)
     if (s.mode == MODE_AC_FIRST) {
         int prevk = s.Ss - 1;
         for (unsigned long long m = mA; m; m &= m - 1) {
@@ -295,11 +299,26 @@ GE_HD void gen_block_m(const Scan &s, const BlockRef &b, const Masks3 &M, unsign
 template <class Sink>
 GE_HD void gen_block(const Scan &s, const BlockRef &b, unsigned group_count, Sink &sk)
 {
-    if (s.mode == MODE_DC_FIRST) { Masks3 none; none.m[0] = none.m[1] = none.m[2] = 0; gen_block_m(s, b, none, group_count, sk); return; }
-    gen_block_m(s, b, make_masks3(b.blk), group_count, sk);
+    if (s.mode == MODE_DC_FIRST) { Masks3 none; none.m[0] = none.m[1] = none.m[2] = 0; gen_block_m(s, s.tbl[b.slot], b, none, group_count, sk); return; }
+    gen_block_m(s, s.tbl[b.slot], b, make_masks3(b.blk), group_count, sk);
 }
 
 // ---- sinks --------------------------------------------------------------------------------------------------------
+// Where the length and emit sinks find a symbol's `code << 8 | length` word (only the low byte, the length, for LenSink):
+// ScanTabs looks it up in a scan's four Tables by kind and table id; KindTabs in one array per kind, the table id being
+// fixed by the caller (the device passes stage the tables of a CTA's scan visits in shared memory this way).
+struct ScanTabs {
+    const Table *t = nullptr;
+    ScanTabs() = default;
+    GE_HD ScanTabs(const Table *p) : t(p) {}
+    GE_HD uint32_t operator()(int kind, int tbl, int symbol) const { return t[kind * 2 + tbl].code_len[symbol]; }
+};
+template <class T>
+struct KindTabs {
+    T *dc, *ac;                 // T = const element type for lookups, a counter type for the statistics pass
+    GE_HD uint32_t operator()(int kind, int, int symbol) const { return (kind ? ac : dc)[symbol]; }
+};
+
 template <class AddFn>
 struct HistSink {               // add(index) must increment counter [kind*2 + tbl][symbol] (atomically on the device)
     AddFn add;
@@ -308,12 +327,14 @@ struct HistSink {               // add(index) must increment counter [kind*2 + t
     GE_HD void raw64(int, unsigned long long) {}
 };
 
-struct LenSink {
-    const Table *tabs;          // [kind*2 + tbl]
+template <class Tabs = ScanTabs>
+struct LenSinkT {
+    Tabs tabs;
     unsigned long long bits = 0;
-    GE_HD void sym(int kind, int tbl, int symbol, int nb, unsigned) { bits += (tabs[kind * 2 + tbl].code_len[symbol] & 0xFFu) + nb; }
+    GE_HD void sym(int kind, int tbl, int symbol, int nb, unsigned) { bits += (tabs(kind, tbl, symbol) & 0xFFu) + nb; }
     GE_HD void raw64(int nb, unsigned long long) { bits += nb; }
 };
+using LenSink = LenSinkT<>;
 
 GE_HD uint32_t shl_or_zero(uint32_t v, int s)      // v << s for s in [0, 32]
 {
@@ -329,16 +350,16 @@ GE_HD uint32_t shl_or_zero(uint32_t v, int s)      // v << s for s in [0, 32]
 // be shared with a neighbouring block: the first completed word and the one finish() writes go through `orw(word_index,
 // value)`, which must OR atomically on the device; every completed word after the first is the block's own and is stored
 // with `stw`.  A caller that writes the blocks one after another may pass its OR function for both.
-template <class OrFn, class StFn = OrFn>
+template <class OrFn, class StFn = OrFn, class Tabs = ScanTabs>
 struct EmitSink {
-    const Table *tabs;
+    Tabs tabs;
     OrFn orw;
     StFn stw;
     long long wpos, first;      // next word index, the block's first word
     uint32_t cur = 0; int n;
-    GE_HD EmitSink(const Table *t, OrFn f, StFn g, long long word_base, unsigned long long bitoff)
+    GE_HD EmitSink(Tabs t, OrFn f, StFn g, long long word_base, unsigned long long bitoff)
         : tabs(t), orw(f), stw(g), wpos(word_base + (long long)(bitoff >> 5)), first(wpos), n((int)(bitoff & 31)) {}
-    GE_HD EmitSink(const Table *t, OrFn f, long long word_base, unsigned long long bitoff) : EmitSink(t, f, f, word_base, bitoff) {}
+    GE_HD EmitSink(Tabs t, OrFn f, long long word_base, unsigned long long bitoff) : EmitSink(t, f, f, word_base, bitoff) {}
     GE_HD void put(uint32_t code, int len)          // the low len bits of code (len <= 32, nothing above them set)
     {
         if (!len) return;
@@ -353,7 +374,7 @@ struct EmitSink {
     GE_HD void sym(int kind, int tbl, int symbol, int nb, unsigned extra)
     {
         // code and value bits leave as one piece: at most 16 + 16 bits
-        const uint32_t e = tabs[kind * 2 + tbl].code_len[symbol];
+        const uint32_t e = tabs(kind, tbl, symbol);
         put(((e >> 8) << nb) | (extra & ((1u << nb) - 1u)), (int)(e & 0xFFu) + nb);
     }
     GE_HD void raw64(int nb, unsigned long long v)

@@ -10,17 +10,62 @@ namespace b200 {
 
 // Block-major view used by the encoder passes: one descriptor per (image, component); a thread owns one block, reads it
 // once, and serves every scan that visits the block (e.g. luma: DC scan + two AC bands + the refinement scan).
+//
+// A CTA copies the component's visit records to shared memory and keeps the Huffman tables of its visits on chip: one slot per
+// table kind a visit codes, the AC tables first (256 symbols each), then the DC table (DC symbols are bit counts 0..16).
+// jpeg_scan_script's progressive luma has three AC visits and one DC visit, a sequential scan one of each.
+constexpr int ENC_MAX_VISITS = 6, ENC_AC_SLOTS = 3, ENC_DC_SLOTS = 1, ENC_DC_SYMBOLS = 17;
+constexpr int ENC_TAB_ENTRIES = ENC_AC_SLOTS * 256 + ENC_DC_SLOTS * ENC_DC_SYMBOLS;   // entry of (AC slot a, symbol) = a * 256 + symbol
+constexpr int ENC_DC_ENTRY = ENC_AC_SLOTS * 256;                                      // entry of (DC slot, symbol) = ENC_DC_ENTRY + symbol
+
+struct EncVisit {                       // one scan visiting the component: what the symbol loops and the unit index need
+    int scan;                           // index into GpuEncPlan::scans
+    int mode, Ss, Se, Al, ns;
+    int tbl;                            // the component's Huffman table id
+    int unit_base;                      // Scan::unit_base (a batch has fewer than 2^31 units)
+    int ac_entry;                       // first on-chip entry of the visit's AC table (unused by a DC-only scan)
+};
+
 struct BlockComp {
     const int16_t *coef;                // image base
     long long comp_off;
     int bw, bh, rbw, rbh, hs, vs;
     int q_base, blocks_per_mcu, mcux;   // position of the component's first block inside an MCU (interleaved scans)
-    int nscan, scan_idx[6];             // indices into GpuEncPlan::scans
+    int nscan;
+    EncVisit visit[ENC_MAX_VISITS];
+    int tab[ENC_AC_SLOTS + ENC_DC_SLOTS];   // batch-wide table index (Scan::tab_base + kind * 2 + tbl) of each slot, -1: unused
     long long mask_base;                // first block of this component in the batch-wide per-block mask array
 };
 
+// the unit of component block (row, col) in a scan with ns components (-1: a padding block the scan does not code)
+GE_HD int enc_unit_of(const BlockComp &bc, int ns, int row, int col)
+{
+    if (ns == 1) return (row < bc.rbh && col < bc.rbw) ? row * bc.rbw + col : -1;
+    const int m = (row / bc.vs) * bc.mcux + col / bc.hs, q = bc.q_base + (row % bc.vs) * bc.hs + (col % bc.hs);
+    return m * bc.blocks_per_mcu + q;
+}
+// the component block (index row * bw + col) whose DC value predicts that of block (row, col) in a scan with ns components, -1
+// for the component's first block in the scan: ge::locate()'s predecessor, walked back on the component's own grid
+GE_HD int enc_dc_prev(const BlockComp &bc, int ns, int row, int col)
+{
+    if (ns == 1) return col > 0 ? row * bc.bw + col - 1 : row > 0 ? (row - 1) * bc.bw + bc.rbw - 1 : -1;
+    if (col % bc.hs) return row * bc.bw + col - 1;                      // earlier block of the same MCU row
+    if (row % bc.vs) return (row - 1) * bc.bw + col + bc.hs - 1;        // last block of the MCU's previous row
+    if (col) return (row + bc.vs - 1) * bc.bw + col - 1;               // last block of the previous MCU
+    if (row) return (row - 1) * bc.bw + bc.mcux * bc.hs - 1;           // ... which ends the previous MCU row
+    return -1;
+}
+
+// the table of on-chip entry k and the entry's symbol; -1 for a slot the component does not use
+GE_HD int enc_entry_table(const BlockComp &bc, int k, int &symbol)
+{
+    if (k < ENC_DC_ENTRY) { symbol = k & 255; return bc.tab[k >> 8]; }
+    symbol = k - ENC_DC_ENTRY; return bc.tab[ENC_AC_SLOTS];
+}
+
 struct GpuEncPlan {
     std::vector<BlockComp> comps;       // image-major
+    bool on_chip = true;                // every component's visits fit ENC_MAX_VISITS and its tables the on-chip slots
     int max_comp_blocks = 0;
     std::vector<ge::Scan> scans;        // image-major: scans of image 0, then image 1, ...
     std::vector<ScanDef> defs;          // one script (shared by all images of the batch)
@@ -64,7 +109,7 @@ inline void gpuenc_plan(const JpegGeom &g, bool progressive, const int16_t *cons
         if (im == 0) { p.units_per_image = unit; p.words_per_image = word; }
     }
     p.total_units = unit; p.total_words = word;
-    p.comps.clear(); p.max_comp_blocks = 0; p.total_comp_blocks = 0;
+    p.comps.clear(); p.max_comp_blocks = 0; p.total_comp_blocks = 0; p.on_chip = true;
     for (int im = 0; im < nimages; im++) {
         int qb = 0;
         for (int c = 0; c < g.ncomp; c++) {
@@ -75,7 +120,20 @@ inline void gpuenc_plan(const JpegGeom &g, bool progressive, const int16_t *cons
             bc.blocks_per_mcu = 0; for (int cc = 0; cc < g.ncomp; cc++) bc.blocks_per_mcu += g.hs[cc] * g.vs[cc];
             qb += g.hs[c] * g.vs[c];
             bc.nscan = 0;
-            for (int si = 0; si < ns; si++) for (int i = 0; i < sc[si].ns; i++) if (sc[si].ci[i] == c && bc.nscan < 6) bc.scan_idx[bc.nscan++] = im * ns + si;
+            int nac = 0, ndc = 0;
+            for (int k = 0; k < ENC_AC_SLOTS + ENC_DC_SLOTS; k++) bc.tab[k] = -1;
+            for (int si = 0; si < ns; si++) for (int i = 0; i < sc[si].ns; i++) {
+                if (sc[si].ci[i] != c) continue;
+                const ge::Scan &s = p.scans[(size_t)im * ns + si];
+                const bool dc = s.mode == ge::MODE_SEQ || s.mode == ge::MODE_DC_FIRST, ac = s.mode != ge::MODE_DC_FIRST;
+                if (bc.nscan == ENC_MAX_VISITS || nac + ac > ENC_AC_SLOTS || ndc + dc > ENC_DC_SLOTS) { p.on_chip = false; continue; }
+                EncVisit &v = bc.visit[bc.nscan++];
+                v.scan = im * ns + si; v.mode = s.mode; v.Ss = s.Ss; v.Se = s.Se; v.Al = s.Al; v.ns = s.ns; v.tbl = s.tbl[i];
+                v.unit_base = (int)s.unit_base;
+                v.ac_entry = ac ? nac * 256 : 0;
+                if (ac) bc.tab[nac++] = s.tab_base + 2 + v.tbl;
+                if (dc) bc.tab[ENC_AC_SLOTS + ndc++] = s.tab_base + v.tbl;
+            }
             bc.mask_base = p.total_comp_blocks; p.total_comp_blocks += (long long)bc.bw * bc.bh;
             p.comps.push_back(bc);
             p.max_comp_blocks = std::max(p.max_comp_blocks, bc.bw * bc.bh);
