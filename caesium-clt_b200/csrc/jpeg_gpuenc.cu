@@ -4,9 +4,11 @@
 // 0xFF stuffing) are resolved with prefix scans (CUB DeviceScan -- plumbing, not one of the path's named kernels).
 //
 // Passes (one launch each for ANY number of images x scans; blockIdx.y = scan):
-//   classify + inline-symbol histogram -> [max-scan: previous event] [sum-scan: trailing correction bits] -> groups + EOBn
-//   histogram -> tables -> lengths -> [sum-scan: bit offsets] -> scan sizes / buffer layout (on the device) -> zero -> emit -> ffcount -> [sum-scan] ->
-//   layout -> scatter (byte stuffing) | D2H: stuffed scans + DHT payloads.  No host wait in between: see "host orchestration".
+//   classify + inline-symbol histogram + correction-bit counts -> [max-scan: previous event] [sum-scan: trailing correction bits] ->
+//   groups + EOBn histogram -> tables + bits per table -> scan sizes / buffer layout (on the device) | D2H: sizes ->
+//   lengths of the interleaved scans' units -> [sum-scan: their bit offsets] -> zero -> emit (single-component scans: CTA runs into a
+//   staging arena) -> [sum-scan: run offsets] -> place runs -> ffcount -> [sum-scan] -> layout -> scatter (byte stuffing) |
+//   D2H: stuffed scans + DHT payloads.  No host wait in between: see "host orchestration".
 #include <cuda_runtime.h>
 #include <cub/device/device_scan.cuh>
 #include <cuda_pipeline.h>
@@ -48,7 +50,8 @@ __global__ void k_ge_groups(const Scan *__restrict__ scans, const uint32_t *__re
 
 // jchuff.c jpeg_gen_optimal_table with the two minimum searches spread over a warp (ties resolve to the LARGEST index,
 // exactly like the sequential `<=` scans); the chain merges and the canonical code assignment stay on lane 0.
-__global__ void k_ge_tables(const uint32_t *__restrict__ hist, Table *__restrict__ tabs, DhtOut *__restrict__ dht)
+// Also the table's share of its scan's size: sum(hist[symbol] * (code length + sym_extra_bits)) into tbits[t].
+__global__ void k_ge_tables(const uint32_t *__restrict__ hist, Table *__restrict__ tabs, DhtOut *__restrict__ dht, unsigned long long *__restrict__ tbits)
 {
     __shared__ long long freq[257];
     __shared__ int codesize[257], others[257];
@@ -108,41 +111,62 @@ __global__ void k_ge_tables(const uint32_t *__restrict__ hist, Table *__restrict
         for (int k2 = 0; k2 < 17; k2++) D.bits[k2] = bits[k2];
         for (int k2 = 0; k2 < p; k2++) D.vals[k2] = T.vals[k2];
     }
+    __syncwarp();                           // lane 0's code lengths are visible to the warp
+    const int kind = (t & 3) >> 1;
+    unsigned long long nb = 0;
+    for (int i = lane; i < 256; i += 32) if (f[i]) nb += (unsigned long long)f[i] * ((tabs[t].code_len[i] & 0xFFu) + (unsigned)sym_extra_bits(kind, i));
+    for (int d = 16; d; d >>= 1) nb += __shfl_xor_sync(0xFFFFFFFFu, nb, d);
+    if (lane == 0) tbits[t] = nb;
 }
 
-// Sizes on the device: bits per scan from the bit-offset scan, then every scan's place in the group's bit buffer (word_base),
-// its byte / 16-byte-group counts and the group index base -- what the host used to compute between two halves of the pipeline
-// (one stream wait per megabatch less).  The buffers are sized from an ESTIMATE of the output (the input's size for a re-encode);
+// Sizes on the device: bits per scan (its four tables' bits + its correction bits), then every scan's place in the group's bit
+// buffer (word_base) and, for a single-component scan, in the staging arena of its CTA runs (arena_base: a run takes whole words,
+// so a scan takes at most its words plus one per run), its byte / 16-byte-group counts and the group index base -- what the host
+// used to compute between two halves of the pipeline (one stream wait per megabatch less).  The buffers are sized from an ESTIMATE of the output (the input's size for a re-encode);
 // if the real sizes do not fit, flags[0] is raised, every scan is given zero length so the back half does nothing, and the host
 // re-runs the back half with exact sizes (flags[1..2] = words / groups needed).  One warp; scans in chunks of 32.
-__global__ void k_ge_scanout(const Scan *__restrict__ scans, int nscans, const uint32_t *__restrict__ bitlen, const uint32_t *__restrict__ bitoff, uint32_t *__restrict__ total,
-                             ScanOut *__restrict__ so, uint32_t words_cap, uint32_t groups_cap, uint32_t *__restrict__ flags)
+__global__ void k_ge_scanout(const Scan *__restrict__ scans, int nscans, const unsigned long long *__restrict__ tbits, const uint32_t *__restrict__ corr,
+                             uint32_t *__restrict__ total, ScanOut *__restrict__ so, uint32_t words_cap, uint32_t groups_cap, uint32_t *__restrict__ flags)
 {
     const int lane = threadIdx.x;
-    uint32_t wbase = 0, gbase = 0;
+    uint32_t wbase = 0, gbase = 0, abase = 0;
     for (int c0 = 0; c0 < nscans; c0 += 32) {
         const int i = c0 + lane;
-        uint32_t tb = 0;
-        if (i < nscans) { const Scan s = scans[i]; const long long last = s.unit_base + s.nblocks - 1; tb = s.nblocks ? bitoff[last] + bitlen[last] - bitoff[s.unit_base] : 0; }
+        uint32_t tb = 0, na = 0;
+        if (i < nscans) {
+            tb = (uint32_t)(tbits[4 * i] + tbits[4 * i + 1] + tbits[4 * i + 2] + tbits[4 * i + 3] + corr[i]);
+            na = scans[i].nruns ? (tb + 31) / 32 + scans[i].nruns : 0;
+        }
         const uint32_t nbytes = (tb + 7) / 8, ng = (nbytes + 15) / 16, nw = i < nscans ? (tb + 31) / 32 + 1 : 0;
-        uint32_t wi = nw, gi = i < nscans ? ng : 0;                  // inclusive warp scans
-        for (int d = 1; d < 32; d <<= 1) { const uint32_t a = __shfl_up_sync(0xFFFFFFFFu, wi, d), b = __shfl_up_sync(0xFFFFFFFFu, gi, d); if (lane >= d) { wi += a; gi += b; } }
-        if (i < nscans) { total[i] = tb; ScanOut o; o.total_bits = tb; o.nbytes = nbytes; o.ngroups = ng; o.group_base = gbase + gi - ng; o.word_base = wbase + wi - nw; o.pad_ = 0; so[i] = o; }
-        wbase += __shfl_sync(0xFFFFFFFFu, wi, 31); gbase += __shfl_sync(0xFFFFFFFFu, gi, 31);
+        uint32_t wi = nw, gi = i < nscans ? ng : 0, ai = na;        // inclusive warp scans
+        for (int d = 1; d < 32; d <<= 1) {
+            const uint32_t a = __shfl_up_sync(0xFFFFFFFFu, wi, d), b = __shfl_up_sync(0xFFFFFFFFu, gi, d), c = __shfl_up_sync(0xFFFFFFFFu, ai, d);
+            if (lane >= d) { wi += a; gi += b; ai += c; }
+        }
+        if (i < nscans) {
+            total[i] = tb;
+            ScanOut o; o.total_bits = tb; o.nbytes = nbytes; o.ngroups = ng; o.group_base = gbase + gi - ng; o.word_base = wbase + wi - nw; o.arena_base = abase + ai - na;
+            so[i] = o;
+        }
+        wbase += __shfl_sync(0xFFFFFFFFu, wi, 31); gbase += __shfl_sync(0xFFFFFFFFu, gi, 31); abase += __shfl_sync(0xFFFFFFFFu, ai, 31);
     }
     __syncwarp();
-    const bool ovf = wbase > words_cap || gbase > groups_cap;
+    const bool ovf = wbase > words_cap || gbase > groups_cap;       // the arena holds words_cap + total_runs words: it fits when the words do
     if (lane == 0) { flags[0] = ovf ? 1u : 0u; flags[1] = wbase; flags[2] = gbase; flags[3] = 0; flags[4] = 0; }
-    if (ovf) for (int i = lane; i < nscans; i += 32) { so[i].total_bits = 0; so[i].nbytes = 0; so[i].ngroups = 0; so[i].group_base = 0; so[i].word_base = 0; }
+    if (ovf) for (int i = lane; i < nscans; i += 32) { so[i].total_bits = 0; so[i].nbytes = 0; so[i].ngroups = 0; so[i].group_base = 0; so[i].word_base = 0; so[i].arena_base = 0; }
 }
 
-__global__ void k_ge_zero(const ScanOut *__restrict__ so, uint32_t *__restrict__ words)
+// a scan's bit buffer, and for a single-component scan its part of the staging arena (the runs' edge words are ORed)
+__global__ void k_ge_zero(const Scan *__restrict__ scans, const ScanOut *__restrict__ so, uint32_t *__restrict__ words, uint32_t *__restrict__ arena)
 {
     const ScanOut o = so[blockIdx.y];
     if (!o.total_bits) return;
-    const uint32_t n = (o.total_bits + 31) / 32 + 1;
-    uint32_t *w = words + o.word_base;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) w[i] = 0;
+    const uint32_t n = (o.total_bits + 31) / 32 + 1, nruns = (uint32_t)scans[blockIdx.y].nruns, na = nruns ? n - 1 + nruns : 0;
+    uint32_t *w = words + o.word_base, *a = arena + o.arena_base;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < max(n, na); i += gridDim.x * blockDim.x) {
+        if (i < n) w[i] = 0;
+        if (i < na) a[i] = 0;
+    }
 }
 
 // ---- block-major passes: one thread per block; the block is read (and its threshold masks built) once per pass and
@@ -151,7 +175,6 @@ __global__ void k_ge_zero(const ScanOut *__restrict__ so, uint32_t *__restrict__
 // coefficients, staged in shared memory with coalesced 16-byte loads so that the symbol loops read their scattered non-zero
 // coefficients from the tile instead of with one dependent global load each.  Rows are 144 bytes apart: the 16-byte reads of a
 // quarter warp (eight consecutive blocks at the same offset) then fall on distinct banks.
-constexpr int ENC_THREADS = 128;
 constexpr int TILE_PITCH = 72;                  // int16 per tile row
 typedef int16_t Tile[ENC_THREADS][TILE_PITCH];
 
@@ -213,17 +236,20 @@ struct SmemHist {
     __device__ void sym(int kind, int, int symbol, int, unsigned) { atomicAdd((kind ? h.ac : h.dc) + symbol, 1u); }
     __device__ void raw64(int, unsigned long long) {}
 };
+// Also each refinement scan's correction bits (corr[scan]), the one part of a scan's size that is not in its histograms.
 __global__ void __launch_bounds__(ENC_THREADS) k_geb_classify(const BlockComp *__restrict__ comps, uint32_t *__restrict__ meta, int *__restrict__ evkey,
-                                                              uint32_t *__restrict__ tail, Masks3 *__restrict__ masks, uint32_t *__restrict__ hist)
+                                                              uint32_t *__restrict__ tail, Masks3 *__restrict__ masks, uint32_t *__restrict__ hist, uint32_t *__restrict__ corr)
 {
     __shared__ __align__(16) Tile tile;
     __shared__ uint32_t h[ENC_TAB_ENTRIES];
     __shared__ EncVisit vis[ENC_MAX_VISITS];
+    __shared__ uint32_t vcorr[ENC_MAX_VISITS];
     const BlockComp &bc = comps[blockIdx.y];
     const int nblk = bc.bw * bc.bh, i0 = blockIdx.x * ENC_THREADS, i = i0 + threadIdx.x;
     if (i0 >= nblk) return;
     stage_tile(tile, bc, i0, nblk);
     for (int k = threadIdx.x; k < ENC_TAB_ENTRIES; k += ENC_THREADS) h[k] = 0;
+    if (threadIdx.x < ENC_MAX_VISITS) vcorr[threadIdx.x] = 0;
     stage_visits(vis, bc);
     wait_tile();
     if (i < nblk) {
@@ -239,9 +265,12 @@ __global__ void __launch_bounds__(ENC_THREADS) k_geb_classify(const BlockComp *_
             meta[g] = m; evkey[g] = meta_event(m) ? g : -1; tail[g] = (uint32_t)meta_tail(m);
             SmemHist sk{kind_tabs(h, v)};
             gen_block_m(v, v.tbl, ref_of(v, bc, tile, i0, row, col), M, 0, sk);
+            const int nc = corr_bits_m(v, M);
+            if (nc) atomicAdd(&vcorr[j], (uint32_t)nc);
         }
     }
     __syncthreads();
+    if ((int)threadIdx.x < bc.nscan && vcorr[threadIdx.x]) atomicAdd(&corr[vis[threadIdx.x].scan], vcorr[threadIdx.x]);
     for (int k = threadIdx.x; k < ENC_TAB_ENTRIES; k += ENC_THREADS) {
         int symbol; const int t = enc_entry_table(bc, k, symbol);
         if (h[k]) atomicAdd(&hist[(size_t)t * 256 + symbol], h[k]);     // an unused slot counts nothing
@@ -250,6 +279,8 @@ __global__ void __launch_bounds__(ENC_THREADS) k_geb_classify(const BlockComp *_
 
 // The length and emit passes load the tables of the CTA's visits once (k_ge_tables wrote them): the per-symbol lookup on the
 // symbol's dependent chain is a shared-memory read.  len keeps the code lengths only.
+// len runs over the visits of interleaved scans (ns > 1) only: the blocks of a CTA are not consecutive units there, so emit needs
+// every unit's bit offset.
 __global__ void __launch_bounds__(ENC_THREADS) k_geb_len(const BlockComp *__restrict__ comps, const uint32_t *__restrict__ gcount, const Table *__restrict__ tabs,
                                                          uint32_t *__restrict__ bitlen, const Masks3 *__restrict__ masks)
 {
@@ -271,51 +302,145 @@ __global__ void __launch_bounds__(ENC_THREADS) k_geb_len(const BlockComp *__rest
     const int row = i / bc.bw, col = i - row * bc.bw;
     for (int j = 0; j < bc.nscan; j++) {
         const EncVisit &v = vis[j];
+        if (v.ns == 1) continue;
         const int u = enc_unit_of(bc, v.ns, row, col);
         if (u < 0) continue;
         LenSinkT<KindTabs<const uint8_t>> sk{kind_tabs<const uint8_t>(tl, v)};
         gen_block_m(v, v.tbl, ref_of(v, bc, tile, i0, row, col), M, gcount[v.unit_base + u], sk);
-        bitlen[v.unit_base + u] = (uint32_t)sk.bits;
+        bitlen[v.lu_base + u] = (uint32_t)sk.bits;
+    }
+}
+// The same when every interleaved visit is a DC-first one (the progressive script): a unit is one DC difference, so a thread reads
+// its block's and the predecessor's DC coefficient and one code length from global memory -- no tile, masks or table staging.
+constexpr int LEN_DC_THREADS = 256;
+__global__ void __launch_bounds__(LEN_DC_THREADS) k_geb_len_dc(const BlockComp *__restrict__ comps, const Table *__restrict__ tabs, uint32_t *__restrict__ bitlen)
+{
+    const BlockComp &bc = comps[blockIdx.y];
+    const int nblk = bc.bw * bc.bh, i = blockIdx.x * LEN_DC_THREADS + threadIdx.x;
+    if (i >= nblk) return;
+    const int row = i / bc.bw, col = i - row * bc.bw;
+    const int16_t *cb = bc.coef + bc.comp_off;
+    const Masks3 none{};
+    for (int j = 0; j < bc.nscan; j++) {
+        const EncVisit v = bc.visit[j];
+        if (v.ns == 1) continue;
+        const int p = enc_dc_prev(bc, v.ns, row, col);
+        const BlockRef r{cb + (long long)i * 64, p >= 0 ? cb + (long long)p * 64 : nullptr, 0};
+        LenSinkT<KindTabs<const uint32_t>> sk{KindTabs<const uint32_t>{tabs[bc.tab[ENC_AC_SLOTS]].code_len, nullptr}};
+        gen_block_m(v, v.tbl, r, none, 0, sk);
+        bitlen[v.lu_base + enc_unit_of(bc, v.ns, row, col)] = (uint32_t)sk.bits;
     }
 }
 
+// exclusive prefix sum of x over the CTA, and the CTA's total; every thread calls it (it has a barrier)
+__device__ __forceinline__ uint32_t cta_exclusive_sum(uint32_t x, uint32_t *wsum /*ENC_THREADS / 32*/, uint32_t &total)
+{
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    uint32_t inc = x;
+    for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, inc, d); if (lane >= d) inc += y; }
+    if (lane == 31) wsum[w] = inc;
+    __syncthreads();
+    uint32_t base = 0, tot = 0;
+#pragma unroll
+    for (int k = 0; k < ENC_THREADS / 32; k++) { const uint32_t sk = wsum[k]; if (k < w) base += sk; tot += sk; }
+    total = tot;
+    return base + inc - x;
+}
+
+// Emit.  A visit of an interleaved scan writes each unit at the bit offset k_geb_len's lengths gave it.  A visit of a single-component
+// scan codes its units once for length and bits together: the CTA's units are consecutive units of the scan, so their offsets inside
+// the CTA's run follow from the lengths, and the run's place in the scan from the other runs' lengths (k_ge_place):
+//   - each thread codes its unit into its slot of ENC_SLOT_WORDS words in shared memory, counting bits past the slot's end;
+//   - a CTA-wide prefix sum gives each unit's offset in the run and the run's length;
+//   - the run takes its words in the scan's part of the staging arena (a per-scan counter: the order of the runs in the arena does
+//     not matter, k_ge_place finds each through runpos), and each unit is copied there from its slot -- or, when it overflowed the
+//     slot, coded a second time straight to its place.
+constexpr int ENC_SLOT_WORDS = 8;
 __global__ void __launch_bounds__(ENC_THREADS) k_geb_emit(const BlockComp *__restrict__ comps, const uint32_t *__restrict__ gcount, const Table *__restrict__ tabs,
                                                           const uint32_t *__restrict__ bitoff, uint32_t *__restrict__ words, const Masks3 *__restrict__ masks, const ScanOut *__restrict__ so,
-                                                          const uint32_t *__restrict__ flags)
+                                                          const uint32_t *__restrict__ flags, uint32_t *__restrict__ arena, uint32_t *__restrict__ cursor,
+                                                          uint32_t *__restrict__ runlen, uint32_t *__restrict__ runpos)
 {
     __shared__ __align__(16) Tile tile;
     __shared__ uint32_t tc[ENC_TAB_ENTRIES];
     __shared__ EncVisit vis[ENC_MAX_VISITS];
-    __shared__ uint32_t vword[ENC_MAX_VISITS], vbit0[ENC_MAX_VISITS];     // each visit's scan: first word, bit offset of unit 0
+    __shared__ uint32_t vword[ENC_MAX_VISITS], vbit0[ENC_MAX_VISITS];     // interleaved scan: first word, bit offset of unit 0; else arena base
+    __shared__ uint32_t slot[ENC_SLOT_WORDS][ENC_THREADS];                // word-major: a warp's stores to its slots hit 32 banks
+    __shared__ uint32_t wsum[ENC_THREADS / 32], run_word;
     if (flags[0]) return;                   // the bit buffer is too small for this batch: the host re-runs this half with exact sizes
     const BlockComp &bc = comps[blockIdx.y];
     const int nblk = bc.bw * bc.bh, i0 = blockIdx.x * ENC_THREADS, i = i0 + threadIdx.x;
     if (i0 >= nblk) return;
+    const bool live = i < nblk;
     stage_tile(tile, bc, i0, nblk);
     const Masks3 M = load_masks(masks, bc, min(i, nblk - 1));   // in flight with the tile
     stage_visits(vis, bc);
     if ((int)threadIdx.x < bc.nscan) {
         const EncVisit &v = bc.visit[threadIdx.x];
-        vword[threadIdx.x] = so[v.scan].word_base; vbit0[threadIdx.x] = bitoff[v.unit_base];
+        const ScanOut &o = so[v.scan];
+        vword[threadIdx.x] = v.ns > 1 ? o.word_base : o.arena_base; vbit0[threadIdx.x] = v.ns > 1 ? bitoff[v.lu_base] : 0;
     }
     for (int k = threadIdx.x; k < ENC_TAB_ENTRIES; k += ENC_THREADS) {
         int symbol; const int t = enc_entry_table(bc, k, symbol);
         if (t >= 0) tc[k] = tabs[t].code_len[symbol];
     }
     wait_tile();
-    if (i >= nblk) return;
     const int row = i / bc.bw, col = i - row * bc.bw;
     auto orw = [&](long long w, uint32_t v) { if (v) atomicOr(&words[w], v); };
     auto stw = [&](long long w, uint32_t v) { words[w] = v; };
-    for (int j = 0; j < bc.nscan; j++) {
+    auto ora = [&](long long w, uint32_t v) { if (v) atomicOr(&arena[w], v); };
+    auto sta = [&](long long w, uint32_t v) { arena[w] = v; };
+    auto sls = [&](long long w, uint32_t v) { if (w < ENC_SLOT_WORDS) slot[w][threadIdx.x] = v; };
+    typedef KindTabs<const uint32_t> KT;
+    for (int j = 0; j < bc.nscan; j++) {                        // v.ns is the same for the whole CTA: the barriers below are uniform
         const EncVisit &v = vis[j];
-        const int u = enc_unit_of(bc, v.ns, row, col);
-        if (u < 0) continue;
-        EmitSink<decltype(orw), decltype(stw), KindTabs<const uint32_t>> sk(kind_tabs<const uint32_t>(tc, v), orw, stw, (long long)vword[j],
-                                                                            (unsigned long long)(bitoff[v.unit_base + u] - vbit0[j]));
-        gen_block_m(v, v.tbl, ref_of(v, bc, tile, i0, row, col), M, gcount[v.unit_base + u], sk);
-        sk.finish();
+        const int u = live ? enc_unit_of(bc, v.ns, row, col) : -1;
+        if (v.ns > 1) {
+            if (u < 0) continue;
+            EmitSink<decltype(orw), decltype(stw), KT> sk(kind_tabs<const uint32_t>(tc, v), orw, stw, (long long)vword[j], (unsigned long long)(bitoff[v.lu_base + u] - vbit0[j]));
+            gen_block_m(v, v.tbl, ref_of(v, bc, tile, i0, row, col), M, gcount[v.unit_base + u], sk);
+            sk.finish();
+            continue;
+        }
+        uint32_t nb = 0;
+        if (u >= 0) {
+            EmitSink<decltype(sls), decltype(sls), KT> sk(kind_tabs<const uint32_t>(tc, v), sls, sls, 0, 0);
+            gen_block_m(v, v.tbl, ref_of(v, bc, tile, i0, row, col), M, gcount[v.unit_base + u], sk);
+            sk.finish();
+            nb = (uint32_t)sk.bits_written(0);
+        }
+        uint32_t L;
+        const uint32_t off = cta_exclusive_sum(nb, wsum, L);
+        if (threadIdx.x == 0) {
+            const uint32_t a = vword[j] + atomicAdd(&cursor[v.scan], (L + 31) / 32);
+            run_word = a; runlen[v.run_base + blockIdx.x] = L; runpos[v.run_base + blockIdx.x] = a;
+        }
+        __syncthreads();
+        const unsigned long long at = (unsigned long long)run_word * 32 + off;
+        if (nb <= ENC_SLOT_WORDS * 32) place_bits([&](long long k) { return slot[k][threadIdx.x]; }, nb, at, ora, sta);
+        else {                              // rare: the unit overflowed its slot
+            EmitSink<decltype(ora), decltype(sta), KT> sk(kind_tabs<const uint32_t>(tc, v), ora, sta, 0, at);
+            gen_block_m(v, v.tbl, ref_of(v, bc, tile, i0, row, col), M, gcount[v.unit_base + u], sk);
+            sk.finish();
+        }
     }
+}
+
+// Runs of the single-component scans to their place in the scan's bit buffer: run r of scan y starts runoff[r] - runoff[first run]
+// bits into the scan (an exclusive sum over the run lengths); one warp per run, funnel-shifting the run's whole arena words.
+constexpr int PLACE_THREADS = 128;
+__global__ void __launch_bounds__(PLACE_THREADS) k_ge_place(const Scan *__restrict__ scans, const ScanOut *__restrict__ so, const uint32_t *__restrict__ runlen,
+                                                            const uint32_t *__restrict__ runoff, const uint32_t *__restrict__ runpos, const uint32_t *__restrict__ arena,
+                                                            uint32_t *__restrict__ words, const uint32_t *__restrict__ flags)
+{
+    if (flags[0]) return;
+    const int nruns = scans[blockIdx.y].nruns, x = blockIdx.x * (PLACE_THREADS / 32) + (threadIdx.x >> 5);
+    if (x >= nruns) return;
+    const int r0 = scans[blockIdx.y].run_base, r = r0 + x;
+    const uint32_t *src = arena + runpos[r];
+    uint32_t *dst = words + so[blockIdx.y].word_base;
+    place_bits([&](long long k) { return src[k]; }, runlen[r], runoff[r] - runoff[r0],
+               [&](long long w, uint32_t v) { atomicOr(&dst[w], v); }, [&](long long w, uint32_t v) { dst[w] = v; }, threadIdx.x & 31, 32);
 }
 
 // byte i of a scan's unstuffed stream (big-endian within words), with flush_bits' padding ones in the last byte
@@ -402,7 +527,7 @@ __global__ void k_ge_fill_dummy(int16_t *__restrict__ coef, long long comp_off, 
 // Three steps so that a megabatch costs the host one wait that overlaps device work plus the final one, and so that a caller with
 // everything resident in HBM (bench.py's device-only figure) can enqueue the whole pass sequence without any wait:
 //   prepare()  plan + buffers (sized from an estimate of the output) + H2D of the descriptors
-//   enqueue()  every kernel; D2H of the sizes right after the bit-offset scan (event), D2H of DHT payloads / stuffed lengths at the end
+//   enqueue()  every kernel; D2H of the sizes right after the tables (event), D2H of DHT payloads / stuffed lengths at the end
 //   finish()   wait for the sizes (the emit / stuffing kernels are still running), size and enqueue the D2H of the stuffed scans,
 //              final wait; a batch that outgrew the estimate re-runs the back half with exact sizes
 static inline size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
@@ -420,15 +545,17 @@ bool GpuEncoder::size_back_buffers(size_t image_bytes, std::string &err)
     const int NS = (int)plan.scans.size();
     // capacities only grow (per image count): they are kernel arguments of the launch sequence, and a sequence whose arguments do
     // not change from megabatch to megabatch can be replayed as a CUDA graph
+    auto grow = [&](auto &buf, size_t need) { return buf.reserve(need, Grow::Pow2Half, err, &generation); };
+    // the staging arena of the single-component scans' runs: at most the scans' words plus one per run (k_ge_scanout)
+    auto grow_arena = [&]() { return grow(d_arena, ((size_t)words_cap + (size_t)plan.total_runs) * 4 + 64); };
     if (nimg != cap_nimg) { cap_nimg = nimg; est_image_bytes = 0; }
-    if (image_bytes <= est_image_bytes && words_cap) return true;
+    if (image_bytes <= est_image_bytes && words_cap) return grow_arena();
     est_image_bytes = image_bytes + image_bytes / 8;
     image_bytes = est_image_bytes;
     words_cap = (uint32_t)std::min<size_t>((size_t)nimg * (image_bytes / 4 + 1) + 2 * (size_t)NS + 64, 0xFFFFFF00u);
     groups_cap = (uint32_t)((size_t)words_cap / 4 + NS + 1);
     out_stride = align_up(image_bytes + image_bytes / 8 + 1024, 256);
-    auto grow = [&](auto &buf, size_t need) { return buf.reserve(need, Grow::Pow2Half, err, &generation); };
-    if (!grow(d_words, (size_t)words_cap * 4 + 64) || !grow(d_ffcount, (size_t)groups_cap * 4 + 4) || !grow(d_ffoff, (size_t)groups_cap * 4 + 4) ||
+    if (!grow_arena() || !grow(d_words, (size_t)words_cap * 4 + 64) || !grow(d_ffcount, (size_t)groups_cap * 4 + 4) || !grow(d_ffoff, (size_t)groups_cap * 4 + 4) ||
         !grow(d_out, out_stride * nimg)) return false;
     size_t tb3 = 0; cub::DeviceScan::ExclusiveSum((void *)nullptr, tb3, d_ffcount.get(), d_ffoff.get(), (int)groups_cap, (cudaStream_t)0);
     return grow(d_temp, tb3 + 256);
@@ -443,7 +570,8 @@ bool GpuEncoder::prepare(const JpegGeom &g, bool progressive, int16_t *const *d_
     gpuenc_plan(g, progressive, bases.data(), nimages, plan);
     nimg = nimages;
     const int NS = (int)plan.scans.size();
-    const long long U = plan.total_units;
+    const long long U = plan.total_units, LU = std::max(plan.total_lunits, 1ll);
+    const int R = std::max(plan.total_runs, 1);
     if (U >= (1ll << 31)) { err = "batch too large for the entropy encoder"; return false; }
     overflow = false;
     for (auto &sc_ : plan.scans) if (!masks_cover(sc_.mode, sc_.Al)) { err = "scan script outside the device encoder's mask range"; overflow = true; return false; }
@@ -454,7 +582,8 @@ bool GpuEncoder::prepare(const JpegGeom &g, bool progressive, int16_t *const *d_
     const int NC = (int)plan.comps.size();
     if (!grow(d_scans, NS * sizeof(Scan)) || !grow(d_comps, NC * sizeof(BlockComp)) ||
         !grow(d_meta, U * 4) || !grow(d_evkey, U * 4) || !grow(d_prev, U * 4) || !grow(d_tail, U * 4) || !grow(d_tsum, U * 4) ||
-        !grow(d_gcount, U * 4) || !grow(d_bitlen, U * 4) || !grow(d_bitoff, U * 4) ||
+        !grow(d_gcount, U * 4) || !grow(d_bitlen, LU * 4) || !grow(d_bitoff, LU * 4) || !grow(d_corr, (size_t)NS * 4) || !grow(d_tbits, (size_t)NS * 4 * 8) ||
+        !grow(d_cursor, (size_t)NS * 4) || !grow(d_runlen, (size_t)R * 4) || !grow(d_runoff, (size_t)R * 4) || !grow(d_runpos, (size_t)R * 4) ||
         !grow(d_hist, (size_t)NS * 4 * 256 * 4) || !grow(d_tabs, (size_t)NS * 4 * sizeof(Table)) || !grow(d_dht, (size_t)NS * 4 * sizeof(DhtOut)) ||
         !grow(d_total, (size_t)NS * 4) || !grow(d_so, (size_t)NS * sizeof(ScanOut)) || !grow(d_outoff, (size_t)NS * 4) || !grow(d_outlen, (size_t)NS * 4) ||
         !grow(d_flags, 64) || !grow(d_masks, (size_t)plan.total_comp_blocks * sizeof(Masks3))) return false;
@@ -463,10 +592,12 @@ bool GpuEncoder::prepare(const JpegGeom &g, bool progressive, int16_t *const *d_
     o_flags = o_comps + align_up((size_t)NC * sizeof(BlockComp), 256);
     const size_t small_bytes = o_flags + 256;
     if (!grow(h_small, small_bytes)) return false;
-    size_t tb1 = 0, tb2 = 0;
+    size_t tb1 = 0, tb2 = 0, tb3 = 0, tb4 = 0;
     cub::DeviceScan::ExclusiveScan((void *)nullptr, tb1, d_evkey.get(), d_prev.get(), cub::Max(), -1, (int)U, st);
     cub::DeviceScan::ExclusiveSum((void *)nullptr, tb2, d_tail.get(), d_tsum.get(), (int)U, st);
-    if (!grow(d_temp, std::max(tb1, tb2) + 256)) return false;
+    cub::DeviceScan::ExclusiveSum((void *)nullptr, tb3, d_bitlen.get(), d_bitoff.get(), (int)LU, st);
+    cub::DeviceScan::ExclusiveSum((void *)nullptr, tb4, d_runlen.get(), d_runoff.get(), R, st);
+    if (!grow(d_temp, std::max(std::max(tb1, tb2), std::max(tb3, tb4)) + 256)) return false;
     // ---- buffers whose size follows the OUTPUT: estimate now, exact on a retry.  A re-encode at lower quality does not grow, so
     // the caller's hint is the input's entropy-coded size; without a hint a third of the coefficient bytes (~ 1 byte / pixel).
     const size_t coef_bytes = (size_t)g.total_coefs * 2;
@@ -501,6 +632,7 @@ unsigned long long GpuEncoder::signature() const
     for (auto pb : coef_bases) mix((unsigned long long)(uintptr_t)pb);
     int max_units = 0; for (auto &sc : plan.scans) max_units = std::max(max_units, sc.nblocks);
     mix((unsigned long long)max_units);
+    mix((unsigned long long)plan.total_lunits); mix((unsigned long long)plan.total_runs); mix((unsigned long long)plan.max_runs);
     return h;
 }
 
@@ -510,7 +642,7 @@ bool GpuEncoder::enqueue_sizes(void *stream_, std::string &err)
     cudaStream_t st = (cudaStream_t)stream_;
     const int NS = (int)plan.scans.size();
     uint32_t *h_total = reinterpret_cast<uint32_t *>(h_small + o_total), *h_flags = reinterpret_cast<uint32_t *>(h_small + o_flags);
-    k_ge_scanout<<<1, 32, 0, st>>>(d_scans, NS, d_bitlen, d_bitoff, d_total, d_so, words_cap, groups_cap, d_flags);
+    k_ge_scanout<<<1, 32, 0, st>>>(d_scans, NS, d_tbits, d_corr, d_total, d_so, words_cap, groups_cap, d_flags);
     LT_MARK("k_ge_scanout");
     CU(cudaMemcpyAsync(h_total, d_total, (size_t)NS * 4, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(h_flags, d_flags, 12, cudaMemcpyDeviceToHost, st));
@@ -529,10 +661,36 @@ bool GpuEncoder::enqueue_back(void *stream_, std::string &err)
     const int NS = (int)plan.scans.size(), NC = (int)plan.comps.size();
     uint32_t *h_flags = reinterpret_cast<uint32_t *>(h_small + o_flags);
     const dim3 gb(cdiv(plan.max_comp_blocks, ENC_THREADS), NC);
-    k_ge_zero<<<dim3(64, NS), 256, 0, st>>>(d_so, d_words);
+    int n = 6;
+    if (plan.total_lunits) {                // units of the interleaved scans: lengths, then bit offsets
+        bool dc_only = true;
+        for (auto &sc : plan.scans) if (sc.ns > 1 && sc.mode != MODE_DC_FIRST) dc_only = false;
+        if (dc_only) {
+            k_geb_len_dc<<<dim3(cdiv(plan.max_comp_blocks, LEN_DC_THREADS), NC), LEN_DC_THREADS, 0, st>>>(d_comps, d_tabs, d_bitlen);
+            LT_MARK("k_geb_len_dc");
+        } else {
+            k_geb_len<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_gcount, d_tabs, d_bitlen, d_masks);
+            LT_MARK("k_geb_len");
+        }
+        size_t tb = d_temp.capacity();
+        cub::DeviceScan::ExclusiveSum(d_temp, tb, d_bitlen.get(), d_bitoff.get(), (int)plan.total_lunits, st);
+        LT_MARK("cub_scan");
+        n += 2;
+    }
+    CU(cudaMemsetAsync(d_cursor, 0, (size_t)NS * 4, st));
+    LT_MARK("memset");
+    k_ge_zero<<<dim3(64, NS), 256, 0, st>>>(d_scans, d_so, d_words, d_arena);
     LT_MARK("k_ge_zero");
-    k_geb_emit<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_gcount, d_tabs, d_bitoff, d_words, d_masks, d_so, d_flags);
+    k_geb_emit<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_gcount, d_tabs, d_bitoff, d_words, d_masks, d_so, d_flags, d_arena, d_cursor, d_runlen, d_runpos);
     LT_MARK("k_geb_emit");
+    if (plan.total_runs) {                  // runs of the single-component scans: offsets, then placement
+        size_t tb = d_temp.capacity();
+        cub::DeviceScan::ExclusiveSum(d_temp, tb, d_runlen.get(), d_runoff.get(), plan.total_runs, st);
+        LT_MARK("cub_scan");
+        k_ge_place<<<dim3(cdiv(plan.max_runs, PLACE_THREADS / 32), NS), PLACE_THREADS, 0, st>>>(d_scans, d_so, d_runlen, d_runoff, d_runpos, d_arena, d_words, d_flags);
+        LT_MARK("k_ge_place");
+        n += 2;
+    }
     k_ge_ffcount<<<dim3(32, NS + 1), 128, 0, st>>>(d_so, NS, d_words, d_ffcount, groups_cap, d_flags);
     LT_MARK("k_ge_ffcount");
     size_t tb = d_temp.capacity();
@@ -546,7 +704,7 @@ bool GpuEncoder::enqueue_back(void *stream_, std::string &err)
     CU(cudaMemcpyAsync(h_small + o_dht, d_dht, (size_t)NS * 4 * sizeof(DhtOut), cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(h_flags + 4, d_flags, 32, cudaMemcpyDeviceToHost, st));         // second snapshot: image-level overflow (flags[3..4])
     CU(cudaGetLastError());
-    launches += 7;
+    launches += n;
     return true;
 }
 
@@ -575,7 +733,9 @@ bool GpuEncoder::enqueue_front(void *stream_, bool fill_dummy, std::string &err)
     const dim3 gu1(cdiv(max_units + 1, 128), NS);
     CU(cudaMemsetAsync(d_hist, 0, (size_t)NS * 4 * 256 * 4, st));
     LT_MARK("memset");
-    k_geb_classify<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_meta, d_evkey, d_tail, d_masks, d_hist);
+    CU(cudaMemsetAsync(d_corr, 0, (size_t)NS * 4, st));
+    LT_MARK("memset");
+    k_geb_classify<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_meta, d_evkey, d_tail, d_masks, d_hist, d_corr);
     LT_MARK("k_geb_classify");
     size_t tb = d_temp.capacity();
     cub::DeviceScan::ExclusiveScan(d_temp, tb, d_evkey.get(), d_prev.get(), cub::Max(), -1, (int)U, st);
@@ -587,14 +747,9 @@ bool GpuEncoder::enqueue_front(void *stream_, bool fill_dummy, std::string &err)
     LT_MARK("memset");
     k_ge_groups<<<gu1, 128, 0, st>>>(d_scans, d_meta, d_evkey, d_prev, d_tsum, d_gcount, d_hist);
     LT_MARK("k_ge_groups");
-    k_ge_tables<<<NS * 4, 32, 0, st>>>(d_hist, d_tabs, d_dht);
+    k_ge_tables<<<NS * 4, 32, 0, st>>>(d_hist, d_tabs, d_dht, d_tbits);
     LT_MARK("k_ge_tables");
-    k_geb_len<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_gcount, d_tabs, d_bitlen, d_masks);
-    LT_MARK("k_geb_len");
-    tb = d_temp.capacity();
-    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_bitlen.get(), d_bitoff.get(), (int)U, st);
-    LT_MARK("cub_scan");
-    launches += 7;
+    launches += 5;
     CU(cudaGetLastError());
     return true;
 }

@@ -10,7 +10,7 @@
 namespace b200 {
 
 struct DhtOut { uint8_t bits[17]; uint8_t vals[256]; int32_t nvals; };
-struct ScanOut { uint32_t total_bits, nbytes, ngroups, group_base, word_base, pad_; };   // filled on the device (k_ge_scanout)
+struct ScanOut { uint32_t total_bits, nbytes, ngroups, group_base, word_base, arena_base; };   // filled on the device (k_ge_scanout)
 
 // One encoder instance per slot (or per megabatch): owns its device / pinned buffers and grows them on demand.
 class GpuEncoder {
@@ -58,7 +58,11 @@ private:
     size_t o_scans = 0, o_total = 0, o_outlen = 0, o_dht = 0, o_comps = 0, o_flags = 0;
     DeviceBuffer<ge::Scan> d_scans;
     DeviceBuffer<BlockComp> d_comps;
-    DeviceBuffer<uint32_t> d_meta, d_tail, d_tsum, d_gcount, d_bitlen, d_bitoff;
+    DeviceBuffer<uint32_t> d_meta, d_tail, d_tsum, d_gcount;
+    DeviceBuffer<uint32_t> d_bitlen, d_bitoff;          // per unit of the interleaved scans (Scan::lu_base)
+    DeviceBuffer<uint32_t> d_corr;                      // correction bits per scan (k_geb_classify)
+    DeviceBuffer<unsigned long long> d_tbits;           // bits coded with each table (k_ge_tables)
+    DeviceBuffer<uint32_t> d_cursor, d_runlen, d_runoff, d_runpos, d_arena;   // CTA runs of the single-component scans (k_geb_emit, k_ge_place)
     DeviceBuffer<int> d_evkey, d_prev;
     DeviceBuffer<uint32_t> d_hist;
     DeviceBuffer<ge::Table> d_tabs;

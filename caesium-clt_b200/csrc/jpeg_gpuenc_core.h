@@ -44,7 +44,9 @@ struct Scan {
     int rbw, rbh;               // single-component geometry (real blocks)
     int nblocks;                // units in this scan
     long long unit_base;        // index of unit 0 in the batch-wide per-unit arrays
-    int tab_base;               // index of this scan's first table in the batch-wide table array (4 per scan: [kind*2+tbl])
+    long long lu_base;          // ns > 1: index of unit 0 in the per-unit bit length / offset arrays (only these scans have them)
+    int run_base, nruns;        // ns == 1: the scan's first CTA run in the batch-wide run arrays, and its run count
+    int tab_base;              // index of this scan's first table in the batch-wide table array (4 per scan: [kind*2+tbl])
     long long word_base;        // first word of this scan's unstuffed bit buffer
     long long word_cap;         // capacity in 32-bit words
 };
@@ -207,6 +209,12 @@ GE_HD uint32_t classify_m(const S &s, const Masks3 &M)
     else tail = popc64(mB & ~((2ull << last_new) - 1ull));
     return meta_pack(last_new >= 0, last_new < s.Se, tail);
 }
+// correction bits a block writes in a scan: one per coefficient of the band that was already non-zero (refinement scans only)
+template <class S>
+GE_HD int corr_bits_m(const S &s, const Masks3 &M)
+{
+    return s.mode == MODE_AC_REFINE ? popc64(mask_at(M, s.Al + 1) & band_mask(s.Ss, s.Se)) : 0;
+}
 GE_HD uint32_t classify(const Scan &s, const int16_t *blk)
 {
     if (s.mode == MODE_SEQ || s.mode == MODE_DC_FIRST) return meta_pack(true, false, 0);
@@ -225,6 +233,14 @@ GE_HD void gen_dc(int value_shifted, int pred_shifted, int tbl, Sink &sk)
 }
 
 GE_HD int eob_symbol(unsigned count) { return (nbits_of(count) - 1) << 4; }     // EOBn: AC symbol of a group of `count` blocks
+// The value bits that follow a Huffman symbol depend on the symbol alone: a DC symbol is its bit count; an AC run/size symbol
+// carries `size` bits, EOBn (n << 4, n < 15) carries n, ZRL (0xF0) and EOB (0x00) none.  So a scan's size is
+// sum(hist[symbol] * (code length + sym_extra_bits)) over its tables, plus the correction bits of a refinement scan.
+GE_HD int sym_extra_bits(int kind, int symbol)
+{
+    if (kind == 0) return symbol;
+    return (symbol & 15) ? (symbol & 15) : symbol == 0xF0 ? 0 : symbol >> 4;
+}
 template <class Sink>
 GE_HD void gen_eob_token(unsigned count, int tbl, Sink &sk)
 {
@@ -382,7 +398,25 @@ struct EmitSink {
         if (nb > 32) { put((unsigned)(v >> 32), nb - 32); put((unsigned)v, 32); } else put((unsigned)v, nb);   // v < 2^nb
     }
     GE_HD void finish() { if (n > 0) orw(wpos, cur); }
+    GE_HD unsigned long long bits_written(long long word_base) const { return (unsigned long long)(wpos - word_base) * 32 + n; }   // from a word-aligned start
 };
+
+// Copies bits [0, nbits) of the MSB-first word sequence src(0), src(1), ... (nothing set past nbits) to bit `bitoff` of a
+// zero-initialised word buffer.  Destination words k = k0, k0 + dk, ... of the range are produced: the first and the last, which a
+// neighbouring range may share, go through orw (atomic on the device), the others through stw.
+template <class Src, class OrFn, class StFn>
+GE_HD void place_bits(Src src, unsigned long long nbits, unsigned long long bitoff, OrFn &&orw, StFn &&stw, int k0 = 0, int dk = 1)
+{
+    if (!nbits) return;
+    const int s = (int)(bitoff & 31);
+    const long long w0 = (long long)(bitoff >> 5), nsrc = (long long)((nbits + 31) / 32), nout = (long long)((s + nbits + 31) / 32);
+    for (long long k = k0; k < nout; k += dk) {
+        const uint32_t hi = k > 0 ? src(k - 1) : 0u, lo = k < nsrc ? src(k) : 0u;
+        const uint32_t v = s ? (hi << (32 - s)) | (lo >> s) : lo;
+        if (k == 0 || k == nout - 1) { if (v) orw(w0 + k, v); }
+        else stw(w0 + k, v);
+    }
+}
 
 // ---- EOB groups (pass "groups"): called for every event unit b and once for b == nblocks (end of scan) -------------
 // prev_ev = index of the last event unit before b (-1 if none); meta/tsum are the scan's per-unit arrays (tsum =

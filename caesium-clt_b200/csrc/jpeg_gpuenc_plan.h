@@ -14,6 +14,9 @@ namespace b200 {
 // A CTA copies the component's visit records to shared memory and keeps the Huffman tables of its visits on chip: one slot per
 // table kind a visit codes, the AC tables first (256 symbols each), then the DC table (DC symbols are bit counts 0..16).
 // jpeg_scan_script's progressive luma has three AC visits and one DC visit, a sequential scan one of each.
+// A CTA of the block-major passes owns ENC_THREADS consecutive blocks of one component.  In a scan with one component these are
+// consecutive units: the CTA's part of such a scan is one run of the scan's bits, coded in one pass (see k_geb_emit).
+constexpr int ENC_THREADS = 128;
 constexpr int ENC_MAX_VISITS = 6, ENC_AC_SLOTS = 3, ENC_DC_SLOTS = 1, ENC_DC_SYMBOLS = 17;
 constexpr int ENC_TAB_ENTRIES = ENC_AC_SLOTS * 256 + ENC_DC_SLOTS * ENC_DC_SYMBOLS;   // entry of (AC slot a, symbol) = a * 256 + symbol
 constexpr int ENC_DC_ENTRY = ENC_AC_SLOTS * 256;                                      // entry of (DC slot, symbol) = ENC_DC_ENTRY + symbol
@@ -23,6 +26,8 @@ struct EncVisit {                       // one scan visiting the component: what
     int mode, Ss, Se, Al, ns;
     int tbl;                            // the component's Huffman table id
     int unit_base;                      // Scan::unit_base (a batch has fewer than 2^31 units)
+    int lu_base;                        // ns > 1: Scan::lu_base
+    int run_base;                       // ns == 1: Scan::run_base
     int ac_entry;                       // first on-chip entry of the visit's AC table (unused by a DC-only scan)
 };
 
@@ -72,6 +77,8 @@ struct GpuEncPlan {
     int scans_per_image = 0;
     long long units_per_image = 0, words_per_image = 0;
     long long total_units = 0, total_words = 0, total_comp_blocks = 0;
+    long long total_lunits = 0;         // units of the scans with ns > 1 (the ones coded unit by unit)
+    int total_runs = 0, max_runs = 0;   // CTA runs of the scans with ns == 1: in all, and in the largest scan
 };
 
 // coef_base[i] = device (or host) pointer to image i's coefficient buffer (geometry g, zigzag)
@@ -82,7 +89,9 @@ inline void gpuenc_plan(const JpegGeom &g, bool progressive, const int16_t *cons
     p.defs.assign(sc, sc + ns);
     p.scans_per_image = ns;
     p.scans.clear();
-    long long unit = 0, word = 0;
+    long long unit = 0, word = 0, lunit = 0;
+    int run = 0;
+    p.max_runs = 0;
     for (int im = 0; im < nimages; im++) {
         for (int si = 0; si < ns; si++) {
             const ScanDef &d = sc[si];
@@ -102,13 +111,16 @@ inline void gpuenc_plan(const JpegGeom &g, bool progressive, const int16_t *cons
             s.rbw = g.rbw[d.ci[0]]; s.rbh = g.rbh[d.ci[0]];
             s.nblocks = d.ns > 1 ? g.mcux * g.mcuy * s.blocks_per_mcu : s.rbw * s.rbh;
             s.unit_base = unit; unit += s.nblocks;
+            s.lu_base = -1; s.run_base = -1; s.nruns = 0;
+            if (d.ns > 1) { s.lu_base = lunit; lunit += s.nblocks; }
+            else { s.run_base = run; s.nruns = (g.bw[d.ci[0]] * g.bh[d.ci[0]] + ENC_THREADS - 1) / ENC_THREADS; run += s.nruns; p.max_runs = std::max(p.max_runs, s.nruns); }
             s.tab_base = (int)p.scans.size() * 4;
             s.word_base = word; s.word_cap = (long long)s.nblocks * 32 + 64; word += s.word_cap;   // 128 B per block: the size of its coefficients
             p.scans.push_back(s);
         }
         if (im == 0) { p.units_per_image = unit; p.words_per_image = word; }
     }
-    p.total_units = unit; p.total_words = word;
+    p.total_units = unit; p.total_words = word; p.total_lunits = lunit; p.total_runs = run;
     p.comps.clear(); p.max_comp_blocks = 0; p.total_comp_blocks = 0; p.on_chip = true;
     for (int im = 0; im < nimages; im++) {
         int qb = 0;
@@ -129,7 +141,7 @@ inline void gpuenc_plan(const JpegGeom &g, bool progressive, const int16_t *cons
                 if (bc.nscan == ENC_MAX_VISITS || nac + ac > ENC_AC_SLOTS || ndc + dc > ENC_DC_SLOTS) { p.on_chip = false; continue; }
                 EncVisit &v = bc.visit[bc.nscan++];
                 v.scan = im * ns + si; v.mode = s.mode; v.Ss = s.Ss; v.Se = s.Se; v.Al = s.Al; v.ns = s.ns; v.tbl = s.tbl[i];
-                v.unit_base = (int)s.unit_base;
+                v.unit_base = (int)s.unit_base; v.lu_base = (int)s.lu_base; v.run_base = s.run_base;
                 v.ac_entry = ac ? nac * 256 : 0;
                 if (ac) bc.tab[nac++] = s.tab_base + 2 + v.tbl;
                 if (dc) bc.tab[ENC_AC_SLOTS + ndc++] = s.tab_base + v.tbl;
