@@ -171,10 +171,12 @@ inline bool build_dec_tables(const uint8_t *const dht_bits[8], const uint8_t *co
     }
     if (!ok) {
         // a refused set is never trusted (T.ok = 0 sends the image to the host decoder): its entries only have to keep the passes
-        // in bounds and moving, so every one is a plain 16-bit skip
+        // in bounds and moving, so every one is a plain 16-bit skip.  The kernels stage only the first nlook slots, so every
+        // selector goes back to slot 0: one left on a later slot would read first-level entries that were never staged.
         const uint16_t SKIP = (uint16_t)(16 << 8);
         for (int i = 0; i < MAX_TABLES * LOOK_N; i++) T.look[i] = SKIP;
         for (int i = 0; i < EXT_N; i++) T.ext[i] = SKIP;
+        for (int i = 0; i < 20; i++) T.sel[i] = 0;
         T.nlook = 1; T.next = 0; T.ok = 0;
         return false;
     }

@@ -970,5 +970,19 @@ int orc_jpeg_lossless(const uint8_t *data, size_t len, const orc_jpeg_params *p,
     fill_dummy_blocks(&in);
     int rc = orc_jpeg_write(&in, p, &in, out, out_len, err);
     orc_jpeg_free(&in);
+    /* jpeg_copy_critical_parameters also copies the source's JFIF version (major 1 or 2) and density: patch them into the
+       APP0 orc_jpeg_write put at out[2] (version at +9, units at +11, X / Y density at +12 / +14) */
+    for (size_t i = 2; rc == 0 && i + 4 <= len && data[i] == 0xFF; ) {
+        unsigned m = data[i + 1];
+        if (m == 0xFF) { i++; continue; }
+        size_t L = ((size_t)data[i + 2] << 8) | data[i + 3];
+        if (m == 0xDA || m == 0xD9 || L < 2 || i + 2 + L > len) break;
+        if (m == 0xE0 && L >= 16 && !memcmp(data + i + 4, "JFIF\0", 5)) {
+            if (data[i + 9] == 1 || data[i + 9] == 2) memcpy(*out + 11, data + i + 9, 2);
+            memcpy(*out + 13, data + i + 11, 5);
+            break;
+        }
+        i += 2 + L;
+    }
     return rc;
 }

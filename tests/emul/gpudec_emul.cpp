@@ -148,6 +148,8 @@ extern "C" int emul_build_tables_raw(const uint8_t *ac_bits, const uint8_t *ac_v
     std::vector<gd::DecTables> T(1);
     const bool ok = gd::build_dec_tables(db, dv, G, T[0]);
     *pool_used = T[0].next; *bad = 0;
+    // the kernels stage the first nlook slots only: a selector past them would read first-level entries nobody staged
+    for (int i = 0; i < 20; i++) if (T[0].sel[i] >= T[0].nlook * gd::LOOK_N) (*bad)++;
     if (!ok) {
         for (int i = 0; i < gd::MAX_TABLES * gd::LOOK_N; i++) if (T[0].look[i] != (16 << 8)) (*bad)++;      // refused: all-invalid tables
         return 0;

@@ -90,7 +90,8 @@ def test_kernel_form_tables_equal_the_jdhuff_search(emul, golden):
 def test_adversarial_tables_fit_or_are_refused_cleanly(emul):
     """DHTs built to spread long codes over many 9-bit prefixes: the second-level pool either holds them (and the lookup equals the
     jdhuff.c search everywhere) or the table set is refused with an all-invalid, in-bounds result -- the image then goes to the
-    host decoder, like a stream that does not converge."""
+    host decoder, like a stream that does not converge.  Either way every block's selector names one of the first nlook slots,
+    the only ones the kernels stage: a selector past them would read shared memory nobody wrote."""
     dc_bits = np.zeros(17, np.uint8); dc_bits[2] = 1; dc_bits[3] = 5; dc_bits[4] = 1; dc_bits[5] = 1; dc_bits[6] = 1; dc_bits[7] = 1; dc_bits[8] = 1; dc_bits[9] = 1
     dc_vals = np.zeros(256, np.uint8); dc_vals[:12] = np.arange(12)
     outcomes = set()
