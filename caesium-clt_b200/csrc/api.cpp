@@ -6,6 +6,7 @@
 #include "../../include/b200_caesium_jpeg_trellis.h"
 #include "../../include/b200_caesium_gif.h"
 #include "../../include/b200_caesium_png_resize.h"
+#include "../../include/b200_caesium_webp_lossless.h"
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -29,6 +30,7 @@
 #include "png_host.h"
 #include "png_device.h"
 #include "png_quant.h"
+#include "png_webp.h"
 #include "vp8_host.h"
 #include "webp_device.h"
 #include "vp8l_device.h"
@@ -39,6 +41,7 @@
 #include "jpeg_pipe.h"
 #include "topology.h"
 #include "launch_timer.h"
+#include "stream_wait.h"
 
 using namespace b200;
 
@@ -74,6 +77,7 @@ std::atomic<int> g_entropy_mode{-1};     // -1 unset (env B200_ENTROPY); bit 0 =
 std::atomic<int> g_png_lossy{-1};        // -1 unset (env B200_PNG_LOSSY); 1 = lossy PNG on the device's quantiser, 0 = refused (code 3)
 std::atomic<int> g_gif{-1};              // -1 unset (env B200_GIF); 1 = GIF re-encoded on the device, 0 = refused (code 3)
 std::atomic<int> g_png_resize{-1};       // -1 unset (env B200_PNG_RESIZE); 1 = PNG -> PNG with width / height on the device, 0 = refused (code 3)
+std::atomic<int> g_webp_lossless_convert{-1};   // -1 unset (env B200_WEBP_LOSSLESS_CONVERT); 1 = JPEG / PNG -> lossless WebP on the device, 0 = refused (code 3)
 
 // runtime_init is idempotent while initialised, so after b200_shutdown (which frees every slot's device buffers) the next call
 // initialises again: a long-running host can hand the memory of one workload's slots back before starting another
@@ -114,6 +118,16 @@ bool png_resize()
         g_png_resize.store(e && !strcmp(e, "gpu") ? 1 : 0);
     }
     return g_png_resize.load() == 1;
+}
+
+// JPEG / PNG -> lossless WebP on the device: b200_set_webp_lossless_convert, else B200_WEBP_LOSSLESS_CONVERT=gpu, read once; off by default
+bool webp_lossless_convert()
+{
+    if (g_webp_lossless_convert.load() < 0) {
+        const char *e = getenv("B200_WEBP_LOSSLESS_CONVERT");
+        g_webp_lossless_convert.store(e && !strcmp(e, "gpu") ? 1 : 0);
+    }
+    return g_webp_lossless_convert.load() == 1;
 }
 
 // GIF sources on the device: b200_set_gif, else B200_GIF=gpu, read once; off by default
@@ -884,6 +898,121 @@ b200_status png_to_webp(const uint8_t *in, size_t in_len, const b200_params *p, 
     return rgb_to_webp(rgb, info.width, info.height, p, prefer_dev, out, has_alpha ? &alpha : nullptr);
 }
 
+// ---- conversion to lossless WebP (VP8L; the switch on) ----------------------------------------------------------------
+// libcaesium convert with webp.lossless: decode -> (resize) -> the lossless encoder.  The samples never leave the device: the JPEG
+// leg's planes and the PNG leg's un-filtered rows feed the encoder (vp8l_encode.cpp) where they lie.  B200_TRACE=2 prints one line
+// per call with the stages; to give each stage its own time the trace waits for the device after each of them.
+struct ConvertStages {
+    static bool verbose() { static const bool v = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2; return v; }
+    std::chrono::steady_clock::time_point t = std::chrono::steady_clock::now();
+    double ms[4] = {0, 0, 0, 0};            // parse + decode / inflate, device front end, resize, encode
+    void lap(int k, void *stream)
+    {
+        if (!verbose()) return;
+        if (stream) cudaStreamSynchronize((cudaStream_t)stream);
+        const auto n = std::chrono::steady_clock::now();
+        ms[k] += std::chrono::duration<double, std::milli>(n - t).count(); t = n;
+    }
+    void print(const char *src, uint32_t w, uint32_t h, uint32_t nw, uint32_t nh, const Vp8lDevice *v, const char *stage0) const
+    {
+        if (!verbose()) return;
+        fprintf(stderr, "[b200 trace] webp-lossless-convert %s %ux%u -> %ux%u: %s %.3f ms, front end %.3f ms, resize %.3f ms, encode %.3f ms (cache bits %d); "
+                        "fetched %zu bytes (encoder), sample planes fetched 0\n",
+                src, w, h, nw, nh, stage0, ms[0], ms[1], ms[2], ms[3], v->last_cache_bits, v->last_d2h_bytes);
+    }
+};
+
+// JPEG -> lossless WebP: the header checks, refusals and target size of jpeg_to_webp; the device-decoded RGB planes (K3 when
+// width / height are set) go to the encoder's plane entry.
+b200_status jpeg_to_webp_lossless(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
+{
+    std::string err;
+    ConvertStages tr;
+    JpegReader rd(in, in_len);
+    if (!rd.read_header(err)) return header_status(err);
+    const JpegGeom &gin = rd.geom();
+    if (fractional_sampling(gin)) return make_status(B200_ERR_UNSUPPORTED, kFractional);
+    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
+    uint32_t nw, nh;
+    b200_status st = target_size((uint32_t)gin.width, (uint32_t)gin.height, p, 16383, nw, nh, "invalid target dimensions for WebP");
+    if (st.code) return st;
+    SlotLease s(prefer_dev);
+    if (!s) return s.failure();
+    if (!s->ensure((size_t)gin.total_coefs * 2, 0, 0, 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    bool on_device;
+    if ((st = decode_into_slot(s, rd, on_device, err)).code) return st;
+    tr.lap(0, s->stream);
+    SamplePlan sp;
+    uint8_t *full[3], *rgb[3];
+    if (!(plan_samples(s, gin, (int)nw, (int)nh, nullptr, sp, err) && samples_from_coefs(s, gin, sp, !on_device, true, full, err))) return make_status(B200_ERR_CUDA, err);
+    tr.lap(1, s->stream);
+    if (!resize_samples(s, full, sp, rgb, err)) return make_status(B200_ERR_CUDA, err);
+    tr.lap(2, s->stream);
+    Vp8lDevice *v = s->vp8l_dev();
+    const int g = gin.ncomp == 3;          // a grey source is its one plane three times
+    if (!v->encode_planes(rgb[0], rgb[g], rgb[2 * g], nullptr, (int)nw, (int)nh, s->stream, out, err)) return make_status(B200_ERR_CUDA, err);
+    tr.lap(3, nullptr);
+    tr.print("jpeg", (uint32_t)gin.width, (uint32_t)gin.height, nw, nh, v, on_device ? "parse + device entropy decode" : "parse + host entropy decode");
+    return ok_status();
+}
+
+// PNG -> lossless WebP: parse and inflate into the slot's staging buffer as png_compress does, the device un-filter with its filter-
+// byte and Adler-32 checks (code 4), then the rows become the encoder's ARGB pixels (k_png_rows_argb).  With a resize the rows
+// become 8-bit planes (k_png_rows_planes; alpha only when the image is translucent), K3 resamples them and the plane entry packs them.
+b200_status png_to_webp_lossless(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
+{
+    std::string err;
+    ConvertStages tr;
+    PngInfo info; PngIdat idat;
+    if (!png_parse_chunks(in, in_len, false, info, idat, err)) return png_status(err);
+    uint32_t nw, nh;
+    const b200_status st = target_size(info.width, info.height, p, 16383, nw, nh, "invalid dimensions for WebP");
+    if (st.code) return st;
+    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
+    SlotLease s(prefer_dev);
+    if (!s) return s.failure();
+    PngDevice *png = s->png_dev();
+    Vp8lDevice *v = s->vp8l_dev();
+    const size_t nin = (info.row_bytes + 1) * (size_t)info.height;
+    size_t cap = 0, got = 0; uint32_t stored_adler = 0;
+    uint8_t *buf = png->input_buffer(nin, cap, err);
+    if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    if (!zlib_inflate_to(idat.p, idat.n, buf, cap, nin, &got, &stored_adler, err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
+    if (got < nin) return make_status(B200_ERR_CORRUPT_INPUT, "IDAT too short");
+    tr.lap(0, nullptr);
+    std::vector<uint8_t> none;
+    if (!png->from_filtered(info, got, stored_adler, 0, s->stream, none, nullptr, err, PngDevice::Tail::Samples, 0, 0)) return png_device_status(png, false, err);
+    const uint32_t w = info.width, h = info.height;
+    uint32_t *argb, *flags;
+    if (!v->reserve((int)nw, (int)nh, argb, flags, err)) return make_status(B200_ERR_CUDA, err);
+    if (nw == w && nh == h) {
+        if (!launch_ok(launch_png_rows_argb(png->d_raw, info, argb, flags, s->stream), "png rows", err)) return make_status(B200_ERR_CUDA, err);
+        tr.lap(1, s->stream);
+        if (!v->encode_packed((int)nw, (int)nh, s->stream, out, err)) return make_status(B200_ERR_CUDA, err);
+    } else {
+        const size_t n = (size_t)w * h, nn = (size_t)nw * nh;
+        const bool may_alpha = png_may_be_translucent(info);
+        if (!png->d_planes.reserve(4 * n + 64, Grow::Pow2Quarter, err) || !png->d_rplanes.reserve(4 * nn + 64, Grow::Pow2Quarter, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+        uint8_t *src[4], *dst[4];
+        for (int c = 0; c < 4; c++) { src[c] = png->d_planes + c * n; dst[c] = png->d_rplanes + c * nn; }
+        uint32_t *d_flag = png->d_hist, *h_flag = reinterpret_cast<uint32_t *>(png->h_small.get());
+        if (!launch_ok(launch_png_rows_planes(png->d_raw, info, src[0], src[1], src[2], may_alpha ? src[3] : nullptr, d_flag, s->stream), "png rows", err)) return make_status(B200_ERR_CUDA, err);
+        bool translucent = false;
+        if (may_alpha) {   // the alpha plane is resampled only when some pixel is translucent
+            const cudaError_t e = cudaMemcpyAsync(h_flag, d_flag, 4, cudaMemcpyDeviceToHost, (cudaStream_t)s->stream);
+            if (e != cudaSuccess || stream_wait((cudaStream_t)s->stream) != cudaSuccess) return make_status(B200_ERR_CUDA, "translucency flag fetch failed");
+            translucent = (*h_flag & 1u) != 0;
+        }
+        tr.lap(1, s->stream);
+        if (!png->resampler.run<uint8_t>(src, (int)w, (int)h, dst, (int)nw, (int)nh, translucent ? 4 : 3, s->stream, err)) return make_status(B200_ERR_CUDA, err);
+        tr.lap(2, s->stream);
+        if (!v->encode_planes(dst[0], dst[1], dst[2], translucent ? dst[3] : nullptr, (int)nw, (int)nh, s->stream, out, err)) return make_status(B200_ERR_CUDA, err);
+    }
+    tr.lap(3, nullptr);
+    tr.print("png", w, h, nw, nh, v, "parse + inflate");
+    return ok_status();
+}
+
 // Planar RGB on the host -> lossless PNG (K3 resize when asked, then the PNG leg's raw-sample entry point)
 b200_status rgb_to_png(const std::vector<uint8_t> &rgb, uint32_t w, uint32_t h, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out,
                        const std::vector<uint8_t> *alpha = nullptr)
@@ -924,7 +1053,11 @@ b200_status convert_dispatch(const uint8_t *in, size_t in_len, uint32_t src, uin
     }
     const bool to_webp = fmt == B200_FMT_WEBP, png_to_jpg = fmt == B200_FMT_JPEG && src == B200_FMT_PNG;
     if (!to_webp && !png_to_jpg) return make_status(B200_ERR_UNSUPPORTED, "this conversion is outside the GPU path (route to caesium::convert_in_memory)");
-    if (to_webp && p->webp_lossless) return make_status(B200_ERR_UNSUPPORTED, "lossless WebP (VP8L) is outside the GPU path (route to caesium::convert_in_memory)");
+    if (to_webp && p->webp_lossless) {
+        if (webp_lossless_convert() && src == B200_FMT_JPEG) return jpeg_to_webp_lossless(in, in_len, p, -1, out);
+        if (webp_lossless_convert() && src == B200_FMT_PNG) return png_to_webp_lossless(in, in_len, p, -1, out);
+        return make_status(B200_ERR_UNSUPPORTED, "lossless WebP (VP8L) is outside the GPU path (route to caesium::convert_in_memory)");
+    }
     if (png_to_jpg && p->jpeg_optimize) return make_status(B200_ERR_UNSUPPORTED, "lossless conversion to JPEG is outside the GPU path (route to caesium::convert_in_memory)");
     if (png_to_jpg) return png_to_jpeg(in, in_len, p, -1, out);
     if (src == B200_FMT_JPEG) return jpeg_to_webp(in, in_len, p, -1, out);
@@ -1067,6 +1200,7 @@ int b200_set_entropy_mode(int mode) { if (mode < 0 || mode > 3) return B200_ERR_
 int b200_set_png_lossy(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_png_lossy.store(on); return B200_OK; }
 int b200_set_gif(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_gif.store(on); return B200_OK; }
 int b200_set_png_resize(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_png_resize.store(on); return B200_OK; }
+int b200_set_webp_lossless_convert(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_webp_lossless_convert.store(on); return B200_OK; }
 int b200_set_jpeg_trellis(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; set_jpeg_trellis(on == 1); return B200_OK; }
 
 uint32_t b200_sniff_format(const uint8_t *d, size_t n)

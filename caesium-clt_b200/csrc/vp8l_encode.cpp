@@ -47,24 +47,48 @@ PrefixCode zero_code(int n) { PrefixCode pc; pc.len.assign(n, 0); pc.code.assign
 
 } // namespace
 
-bool Vp8lDevice::encode(const uint8_t *rgb, const uint8_t *alpha, int w, int h, void *stream_, std::vector<uint8_t> &out, std::string &err)
+bool Vp8lDevice::reserve(int w, int h, uint32_t *&argb, uint32_t *&flags, std::string &err)
 {
-    cudaStream_t st = (cudaStream_t)stream_;
     if (w < 1 || h < 1 || w > 16384 || h > 16384) { err = "VP8L dimensions out of range"; return false; }
     const size_t n = (size_t)w * h;
     const int nchunks = (int)((n + VP8L_CHUNK - 1) / VP8L_CHUNK);
-    const int tiles_x = (w + VP8L_TILE - 1) >> VP8L_TILE_BITS, tiles_y = (h + VP8L_TILE - 1) >> VP8L_TILE_BITS, tiles = tiles_x * tiles_y;
-    Vp8lBuffers B;
+    const int tiles = ((w + VP8L_TILE - 1) >> VP8L_TILE_BITS) * ((h + VP8L_TILE - 1) >> VP8L_TILE_BITS);
     const size_t arena = carve(nullptr, n, nchunks, tiles, B);
-    const size_t hist_bytes = sizeof(uint32_t) * VP8L_NCACHE * VP8L_HIST, small = hist_bytes + 16 + (size_t)tiles;
-    if (!grow(d_arena, arena, err) || !grow(h_in, 4 * n, err) || !grow(h_small, small, err) ||
-        !grow(h_codes, sizeof(Vp8lCodes), err)) return false;
+    const size_t small = sizeof(uint32_t) * VP8L_NCACHE * VP8L_HIST + 16 + (size_t)tiles;
+    if (!grow(d_arena, arena, err) || !grow(h_small, small, err) || !grow(h_codes, sizeof(Vp8lCodes), err)) return false;
     carve(d_arena, n, nchunks, tiles, B);
-    // ---- analysis: everything that decides the bitstream, for every cache candidate at once
+    argb = B.argb; flags = B.flags;
+    return true;
+}
+
+bool Vp8lDevice::encode(const uint8_t *rgb, const uint8_t *alpha, int w, int h, void *stream_, std::vector<uint8_t> &out, std::string &err)
+{
+    cudaStream_t st = (cudaStream_t)stream_;
+    uint32_t *argb, *flags;
+    if (!reserve(w, h, argb, flags, err)) return false;
+    const size_t n = (size_t)w * h;
+    if (!grow(h_in, 4 * n, err)) return false;
     memcpy(h_in, rgb, 3 * n);
     if (alpha) memcpy(h_in + 3 * n, alpha, n);
     CU(cudaMemcpyAsync(B.planes, h_in, (alpha ? 4 : 3) * n, cudaMemcpyHostToDevice, st));
-    int rc = launch_vp8l_analyse(B, w, h, alpha ? 1 : 0, st);
+    return encode_planes(B.planes, B.planes + n, B.planes + 2 * n, alpha ? B.planes + 3 * n : nullptr, w, h, stream_, out, err);
+}
+
+bool Vp8lDevice::encode_planes(const uint8_t *r, const uint8_t *g, const uint8_t *b, const uint8_t *a, int w, int h, void *stream, std::vector<uint8_t> &out, std::string &err)
+{
+    uint32_t *argb, *flags;
+    if (!reserve(w, h, argb, flags, err)) return false;
+    if (!launch_ok(launch_vp8l_pack(r, g, b, a, B, w, h, stream), "vp8l kernels", err)) return false;
+    return encode_packed(w, h, stream, out, err);
+}
+
+// ---- analysis: everything that decides the bitstream, for every cache candidate at once
+bool Vp8lDevice::encode_packed(int w, int h, void *stream_, std::vector<uint8_t> &out, std::string &err)
+{
+    cudaStream_t st = (cudaStream_t)stream_;
+    const int tiles_x = (w + VP8L_TILE - 1) >> VP8L_TILE_BITS, tiles_y = (h + VP8L_TILE - 1) >> VP8L_TILE_BITS, tiles = tiles_x * tiles_y;
+    const size_t hist_bytes = sizeof(uint32_t) * VP8L_NCACHE * VP8L_HIST;
+    int rc = launch_vp8l_analyse(B, w, h, st);
     if (!launch_ok(rc, "vp8l kernels", err)) return false;
     uint32_t *h_hist = (uint32_t *)h_small.get(), *h_flags = (uint32_t *)(h_small + hist_bytes);
     unsigned long long *h_total = (unsigned long long *)(h_small + hist_bytes + 8);
@@ -121,6 +145,7 @@ bool Vp8lDevice::encode(const uint8_t *rgb, const uint8_t *alpha, int w, int h, 
     const size_t words = (size_t)((total + 31) / 32), nbytes = (size_t)((total + 7) / 8);
     if (!grow(d_words, words * 4, err) || !grow(h_words, words * 4, err)) return false;
     B.words = d_words;
+    last_d2h_bytes = hist_bytes + 4 + (size_t)tiles + 8 + words * 4;
     rc = launch_vp8l_emit(B, w, h, cand, words, st);
     if (!launch_ok(rc, "vp8l kernels", err)) return false;
     CU(cudaMemcpyAsync(h_words, d_words, words * 4, cudaMemcpyDeviceToHost, st));

@@ -1,6 +1,6 @@
 // vp8l_kernels.cu -- the per-pixel work of the lossless WebP (VP8L) encoder; the rules are vp8l_enc_core.h's, the host side is
 // vp8l_encode.cpp.
-//   k_vp8l_pack         planar R, G, B (+ alpha) -> ARGB with subtract-green applied; flags an alpha value below 255
+//   k_vp8l_pack         R, G, B (+ alpha) planes anywhere on the device -> ARGB with subtract-green applied; flags an alpha below 255
 //   k_vp8l_predict      CTA per 16x16 tile: the 14 modes scored in shared-memory histograms -> mode image, residual image
 //   k_vp8l_cache_last   CTA per (parse chunk, cache candidate): last position of every cache key inside the chunk
 //   k_vp8l_cache_carry  thread per (key, candidate): the last position before each chunk (a running scan over the chunks)
@@ -25,12 +25,14 @@ constexpr int V_THREADS = 256, V_PER = VP8L_CHUNK / V_THREADS, V_WORDS = VP8L_CH
 __host__ __device__ __forceinline__ int cache_table_offset(int cand) { return cand <= 1 ? 0 : cand == 2 ? 64 : 320; }   // keys of candidates 1..3: 64, 256, 1024
 constexpr int CACHE_TABLE_KEYS = 64 + 256 + 1024;
 
-__global__ void __launch_bounds__(V_THREADS) k_vp8l_pack(const uint8_t *__restrict__ planes, int has_alpha, uint32_t n, uint32_t *__restrict__ argb, uint32_t *__restrict__ flags)
+// a: nullptr for an opaque image; a grey source passes one plane as r, g and b
+__global__ void __launch_bounds__(V_THREADS) k_vp8l_pack(const uint8_t *__restrict__ r_, const uint8_t *__restrict__ g_, const uint8_t *__restrict__ b_,
+                                                          const uint8_t *__restrict__ a_, uint32_t n, uint32_t *__restrict__ argb, uint32_t *__restrict__ flags)
 {
     const uint32_t i = blockIdx.x * V_THREADS + threadIdx.x;
     bool translucent = false;
     if (i < n) {
-        const uint32_t r = planes[i], g = planes[(size_t)n + i], b = planes[2 * (size_t)n + i], a = has_alpha ? planes[3 * (size_t)n + i] : 255u;
+        const uint32_t r = r_[i], g = g_[i], b = b_[i], a = a_ ? a_[i] : 255u;
         translucent = a != 255u;
         argb[i] = vp8l_sub_green((a << 24) | (r << 16) | (g << 8) | b);
     }
@@ -357,14 +359,21 @@ __global__ void __launch_bounds__(V_THREADS) k_vp8l_emit(const uint2 *__restrict
 
 static inline unsigned cdiv(size_t a, size_t b) { return (unsigned)((a + b - 1) / b); }
 
-int launch_vp8l_analyse(const Vp8lBuffers &B, int w, int h, int has_alpha, void *stream_)
+int launch_vp8l_pack(const uint8_t *r, const uint8_t *g, const uint8_t *b, const uint8_t *a, const Vp8lBuffers &B, int w, int h, void *stream_)
+{
+    cudaStream_t st = (cudaStream_t)stream_;
+    const uint32_t n = (uint32_t)w * (uint32_t)h;
+    cudaMemsetAsync(B.flags, 0, 4, st); LT_MARK("upload+memset");
+    k_vp8l_pack<<<cdiv(n, V_THREADS), V_THREADS, 0, st>>>(r, g, b, a, n, B.argb, B.flags); LT_MARK("k_vp8l_pack");
+    return (int)cudaGetLastError();
+}
+
+int launch_vp8l_analyse(const Vp8lBuffers &B, int w, int h, void *stream_)
 {
     cudaStream_t st = (cudaStream_t)stream_;
     const uint32_t n = (uint32_t)w * (uint32_t)h;
     const int nchunks = (int)cdiv(n, VP8L_CHUNK), tiles_x = (w + VP8L_TILE - 1) >> VP8L_TILE_BITS, tiles = tiles_x * ((h + VP8L_TILE - 1) >> VP8L_TILE_BITS);
-    cudaMemsetAsync(B.flags, 0, 4, st);
-    cudaMemsetAsync(B.hist, 0, sizeof(uint32_t) * VP8L_NCACHE * VP8L_HIST, st); LT_MARK("upload+memset");
-    k_vp8l_pack<<<cdiv(n, V_THREADS), V_THREADS, 0, st>>>(B.planes, has_alpha, n, B.argb, B.flags); LT_MARK("k_vp8l_pack");
+    cudaMemsetAsync(B.hist, 0, sizeof(uint32_t) * VP8L_NCACHE * VP8L_HIST, st); LT_MARK("memset");
     k_vp8l_predict<<<tiles, V_THREADS, 0, st>>>(B.argb, w, h, tiles_x, B.res, B.modes); LT_MARK("k_vp8l_predict");
     k_vp8l_cache_last<<<dim3(nchunks, VP8L_NCACHE - 1), V_THREADS, 0, st>>>(B.res, n, nchunks, B.cache_tab); LT_MARK("k_vp8l_cache_last");
     k_vp8l_cache_carry<<<dim3(cdiv(1 << VP8L_MAX_CACHE_BITS, V_THREADS), VP8L_NCACHE - 1), V_THREADS, 0, st>>>(nchunks, B.cache_tab); LT_MARK("k_vp8l_cache_carry");

@@ -11,7 +11,7 @@ namespace b200 {
 struct Vp8lCodes { uint16_t code[VP8L_HIST]; uint8_t len[VP8L_HIST]; };
 
 struct Vp8lBuffers {
-    uint8_t *planes;                    // R | G | B | A planes of n bytes each
+    uint8_t *planes;                    // R | G | B | A planes of n bytes each: the host entry's upload
     uint32_t *argb, *res, *best;        // n each: subtract-green pixels, residuals, best copy per pixel
     uint8_t *modes;                     // one per 16x16 tile
     int *cache_tab;                     // vp8l_cache_table_ints(nchunks)
@@ -26,8 +26,10 @@ struct Vp8lBuffers {
 };
 
 size_t vp8l_cache_table_ints(int nchunks);
-// pack, predictor choice, colour-cache hits, match search, parse and the histograms of every cache candidate
-int launch_vp8l_analyse(const Vp8lBuffers &B, int w, int h, int has_alpha, void *stream);
+// R, G, B planes (+ alpha; nullptr: opaque) of w x h bytes anywhere on the device -> B.argb (subtract-green) and B.flags
+int launch_vp8l_pack(const uint8_t *r, const uint8_t *g, const uint8_t *b, const uint8_t *a, const Vp8lBuffers &B, int w, int h, void *stream);
+// predictor choice, colour-cache hits, match search, parse and the histograms of every cache candidate over B.argb
+int launch_vp8l_analyse(const Vp8lBuffers &B, int w, int h, void *stream);
 // bit offsets of every chunk's and thread's tokens under B.codes for cache candidate `cand`; *B.total = bit_base + their bits
 int launch_vp8l_size(const Vp8lBuffers &B, int w, int h, int cand, unsigned long long bit_base, void *stream);
 // the tokens into B.words (words of them are zeroed first)
