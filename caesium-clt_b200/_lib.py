@@ -68,7 +68,7 @@ _SYMBOLS = [
     "b200_webp_encode_rgb", "b200_webp_write_levels", "b200_webp_qindex",
     "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_jpeg_pipe_destroy", "b200_device_jobs", "b200_device_numa_node", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba", "b200_webp_alpha_filter", "b200_webp_d2h_bytes",
     "b200_set_png_lossy", "b200_png_quantize", "b200_set_jpeg_trellis", "b200_set_gif", "b200_gif_decode", "b200_gif_lzw",
-    "b200_set_png_resize", "b200_png_resize_samples", "b200_set_webp_lossless_convert",
+    "b200_set_png_resize", "b200_png_resize_samples", "b200_set_webp_lossless_convert", "b200_set_png_interlaced",
 ]
 
 
@@ -244,6 +244,12 @@ def set_webp_lossless_convert(on):
     """b200_set_webp_lossless_convert: convert_in_memory to WebP with webp_lossless on JPEG and PNG sources runs on the device (1) or
     is refused with code 3 (0, the default).  Any other value is refused with B200_ERR_INVALID_ARGUMENT."""
     return lib().b200_set_webp_lossless_convert(int(on))
+
+
+def set_png_interlaced(on):
+    """b200_set_png_interlaced: Adam7-interlaced PNG sources are accepted by every PNG leg (1) or refused with code 3 (0, the default).
+    Any other value is refused with B200_ERR_INVALID_ARGUMENT."""
+    return lib().b200_set_png_interlaced(int(on))
 
 
 def set_jpeg_trellis(on):

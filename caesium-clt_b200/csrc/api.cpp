@@ -7,6 +7,7 @@
 #include "../../include/b200_caesium_gif.h"
 #include "../../include/b200_caesium_png_resize.h"
 #include "../../include/b200_caesium_webp_lossless.h"
+#include "../../include/b200_caesium_png_interlaced.h"
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -78,6 +79,7 @@ std::atomic<int> g_png_lossy{-1};        // -1 unset (env B200_PNG_LOSSY); 1 = l
 std::atomic<int> g_gif{-1};              // -1 unset (env B200_GIF); 1 = GIF re-encoded on the device, 0 = refused (code 3)
 std::atomic<int> g_png_resize{-1};       // -1 unset (env B200_PNG_RESIZE); 1 = PNG -> PNG with width / height on the device, 0 = refused (code 3)
 std::atomic<int> g_webp_lossless_convert{-1};   // -1 unset (env B200_WEBP_LOSSLESS_CONVERT); 1 = JPEG / PNG -> lossless WebP on the device, 0 = refused (code 3)
+std::atomic<int> g_png_interlaced{-1};   // -1 unset (env B200_PNG_INTERLACED); 1 = Adam7 PNG sources accepted, 0 = refused (code 3)
 
 // runtime_init is idempotent while initialised, so after b200_shutdown (which frees every slot's device buffers) the next call
 // initialises again: a long-running host can hand the memory of one workload's slots back before starting another
@@ -129,6 +131,21 @@ bool webp_lossless_convert()
     }
     return g_webp_lossless_convert.load() == 1;
 }
+
+} // namespace
+
+// Adam7 PNG sources on every PNG leg: b200_set_png_interlaced, else B200_PNG_INTERLACED=gpu, read once; off by default.  Asked by
+// png_parse_chunks (png_host.cpp), which every PNG leg goes through.
+bool b200::png_interlaced()
+{
+    if (g_png_interlaced.load() < 0) {
+        const char *e = getenv("B200_PNG_INTERLACED");
+        g_png_interlaced.store(e && !strcmp(e, "gpu") ? 1 : 0);
+    }
+    return g_png_interlaced.load() == 1;
+}
+
+namespace {
 
 // GIF sources on the device: b200_set_gif, else B200_GIF=gpu, read once; off by default
 bool gif_on()
@@ -473,7 +490,7 @@ b200_status png_compress(const uint8_t *in, size_t in_len, const b200_params *p,
         PngDevice *png = s->png_dev();
         // the IDAT stream is inflated straight into the slot's pinned staging buffer; from there on everything is device work
         // (un-filter, checksum, reductions, filter trials, LZ77, DEFLATE coding) until the finished zlib stream comes back
-        const size_t nin = (info.row_bytes + 1) * (size_t)info.height;
+        const size_t nin = png_inflated_size(info);
         size_t cap = 0, got = 0; uint32_t stored_adler = 0;
         uint8_t *buf = png->input_buffer(nin, cap, err);
         if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
@@ -495,7 +512,8 @@ b200_status png_compress(const uint8_t *in, size_t in_len, const b200_params *p,
         fprintf(stderr, "[b200 trace] png %ux%u: parse + inflate %.1f ms, device (un-filter, filter trials, LZ77, DEFLATE coding; host Huffman %.1f) %.1f ms, container %.1f ms\n",
                 info.width, info.height, ms(t0, t1), deflate_ms, ms(t1, t3), ms(t3, std::chrono::steady_clock::now()));
         auto at = [&](const char *k) { auto it = ev.find(k); return it == ev.end() ? 0.0 : it->second.first; };
-        const double up = at("h2d") + at("png_unfilter"), rz = at("png_resize");
+        const double up = at("h2d") + at("k_png_adler") + at("k_png_unfilter") + at("k_png_adam7_unfilter") + at("k_png_adam7_gather") + at("png_unfilter"),
+                     rz = at("png_resize");
         fprintf(stderr, "[b200 trace] png stages %ux%u -> %ux%u: parse + inflate %.3f ms, h2d + un-filter %.3f ms, expand + K3 + pack %.3f ms, back end %.3f ms\n",
                 sw, sh, info.width, info.height, ms(t0, t1), up, rz, ms(t1, t3) - up - rz);
     }
@@ -549,7 +567,7 @@ b200_status png_lossy_load(Slot *s, PngInfo &info, const PngIdat &idat, uint32_t
     const bool grey = info.color_type == 0 || info.color_type == 4;
     drop_colour_chunks(info.kept_before_idat, grey); drop_colour_chunks(info.kept_after_idat, grey);
     PngDevice *png = s->png_dev();
-    const size_t nin = (info.row_bytes + 1) * (size_t)info.height;
+    const size_t nin = png_inflated_size(info);
     size_t cap = 0, got = 0; uint32_t stored_adler = 0;
     uint8_t *buf = png->input_buffer(nin, cap, err);
     if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
@@ -973,7 +991,7 @@ b200_status png_to_webp_lossless(const uint8_t *in, size_t in_len, const b200_pa
     if (!s) return s.failure();
     PngDevice *png = s->png_dev();
     Vp8lDevice *v = s->vp8l_dev();
-    const size_t nin = (info.row_bytes + 1) * (size_t)info.height;
+    const size_t nin = png_inflated_size(info);
     size_t cap = 0, got = 0; uint32_t stored_adler = 0;
     uint8_t *buf = png->input_buffer(nin, cap, err);
     if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
@@ -1201,6 +1219,7 @@ int b200_set_png_lossy(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_A
 int b200_set_gif(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_gif.store(on); return B200_OK; }
 int b200_set_png_resize(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_png_resize.store(on); return B200_OK; }
 int b200_set_webp_lossless_convert(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_webp_lossless_convert.store(on); return B200_OK; }
+int b200_set_png_interlaced(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_png_interlaced.store(on); return B200_OK; }
 int b200_set_jpeg_trellis(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; set_jpeg_trellis(on == 1); return B200_OK; }
 
 uint32_t b200_sniff_format(const uint8_t *d, size_t n)
@@ -1774,7 +1793,7 @@ b200_status b200_png_device_times(const uint8_t *in, size_t in_len, int level, i
         SlotLease s(-1);
         if (!s) return s.failure();
         PngDevice *png = s->png_dev();
-        const size_t nin = (info0.row_bytes + 1) * (size_t)info0.height;
+        const size_t nin = png_inflated_size(info0);
         size_t bcap = 0, got = 0; uint32_t adler = 0;
         uint8_t *buf = png->input_buffer(nin, bcap, err);
         if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
@@ -1832,7 +1851,7 @@ b200_status b200_png_resize_samples(const uint8_t *in, size_t in_len, uint32_t w
         SlotLease s(-1);
         if (!s) return s.failure();
         PngDevice *png = s->png_dev();
-        const size_t nin = (pi.row_bytes + 1) * (size_t)pi.height;
+        const size_t nin = png_inflated_size(pi);
         size_t cap = 0, got = 0; uint32_t stored_adler = 0;
         uint8_t *buf = png->input_buffer(nin, cap, err);
         if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);

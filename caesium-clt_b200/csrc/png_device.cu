@@ -185,10 +185,20 @@ bool PngDevice::from_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler
     cudaStream_t st = (cudaStream_t)stream_;
     corrupt = false;
     const int h = (int)info.height; const size_t rb = info.row_bytes; const int bpp = info.bpp;
-    const size_t nraw = (size_t)h * rb, nin = (size_t)h * (rb + 1);
+    // Adam7: the seven passes are un-filtered into d_raw2 (pass-packed) and gathered into d_raw; from there on the image is the
+    // non-interlaced one and every tail sees full-image rows
+    const bool adam7 = info.interlace == 1;
+    const uint32_t w = info.width; const int bits = info.bits_per_pixel;      // the source's (a resize rewrites info below)
+    Adam7Layout L;
+    if (adam7) adam7_layout(w, info.height, bits, L);
+    info.interlace = 0;
+    const size_t nraw = (size_t)h * rb, nin = adam7 ? L.filt_bytes : (size_t)h * (rb + 1);
     if (nfilt < nin) { err = "IDAT too short"; corrupt = true; return false; }
+    size_t ngroups = ((size_t)h + 31) / 32;
+    if (adam7) { ngroups = 0; for (const Adam7Pass &P : L.pass) ngroups += (P.h + 31) / 32; }
     const size_t nmax = nin + 64;
     if (!ensure_buffers(nraw, nmax, rb, st, err) || !grow(d_fin, nmax + 64, err)) return false;
+    if (adam7 && (!grow(d_raw2, L.raw_bytes + 64, err) || !grow(d_sync, (ngroups + 16) * 4 + 2048 * 4 + 64, err))) return false;
     const bool resize = nw && nh;
     const PngInfo src = resize ? info : PngInfo();
     if (resize) {   // every buffer of the back end for the larger of the two images
@@ -198,8 +208,9 @@ bool PngDevice::from_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler
     CU(cudaMemcpyAsync(d_fin, h_raw, nin, cudaMemcpyHostToDevice, st)); LT_MARK("h2d");
     int rc = launch_png_adler(d_fin, nin, d_sums_in, st);
     uint32_t *d_un = d_sync, *d_flags = d_hist;
-    uint32_t *d_set = reinterpret_cast<uint32_t *>(((uintptr_t)(d_sync + ((size_t)(h + 31) / 32 + 8)) + 7) & ~(uintptr_t)7);
-    if (!rc) rc = launch_png_unfilter(d_fin, d_raw, h, (int)rb, bpp, d_un, st);
+    uint32_t *d_set = reinterpret_cast<uint32_t *>(((uintptr_t)(d_sync + (ngroups + 8)) + 7) & ~(uintptr_t)7);
+    if (!rc) rc = adam7 ? launch_png_adam7_unfilter(d_fin, d_raw2, d_raw, L, w, (uint32_t)h, bits, bpp, d_un, st)
+                        : launch_png_unfilter(d_fin, d_raw, h, (int)rb, bpp, d_un, st);
     if (!launch_ok(rc, "png unfilter", err)) return false;
     LT_MARK("png_unfilter");
     if (resize && !resize_raw(src, info, st, err)) return false;

@@ -3,6 +3,7 @@
 // the chunks StripChunks::Safe keeps, and wrap the re-compressed image data.
 #include "png_host.h"
 #include "dfl_core.h"
+#include "png_adam7_core.h"
 #include <emmintrin.h>
 #include <immintrin.h>
 #include <algorithm>
@@ -453,36 +454,41 @@ bool png_parse_chunks(const uint8_t *d, size_t n, bool keep_all, PngInfo &info, 
         i += 12 + L;
     }
     if (!have_ihdr || !seen_idat || !seen_end) { err = "incomplete PNG"; return false; }
-    if (info.interlace) { err = "interlaced PNG is not supported on the GPU path"; return false; }
-    const size_t stride = info.row_bytes + 1;
-    if (stride > ((size_t)1 << 40) / info.height) { err = "PNG dimensions too large"; return false; }      // 1 TiB of samples: no overflow below
+    if (info.interlace > 1 || (info.interlace == 1 && !png_interlaced())) { err = "interlaced PNG is not supported on the GPU path"; return false; }
+    // 1 TiB of samples: no overflow below.  The first test keeps png_inflated_size from overflowing; an Adam7 stream is larger (up to
+    // about 15 h / 8 filter bytes and a padded last byte per pass row), so it is bounded on its own.
+    const size_t stride = info.row_bytes + 1, most = (size_t)1 << 40;
+    if (stride > most / info.height || png_inflated_size(info) > most) { err = "PNG dimensions too large"; return false; }
     if (nidat == 1) { idat_out.p = first_idat; idat_out.n = first_len; } else { idat_out.p = idat.data(); idat_out.n = idat.size(); }
     return true;
+}
+
+size_t png_inflated_size(const PngInfo &info)
+{
+    if (info.interlace != 1) return (info.row_bytes + 1) * (size_t)info.height;
+    Adam7Layout L;
+    adam7_layout(info.width, info.height, info.bits_per_pixel, L);
+    return L.filt_bytes;
 }
 
 bool png_parse_inflate(const uint8_t *d, size_t n, bool keep_all, PngInfo &info, std::vector<uint8_t> &filt, std::string &err)
 {
     PngIdat idat;
     if (!png_parse_chunks(d, n, keep_all, info, idat, err)) return false;
-    const size_t stride = info.row_bytes + 1;
-    if (!zlib_inflate(idat.p, idat.n, filt, stride * info.height, err)) return false;
-    if (filt.size() < stride * info.height) { err = "IDAT too short"; return false; }
+    const size_t nin = png_inflated_size(info);
+    if (!zlib_inflate(idat.p, idat.n, filt, nin, err)) return false;
+    if (filt.size() < nin) { err = "IDAT too short"; return false; }
     return true;
 }
 
-bool png_decode(const uint8_t *d, size_t n, bool keep_all, PngInfo &info, std::vector<uint8_t> &raw, std::string &err)
+// PNG 9.2 reconstruction of h rows of rb bytes: filt holds each row's filter byte and filtered bytes, raw receives the rows.  Both
+// have 16 bytes of slack after them (the 4-byte-wide Paeth path reads and stores past a 3-byte pixel); zero_row has rb + 16 zeros.
+static bool unfilter_rows(const uint8_t *filt, uint8_t *raw, size_t h, size_t rb, size_t bpp, const uint8_t *zero_row, std::string &err)
 {
-    std::vector<uint8_t> filt;
-    if (!png_parse_inflate(d, n, keep_all, info, filt, err)) return false;
-    const size_t stride = info.row_bytes + 1;
-    const size_t nraw = info.row_bytes * info.height;
-    raw.resize(nraw + 16);                          // slack: the 4-byte-wide Paeth path stores one byte past a 3-byte pixel
-    filt.resize(filt.size() + 16);
-    const size_t bpp = (size_t)info.bpp, rb = info.row_bytes;
-    const std::vector<uint8_t> zero_row(rb + 16, 0);
-    for (uint32_t y = 0; y < info.height; y++) {   // PNG 9.2 reconstruction
-        const uint8_t *f = filt.data() + (size_t)y * stride; const int ft = f[0]; f++;
-        uint8_t *r = raw.data() + (size_t)y * rb; const uint8_t *up = y ? r - rb : zero_row.data();
+    const size_t stride = rb + 1;
+    for (size_t y = 0; y < h; y++) {
+        const uint8_t *f = filt + y * stride; const int ft = f[0]; f++;
+        uint8_t *r = raw + y * rb; const uint8_t *up = y ? r - rb : zero_row;
         switch (ft) {
             case 0: memcpy(r, f, rb); break;
             case 1:
@@ -504,7 +510,32 @@ bool png_decode(const uint8_t *d, size_t n, bool keep_all, PngInfo &info, std::v
             default: err = "bad filter type"; return false;
         }
     }
+    return true;
+}
+
+bool png_decode(const uint8_t *d, size_t n, bool keep_all, PngInfo &info, std::vector<uint8_t> &raw, std::string &err)
+{
+    std::vector<uint8_t> filt;
+    if (!png_parse_inflate(d, n, keep_all, info, filt, err)) return false;
+    const size_t nraw = info.row_bytes * info.height, bpp = (size_t)info.bpp, rb = info.row_bytes;
+    filt.resize(filt.size() + 16);
+    const std::vector<uint8_t> zero_row(rb + 16, 0);
+    if (info.interlace != 1) {
+        raw.resize(nraw + 16);
+        if (!unfilter_rows(filt.data(), raw.data(), info.height, rb, bpp, zero_row.data(), err)) return false;
+        raw.resize(nraw);
+        return true;
+    }
+    // Adam7: each pass is un-filtered as an image of its own into a pass-packed buffer, then the full rows are gathered from it
+    Adam7Layout L;
+    adam7_layout(info.width, info.height, info.bits_per_pixel, L);
+    std::vector<uint8_t> packed(L.raw_bytes + 16);
+    for (const Adam7Pass &P : L.pass)
+        if (P.h && !unfilter_rows(filt.data() + P.filt_off, packed.data() + P.raw_off, P.h, P.rb, bpp, zero_row.data(), err)) return false;
     raw.resize(nraw);
+    for (uint32_t y = 0; y < info.height; y++)
+        for (size_t i = 0; i < rb; i++) raw[(size_t)y * rb + i] = adam7_gather_byte(packed.data(), L, info.bits_per_pixel, info.width, y, i);
+    info.interlace = 0;
     return true;
 }
 

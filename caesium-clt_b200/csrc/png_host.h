@@ -19,13 +19,22 @@ struct PngInfo {
     std::vector<uint8_t> kept_before_idat, kept_after_idat;   // ancillary chunks carried over, serialised (len|type|data|crc)
 };
 
+// Whether Adam7-interlaced files are accepted (b200_set_png_interlaced, else B200_PNG_INTERLACED=gpu; off by default).  The switch
+// belongs to the C ABI (api.cpp); png_parse_chunks asks it, so every leg that parses a PNG follows it.
+bool png_interlaced();
+
 // Container parse only (chunk CRCs checked, IHDR validated, PLTE / tRNS / kept chunks collected): where the zlib stream lies.
+// Interlace method 1 (Adam7) is refused with "interlaced PNG is not supported on the GPU path" unless png_interlaced(); any other
+// non-zero method always is.
 struct PngIdat { const uint8_t *p = nullptr; size_t n = 0; std::vector<uint8_t> joined; };      // p points into the file (one IDAT) or into joined
 bool png_parse_chunks(const uint8_t *data, size_t len, bool keep_all_metadata, PngInfo &info, PngIdat &idat, std::string &err);
-// Container parse + inflate only: filt = height * (row_bytes + 1) bytes, every row led by its filter-type byte (the lossless path
-// un-filters on the device, png_kernels.cu k_png_unfilter).
+// Bytes of the inflated image data: height * (row_bytes + 1), or for an Adam7 file the rows of its seven passes (png_adam7_core.h).
+size_t png_inflated_size(const PngInfo &info);
+// Container parse + inflate only: filt = png_inflated_size(info) bytes, every row led by its filter-type byte (the lossless path
+// un-filters on the device, png_kernels.cu k_png_unfilter / k_png_adam7_unfilter).
 bool png_parse_inflate(const uint8_t *data, size_t len, bool keep_all_metadata, PngInfo &info, std::vector<uint8_t> &filt, std::string &err);
-// Parse + inflate + unfilter.  raw = height * row_bytes bytes of packed samples (no filter bytes).
+// Parse + inflate + unfilter (+ de-interlace).  raw = height * row_bytes bytes of packed samples (no filter bytes); info.interlace
+// is 0 afterwards.
 bool png_decode(const uint8_t *data, size_t len, bool keep_all_metadata, PngInfo &info, std::vector<uint8_t> &raw, std::string &err);
 
 // oxipng reduction::palette (lossless): an 8-bit RGB / RGBA image with at most 256 distinct pixel values becomes an 8-bit

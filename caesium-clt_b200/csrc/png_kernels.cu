@@ -7,6 +7,7 @@
 // (pixel-multiple distances and the row above); parsing is sequential inside 4 KiB chunks, parallel across them.
 // All integer/byte work, HBM-bound; no tensor cores.
 #include <cuda_runtime.h>
+#include <algorithm>
 #include <cub/block/block_radix_sort.cuh>
 #include <cmath>
 #include <cstdint>
@@ -526,15 +527,13 @@ __global__ void k_png_repack(const uint8_t *__restrict__ raw, uint8_t *__restric
 // x and pixel x - 1) are that lane's results of the previous two steps and arrive by shuffle.  Lane 0's "row above" is the last
 // row of the previous group, read back from HBM behind that group's progress counter; groups are handed out by an atomic ticket,
 // so a waiting warp only ever waits for a warp that is already running (the K8 pattern).  BPP = filter distance in bytes (1..8).
+// One group g of an image of h rows of rb bytes; progress[g - 1] is the previous group's counter.
 template <int BPP>
-__global__ void __launch_bounds__(32) k_png_unfilter(const uint8_t *__restrict__ filt, uint8_t *raw, int h, int rb, uint32_t *__restrict__ ticket,
-                                                     volatile uint32_t *__restrict__ progress, uint32_t *__restrict__ bad)
+__device__ __forceinline__ void unfilter_group(const uint8_t *__restrict__ filt, uint8_t *raw, int h, int rb, int g, volatile uint32_t *__restrict__ progress,
+                                               uint32_t *__restrict__ bad)
 {
     __shared__ uint8_t sh_up[2][32 * BPP];               // the row above lane 0, 32 pixels at a time, double buffered
     const int lane = threadIdx.x;
-    int g = 0;
-    if (lane == 0) g = (int)atomicAdd(ticket, 1u);
-    g = __shfl_sync(0xFFFFFFFFu, g, 0);
     const int y = g * 32 + lane;
     const bool live = y < h;
     const int npix = (rb + BPP - 1) / BPP;
@@ -586,6 +585,47 @@ __global__ void __launch_bounds__(32) k_png_unfilter(const uint8_t *__restrict__
         // the last lane publishes its progress for the next group, 32 pixels at a time
         if (lane == 31 && on && ((x & 31) == 31 || x == npix - 1)) { __threadfence(); progress[g] = (uint32_t)(x + 1); }
     }
+}
+
+template <int BPP>
+__global__ void __launch_bounds__(32) k_png_unfilter(const uint8_t *__restrict__ filt, uint8_t *raw, int h, int rb, uint32_t *__restrict__ ticket,
+                                                     volatile uint32_t *__restrict__ progress, uint32_t *__restrict__ bad)
+{
+    int g = 0;
+    if (threadIdx.x == 0) g = (int)atomicAdd(ticket, 1u);
+    g = __shfl_sync(0xFFFFFFFFu, g, 0);
+    unfilter_group<BPP>(filt, raw, h, rb, g, progress, bad);
+}
+
+// ---- Adam7: the seven passes in one wavefront launch ---------------------------------------------------------------------------
+// Each pass is a PNG image of its own.  Groups take their tickets across all passes (pass p owns tickets first[p] .. first[p + 1] - 1);
+// a pass's group 0 has no row above, and a group waits only for its predecessor in the same pass, which holds a lower ticket -- so,
+// as in k_png_unfilter, a waiting warp only ever waits for one already running.  The passes run side by side: the launch takes about
+// as long as the tallest pass's wavefront, not the sum of the seven.
+struct Adam7Groups {
+    int h[7], rb[7];
+    unsigned long long filt_off[7], raw_off[7];
+    int first[8];
+};
+
+template <int BPP>
+__global__ void __launch_bounds__(32) k_png_adam7_unfilter(const uint8_t *__restrict__ filt, uint8_t *packed, const Adam7Groups d, uint32_t *__restrict__ ticket,
+                                                           volatile uint32_t *__restrict__ progress, uint32_t *__restrict__ bad)
+{
+    int g = 0;
+    if (threadIdx.x == 0) g = (int)atomicAdd(ticket, 1u);
+    g = __shfl_sync(0xFFFFFFFFu, g, 0);
+    int p = 0;
+    while (p < 6 && g >= d.first[p + 1]) p++;          // empty passes own no tickets and are stepped over
+    unfilter_group<BPP>(filt + d.filt_off[p], packed + d.raw_off[p], d.h[p], d.rb[p], g - d.first[p], progress + d.first[p], bad);
+}
+
+// the full image's rows from the pass-packed rows: one thread per output byte (so no two threads write one byte); blockIdx.y strides rows
+__global__ void k_png_adam7_gather(const uint8_t *__restrict__ packed, uint8_t *__restrict__ raw, const Adam7Layout L, int bits, uint32_t w, uint32_t h, uint32_t rb)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= rb) return;
+    for (uint32_t y = blockIdx.y; y < h; y += gridDim.y) raw[(size_t)y * rb + i] = adam7_gather_byte(packed, L, bits, w, y, i);
 }
 
 // ---- palette probe: does the image have at most 256 distinct pixel values?  (8-bit RGB / RGBA; oxipng reduction::palette) -----------
@@ -688,6 +728,35 @@ int launch_png_unfilter(const uint8_t *d_filt, uint8_t *d_raw, int h, int rb, in
         default: return (int)cudaErrorInvalidValue;
     }
     LT_MARK("k_png_unfilter");
+    return (int)cudaGetLastError();
+}
+int launch_png_adam7_unfilter(const uint8_t *d_filt, uint8_t *d_packed, uint8_t *d_raw, const Adam7Layout &L, uint32_t w, uint32_t h, int bits, int bpp,
+                              uint32_t *d_sync, void *stream)
+{
+    cudaStream_t st = (cudaStream_t)stream;
+    Adam7Groups d;
+    d.first[0] = 0;
+    for (int p = 0; p < 7; p++) {
+        const Adam7Pass &P = L.pass[p];
+        d.h[p] = (int)P.h; d.rb[p] = (int)P.rb; d.filt_off[p] = P.filt_off; d.raw_off[p] = P.raw_off;
+        d.first[p + 1] = d.first[p] + (int)((P.h + 31) / 32);
+    }
+    const int groups = d.first[7];
+    cudaMemsetAsync(d_sync, 0, (size_t)(groups + 2) * 4, st);
+    uint32_t *ticket = d_sync, *bad = d_sync + 1, *progress = d_sync + 2;
+    switch (bpp) {
+        case 1: k_png_adam7_unfilter<1><<<groups, 32, 0, st>>>(d_filt, d_packed, d, ticket, progress, bad); break;
+        case 2: k_png_adam7_unfilter<2><<<groups, 32, 0, st>>>(d_filt, d_packed, d, ticket, progress, bad); break;
+        case 3: k_png_adam7_unfilter<3><<<groups, 32, 0, st>>>(d_filt, d_packed, d, ticket, progress, bad); break;
+        case 4: k_png_adam7_unfilter<4><<<groups, 32, 0, st>>>(d_filt, d_packed, d, ticket, progress, bad); break;
+        case 6: k_png_adam7_unfilter<6><<<groups, 32, 0, st>>>(d_filt, d_packed, d, ticket, progress, bad); break;
+        case 8: k_png_adam7_unfilter<8><<<groups, 32, 0, st>>>(d_filt, d_packed, d, ticket, progress, bad); break;
+        default: return (int)cudaErrorInvalidValue;
+    }
+    LT_MARK("k_png_adam7_unfilter");
+    const uint32_t rb = (uint32_t)(((size_t)w * bits + 7) / 8);
+    k_png_adam7_gather<<<dim3(cdivu(rb, 256), std::min<uint32_t>(h, 65535)), 256, 0, st>>>(d_packed, d_raw, L, bits, w, h, rb);
+    LT_MARK("k_png_adam7_gather");
     return (int)cudaGetLastError();
 }
 int launch_png_colours(const uint8_t *d_raw, size_t npixels, int channels, uint32_t *d_set /*2048 words, 8-byte aligned*/, uint32_t *d_flags, void *stream)

@@ -3,6 +3,7 @@
 #pragma once
 #include <cstdint>
 #include <cstddef>
+#include "png_adam7_core.h"
 
 namespace b200 {
 
@@ -32,6 +33,11 @@ int launch_png_adler(const uint8_t *d_filt, size_t n, unsigned long long *d_sums
 int launch_png_probe(const uint8_t *d_raw, size_t npixels, int channels, uint32_t *d_flags, void *stream);
 // wavefront un-filtering: filtered [h][rb + 1] -> raw [h][rb]; d_sync[1] != 0 afterwards = a row had a filter type > 4
 int launch_png_unfilter(const uint8_t *d_filt, uint8_t *d_raw, int h, int rb, int bpp, uint32_t *d_sync /*2 + ceil(h/32) words*/, void *stream);
+// Adam7: the seven passes of the inflated stream d_filt (layout L of a w x h image, bits per pixel, filter distance bpp) un-filtered in
+// one wavefront launch into d_packed (L.raw_bytes), then the full rows gathered into d_raw [h][row_bytes]; d_sync[1] != 0 afterwards =
+// a row had a filter type > 4.  d_sync: 2 + sum over the passes of ceil(pass height / 32) words.
+int launch_png_adam7_unfilter(const uint8_t *d_filt, uint8_t *d_packed, uint8_t *d_raw, const Adam7Layout &L, uint32_t w, uint32_t h, int bits, int bpp,
+                              uint32_t *d_sync, void *stream);
 // palette probe (8-bit RGB / RGBA): flags[2] = number of distinct pixel values, saturating above 256
 int launch_png_colours(const uint8_t *d_raw, size_t npixels, int channels, uint32_t *d_set /*2048 words*/, uint32_t *d_flags, void *stream);
 // repack pixels keeping `keep_mask` channels (bit c = keep channel c) : 8-bit samples only

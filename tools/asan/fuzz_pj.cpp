@@ -7,6 +7,7 @@
 #include "png_host.h"
 #include "jpeg_host.h"
 using namespace b200;
+bool b200::png_interlaced() { return true; }          // the C ABI's switch (api.cpp): Adam7 files are fuzzed too
 static std::vector<uint8_t> slurp(const char *p) { FILE *f = fopen(p, "rb"); std::vector<uint8_t> v; if (!f) return v; fseek(f, 0, SEEK_END); v.resize(ftell(f)); fseek(f, 0, SEEK_SET); if (fread(v.data(), 1, v.size(), f)) {} fclose(f); return v; }
 int main(int argc, char **argv)
 {
@@ -27,7 +28,7 @@ int main(int argc, char **argv)
             if (is_png) {
                 PngInfo info; PngIdat idat;
                 if (!png_parse_chunks(d.data(), d.size(), false, info, idat, err)) { bad++; continue; }
-                const unsigned long long nin = (unsigned long long)(info.row_bytes + 1) * info.height;
+                const unsigned long long nin = png_inflated_size(info);
                 if (nin > 50000000ull) { bad++; continue; }
                 // the product's shape: inflate into a fixed buffer of nin + 4096 (+ 64) bytes
                 std::vector<uint8_t> buf(nin + 4096 + 64); size_t got = 0; uint32_t ad = 0;
