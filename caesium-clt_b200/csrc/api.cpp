@@ -75,11 +75,25 @@ const char *const kFractional = "fractional sampling ratio unsupported (upsampli
 
 int g_forced_device = -1, g_forced_ngpus = 0;
 std::atomic<int> g_entropy_mode{-1};     // -1 unset (env B200_ENTROPY); bit 0 = device entropy encoder, bit 1 = device entropy decoder (default 3)
-std::atomic<int> g_png_lossy{-1};        // -1 unset (env B200_PNG_LOSSY); 1 = lossy PNG on the device's quantiser, 0 = refused (code 3)
-std::atomic<int> g_gif{-1};              // -1 unset (env B200_GIF); 1 = GIF re-encoded on the device, 0 = refused (code 3)
-std::atomic<int> g_png_resize{-1};       // -1 unset (env B200_PNG_RESIZE); 1 = PNG -> PNG with width / height on the device, 0 = refused (code 3)
-std::atomic<int> g_webp_lossless_convert{-1};   // -1 unset (env B200_WEBP_LOSSLESS_CONVERT); 1 = JPEG / PNG -> lossless WebP on the device, 0 = refused (code 3)
-std::atomic<int> g_png_interlaced{-1};   // -1 unset (env B200_PNG_INTERLACED); 1 = Adam7 PNG sources accepted, 0 = refused (code 3)
+
+// An opt-in device leg, off by default: its b200_set_* setter, else its environment variable set to "gpu", read once.  Off, the
+// leg's inputs are refused with code 3.
+struct OptIn {
+    const char *env;
+    std::atomic<int> v{-1};              // -1: not set yet
+    constexpr explicit OptIn(const char *e) : env(e) {}
+    bool on()
+    {
+        if (v.load() < 0) { const char *e = getenv(env); v.store(e && !strcmp(e, "gpu") ? 1 : 0); }
+        return v.load() == 1;
+    }
+    int set(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; v.store(on); return B200_OK; }
+};
+OptIn g_png_lossy{"B200_PNG_LOSSY"};                          // lossy PNG (png.optimize == false) on the device's quantiser
+OptIn g_gif{"B200_GIF"};                                      // GIF re-encoded on the device
+OptIn g_png_resize{"B200_PNG_RESIZE"};                        // PNG -> PNG with width / height on the device
+OptIn g_webp_lossless_convert{"B200_WEBP_LOSSLESS_CONVERT"};  // JPEG / PNG -> lossless WebP on the device
+OptIn g_png_interlaced{"B200_PNG_INTERLACED"};                // Adam7 PNG sources on every PNG leg
 
 // runtime_init is idempotent while initialised, so after b200_shutdown (which frees every slot's device buffers) the next call
 // initialises again: a long-running host can hand the memory of one workload's slots back before starting another
@@ -102,60 +116,12 @@ int entropy_mode()
     return g_entropy_mode.load();
 }
 
-// lossy PNG (png.optimize == false) on the device: b200_set_png_lossy, else B200_PNG_LOSSY=gpu, read once; off by default
-bool png_lossy()
-{
-    if (g_png_lossy.load() < 0) {
-        const char *e = getenv("B200_PNG_LOSSY");
-        g_png_lossy.store(e && !strcmp(e, "gpu") ? 1 : 0);
-    }
-    return g_png_lossy.load() == 1;
-}
-
-// PNG -> PNG with a target size on the device: b200_set_png_resize, else B200_PNG_RESIZE=gpu, read once; off by default
-bool png_resize()
-{
-    if (g_png_resize.load() < 0) {
-        const char *e = getenv("B200_PNG_RESIZE");
-        g_png_resize.store(e && !strcmp(e, "gpu") ? 1 : 0);
-    }
-    return g_png_resize.load() == 1;
-}
-
-// JPEG / PNG -> lossless WebP on the device: b200_set_webp_lossless_convert, else B200_WEBP_LOSSLESS_CONVERT=gpu, read once; off by default
-bool webp_lossless_convert()
-{
-    if (g_webp_lossless_convert.load() < 0) {
-        const char *e = getenv("B200_WEBP_LOSSLESS_CONVERT");
-        g_webp_lossless_convert.store(e && !strcmp(e, "gpu") ? 1 : 0);
-    }
-    return g_webp_lossless_convert.load() == 1;
-}
-
 } // namespace
 
-// Adam7 PNG sources on every PNG leg: b200_set_png_interlaced, else B200_PNG_INTERLACED=gpu, read once; off by default.  Asked by
-// png_parse_chunks (png_host.cpp), which every PNG leg goes through.
-bool b200::png_interlaced()
-{
-    if (g_png_interlaced.load() < 0) {
-        const char *e = getenv("B200_PNG_INTERLACED");
-        g_png_interlaced.store(e && !strcmp(e, "gpu") ? 1 : 0);
-    }
-    return g_png_interlaced.load() == 1;
-}
+// asked by png_parse_chunks (png_host.cpp), which every PNG leg goes through
+bool b200::png_interlaced() { return g_png_interlaced.on(); }
 
 namespace {
-
-// GIF sources on the device: b200_set_gif, else B200_GIF=gpu, read once; off by default
-bool gif_on()
-{
-    if (g_gif.load() < 0) {
-        const char *e = getenv("B200_GIF");
-        g_gif.store(e && !strcmp(e, "gpu") ? 1 : 0);
-    }
-    return g_gif.load() == 1;
-}
 
 // One slot of one device (prefer_dev < 0: the next device round-robin), held until the lease goes out of scope.  The runtime
 // must already be up (ensure_runtime): where a leg calls that decides which status a machine without a device answers.
@@ -271,10 +237,11 @@ struct StageTimer {
         const long long ns = std::chrono::duration_cast<std::chrono::nanoseconds>(n - t).count();
         g_stage_ns[i] += ns; t = n;
         if (i == 5) g_stage_n++;
-        static const bool verbose = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2;
-        if (verbose) fprintf(stderr, "[b200 trace] stage %d: %.3f ms\n", i, ns / 1e6);
+        if (trace_level() >= 2) fprintf(stderr, "[b200 trace] stage %d: %.3f ms\n", i, ns / 1e6);
     }
 };
+double ms_between(std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); }
+
 void print_trace()
 {
     if (!g_trace || !g_stage_n.load()) return;
@@ -462,16 +429,30 @@ b200_status png_target(const PngInfo &info, const b200_params *p, uint32_t &nw, 
     return target_size(info.width, info.height, p, 65535, nw, nh, "invalid target dimensions");
 }
 
+// The IDAT stream inflated straight into the PngDevice's pinned staging buffer: nfilt filtered bytes and the stream's stored Adler-32
+b200_status png_inflate(PngDevice *png, const PngInfo &info, const PngIdat &idat, size_t &nfilt, uint32_t &stored_adler)
+{
+    std::string err;
+    const size_t nin = png_inflated_size(info);
+    size_t cap = 0;
+    nfilt = 0; stored_adler = 0;
+    uint8_t *buf = png->input_buffer(nin, cap, err);
+    if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    if (!zlib_inflate_to(idat.p, idat.n, buf, cap, nin, &nfilt, &stored_adler, err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
+    if (nfilt < nin) return make_status(B200_ERR_CORRUPT_INPUT, "IDAT too short");
+    return ok_status();
+}
+
 // ---- PNG (lossless) through the device ---------------------------------------------------------------------------
 // libcaesium png::compress: optimize == true -> png::lossless (oxipng, level = png.optimization_level); otherwise the lossy
 // palette quantiser (imagequant) when the lossy switch is on.  Resizing (width / height) runs on the device when the resize switch is on.
 b200_status png_compress(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
 {
-    if (!p->png_optimize && !png_lossy()) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::compress_in_memory)");
-    if ((p->width || p->height) && !png_resize()) return make_status(B200_ERR_UNSUPPORTED, "PNG resize is outside the GPU path (route to caesium::compress_in_memory)");
+    if (!p->png_optimize && !g_png_lossy.on()) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::compress_in_memory)");
+    if ((p->width || p->height) && !g_png_resize.on()) return make_status(B200_ERR_UNSUPPORTED, "PNG resize is outside the GPU path (route to caesium::compress_in_memory)");
     std::string err;
     PngInfo info; PngIdat idat;
-    static const bool verbose = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2;
+    const bool verbose = trace_level() >= 2;
     const auto t0 = std::chrono::steady_clock::now();
     if (!png_parse_chunks(in, in_len, p->keep_metadata != 0, info, idat, err)) return png_status(err);
     uint32_t nw, nh;
@@ -490,32 +471,27 @@ b200_status png_compress(const uint8_t *in, size_t in_len, const b200_params *p,
         PngDevice *png = s->png_dev();
         // the IDAT stream is inflated straight into the slot's pinned staging buffer; from there on everything is device work
         // (un-filter, checksum, reductions, filter trials, LZ77, DEFLATE coding) until the finished zlib stream comes back
-        const size_t nin = png_inflated_size(info);
-        size_t cap = 0, got = 0; uint32_t stored_adler = 0;
-        uint8_t *buf = png->input_buffer(nin, cap, err);
-        if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
-        if (!zlib_inflate_to(idat.p, idat.n, buf, cap, nin, &got, &stored_adler, err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
-        if (got < nin) return make_status(B200_ERR_CORRUPT_INPUT, "IDAT too short");
+        size_t nfilt; uint32_t stored_adler;
+        const b200_status ist = png_inflate(png, info, idat, nfilt, stored_adler);
+        if (ist.code) return ist;
         t1 = std::chrono::steady_clock::now();
-        LaunchTimer lt;
-        if (verbose) { lt.begin((cudaStream_t)s->stream); tl_launch_timer = &lt; }
-        const bool ok = png->compress_filtered(info, got, stored_adler, std::min((int)p->png_optimization_level, 6), s->stream, z, nullptr, err, nw, nh);
-        tl_launch_timer = nullptr;
-        if (verbose) { cudaStreamSynchronize((cudaStream_t)s->stream); lt.collect(ev); }
+        LaunchTrace tr(s->stream, verbose);
+        const bool ok = png->unfilter(info, nfilt, stored_adler, s->stream, err, nw, nh, true) &&
+                        png->code_unfiltered(info, std::min((int)p->png_optimization_level, 6), s->stream, z, nullptr, err);
+        if (verbose) { cudaStreamSynchronize((cudaStream_t)s->stream); tr.lt.collect(ev); }
         if (!ok) return png_device_status(png, nw != 0, err);
         deflate_ms = png->last_deflate_ms;
     }
     const auto t3 = std::chrono::steady_clock::now();
     png_write(info, z, out);
     if (verbose) {
-        auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
         fprintf(stderr, "[b200 trace] png %ux%u: parse + inflate %.1f ms, device (un-filter, filter trials, LZ77, DEFLATE coding; host Huffman %.1f) %.1f ms, container %.1f ms\n",
-                info.width, info.height, ms(t0, t1), deflate_ms, ms(t1, t3), ms(t3, std::chrono::steady_clock::now()));
+                info.width, info.height, ms_between(t0, t1), deflate_ms, ms_between(t1, t3), ms_between(t3, std::chrono::steady_clock::now()));
         auto at = [&](const char *k) { auto it = ev.find(k); return it == ev.end() ? 0.0 : it->second.first; };
         const double up = at("h2d") + at("k_png_adler") + at("k_png_unfilter") + at("k_png_adam7_unfilter") + at("k_png_adam7_gather") + at("png_unfilter"),
                      rz = at("png_resize");
         fprintf(stderr, "[b200 trace] png stages %ux%u -> %ux%u: parse + inflate %.3f ms, h2d + un-filter %.3f ms, expand + K3 + pack %.3f ms, back end %.3f ms\n",
-                sw, sh, info.width, info.height, ms(t0, t1), up, rz, ms(t1, t3) - up - rz);
+                sw, sh, info.width, info.height, ms_between(t0, t1), up, rz, ms_between(t1, t3) - up - rz);
     }
     return ok_status();
 }
@@ -539,22 +515,16 @@ void drop_colour_chunks(std::vector<uint8_t> &kept, bool grey_source)
 // B200_TRACE=2 prints the per-kernel event times.
 b200_status png_lossy_code(Slot *s, PngInfo info, int quality, int level, std::vector<uint8_t> &out)
 {
-    static const bool verbose = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2;
+    const bool verbose = trace_level() >= 2;
     std::string err;
     std::vector<uint8_t> z;
-    LaunchTimer lt;
-    if (verbose) { lt.begin((cudaStream_t)s->stream); tl_launch_timer = &lt; }
+    LaunchTrace tr(s->stream, verbose);
     const auto t0 = std::chrono::steady_clock::now();
-    const bool ok = s->png_dev()->code_quantized(info, quality < 0 ? 0 : quality > 100 ? 100 : quality, std::min(level, 6), s->stream, z, err);
-    tl_launch_timer = nullptr;
-    if (!ok) return make_status(B200_ERR_CUDA, err);
+    if (!s->png_dev()->code_quantized(info, quality < 0 ? 0 : quality > 100 ? 100 : quality, std::min(level, 6), s->stream, z, err)) return make_status(B200_ERR_CUDA, err);
     if (verbose) {
-        std::map<std::string, std::pair<double, int>> acc;
-        lt.collect(acc);
-        std::string kt;
-        for (auto &kv : acc) { char b[96]; snprintf(b, sizeof b, " %s=%.4f", kv.first.c_str(), kv.second.first); kt += b; }
+        const std::string kt = tr.kernel_ms();
         fprintf(stderr, "[b200 trace] png-lossy %ux%u q%d: %d colours, device %.3f ms (median cut %.3f); kernels ms:%s\n", info.width, info.height, quality,
-                (int)(info.plte.size() / 3), std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count(), s->png_dev()->quantiser()->last_cut_ms, kt.c_str());
+                (int)(info.plte.size() / 3), ms_between(t0, std::chrono::steady_clock::now()), s->png_dev()->quantiser()->last_cut_ms, kt.c_str());
     }
     png_write(info, z, out);
     return ok_status();
@@ -567,13 +537,11 @@ b200_status png_lossy_load(Slot *s, PngInfo &info, const PngIdat &idat, uint32_t
     const bool grey = info.color_type == 0 || info.color_type == 4;
     drop_colour_chunks(info.kept_before_idat, grey); drop_colour_chunks(info.kept_after_idat, grey);
     PngDevice *png = s->png_dev();
-    const size_t nin = png_inflated_size(info);
-    size_t cap = 0, got = 0; uint32_t stored_adler = 0;
-    uint8_t *buf = png->input_buffer(nin, cap, err);
-    if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
-    if (!zlib_inflate_to(idat.p, idat.n, buf, cap, nin, &got, &stored_adler, err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
-    if (got < nin) return make_status(B200_ERR_CORRUPT_INPUT, "IDAT too short");
-    if (!png->load_filtered_lossy(info, got, stored_adler, s->stream, err, nw, nh)) return png_device_status(png, nw != 0, err);
+    size_t nfilt; uint32_t stored_adler;
+    const b200_status st = png_inflate(png, info, idat, nfilt, stored_adler);
+    if (st.code) return st;
+    if (!png->unfilter(info, nfilt, stored_adler, s->stream, err, nw, nh) || !png->quantiser()->expand(png->d_raw, info, s->stream, err) || !png->quant->prepare(s->stream, err))
+        return png_device_status(png, nw != 0, err);
     return ok_status();
 }
 
@@ -637,6 +605,44 @@ bool resize_to_host(Slot *s, const uint8_t *src, uint32_t w, uint32_t h, uint32_
     return resize_host_planes(s, src, w, h, nw, nh, nc, rz, err) && slot_fetch_planes(s, rz, nc, (size_t)nw * nh, dst.data(), err);
 }
 
+// Host RGB planes `rgb` and an optional alpha plane `alpha` (null: none) at nw x nh: unchanged at the source's size, else resized into
+// `planes` and `ra` and pointed there (the alpha plane takes the same Lanczos3 as the colour planes)
+bool resize_rgba_to_host(Slot *s, const uint8_t *&rgb, const uint8_t *&alpha, uint32_t w, uint32_t h, uint32_t nw, uint32_t nh, std::vector<uint8_t> &planes,
+                         std::vector<uint8_t> &ra, std::string &err)
+{
+    if (nw == w && nh == h) return true;
+    if (!resize_to_host(s, rgb, w, h, nw, nh, 3, planes, err) || (alpha && !resize_to_host(s, alpha, w, h, nw, nh, 1, ra, err))) return false;
+    rgb = planes.data();
+    if (alpha) alpha = ra.data();
+    return true;
+}
+
+// The legs that decode a JPEG to RGB (or grey) planes and resample them (JPEG -> WebP, PNG, lossless WebP) start alike.  First,
+// before any slot is taken: the header and its refusals, the device, then the target size at `limit` (`msg` when out of range).
+b200_status jpeg_planes_target(JpegReader &rd, const b200_params *p, uint32_t limit, const char *msg, uint32_t &nw, uint32_t &nh)
+{
+    std::string err;
+    if (!rd.read_header(err)) return header_status(err);
+    const JpegGeom &gin = rd.geom();
+    if (fractional_sampling(gin)) return make_status(B200_ERR_UNSUPPORTED, kFractional);
+    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
+    return target_size((uint32_t)gin.width, (uint32_t)gin.height, p, limit, nw, nh, msg);
+}
+
+// Then, on the caller's slot: the entropy decode (`decoded` runs right after it, for the legs' trace laps), the resample plan to
+// nw x nh and the source's full-size planes in `full`, ready for resize_samples
+b200_status jpeg_planes_decode(Slot *s, JpegReader &rd, uint32_t nw, uint32_t nh, bool &on_device, SamplePlan &sp, uint8_t **full, std::string &err,
+                               const std::function<void()> &decoded = nullptr)
+{
+    const JpegGeom &gin = rd.geom();
+    if (!s->ensure((size_t)gin.total_coefs * 2, 0, 0, 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    const b200_status st = decode_into_slot(s, rd, on_device, err);
+    if (st.code) return st;
+    if (decoded) decoded();
+    if (!(plan_samples(s, gin, (int)nw, (int)nh, nullptr, sp, err) && samples_from_coefs(s, gin, sp, !on_device, true, full, err))) return make_status(B200_ERR_CUDA, err);
+    return ok_status();
+}
+
 // ---- conversion to WebP (lossy VP8) ----------------------------------------------------------------------------------
 // libcaesium convert: decode -> (resize) -> webp::compress at parameters.webp.quality.  JPEG sources are decoded on the
 // device (entropy decode, IDCT, upsample, YCbCr -> RGB, Lanczos3 when width/height are set) and never leave HBM before K8.
@@ -644,34 +650,26 @@ b200_status jpeg_to_webp(const uint8_t *in, size_t in_len, const b200_params *p,
 {
     std::string err;
     JpegReader rd(in, in_len);
-    if (!rd.read_header(err)) return header_status(err);
-    const JpegGeom &gin = rd.geom();
-    if (fractional_sampling(gin)) return make_status(B200_ERR_UNSUPPORTED, kFractional);
-    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
     uint32_t nw, nh;
-    b200_status st = target_size((uint32_t)gin.width, (uint32_t)gin.height, p, 16383, nw, nh, "invalid target dimensions for WebP");
+    b200_status st = jpeg_planes_target(rd, p, 16383, "invalid target dimensions for WebP", nw, nh);
     if (st.code) return st;
     SlotLease s(prefer_dev);
     if (!s) return s.failure();
-    static const bool verbose = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2;
+    const JpegGeom &gin = rd.geom();
     const auto t0 = std::chrono::steady_clock::now();
-    if (!s->ensure((size_t)gin.total_coefs * 2, 0, 0, 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    auto t1 = t0;
     bool on_device;
-    if ((st = decode_into_slot(s, rd, on_device, err)).code) return st;
-    const auto t1 = std::chrono::steady_clock::now();
     SamplePlan sp;
     uint8_t *full[3], *rgb[3];
-    if (!(plan_samples(s, gin, (int)nw, (int)nh, nullptr, sp, err) && samples_from_coefs(s, gin, sp, !on_device, true, full, err) && resize_samples(s, full, sp, rgb, err)))
-        return make_status(B200_ERR_CUDA, err);
+    if ((st = jpeg_planes_decode(s, rd, nw, nh, on_device, sp, full, err, [&] { t1 = std::chrono::steady_clock::now(); })).code) return st;
+    if (!resize_samples(s, full, sp, rgb, err)) return make_status(B200_ERR_CUDA, err);
     const auto t2 = std::chrono::steady_clock::now();
     WebpDevice *webp = s->webp_dev();
     const int g = gin.ncomp == 3;          // a grey source is its one plane three times
     if (!webp->encode_planes(rgb[0], rgb[g], rgb[2 * g], (int)nw, (int)nh, (int)p->webp_quality, s->stream, out, err)) return make_status(B200_ERR_CUDA, err);
-    if (verbose) {
-        auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
+    if (trace_level() >= 2)
         fprintf(stderr, "[b200 trace] jpeg %dx%d -> webp %ux%u: segment walk + entropy decode (device %d) %.1f ms, transform + resize launch %.1f ms, VP8 (wait for the device %.1f ms, boolean coder %.1f ms) %.1f ms\n",
-                gin.width, gin.height, nw, nh, (int)on_device, ms(t0, t1), ms(t1, t2), webp->last_wait_ms, webp->last_code_ms, ms(t2, std::chrono::steady_clock::now()));
-    }
+                gin.width, gin.height, nw, nh, (int)on_device, ms_between(t0, t1), ms_between(t1, t2), webp->last_wait_ms, webp->last_code_ms, ms_between(t2, std::chrono::steady_clock::now()));
     return ok_status();
 }
 
@@ -679,28 +677,21 @@ b200_status jpeg_to_webp(const uint8_t *in, size_t in_len, const b200_params *p,
 // the lossless PNG leg (K6 filter selection, K7 LZ77).  A greyscale JPEG becomes a greyscale PNG.
 b200_status jpeg_to_png(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
 {
-    if (!p->png_optimize && !png_lossy()) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::convert_in_memory)");
+    if (!p->png_optimize && !g_png_lossy.on()) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::convert_in_memory)");
     std::string err;
     JpegReader rd(in, in_len);
-    if (!rd.read_header(err)) return header_status(err);
-    const JpegGeom &gin = rd.geom();
-    if (fractional_sampling(gin)) return make_status(B200_ERR_UNSUPPORTED, kFractional);
-    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
     uint32_t nw, nh;
-    b200_status st = target_size((uint32_t)gin.width, (uint32_t)gin.height, p, 65535, nw, nh, "invalid target dimensions");
+    b200_status st = jpeg_planes_target(rd, p, 65535, "invalid target dimensions", nw, nh);
     if (st.code) return st;
     SlotLease s(prefer_dev);
     if (!s) return s.failure();
-    if (!s->ensure((size_t)gin.total_coefs * 2, 0, 0, 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
     bool on_device;
-    if ((st = decode_into_slot(s, rd, on_device, err)).code) return st;
-    const int nc = gin.ncomp == 1 ? 1 : 3;
     SamplePlan sp;
     uint8_t *full[3], *rgb[3];
+    if ((st = jpeg_planes_decode(s, rd, nw, nh, on_device, sp, full, err)).code) return st;
+    const int nc = rd.geom().ncomp == 1 ? 1 : 3;
     std::vector<uint8_t> planes((size_t)nc * nw * nh);
-    if (!(plan_samples(s, gin, (int)nw, (int)nh, nullptr, sp, err) && samples_from_coefs(s, gin, sp, !on_device, true, full, err) && resize_samples(s, full, sp, rgb, err) &&
-          slot_fetch_planes(s, rgb, nc, (size_t)nw * nh, planes.data(), err)))
-        return make_status(B200_ERR_CUDA, err);
+    if (!(resize_samples(s, full, sp, rgb, err) && slot_fetch_planes(s, rgb, nc, (size_t)nw * nh, planes.data(), err))) return make_status(B200_ERR_CUDA, err);
     return png_from_planes(s, planes.data(), nc, nullptr, nw, nh, false, p, out, err);
 }
 
@@ -851,7 +842,7 @@ b200_status webp_decode_status(const uint8_t *in, size_t in_len, WebpInfo &info,
 b200_status webp_lossless_compress(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
 {
     std::string err;
-    static const bool verbose = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2;
+    const bool verbose = trace_level() >= 2;
     const auto t0 = std::chrono::steady_clock::now();
     WebpInfo info; std::vector<uint8_t> rgb, alpha;
     b200_status st = webp_decode_status(in, in_len, info, rgb, &alpha);
@@ -865,26 +856,15 @@ b200_status webp_lossless_compress(const uint8_t *in, size_t in_len, const b200_
     const auto t1 = std::chrono::steady_clock::now();
     const uint8_t *src = rgb.data(), *ap = alpha.empty() ? nullptr : alpha.data();
     std::vector<uint8_t> planes, ra;
-    if (nw != w || nh != h) {
-        if (!resize_to_host(s, src, w, h, nw, nh, 3, planes, err) || (ap && !resize_to_host(s, ap, w, h, nw, nh, 1, ra, err))) return make_status(B200_ERR_CUDA, err);
-        src = planes.data();
-        if (ap) ap = ra.data();
-    }
+    if (!resize_rgba_to_host(s, src, ap, w, h, nw, nh, planes, ra, err)) return make_status(B200_ERR_CUDA, err);
     const auto t2 = std::chrono::steady_clock::now();
     Vp8lDevice *v = s->vp8l_dev();
-    LaunchTimer lt;
-    if (verbose) { lt.begin((cudaStream_t)s->stream); tl_launch_timer = &lt; }
-    const bool ok = v->encode(src, ap, (int)nw, (int)nh, s->stream, out, err);
-    tl_launch_timer = nullptr;
-    if (!ok) return make_status(B200_ERR_CUDA, err);
+    LaunchTrace tr(s->stream, verbose);
+    if (!v->encode(src, ap, (int)nw, (int)nh, s->stream, out, err)) return make_status(B200_ERR_CUDA, err);
     if (verbose) {
-        auto ms = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
-        std::map<std::string, std::pair<double, int>> acc;
-        lt.collect(acc);
-        std::string kt;
-        for (auto &kv : acc) { char b[96]; snprintf(b, sizeof b, " %s=%.4f", kv.first.c_str(), kv.second.first); kt += b; }
+        const std::string kt = tr.kernel_ms();
         fprintf(stderr, "[b200 trace] webp-lossless %ux%u -> %ux%u: host decode %.3f ms, resize %.3f ms, device encode %.3f ms (analysis wait %.3f, cache bits %d, codes + emission %.3f); kernels ms:%s\n",
-                w, h, nw, nh, ms(t0, t1), ms(t1, t2), ms(t2, std::chrono::steady_clock::now()), v->last_analyse_ms, v->last_cache_bits, v->last_code_ms, kt.c_str());
+                w, h, nw, nh, ms_between(t0, t1), ms_between(t1, t2), ms_between(t2, std::chrono::steady_clock::now()), v->last_analyse_ms, v->last_cache_bits, v->last_code_ms, kt.c_str());
     }
     return ok_status();
 }
@@ -921,7 +901,7 @@ b200_status png_to_webp(const uint8_t *in, size_t in_len, const b200_params *p, 
 // leg's planes and the PNG leg's un-filtered rows feed the encoder (vp8l_encode.cpp) where they lie.  B200_TRACE=2 prints one line
 // per call with the stages; to give each stage its own time the trace waits for the device after each of them.
 struct ConvertStages {
-    static bool verbose() { static const bool v = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2; return v; }
+    static bool verbose() { return trace_level() >= 2; }
     std::chrono::steady_clock::time_point t = std::chrono::steady_clock::now();
     double ms[4] = {0, 0, 0, 0};            // parse + decode / inflate, device front end, resize, encode
     void lap(int k, void *stream)
@@ -947,22 +927,16 @@ b200_status jpeg_to_webp_lossless(const uint8_t *in, size_t in_len, const b200_p
     std::string err;
     ConvertStages tr;
     JpegReader rd(in, in_len);
-    if (!rd.read_header(err)) return header_status(err);
-    const JpegGeom &gin = rd.geom();
-    if (fractional_sampling(gin)) return make_status(B200_ERR_UNSUPPORTED, kFractional);
-    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
     uint32_t nw, nh;
-    b200_status st = target_size((uint32_t)gin.width, (uint32_t)gin.height, p, 16383, nw, nh, "invalid target dimensions for WebP");
+    b200_status st = jpeg_planes_target(rd, p, 16383, "invalid target dimensions for WebP", nw, nh);
     if (st.code) return st;
     SlotLease s(prefer_dev);
     if (!s) return s.failure();
-    if (!s->ensure((size_t)gin.total_coefs * 2, 0, 0, 1 << 14, err)) return make_status(B200_ERR_OUT_OF_MEMORY, err);
+    const JpegGeom &gin = rd.geom();
     bool on_device;
-    if ((st = decode_into_slot(s, rd, on_device, err)).code) return st;
-    tr.lap(0, s->stream);
     SamplePlan sp;
     uint8_t *full[3], *rgb[3];
-    if (!(plan_samples(s, gin, (int)nw, (int)nh, nullptr, sp, err) && samples_from_coefs(s, gin, sp, !on_device, true, full, err))) return make_status(B200_ERR_CUDA, err);
+    if ((st = jpeg_planes_decode(s, rd, nw, nh, on_device, sp, full, err, [&] { tr.lap(0, s->stream); })).code) return st;
     tr.lap(1, s->stream);
     if (!resize_samples(s, full, sp, rgb, err)) return make_status(B200_ERR_CUDA, err);
     tr.lap(2, s->stream);
@@ -991,15 +965,11 @@ b200_status png_to_webp_lossless(const uint8_t *in, size_t in_len, const b200_pa
     if (!s) return s.failure();
     PngDevice *png = s->png_dev();
     Vp8lDevice *v = s->vp8l_dev();
-    const size_t nin = png_inflated_size(info);
-    size_t cap = 0, got = 0; uint32_t stored_adler = 0;
-    uint8_t *buf = png->input_buffer(nin, cap, err);
-    if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
-    if (!zlib_inflate_to(idat.p, idat.n, buf, cap, nin, &got, &stored_adler, err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
-    if (got < nin) return make_status(B200_ERR_CORRUPT_INPUT, "IDAT too short");
+    size_t nfilt; uint32_t stored_adler;
+    const b200_status ist = png_inflate(png, info, idat, nfilt, stored_adler);
+    if (ist.code) return ist;
     tr.lap(0, nullptr);
-    std::vector<uint8_t> none;
-    if (!png->from_filtered(info, got, stored_adler, 0, s->stream, none, nullptr, err, PngDevice::Tail::Samples, 0, 0)) return png_device_status(png, false, err);
+    if (!png->unfilter(info, nfilt, stored_adler, s->stream, err)) return png_device_status(png, false, err);
     const uint32_t w = info.width, h = info.height;
     uint32_t *argb, *flags;
     if (!v->reserve((int)nw, (int)nh, argb, flags, err)) return make_status(B200_ERR_CUDA, err);
@@ -1044,11 +1014,7 @@ b200_status rgb_to_png(const std::vector<uint8_t> &rgb, uint32_t w, uint32_t h, 
     if (!s) return s.failure();
     const uint8_t *src = rgb.data(), *ap = alpha ? alpha->data() : nullptr;
     std::vector<uint8_t> planes, ra;
-    if (nw != w || nh != h) {   // transparency stays: the alpha plane takes the same Lanczos3 as the colour planes
-        if (!resize_to_host(s, src, w, h, nw, nh, 3, planes, err) || (ap && !resize_to_host(s, ap, w, h, nw, nh, 1, ra, err))) return make_status(B200_ERR_CUDA, err);
-        src = planes.data();
-        if (ap) ap = ra.data();
-    }
+    if (!resize_rgba_to_host(s, src, ap, w, h, nw, nh, planes, ra, err)) return make_status(B200_ERR_CUDA, err);
     return png_from_planes(s, src, 3, ap, nw, nh, true, p, out, err);
 }
 
@@ -1061,7 +1027,7 @@ b200_status convert_dispatch(const uint8_t *in, size_t in_len, uint32_t src, uin
     if (src == B200_FMT_WEBP && (fmt == B200_FMT_JPEG || fmt == B200_FMT_PNG)) {
         // WebP source: decoded on the calling thread (vp8_decode.cpp), then the same back ends as a PNG source
         if (fmt == B200_FMT_JPEG && p->jpeg_optimize) return make_status(B200_ERR_UNSUPPORTED, "lossless conversion to JPEG is outside the GPU path (route to caesium::convert_in_memory)");
-        if (fmt == B200_FMT_PNG && !p->png_optimize && !png_lossy()) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::convert_in_memory)");
+        if (fmt == B200_FMT_PNG && !p->png_optimize && !g_png_lossy.on()) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::convert_in_memory)");
         WebpInfo wi; std::vector<uint8_t> rgb, alpha;
         const b200_status s = webp_decode_status(in, in_len, wi, rgb, &alpha);
         if (s.code) return s;
@@ -1072,8 +1038,8 @@ b200_status convert_dispatch(const uint8_t *in, size_t in_len, uint32_t src, uin
     const bool to_webp = fmt == B200_FMT_WEBP, png_to_jpg = fmt == B200_FMT_JPEG && src == B200_FMT_PNG;
     if (!to_webp && !png_to_jpg) return make_status(B200_ERR_UNSUPPORTED, "this conversion is outside the GPU path (route to caesium::convert_in_memory)");
     if (to_webp && p->webp_lossless) {
-        if (webp_lossless_convert() && src == B200_FMT_JPEG) return jpeg_to_webp_lossless(in, in_len, p, -1, out);
-        if (webp_lossless_convert() && src == B200_FMT_PNG) return png_to_webp_lossless(in, in_len, p, -1, out);
+        if (g_webp_lossless_convert.on() && src == B200_FMT_JPEG) return jpeg_to_webp_lossless(in, in_len, p, -1, out);
+        if (g_webp_lossless_convert.on() && src == B200_FMT_PNG) return png_to_webp_lossless(in, in_len, p, -1, out);
         return make_status(B200_ERR_UNSUPPORTED, "lossless WebP (VP8L) is outside the GPU path (route to caesium::convert_in_memory)");
     }
     if (png_to_jpg && p->jpeg_optimize) return make_status(B200_ERR_UNSUPPORTED, "lossless conversion to JPEG is outside the GPU path (route to caesium::convert_in_memory)");
@@ -1087,9 +1053,8 @@ b200_status convert_dispatch(const uint8_t *in, size_t in_len, uint32_t src, uin
 // quantiser at gif_quality, segmented LZW); the container is written here.  B200_TRACE=2 prints host decode against device time.
 b200_status gif_compress(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
 {
-    if (!gif_on()) return make_status(B200_ERR_UNSUPPORTED, "GIF is outside the GPU path (route to caesium::compress_in_memory)");
+    if (!g_gif.on()) return make_status(B200_ERR_UNSUPPORTED, "GIF is outside the GPU path (route to caesium::compress_in_memory)");
     if (p->width || p->height) return make_status(B200_ERR_UNSUPPORTED, "GIF resize is outside the GPU path (route to caesium::compress_in_memory)");
-    static const bool verbose = getenv("B200_TRACE") && atoi(getenv("B200_TRACE")) >= 2;
     std::string err;
     GifReader rd;
     if (!rd.open(in, in_len, err)) return make_status(rd.unsupported ? B200_ERR_UNSUPPORTED : B200_ERR_CORRUPT_INPUT, err);
@@ -1100,8 +1065,8 @@ b200_status gif_compress(const uint8_t *in, size_t in_len, const b200_params *p,
     bool corrupt = false;
     const int q = (int)std::min<uint32_t>(p->gif_quality, 100);
     if (!s->gif_dev()->encode(rd, *s->png_dev()->quantiser(), q, s->stream, out, corrupt, err)) return make_status(corrupt ? B200_ERR_CORRUPT_INPUT : B200_ERR_CUDA, err);
-    if (verbose) {
-        const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    if (trace_level() >= 2) {
+        const double ms = ms_between(t0, std::chrono::steady_clock::now());
         fprintf(stderr, "[b200 trace] gif %dx%d, %d frames q%d: host decode %.1f ms, device and container %.1f ms\n", rd.width, rd.height, rd.frames, q,
                 s->gif_dev()->decode_ms, ms - s->gif_dev()->decode_ms);
     }
@@ -1215,11 +1180,11 @@ int b200_device_numa_node(int index) { return index < 0 || index >= runtime_devi
 const char *b200_version(void) { return "b200-caesium 0.1.0 (sm_90a)"; }
 void b200_free(void *p) { free(p); }
 int b200_set_entropy_mode(int mode) { if (mode < 0 || mode > 3) return B200_ERR_INVALID_ARGUMENT; g_entropy_mode.store(mode); return B200_OK; }
-int b200_set_png_lossy(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_png_lossy.store(on); return B200_OK; }
-int b200_set_gif(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_gif.store(on); return B200_OK; }
-int b200_set_png_resize(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_png_resize.store(on); return B200_OK; }
-int b200_set_webp_lossless_convert(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_webp_lossless_convert.store(on); return B200_OK; }
-int b200_set_png_interlaced(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; g_png_interlaced.store(on); return B200_OK; }
+int b200_set_png_lossy(int on) { return g_png_lossy.set(on); }
+int b200_set_gif(int on) { return g_gif.set(on); }
+int b200_set_png_resize(int on) { return g_png_resize.set(on); }
+int b200_set_webp_lossless_convert(int on) { return g_webp_lossless_convert.set(on); }
+int b200_set_png_interlaced(int on) { return g_png_interlaced.set(on); }
 int b200_set_jpeg_trellis(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; set_jpeg_trellis(on == 1); return B200_OK; }
 
 uint32_t b200_sniff_format(const uint8_t *d, size_t n)
@@ -1372,8 +1337,8 @@ static b200_status webp_to_size(const uint8_t *in, size_t in_len, b200_params *p
 // refinement, dithering and coding at its png_quality
 static b200_status png_to_size(const uint8_t *in, size_t in_len, b200_params *params, size_t max_output_size, bool return_smallest, std::vector<uint8_t> &result)
 {
-    if (!png_lossy()) return make_status(B200_ERR_UNSUPPORTED, "compress_to_size on a PNG bisects the lossy (imagequant) quality, which is outside the GPU path (route to caesium::compress_to_size_in_memory)");
-    if ((params->width || params->height) && !png_resize()) return make_status(B200_ERR_UNSUPPORTED, "PNG resize is outside the GPU path (route to caesium::compress_to_size_in_memory)");
+    if (!g_png_lossy.on()) return make_status(B200_ERR_UNSUPPORTED, "compress_to_size on a PNG bisects the lossy (imagequant) quality, which is outside the GPU path (route to caesium::compress_to_size_in_memory)");
+    if ((params->width || params->height) && !g_png_resize.on()) return make_status(B200_ERR_UNSUPPORTED, "PNG resize is outside the GPU path (route to caesium::compress_to_size_in_memory)");
     std::string err;
     PngInfo info; PngIdat idat;
     if (!png_parse_chunks(in, in_len, params->keep_metadata != 0, info, idat, err)) return png_status(err);
@@ -1793,20 +1758,16 @@ b200_status b200_png_device_times(const uint8_t *in, size_t in_len, int level, i
         SlotLease s(-1);
         if (!s) return s.failure();
         PngDevice *png = s->png_dev();
-        const size_t nin = png_inflated_size(info0);
-        size_t bcap = 0, got = 0; uint32_t adler = 0;
-        uint8_t *buf = png->input_buffer(nin, bcap, err);
-        if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
-        if (!zlib_inflate_to(idat.p, idat.n, buf, bcap, nin, &got, &adler, err) || got < nin) return make_status(B200_ERR_CORRUPT_INPUT, err.empty() ? "IDAT too short" : err);
+        size_t nfilt; uint32_t adler;
+        const b200_status ist = png_inflate(png, info0, idat, nfilt, adler);
+        if (ist.code) return ist;
         std::vector<uint8_t> z;
         for (int it = 0; it <= iters; it++) {          // iteration 0 warms buffers up and is not counted
             PngInfo info = info0;
-            LaunchTimer lt; lt.begin((cudaStream_t)s->stream);
-            tl_launch_timer = it ? &lt : nullptr;
-            const bool ok = png->compress_filtered(info, got, adler, level < 0 ? 0 : level > 6 ? 6 : level, s->stream, z, nullptr, err);
-            tl_launch_timer = nullptr;
-            if (!ok) return make_status(B200_ERR_CUDA, err);
-            if (it) lt.collect(acc);
+            LaunchTrace tr(s->stream, it > 0);
+            if (!png->unfilter(info, nfilt, adler, s->stream, err, 0, 0, true) ||
+                !png->code_unfiltered(info, level < 0 ? 0 : level > 6 ? 6 : level, s->stream, z, nullptr, err)) return make_status(B200_ERR_CUDA, err);
+            tr.lt.collect(acc);
         }
     }
     std::string out;
@@ -1851,14 +1812,11 @@ b200_status b200_png_resize_samples(const uint8_t *in, size_t in_len, uint32_t w
         SlotLease s(-1);
         if (!s) return s.failure();
         PngDevice *png = s->png_dev();
-        const size_t nin = png_inflated_size(pi);
-        size_t cap = 0, got = 0; uint32_t stored_adler = 0;
-        uint8_t *buf = png->input_buffer(nin, cap, err);
-        if (!buf) return make_status(B200_ERR_OUT_OF_MEMORY, err);
-        if (!zlib_inflate_to(idat.p, idat.n, buf, cap, nin, &got, &stored_adler, err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
-        if (got < nin) return make_status(B200_ERR_CORRUPT_INPUT, "IDAT too short");
+        size_t nfilt; uint32_t stored_adler;
+        const b200_status ist = png_inflate(png, pi, idat, nfilt, stored_adler);
+        if (ist.code) return ist;
         std::vector<uint8_t> r;
-        if (!png->resize_filtered(pi, got, stored_adler, nw, nh, s->stream, r, err)) return png_device_status(png, true, err);
+        if (!png->unfilter(pi, nfilt, stored_adler, s->stream, err, nw, nh) || !png->fetch_rows(pi, r, s->stream, err)) return png_device_status(png, true, err);
         info->width = pi.width; info->height = pi.height; info->bit_depth = pi.bit_depth; info->color_type = pi.color_type; info->bpp = pi.bpp; info->row_bytes = pi.row_bytes;
         size_t n;
         return give(r, raw, &n);

@@ -171,13 +171,10 @@ bool pipe_kernel_times(JpegPipe *P, int iters, std::map<std::string, std::pair<d
     CU(cudaDeviceSynchronize());
     std::map<std::string, std::pair<double, int>> acc;
     for (int it = 0; it < iters; it++) {
-        LaunchTimer lt; lt.begin(st);
-        tl_launch_timer = &lt;
-        const bool ok = enqueue_group(P, G, 0, nullptr, err);
-        tl_launch_timer = nullptr;
-        if (!ok) return false;
+        LaunchTrace tr(st, true);
+        if (!enqueue_group(P, G, 0, nullptr, err)) return false;
         CU(cudaStreamSynchronize(st));
-        lt.collect(acc);
+        tr.lt.collect(acc);
     }
     out.clear();
     for (auto &kv : acc) out[kv.first] = std::make_pair(kv.second.first / kv.second.second, kv.second.second / iters);

@@ -119,33 +119,6 @@ uint8_t *PngDevice::input_buffer(size_t bytes, size_t &cap, std::string &err)
     return h_raw;
 }
 
-// The lossless path proper: the inflated IDAT (filter byte + filtered bytes per row) sits in this object's pinned buffer
-// (input_buffer()); everything from there to the finished zlib stream runs on the device -- un-filter (wavefront), Adler-32 check of
-// the input, reductions, K6 / K7 per strategy, DEFLATE coding -- except a palette reduction, which (at most 256 colours) goes
-// through the host and the raw-sample entry point below.
-bool PngDevice::compress_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, int level, void *stream, std::vector<uint8_t> &zlib_stream, int *chosen, std::string &err,
-                                  uint32_t nw, uint32_t nh)
-{
-    return from_filtered(info, nfilt, stored_adler, level, stream, zlib_stream, chosen, err, Tail::Code, nw, nh);
-}
-
-bool PngDevice::load_filtered_lossy(PngInfo &info, size_t nfilt, uint32_t stored_adler, void *stream, std::string &err, uint32_t nw, uint32_t nh)
-{
-    std::vector<uint8_t> none;
-    return from_filtered(info, nfilt, stored_adler, 0, stream, none, nullptr, err, Tail::Quantise, nw, nh);
-}
-
-bool PngDevice::resize_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, uint32_t nw, uint32_t nh, void *stream_, std::vector<uint8_t> &raw, std::string &err)
-{
-    cudaStream_t st = (cudaStream_t)stream_;
-    std::vector<uint8_t> none;
-    if (!from_filtered(info, nfilt, stored_adler, 0, stream_, none, nullptr, err, Tail::Samples, nw, nh)) return false;
-    raw.resize(info.row_bytes * info.height);
-    CU(cudaMemcpyAsync(raw.data(), d_raw, raw.size(), cudaMemcpyDeviceToHost, st));
-    CU(stream_wait(st));
-    return true;
-}
-
 // K3 of the ch planes of T at `in` (W x H each, one after another) into `out` (NW x NH each)
 template <class T> static bool resample_planes(Resampler &rs, const uint8_t *in, int W, int H, uint8_t *out, int NW, int NH, int ch, void *stream, std::string &err)
 {
@@ -176,11 +149,15 @@ bool PngDevice::resize_raw(const PngInfo &src, const PngInfo &out, void *stream_
     return true;
 }
 
-// Tail::Quantise (the lossy leg): stop after the checks and hand the samples to the quantiser (expand, histogram).  Tail::Samples: stop
-// after the checks.  nw, nh > 0: the resize runs between the un-filter and the checks' host wait (a corrupt input's resized samples
-// are discarded) and info describes the resized image from there on.
-bool PngDevice::from_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, int level, void *stream_, std::vector<uint8_t> &zlib_stream, int *chosen, std::string &err,
-                              Tail tail, uint32_t nw, uint32_t nh)
+// the inputs of the alpha / grey probe: 8-bit samples without tRNS that have colour or alpha to drop
+static bool alpha_grey_candidate(const PngInfo &info)
+{
+    return info.bit_depth == 8 && info.trns.empty() && (info.color_type == 2 || info.color_type == 4 || info.color_type == 6);
+}
+
+// nw, nh > 0: the resize runs between the un-filter and the checks' host wait (a corrupt input's resized samples are discarded)
+// and info describes the resized image from there on
+bool PngDevice::unfilter(PngInfo &info, size_t nfilt, uint32_t stored_adler, void *stream_, std::string &err, uint32_t nw, uint32_t nh, bool probes)
 {
     cudaStream_t st = (cudaStream_t)stream_;
     corrupt = false;
@@ -215,13 +192,9 @@ bool PngDevice::from_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler
     LT_MARK("png_unfilter");
     if (resize && !resize_raw(src, info, st, err)) return false;
     CU(cudaMemsetAsync(d_flags, 0, 16, st));
-    const bool lossless = tail == Tail::Code;
-    const bool eight = info.bit_depth == 8 && info.trns.empty();
-    const bool probe_ag = lossless && eight && (info.color_type == 2 || info.color_type == 4 || info.color_type == 6);
-    const bool probe_pal = lossless && png_palette_candidate(info);
     const size_t npix = (size_t)info.width * info.height;
-    if (probe_ag && launch_png_probe(d_raw, npix, info.channels, d_flags, st)) { err = "png probe launch failed"; return false; }
-    if (probe_pal && launch_png_colours(d_raw, npix, info.channels, d_set, d_flags, st)) { err = "png palette probe launch failed"; return false; }
+    if (probes && alpha_grey_candidate(info) && launch_png_probe(d_raw, npix, info.channels, d_flags, st)) { err = "png probe launch failed"; return false; }
+    if (probes && png_palette_candidate(info) && launch_png_colours(d_raw, npix, info.channels, d_set, d_flags, st)) { err = "png palette probe launch failed"; return false; }
     uint32_t *h_flags = reinterpret_cast<uint32_t *>(h_small.get());
     unsigned long long *h_sums_in = reinterpret_cast<unsigned long long *>(h_z.get());
     const size_t npieces_in = (nin + 4095) / 4096;
@@ -231,16 +204,30 @@ bool PngDevice::from_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler
     CU(stream_wait(st)); LT_MARK("host_wait");
     if (h_flags[5]) { err = "bad filter type"; corrupt = true; return false; }
     if (combine_adler(h_sums_in, nin) != stored_adler) { err = "Adler-32 mismatch"; corrupt = true; return false; }
-    if (tail == Tail::Samples) return true;
-    if (tail == Tail::Quantise) return quantiser()->expand(d_raw, info, st, err) && quant->prepare(st, err);
-    if (probe_pal && h_flags[2] <= 256) {
+    return true;
+}
+
+bool PngDevice::code_unfiltered(PngInfo &info, int level, void *stream_, std::vector<uint8_t> &zlib_stream, int *chosen, std::string &err)
+{
+    const uint32_t *h_flags = reinterpret_cast<const uint32_t *>(h_small.get());
+    const bool probed = alpha_grey_candidate(info);
+    if (png_palette_candidate(info) && h_flags[2] <= 256) {
         // few colours: oxipng's palette reduction (first-appearance order, tRNS layout, bit packing) runs on the host over the
         // reconstructed samples, and the indexed image takes the raw-sample entry point
         std::vector<uint8_t> raw(info.row_bytes * info.height);
         CU(cudaMemcpy(raw.data(), d_raw, raw.size(), cudaMemcpyDeviceToHost));
         if (png_reduce_palette(info, raw)) return compress(info, raw, level, stream_, zlib_stream, chosen, err);
     }
-    return reduce_and_code(info, probe_ag, h_flags, level, stream_, zlib_stream, chosen, err);
+    return reduce_and_code(info, probed, h_flags, level, stream_, zlib_stream, chosen, err);
+}
+
+bool PngDevice::fetch_rows(const PngInfo &info, std::vector<uint8_t> &raw, void *stream_, std::string &err)
+{
+    cudaStream_t st = (cudaStream_t)stream_;
+    raw.resize(info.row_bytes * info.height);
+    CU(cudaMemcpyAsync(raw.data(), d_raw, raw.size(), cudaMemcpyDeviceToHost, st));
+    CU(stream_wait(st));
+    return true;
 }
 
 bool PngDevice::compress(PngInfo &info, const std::vector<uint8_t> &raw_in, int level, void *stream_, std::vector<uint8_t> &zlib_stream, int *chosen, std::string &err)
@@ -255,7 +242,7 @@ bool PngDevice::compress(PngInfo &info, const std::vector<uint8_t> &raw_in, int 
     memcpy(h_raw, raw_in.data(), nraw);
     CU(cudaMemcpyAsync(d_raw, h_raw, nraw, cudaMemcpyHostToDevice, st));
     uint32_t *h_flags = reinterpret_cast<uint32_t *>(h_small.get());
-    const bool probe_ag = info.bit_depth == 8 && info.trns.empty() && (info.color_type == 2 || info.color_type == 4 || info.color_type == 6);
+    const bool probe_ag = alpha_grey_candidate(info);
     if (probe_ag) {
         uint32_t *d_flags = d_hist;
         CU(cudaMemsetAsync(d_flags, 0, 16, st));

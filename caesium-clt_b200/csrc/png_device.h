@@ -31,30 +31,26 @@ struct PngDevice {
     PngDevice();
     ~PngDevice();
 
-    // The lossless path: the caller inflates the IDAT stream into input_buffer() (pinned, `bytes` = height * (row_bytes + 1); the
-    // buffer has 4096 bytes of slack for the inflate) and hands over its length and the stream's stored Adler-32; un-filtering,
-    // checksum verification, reductions, K6 / K7 and the DEFLATE coding run on the device.
+    // The front end of every leg that starts from a PNG's IDAT: the caller inflates the stream into input_buffer() (pinned, `bytes` =
+    // png_inflated_size; the buffer has 4096 bytes of slack for the inflate) and hands over its length and the stream's stored
+    // Adler-32.  unfilter() uploads it, un-filters it into d_raw (Adam7: passes gathered into full rows), waits for the device once
+    // and checks the filter bytes and the Adler-32 (corrupt = true when they fail).  nw, nh > 0: the image is first expanded to the
+    // image crate's decoded type and resized to nw x nh (Lanczos3) before that wait, and info is rewritten to the resized image
+    // (png_resized_info: no source chunks survive).  probes: code_unfiltered() follows, and its alpha / grey and palette probes are
+    // enqueued before the wait.  The caller then runs its own tail over d_raw.
     uint8_t *input_buffer(size_t bytes, size_t &cap, std::string &err);
-    // nw, nh > 0: the image is first expanded to the image crate's decoded type and resized to nw x nh (Lanczos3), and info is rewritten
-    // to the resized image (png_resized_info: no source chunks survive); the back end then codes that image.
-    bool compress_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, int level, void *stream, std::vector<uint8_t> &zlib_stream, int *chosen_strategy, std::string &err,
-                           uint32_t nw = 0, uint32_t nh = 0);
-    // The lossy leg's front end: the same upload, un-filter and checks as compress_filtered, then the samples are expanded to RGBA8
-    // and the quantiser's histogram is built (quantiser(); independent of the quality, so compress_to_size does it once).  nw, nh > 0:
-    // resized first, as in compress_filtered, and info describes the resized image afterwards.
-    bool load_filtered_lossy(PngInfo &info, size_t nfilt, uint32_t stored_adler, void *stream, std::string &err, uint32_t nw = 0, uint32_t nh = 0);
-    // The resize alone (b200_png_resize_samples): the same upload, un-filter, checks and resize, then the rows of the resized image
-    // (info rewritten) come back to the host.
-    bool resize_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, uint32_t nw, uint32_t nh, void *stream, std::vector<uint8_t> &raw, std::string &err);
+    bool unfilter(PngInfo &info, size_t nfilt, uint32_t stored_adler, void *stream, std::string &err, uint32_t nw = 0, uint32_t nh = 0, bool probes = false);
+    // The lossless back end after unfilter(..., probes = true): the palette reduction when the probe found at most 256 colours,
+    // else the alpha / grey reductions, the filter trials, LZ77 and DEFLATE over d_raw.
+    bool code_unfiltered(PngInfo &info, int level, void *stream, std::vector<uint8_t> &zlib_stream, int *chosen_strategy, std::string &err);
+    // the rows in d_raw (info's image) back to the host
+    bool fetch_rows(const PngInfo &info, std::vector<uint8_t> &raw, void *stream, std::string &err);
     // The lossy leg's back end over whatever quantiser() holds: palette + dithered indices at `quality`, packed into d_raw as an
     // indexed image (info becomes colour type 3 with PLTE / tRNS), then the lossless leg's filter trials, LZ77 and DEFLATE.  An
     // image with at most 256 distinct values is not quantised: it takes the lossless leg's exact palette reduction.
     bool code_quantized(PngInfo &info, int quality, int level, void *stream, std::vector<uint8_t> &zlib_stream, std::string &err);
     PngQuant *quantiser();
     std::unique_ptr<PngQuant> quant;
-    enum class Tail { Code, Quantise, Samples };       // what follows the checks: the lossless back end, the quantiser, nothing
-    bool from_filtered(PngInfo &info, size_t nfilt, uint32_t stored_adler, int level, void *stream, std::vector<uint8_t> &zlib_stream, int *chosen_strategy, std::string &err,
-                       Tail tail, uint32_t nw, uint32_t nh);
     // d_raw (the source's un-filtered rows, `src`) -> expansion -> K3 -> packed rows of `out` (png_resized_info) in d_raw
     bool resize_raw(const PngInfo &src, const PngInfo &out, void *stream, std::string &err);
     bool ensure_buffers(size_t nraw, size_t nmax, size_t rb, void *stream, std::string &err);
