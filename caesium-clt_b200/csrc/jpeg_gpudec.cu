@@ -20,36 +20,76 @@ namespace b200 {
 using namespace gd;
 
 // ---- un-stuffing: drop the 0x00 that follows every 0xFF -----------------------------------------------------------------
-__global__ void k_gd_unstuff_count(const DecImage *__restrict__ imgs, const uint8_t *__restrict__ raw_all, uint32_t *__restrict__ cnt, uint32_t *__restrict__ marker)
+// One thread per 16-byte group of the entropy-coded segment, read with one 16-byte load (the raw buffer of every image starts
+// 16-byte aligned and has at least 16 bytes of slack behind it, so the last group's load stays inside the buffer).
+constexpr int UNSTUFF_THREADS = 128;
+__device__ __forceinline__ uint32_t group_byte(const uint4 &q, int t) { const uint32_t w = t < 4 ? q.x : t < 8 ? q.y : t < 12 ? q.z : q.w; return (w >> (8 * (t & 3))) & 0xFFu; }
+
+__global__ void __launch_bounds__(UNSTUFF_THREADS) k_gd_unstuff_count(const DecImage *__restrict__ imgs, const uint8_t *__restrict__ raw_all, uint32_t *__restrict__ cnt, uint32_t *__restrict__ marker)
 {
     const DecImage &im = imgs[blockIdx.y];
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= im.ngrp) return;
     const uint8_t *raw = raw_all + im.raw_off;
+    const uint4 q = reinterpret_cast<const uint4 *>(raw)[g];
+    const uint32_t j0 = g * 16, n = im.nraw - j0 < 16 ? im.nraw - j0 : 16;
+    uint32_t prev = g ? raw[j0 - 1] : 0u;                                       // (byte 0 of the segment is never a stuffed zero)
+    const uint32_t after = j0 + 16 < im.nraw ? raw[j0 + 16] : 0u;
     uint32_t c = 0; bool mark = false;
-    for (uint32_t j = g * 16; j < g * 16 + 16 && j < im.nraw; j++) {
-        c += (j > 0 && raw[j] == 0 && raw[j - 1] == 0xFF);
-        // an 0xFF followed by anything but the stuffed zero is a marker (RSTn, DNL, a second image's EOI ...) or fill: not ours
-        mark |= im.verify && raw[j] == 0xFF && j + 1 < im.nraw && raw[j + 1] != 0x00;
+#pragma unroll
+    for (int t = 0; t < 16; t++) {
+        const uint32_t b = group_byte(q, t), next = t < 15 ? group_byte(q, t + 1) : after;
+        if ((uint32_t)t < n) {
+            c += b == 0 && prev == 0xFF;
+            // an 0xFF followed by anything but the stuffed zero is a marker (RSTn, DNL, a second image's EOI ...) or fill: not ours
+            mark |= im.verify && b == 0xFF && j0 + t + 1 < im.nraw && next != 0x00;
+        }
+        prev = b;
     }
     cnt[im.grp_off + g] = c;
     if (mark) marker[blockIdx.y] = 1;
 }
+// A CTA's groups un-stuff into one contiguous range of the output: the bytes are compacted in shared memory, at the output's
+// word alignment, and leave as aligned 4-byte stores, coalesced across the CTA; only the up to three bytes at either end of the
+// range, whose words the neighbouring CTAs share, leave one by one.
 // (for images the host did not walk, the thread of the last group also publishes the true stream length: g.nbits and g.nsub in
 // the device copy of the descriptor were upper bounds taken from the raw length)
-__global__ void k_gd_unstuff_scatter(DecImage *imgs, const uint8_t *__restrict__ raw_all, const uint32_t *__restrict__ off, const uint32_t *__restrict__ cnt, uint8_t *__restrict__ stream_all)
+__global__ void __launch_bounds__(UNSTUFF_THREADS) k_gd_unstuff_scatter(DecImage *imgs, const uint8_t *__restrict__ raw_all, const uint32_t *__restrict__ off, const uint32_t *__restrict__ cnt, uint8_t *__restrict__ stream_all)
 {
+    __shared__ uint32_t sbuf[UNSTUFF_THREADS * 4 + 1];
+    __shared__ uint32_t range_end;
     DecImage &im = imgs[blockIdx.y];
-    const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
-    if (g >= im.ngrp) return;
+    const uint32_t g0 = blockIdx.x * blockDim.x, g = g0 + threadIdx.x;
+    if (g0 >= im.ngrp) return;
     const uint8_t *raw = raw_all + im.raw_off;
     uint8_t *out = stream_all + im.stream_off;
-    uint32_t o = g * 16 - (off[im.grp_off + g] - off[im.grp_off]);
-    for (uint32_t j = g * 16; j < g * 16 + 16 && j < im.nraw; j++) { if (j > 0 && raw[j] == 0 && raw[j - 1] == 0xFF) continue; out[o++] = raw[j]; }
+    uint8_t *sb = reinterpret_cast<uint8_t *>(sbuf);
+    const uint32_t base = off[im.grp_off];
+    const uint32_t first = g0 * 16 - (off[im.grp_off + g0] - base), aligned = first & ~3u;     // the CTA's first output byte
+    if (g < im.ngrp) {
+        const uint4 q = reinterpret_cast<const uint4 *>(raw)[g];
+        const uint32_t j0 = g * 16, n = im.nraw - j0 < 16 ? im.nraw - j0 : 16;
+        uint32_t prev = g ? raw[j0 - 1] : 0u;
+        uint32_t o = j0 - (off[im.grp_off + g] - base);
+#pragma unroll
+        for (int t = 0; t < 16; t++) {
+            const uint32_t b = group_byte(q, t);
+            if ((uint32_t)t < n && !(b == 0 && prev == 0xFF)) sb[o++ - aligned] = (uint8_t)b;
+            prev = b;
+        }
+        if (g == g0 + blockDim.x - 1 || g == im.ngrp - 1) range_end = o;
+    }
+    __syncthreads();
+    const uint32_t end = range_end;
+    for (uint32_t a = aligned + 4 * threadIdx.x; a < end; a += 4 * blockDim.x) {
+        const uint32_t w = sbuf[(a - aligned) >> 2];
+        if (a >= first && a + 4 <= end) *reinterpret_cast<uint32_t *>(out + a) = w;
+        else for (uint32_t t = 0; t < 4; t++) if (a + t >= first && a + t < end) out[a + t] = (uint8_t)(w >> (8 * t));
+    }
     if (g == im.ngrp - 1) {
         uint32_t ns = im.g.nbits >> 3;
         if (im.verify) {
-            ns = im.nraw - (off[im.grp_off + g] - off[im.grp_off] + cnt[im.grp_off + g]);
+            ns = im.nraw - (off[im.grp_off + g] - base + cnt[im.grp_off + g]);
             im.g.nbits = ns * 8; im.g.nsub = (ns * 8 + im.g.subseq_bits - 1) / im.g.subseq_bits;
         }
         for (uint32_t j = ns; j < ((ns + 3) & ~3u) + 16; j++) out[j] = 0xFF;          // pad: peek32 reads whole words past the end
@@ -339,13 +379,13 @@ bool GpuDecoder::enqueue(void *stream_, std::string &err)
     CU(cudaMemsetAsync(dF, 0, (o_mark - o_flag) + (size_t)4 * N, st));                 // round flags + marker flags
     LT_MARK("memset");
     // ---- unstuff
-    const dim3 gg(cdiv((long long)hw_mgrp, 128), N);
-    k_gd_unstuff_count<<<gg, 128, 0, st>>>(dI, d_raw, d_cnt, dM);
+    const dim3 gg(cdiv((long long)hw_mgrp, UNSTUFF_THREADS), N);
+    k_gd_unstuff_count<<<gg, UNSTUFF_THREADS, 0, st>>>(dI, d_raw, d_cnt, dM);
     LT_MARK("k_gd_unstuff_count");
     size_t tb = d_temp.capacity();
     cub::DeviceScan::ExclusiveSum(d_temp, tb, d_cnt.get(), d_off.get(), (int)hw_grp, st);
     LT_MARK("cub_scan");
-    k_gd_unstuff_scatter<<<gg, 128, 0, st>>>(dIw, d_raw, d_off, d_cnt, d_stream);
+    k_gd_unstuff_scatter<<<gg, UNSTUFF_THREADS, 0, st>>>(dIw, d_raw, d_off, d_cnt, d_stream);
     LT_MARK("k_gd_unstuff_scatter");
     for (int n = 0; n < N; n++) if (coef_bytes[n]) CU(cudaMemsetAsync(coef_ptrs[n], 0, coef_bytes[n], st));      // padding blocks only
     // ---- rounds
