@@ -54,12 +54,13 @@ bool plan_image(const JpegGeom &gin, const JpegGeom &gout, ImagePlan &p, std::st
 
 void append_image_work(const JpegGeom &gin, const JpegGeom &gout, const ImagePlan &plan,
                        const int16_t *d_in, int16_t *d_out, uint8_t *d_scratch,
-                       const uint16_t *d_dq, const QuantDev *d_q, WorkLists &wl)
+                       const uint16_t *d_dq, const QuantDev *d_q, WorkLists &wl, const GpuDecoder::DcSums *dc)
 {
     for (int c = 0; c < gin.ncomp; c++) {
         CompWork w; memset(&w, 0, sizeof(w));
         w.cin = d_in + gin.comp_offset[c]; w.cout = d_out + gout.comp_offset[c];
         w.dq = d_dq + 64 * c; w.q = d_q + gout.tq[c];
+        if (dc && dc[c].sum) { w.dc_sum = dc[c].sum; w.dc_prev = dc[c].prev; w.dc_hs = dc[c].hs; w.dc_vs = dc[c].vs; w.dc_mcux = dc[c].mcux; }
         w.bw_in = gin.bw[c]; w.bh_in = gin.bh[c]; w.rbw_in = gin.rbw[c]; w.rbh_in = gin.rbh[c]; w.cw = gin.cw[c]; w.ch = gin.ch[c];
         w.bw_out = gout.bw[c]; w.bh_out = gout.bh[c]; w.rbw_out = gout.rbw[c]; w.rbh_out = gout.rbh[c];
         w.W = gin.width; w.H = gin.height;
@@ -293,8 +294,9 @@ static const uint16_t *put_dequant(Slot *s, int k, const JpegGeom &gin)
 
 // Quantiser constants, per-image dequantisation tables and the work descriptors of the K images of L into the slot's pinned
 // parameter block.  wl receives the work lists, par_bytes the size of the block, work_off the offset of the descriptors.
-static bool fill_transform_params(Slot *s, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, bool trellis, WorkLists &wl,
-                                  size_t &par_bytes, size_t &work_off, std::string &err)
+// dec: the decoder that decoded the K images of a megabatch (their DC from its prefix sums when it deferred the DC), or null
+static bool fill_transform_params(Slot *s, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, bool trellis, const GpuDecoder *dec,
+                                  WorkLists &wl, size_t &par_bytes, size_t &work_off, std::string &err)
 {
     put_quant(s, gout);
     wl.clear();
@@ -302,8 +304,10 @@ static bool fill_transform_params(Slot *s, const JpegGeom *const *gins, const Jp
         const JpegGeom &gin = *gins[k];
         ImagePlan plan;
         if (!plan_image(gin, gout, plan, err)) return false;
+        GpuDecoder::DcSums dc[4];
+        for (int c = 0; c < 4; c++) dc[c] = dec ? dec->dc_sums(k, c) : GpuDecoder::DcSums{nullptr, nullptr, 1, 1, 1};
         append_image_work(gin, gout, plan, L.coefs(*s, k, true), L.coefs(*s, k, false), s->d_scratch + L.scratch_stride * k,
-                          put_dequant(s, k, gin), dev_quant(s), wl);
+                          put_dequant(s, k, gin), dev_quant(s), wl, dc);
     }
     work_off = par_work_off(L.K);
     if (!trellis) { par_bytes = work_off + flatten_work(wl, reinterpret_cast<CompWork *>(s->h_par + work_off)) * sizeof(CompWork); return true; }
@@ -324,7 +328,7 @@ bool slot_transform(Slot *s, const JpegGeom &gin, const JpegGeom &gout, std::str
     GroupLayout L; L.K = 1;
     const JpegGeom *gins = &gin;
     WorkLists wl; size_t pbytes = 0, work_off = 0;
-    if (!fill_transform_params(s, &gins, gout, L, jpeg_trellis(), wl, pbytes, work_off, err)) return false;
+    if (!fill_transform_params(s, &gins, gout, L, jpeg_trellis(), nullptr, wl, pbytes, work_off, err)) return false;
     CU(cudaMemcpyAsync(s->d_par, s->h_par, pbytes, cudaMemcpyHostToDevice, st));
     if (upload) CU(cudaMemcpyAsync(s->d_in, s->h_in, plan.in_bytes, cudaMemcpyHostToDevice, st));
     const int rc = launch_work(wl, reinterpret_cast<const CompWork *>(s->d_par + work_off), st);
@@ -351,7 +355,7 @@ bool slot_group_layout(Slot *s, const JpegGeom &gin, const JpegGeom &gout, int K
 // host half: the parameter block into the slot's pinned memory, the work lists into s->group_wl
 bool slot_transform_group_prepare(Slot *s, const JpegGeom *const *gins, const JpegGeom &gout, const GroupLayout &L, bool trellis, std::string &err)
 {
-    return fill_transform_params(s, gins, gout, L, trellis, s->group_wl, s->group_par_bytes, s->group_work_off, err);
+    return fill_transform_params(s, gins, gout, L, trellis, s->dec.get(), s->group_wl, s->group_par_bytes, s->group_work_off, err);
 }
 // stream half: parameter block up, the transform kernels
 bool slot_transform_group_enqueue(Slot *s, std::string &err)
@@ -422,6 +426,7 @@ bool slot_run_group(Slot *s, std::vector<GpuDecoder::Item> &items, const JpegGeo
     cudaStream_t st = (cudaStream_t)s->stream;
     const auto t0 = std::chrono::steady_clock::now();
     // ---- host half of all three stages (pinned staging, descriptors, plans); nothing touches the stream yet
+    for (GpuDecoder::Item &it : items) it.defer_dc = !lossless;       // the transform adds the DC; --lossless encodes the blocks as decoded
     if (!s->decoder()->prepare(items, st, err)) return false;
     if (!lossless && !slot_transform_group_prepare(s, gins, gout, L, jpeg_trellis(), err)) return false;
     std::vector<int16_t *> bases((size_t)L.K);

@@ -39,7 +39,7 @@ struct WorkLists {
 // Append one image's work.  d_dq: device uint16[4][64] (per input component, zigzag); d_q: device QuantDev[4] (per output slot).
 void append_image_work(const JpegGeom &gin, const JpegGeom &gout, const ImagePlan &plan,
                        const int16_t *d_in, int16_t *d_out, uint8_t *d_scratch,
-                       const uint16_t *d_dq, const QuantDev *d_q, WorkLists &wl);
+                       const uint16_t *d_dq, const QuantDev *d_q, WorkLists &wl, const GpuDecoder::DcSums *dc = nullptr);   // dc[c]: see CompWork::dc_sum
 // Copy lists into `h_work` (contiguous, order fused|idct|c420|up|down|fdct|trel); returns count.
 size_t flatten_work(const WorkLists &wl, CompWork *h_work);
 // Launch every non-empty list; d_work is the device copy of the flattened array.

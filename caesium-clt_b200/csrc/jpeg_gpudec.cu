@@ -3,7 +3,7 @@
 // Batched: every pass is one launch for all images of the batch (blockIdx.y = image), which is what keeps the launch
 // count per image low when b200_compress_batch packs images into megabatches.
 // Pass order: unstuff (count, scan, scatter) -> round 0 -> rounds (in groups, one host check per group) -> block-count
-// scan -> write (coefficients and DC differences) -> DC scan / scatter.  Coefficients land directly in the transform kernels' input buffers, so the
+// scan -> write (coefficients and DC differences) -> DC scan / scatter (no scatter when the batch defers the DC to the transform).  Coefficients land directly in the transform kernels' input buffers, so the
 // host never sees them.
 #include <cuda_runtime.h>
 #include <cub/device/device_scan.cuh>
@@ -269,6 +269,8 @@ bool GpuDecoder::prepare(std::vector<Item> &items, void *stream_, std::string &e
     // ---- per-image descriptors
     imgs.assign((size_t)N, DecImage());
     coef_ptrs.resize((size_t)N); coef_bytes.resize((size_t)N);
+    defer_dc = items[0].defer_dc;
+    for (const Item &it : items) if (it.defer_dc != defer_dc) { err = "a decode batch takes one DC setting"; return false; }
     raw_total = 0; size_t stream_total = 0; grp_total = 0; sub_total = 0; blk_total = 0; max_grp = 0; max_sub = 0; max_blk = 0;
     for (int n = 0; n < N; n++) {
         const JpegReader &rd = *items[n].rd; const JpegReader::DeviceScan &ds = *items[n].ds; const JpegGeom &g = rd.geom();
@@ -360,7 +362,7 @@ unsigned long long GpuDecoder::signature() const
     unsigned long long h = 1469598103934665603ull;
     auto mix = [&](unsigned long long v) { h = (h ^ v) * 1099511628211ull; };
     mix((unsigned long long)nitems); mix(hw_raw); mix(hw_grp); mix(hw_sub); mix(hw_blk); mix(hw_mgrp); mix(hw_msub); mix(hw_mblk); mix(generation);
-    mix(o_flag); mix(o_mark);
+    mix(o_flag); mix(o_mark); mix(defer_dc);
     for (size_t n = 0; n < coef_ptrs.size(); n++) { mix((unsigned long long)(uintptr_t)coef_ptrs[n]); mix(coef_bytes[n]); }
     return h;
 }
@@ -415,11 +417,33 @@ bool GpuDecoder::enqueue(void *stream_, std::string &err)
     tb = d_temp.capacity();
     cub::DeviceScan::InclusiveSum(d_temp, tb, d_dc.get(), d_dcs.get(), (int)hw_blk, st);
     LT_MARK("cub_scan");
-    k_gd_dc_scatter<<<gb, 128, 0, st>>>(dI, d_dcs);
-    LT_MARK("k_gd_dc_scatter");
+    if (!defer_dc) {
+        k_gd_dc_scatter<<<gb, 128, 0, st>>>(dI, d_dcs);
+        LT_MARK("k_gd_dc_scatter");
+    }
     CU(cudaGetLastError());
-    launches = 9 + nrounds;
+    launches = (defer_dc ? 8 : 9) + nrounds;
     return true;
+}
+
+GpuDecoder::DcSums GpuDecoder::dc_sums(int n, int c) const
+{   // the component-major layout of dc_slot_index: a component's blocks in MCU order, hs * vs of them per MCU
+    DcSums d{nullptr, nullptr, 1, 1, 1};
+    if (!defer_dc || n < 0 || n >= nitems) return d;
+    const DecImage &im = imgs[(size_t)n];
+    const ge::Scan &s = im.scan;
+    uint32_t start = 0;
+    for (int i = 0; i < s.ns; i++) {
+        const int hs = s.ns == 1 ? 1 : s.hs[i], vs = s.ns == 1 ? 1 : s.vs[i];
+        if (s.comp[i] == c) {
+            const uint32_t b = im.blk_off + start;
+            d.sum = d_dcs.get() + b; d.prev = b ? d_dcs.get() + b - 1 : nullptr;
+            d.hs = hs; d.vs = vs; d.mcux = s.ns == 1 ? s.rbw : s.mcux;
+            return d;
+        }
+        start += (uint32_t)s.mcux * (uint32_t)s.mcuy * (uint32_t)(hs * vs);
+    }
+    return d;
 }
 
 void GpuDecoder::finish(std::vector<Item> &items)

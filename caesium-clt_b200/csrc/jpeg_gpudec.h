@@ -30,7 +30,9 @@ public:
     GpuDecoder(const GpuDecoder &) = delete;
     GpuDecoder &operator=(const GpuDecoder &) = delete;
     enum Result { OK = 0, NOT_CONVERGED = 1, FAILED = 2 };
-    struct Item { const JpegReader *rd; const JpegReader::DeviceScan *ds; int16_t *d_coefs; Result result; };
+    // defer_dc: leave each block's DC difference in the block and skip the DC scatter; whoever reads the blocks adds the prefix
+    // sum from dc_sums() instead (the transform kernels do, CompWork::dc_sum).  One setting per batch.
+    struct Item { const JpegReader *rd; const JpegReader::DeviceScan *ds; int16_t *d_coefs; Result result; bool defer_dc = false; };
     // Decode every item's scan straight into its d_coefs (device; fully overwritten, whatever it held before).  Per item: OK, or NOT_CONVERGED
     // (the self-synchronisation did not settle within the round budget -- degenerate periodic streams -- or the stream is
     // damaged: a marker inside it, an invalid code, a run past index 63 or an end before the last block; the caller
@@ -46,6 +48,11 @@ public:
     // arguments (sizes are high-water marks), i.e. a captured CUDA graph of them can be replayed
     unsigned long long signature() const;
     void finish(std::vector<Item> &items);
+    // Where the final DC of item n's frame component c comes from after enqueue() of a defer_dc batch: the DC of the block at
+    // (bx, by) of the component is sum[slot] - (prev ? *prev : 0), slot = ((by / vs) * mcux + bx / hs) * hs * vs + (by % vs) * hs +
+    // bx % hs.  sum = null when the batch does not defer the DC (the blocks hold it) or c is not in the scan.
+    struct DcSums { const int32_t *sum, *prev; int hs, vs, mcux; };
+    DcSums dc_sums(int n, int c) const;
     size_t raw_bytes() const { return raw_total; }          // entropy-coded bytes staged by the last prepare()
     int rounds_used = 0, launches = 0;
     // subsequence size: swept 512 .. 8192 on the 4K bench set under full batch load (tools/throughput.py): 512 -> 3,400
@@ -54,7 +61,7 @@ public:
     // one leaves at once: ~2 us); the 4K bench set settles in <= 14.  An image that needs more is decoded on the host.
     static constexpr int SUBSEQ_BITS = 2048, ROUNDS = 24, MAX_ROUNDS = 64;
 private:
-    int nitems = 0;
+    int nitems = 0; bool defer_dc = false;
     std::vector<DecImage> imgs; std::vector<int16_t *> coef_ptrs; std::vector<size_t> coef_bytes; std::vector<char> tables_ok;
     size_t raw_total = 0, o_img = 0, o_tab = 0, o_flag = 0, o_mark = 0, par_bytes = 0;
     size_t hw_raw = 0, hw_stream = 0, hw_grp = 0, hw_sub = 0, hw_blk = 0, hw_mgrp = 0, hw_msub = 0, hw_mblk = 0; int hw_n = 0;

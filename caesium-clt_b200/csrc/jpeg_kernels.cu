@@ -175,6 +175,16 @@ __device__ __forceinline__ void warp_store_blocks(int4 *__restrict__ g, int nval
     __syncwarp();
 }
 
+// A block read from a deferred-DC decode (w.dc_sum set) carries its DC difference: put the DC from the decoder's prefix sums in its
+// place (the low half of the first word, truncated to int16 as the DC scatter would store it).  bx, by: the block in the component.
+__device__ __forceinline__ void put_dc(const CompWork &w, int bx, int by, int4 (&r)[8])
+{
+    const int mx = bx / w.dc_hs, my = by / w.dc_vs;
+    const int slot = (my * w.dc_mcux + mx) * (w.dc_hs * w.dc_vs) + (by - my * w.dc_vs) * w.dc_hs + (bx - mx * w.dc_hs);
+    const int dc = __ldg(w.dc_sum + slot) - (w.dc_prev ? __ldg(w.dc_prev) : 0);
+    r[0].x = (int)(((uint32_t)r[0].x & 0xFFFF0000u) | ((uint32_t)dc & 0xFFFFu));
+}
+
 // zigzag quantised int16 block (8 x int4) -> dequantised natural-order ints
 __device__ __forceinline__ void dequant_dezigzag(const int4 (&r)[8], const Tables &t, int (&v)[64])
 {
@@ -254,6 +264,7 @@ __global__ void __launch_bounds__(THREADS, 2) k_fused_same(const CompWork *__res
     int4 *st = stage + (threadIdx.x >> 5) * STAGE_INT4_PER_WARP;
     int4 r[8];
     warp_load_blocks(reinterpret_cast<const int4 *>(w.cin) + ((size_t)t.by * w.bw_in + t.bx0) * 8, t.nvalid, st, lane, r);
+    if (w.dc_sum && lane < t.nvalid) put_dc(w, t.bx0 + lane, t.by, r);
     int v[64];
     dequant_dezigzag(r, tab, v);
     idct_block(v);
@@ -291,6 +302,7 @@ __global__ void __launch_bounds__(THREADS) k_idct_plane(const CompWork *__restri
     int4 r[8];
     warp_load_blocks(reinterpret_cast<const int4 *>(w.cin) + ((size_t)t.by * w.bw_in + t.bx0) * 8, t.nvalid, stage + (threadIdx.x >> 5) * STAGE_INT4_PER_WARP, lane, r);
     if (lane >= t.nvalid) return;
+    if (w.dc_sum) put_dc(w, t.bx0 + lane, t.by, r);
     int v[64];
     dequant_dezigzag(r, tab, v);
     idct_block(v);

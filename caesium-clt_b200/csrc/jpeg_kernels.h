@@ -77,6 +77,10 @@ struct CompWork {
     int32_t pstride, fstride;
     int32_t up_hx, up_vx;   // decoder upsampling ratio  (hmax/hs, vmax/vs of the input)
     int32_t dn_hx, dn_vx;   // encoder downsampling ratio (hmax/hs, vmax/vs of the output)
+    // dc_sum != null: the input blocks hold their DC DIFFERENCE (GpuDecoder::Item::defer_dc); the DC of block (bx, by) is
+    // dc_sum[slot] - (dc_prev ? *dc_prev : 0), slot as GpuDecoder::DcSums says
+    const int32_t *dc_sum, *dc_prev;
+    int32_t dc_hs, dc_vs, dc_mcux;
 };
 
 inline int work_tiles(int rbw, int rbh) { return ((rbw + 31) / 32) * rbh; }   // row-aligned tiles of 32 blocks

@@ -84,7 +84,7 @@ JpegPipe *pipe_create(const uint8_t *const *in, const size_t *in_len, int n, con
             const int i = i0 + m;
             G->members.push_back(i);
             G->items[m].rd = P->rd[i].get(); G->items[m].ds = &P->ds[i]; G->items[m].result = GpuDecoder::FAILED;
-            G->items[m].d_coefs = G->L.coefs(G->slot, m, true);
+            G->items[m].d_coefs = G->L.coefs(G->slot, m, true); G->items[m].defer_dc = !P->lossless;
             G->gins[m] = &P->rd[i]->geom();
             G->bases[m] = G->L.coefs(G->slot, m, P->lossless);
             raw += P->ds[i].ecs_end - P->ds[i].ecs_begin;
