@@ -354,6 +354,12 @@ b200_status jpeg_compress(const uint8_t *in, size_t in_len, const b200_params *p
     return ok_status();
 }
 
+// Megabatch members that jpeg_compress_group leaves to the per-image path (the device decoder did not settle them: a marker inside
+// the scan, a damaged or periodic stream; or the group could not run).  Such a member still comes out right, only slower, so the
+// count is the one place a clean file wrongly refused by the device decoder shows.  B200_TRACE prints it at exit.
+std::atomic<long> g_mb_members{0}, g_mb_rescued{0};
+struct MbReport { ~MbReport() { if (getenv("B200_TRACE") && g_mb_members.load()) fprintf(stderr, "[b200 trace] megabatch: %ld members, %ld left to the per-image path\n", g_mb_members.load(), g_mb_rescued.load()); } } g_mb_report;
+
 // One megabatch: the images idx[] that are baseline single-scan JPEGs of one shape are decoded, transformed and encoded by
 // ONE sequence of kernel launches on one slot.  done[k] = 1 for every image this function finished (successfully or with
 // a final error in status[]); the caller runs the others through the per-image path.
@@ -375,6 +381,10 @@ void jpeg_compress_group(const uint8_t *const *in, const size_t *in_len, const s
         members.push_back(k);
     }
     if (members.size() < 2) return;
+    struct Tally {          // on every way out: the members not finished here
+        const std::vector<int> &members; const std::vector<char> &done;
+        ~Tally() { long n = 0; for (int k : members) n += !done[k]; g_mb_members += (long)members.size(); g_mb_rescued += n; }
+    } tally{members, done};
     const JpegGeom &gin0 = rd[members[0]]->geom();
     const bool lossless = p->jpeg_optimize != 0;          // jpeg::lossless: decode -> encode, no transform, per-image tables kept
     JpegGeom gout;

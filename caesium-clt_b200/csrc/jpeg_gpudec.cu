@@ -21,9 +21,10 @@ using namespace gd;
 
 // ---- un-stuffing: drop the 0x00 that follows every 0xFF -----------------------------------------------------------------
 // One thread per 16-byte group of the entropy-coded segment, read with one 16-byte load (the raw buffer of every image starts
-// 16-byte aligned and has at least 16 bytes of slack behind it, so the last group's load stays inside the buffer).
+// 16-byte aligned and has at least 16 bytes of slack behind it, so the last group's load stays inside the buffer).  The
+// per-thread bodies are gd::unstuff_count_group / unstuff_place_group / unstuff_store (jpeg_gpudec_core.h).
 constexpr int UNSTUFF_THREADS = 128;
-__device__ __forceinline__ uint32_t group_byte(const uint4 &q, int t) { const uint32_t w = t < 4 ? q.x : t < 8 ? q.y : t < 12 ? q.z : q.w; return (w >> (8 * (t & 3))) & 0xFFu; }
+__device__ __forceinline__ RawGroup load_group(const uint8_t *raw, uint32_t g) { const uint4 q = reinterpret_cast<const uint4 *>(raw)[g]; return RawGroup{q.x, q.y, q.z, q.w}; }
 
 __global__ void __launch_bounds__(UNSTUFF_THREADS) k_gd_unstuff_count(const DecImage *__restrict__ imgs, const uint8_t *__restrict__ raw_all, uint32_t *__restrict__ cnt, uint32_t *__restrict__ marker)
 {
@@ -31,22 +32,8 @@ __global__ void __launch_bounds__(UNSTUFF_THREADS) k_gd_unstuff_count(const DecI
     const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= im.ngrp) return;
     const uint8_t *raw = raw_all + im.raw_off;
-    const uint4 q = reinterpret_cast<const uint4 *>(raw)[g];
-    const uint32_t j0 = g * 16, n = im.nraw - j0 < 16 ? im.nraw - j0 : 16;
-    uint32_t prev = g ? raw[j0 - 1] : 0u;                                       // (byte 0 of the segment is never a stuffed zero)
-    const uint32_t after = j0 + 16 < im.nraw ? raw[j0 + 16] : 0u;
-    uint32_t c = 0; bool mark = false;
-#pragma unroll
-    for (int t = 0; t < 16; t++) {
-        const uint32_t b = group_byte(q, t), next = t < 15 ? group_byte(q, t + 1) : after;
-        if ((uint32_t)t < n) {
-            c += b == 0 && prev == 0xFF;
-            // an 0xFF followed by anything but the stuffed zero is a marker (RSTn, DNL, a second image's EOI ...) or fill: not ours
-            mark |= im.verify && b == 0xFF && j0 + t + 1 < im.nraw && next != 0x00;
-        }
-        prev = b;
-    }
-    cnt[im.grp_off + g] = c;
+    bool mark;
+    cnt[im.grp_off + g] = unstuff_count_group(raw, load_group(raw, g), g, im.nraw, im.verify, &mark);
     if (mark) marker[blockIdx.y] = 1;
 }
 // A CTA's groups un-stuff into one contiguous range of the output: the bytes are compacted in shared memory, at the output's
@@ -67,33 +54,12 @@ __global__ void __launch_bounds__(UNSTUFF_THREADS) k_gd_unstuff_scatter(DecImage
     const uint32_t base = off[im.grp_off];
     const uint32_t first = g0 * 16 - (off[im.grp_off + g0] - base), aligned = first & ~3u;     // the CTA's first output byte
     if (g < im.ngrp) {
-        const uint4 q = reinterpret_cast<const uint4 *>(raw)[g];
-        const uint32_t j0 = g * 16, n = im.nraw - j0 < 16 ? im.nraw - j0 : 16;
-        uint32_t prev = g ? raw[j0 - 1] : 0u;
-        uint32_t o = j0 - (off[im.grp_off + g] - base);
-#pragma unroll
-        for (int t = 0; t < 16; t++) {
-            const uint32_t b = group_byte(q, t);
-            if ((uint32_t)t < n && !(b == 0 && prev == 0xFF)) sb[o++ - aligned] = (uint8_t)b;
-            prev = b;
-        }
+        const uint32_t o = unstuff_place_group(raw, load_group(raw, g), g, im.nraw, g * 16 - (off[im.grp_off + g] - base), aligned, sb);
         if (g == g0 + blockDim.x - 1 || g == im.ngrp - 1) range_end = o;
     }
     __syncthreads();
     const uint32_t end = range_end;
-    for (uint32_t a = aligned + 4 * threadIdx.x; a < end; a += 4 * blockDim.x) {
-        const uint32_t w = sbuf[(a - aligned) >> 2];
-        if (a >= first && a + 4 <= end) *reinterpret_cast<uint32_t *>(out + a) = w;
-        else for (uint32_t t = 0; t < 4; t++) if (a + t >= first && a + t < end) out[a + t] = (uint8_t)(w >> (8 * t));
-    }
-    if (g == im.ngrp - 1) {
-        uint32_t ns = im.g.nbits >> 3;
-        if (im.verify) {
-            ns = im.nraw - (off[im.grp_off + g] - base + cnt[im.grp_off + g]);
-            im.g.nbits = ns * 8; im.g.nsub = (ns * 8 + im.g.subseq_bits - 1) / im.g.subseq_bits;
-        }
-        for (uint32_t j = ns; j < ((ns + 3) & ~3u) + 16; j++) out[j] = 0xFF;          // pad: peek32 reads whole words past the end
-    }
+    unstuff_store(sbuf, aligned, first, end, threadIdx.x, blockDim.x, out, g == im.ngrp - 1, im.verify, im.nraw, off + (im.grp_off + g), cnt + (im.grp_off + g), base, im.g);
 }
 
 // ---- synchronisation rounds ------------------------------------------------------------------------------------------------

@@ -310,6 +310,79 @@ GE_HD void decode_owned_blocks(const uint8_t *__restrict__ stream, const Geometr
 
 struct NullSink { uint32_t nblk = 0; GE_HD void coef(int, int) {} GE_HD void block_done() { nblk++; } };
 
+// ---- un-stuffing: drop the 0x00 that follows every 0xFF ---------------------------------------------------------------------
+// The per-thread bodies of k_gd_unstuff_count / k_gd_unstuff_scatter (jpeg_gpudec.cu), shared with the CPU emulation.  Thread g
+// owns the 16-byte group g of an entropy-coded segment of nraw bytes; q holds that group as it was read, four little-endian
+// words (the bytes past nraw are the raw buffer's slack: read, never used).
+struct RawGroup { uint32_t x, y, z, w; };
+GE_HD uint32_t group_byte(const RawGroup &q, int t) { const uint32_t w = t < 4 ? q.x : t < 8 ? q.y : t < 12 ? q.z : q.w; return (w >> (8 * (t & 3))) & 0xFFu; }
+
+// Stuffed zeros in group g; *mark |= the group holds an 0xFF followed by anything but the stuffed zero (checked with `verify`
+// only; taken by reference so that the kernel reads the descriptor's flag where an 0xFF needs it, as it did before this body
+// moved here).  The byte before the group (raw[16 g - 1]) decides whether its first byte is a stuffed zero.
+GE_HD uint32_t unstuff_count_group(const uint8_t *raw, const RawGroup &q, uint32_t g, uint32_t nraw, const uint32_t &verify, bool *mark)
+{
+    const uint32_t j0 = g * 16, n = nraw - j0 < 16 ? nraw - j0 : 16;
+    uint32_t prev = g ? raw[j0 - 1] : 0u;                                       // (byte 0 of the segment is never a stuffed zero)
+    const uint32_t after = j0 + 16 < nraw ? raw[j0 + 16] : 0u;
+    uint32_t c = 0; bool m = false;
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+    for (int t = 0; t < 16; t++) {
+        const uint32_t b = group_byte(q, t), next = t < 15 ? group_byte(q, t + 1) : after;
+        if ((uint32_t)t < n) {
+            c += b == 0 && prev == 0xFF;
+            // an 0xFF followed by anything but the stuffed zero is a marker (RSTn, DNL, a second image's EOI ...) or fill: not ours
+            m |= verify && b == 0xFF && j0 + t + 1 < nraw && next != 0x00;
+        }
+        prev = b;
+    }
+    *mark = m;
+    return c;
+}
+
+// Place group g's kept bytes at output positions o, o + 1, ... (o = 16 g - stuffed zeros before the group) into the CTA's byte
+// buffer sb, which holds the output from position `aligned` on.  Returns the output position after the group.
+GE_HD uint32_t unstuff_place_group(const uint8_t *raw, const RawGroup &q, uint32_t g, uint32_t nraw, uint32_t o, uint32_t aligned, uint8_t *sb)
+{
+    const uint32_t j0 = g * 16, n = nraw - j0 < 16 ? nraw - j0 : 16;
+    uint32_t prev = g ? raw[j0 - 1] : 0u;
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+    for (int t = 0; t < 16; t++) {
+        const uint32_t b = group_byte(q, t);
+        if ((uint32_t)t < n && !(b == 0 && prev == 0xFF)) sb[o++ - aligned] = (uint8_t)b;
+        prev = b;
+    }
+    return o;
+}
+
+// Thread `tid` of `nthreads` stores the CTA's output range [first, end) from the word buffer sbuf (word i = output bytes
+// aligned + 4 i .. + 3, aligned = first & ~3): whole aligned words, except the words at either end of the range, which the
+// neighbouring CTAs share and which leave byte by byte.  The thread of the segment's last group (`last`) then finishes the
+// stream: with `verify` it replaces the upper bounds in G.nbits / G.nsub by the true length, nraw - the segment's stuffed zeros
+// (*last_off - base: stuffed zeros before the last group, *last_cnt: inside it), and it pads the stream with 0xFF to a word boundary and
+// 16 bytes further, since the decoder's peek32 reads whole words past the end.
+GE_HD void unstuff_store(const uint32_t *sbuf, uint32_t aligned, uint32_t first, uint32_t end, uint32_t tid, uint32_t nthreads, uint8_t *out,
+                         bool last, bool verify, uint32_t nraw, const uint32_t *last_off, const uint32_t *last_cnt, uint32_t base, Geometry &G)
+{
+    for (uint32_t a = aligned + 4 * tid; a < end; a += 4 * nthreads) {
+        const uint32_t w = sbuf[(a - aligned) >> 2];
+        if (a >= first && a + 4 <= end) *reinterpret_cast<uint32_t *>(out + a) = w;
+        else for (uint32_t t = 0; t < 4; t++) if (a + t >= first && a + t < end) out[a + t] = (uint8_t)(w >> (8 * t));
+    }
+    if (last) {
+        uint32_t ns = G.nbits >> 3;
+        if (verify) {
+            ns = nraw - (*last_off - base + *last_cnt);
+            G.nbits = ns * 8; G.nsub = (ns * 8 + G.subseq_bits - 1) / G.subseq_bits;
+        }
+        for (uint32_t j = ns; j < ((ns + 3) & ~3u) + 16; j++) out[j] = 0xFF;
+    }
+}
+
 // jdhuff.c jpeg_make_d_derived_tbl from the DHT payload
 inline void build_dec_table(const uint8_t bits[17], const uint8_t *vals, DecTable &t)
 {
