@@ -8,6 +8,7 @@
 #include "../../include/b200_caesium_png_resize.h"
 #include "../../include/b200_caesium_webp_lossless.h"
 #include "../../include/b200_caesium_png_interlaced.h"
+#include "../../include/b200_caesium_gif_convert.h"
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -94,6 +95,7 @@ OptIn g_gif{"B200_GIF"};                                      // GIF re-encoded 
 OptIn g_png_resize{"B200_PNG_RESIZE"};                        // PNG -> PNG with width / height on the device
 OptIn g_webp_lossless_convert{"B200_WEBP_LOSSLESS_CONVERT"};  // JPEG / PNG -> lossless WebP on the device
 OptIn g_png_interlaced{"B200_PNG_INTERLACED"};                // Adam7 PNG sources on every PNG leg
+OptIn g_gif_convert{"B200_GIF_CONVERT"};                      // JPEG / PNG / WebP -> GIF and GIF -> JPEG / PNG / WebP on the device
 
 // runtime_init is idempotent while initialised, so after b200_shutdown (which frees every slot's device buffers) the next call
 // initialises again: a long-running host can hand the memory of one workload's slots back before starting another
@@ -1028,11 +1030,135 @@ b200_status rgb_to_png(const std::vector<uint8_t> &rgb, uint32_t w, uint32_t h, 
     return png_from_planes(s, src, 3, ap, nw, nh, true, p, out, err);
 }
 
+// ---- conversions to and from GIF (the switch on) ----------------------------------------------------------------------------
+// libcaesium convert with a GIF target: decode -> RGBA8 -> the gif crate's Frame::from_rgba_speed (alpha 0 stays clear, any other
+// alpha becomes 255) -> gifski.  Here the source's front end writes that canvas (gif_canvas_pixel) into the quantiser on the device,
+// and the GIF leg codes it as the one-frame file it writes for a still GIF (GifDevice::encode_canvas).  B200_TRACE=2 prints one line
+// per call with the stages; to give each stage its own time the trace waits for the device after each of them.
+b200_status gif_code_canvas(Slot *s, uint32_t w, uint32_t h, const b200_params *p, ConvertStages &tr, const char *src, const char *stage0, std::vector<uint8_t> &out)
+{
+    std::string err;
+    tr.lap(1, s->stream);
+    const int q = (int)std::min<uint32_t>(p->gif_quality, 100);
+    if (!s->gif_dev()->encode_canvas(*s->png_dev()->quantiser(), (int)w, (int)h, q, s->stream, out, err)) return make_status(B200_ERR_CUDA, err);
+    tr.lap(3, nullptr);
+    if (ConvertStages::verbose())
+        fprintf(stderr, "[b200 trace] gif-convert %s %ux%u -> gif q%d: %s %.3f ms, device front end + canvas %.3f ms, quantise + LZW + container %.3f ms\n", src, w, h, q, stage0,
+                tr.ms[0], tr.ms[1], tr.ms[3]);
+    return ok_status();
+}
+
+// JPEG -> GIF: the device decode of the lossy conversions (entropy decode, IDCT, upsampling, YCbCr -> RGB); the planes never leave HBM
+b200_status jpeg_to_gif(const uint8_t *in, size_t in_len, const b200_params *p, std::vector<uint8_t> &out)
+{
+    std::string err;
+    ConvertStages tr;
+    JpegReader rd(in, in_len);
+    uint32_t nw, nh;
+    b200_status st = jpeg_planes_target(rd, p, 65535, "invalid target dimensions", nw, nh);
+    if (st.code) return st;
+    SlotLease s(-1);
+    if (!s) return s.failure();
+    bool on_device;
+    SamplePlan sp;
+    uint8_t *full[3], *rgb[3];
+    if ((st = jpeg_planes_decode(s, rd, nw, nh, on_device, sp, full, err, [&] { tr.lap(0, s->stream); })).code) return st;
+    const int g = rd.geom().ncomp == 3;          // a grey source is its one plane three times
+    if (!resize_samples(s, full, sp, rgb, err) ||
+        !s->gif_dev()->canvas_from_planes(*s->png_dev()->quantiser(), rgb[0], rgb[g], rgb[2 * g], nullptr, (int)nw, (int)nh, s->stream, err)) return make_status(B200_ERR_CUDA, err);
+    return gif_code_canvas(s, nw, nh, p, tr, "jpeg", on_device ? "parse + device entropy decode" : "parse + host entropy decode", out);
+}
+
+// PNG -> GIF: parse and inflate as png_compress does, the device un-filter with its filter-byte and Adler-32 checks (code 4), then the
+// quantiser's expansion to RGBA8 (palette and tRNS, sub-byte greys scaled, 16-bit samples by their high byte) made a canvas in place
+b200_status png_to_gif(const uint8_t *in, size_t in_len, const b200_params *p, std::vector<uint8_t> &out)
+{
+    std::string err;
+    ConvertStages tr;
+    PngInfo info; PngIdat idat;
+    if (!png_parse_chunks(in, in_len, false, info, idat, err)) return png_status(err);
+    uint32_t nw, nh;
+    b200_status st = target_size(info.width, info.height, p, 65535, nw, nh, "invalid target dimensions");
+    if (st.code) return st;
+    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
+    SlotLease s(-1);
+    if (!s) return s.failure();
+    PngDevice *png = s->png_dev();
+    PngQuant *q = png->quantiser();
+    size_t nfilt; uint32_t stored_adler;
+    if ((st = png_inflate(png, info, idat, nfilt, stored_adler)).code) return st;
+    tr.lap(0, nullptr);
+    if (!png->unfilter(info, nfilt, stored_adler, s->stream, err) || !q->expand(png->d_raw, info, s->stream, err)) return png_device_status(png, false, err);
+    if (!s->gif_dev()->canvas_from_rgba(*q, s->stream, err)) return make_status(B200_ERR_CUDA, err);
+    return gif_code_canvas(s, nw, nh, p, tr, "png", "parse + inflate", out);
+}
+
+// WebP -> GIF: the host decoder's RGB and alpha plane, uploaded once
+b200_status webp_to_gif(const uint8_t *in, size_t in_len, const b200_params *p, std::vector<uint8_t> &out)
+{
+    std::string err;
+    ConvertStages tr;
+    WebpInfo wi; std::vector<uint8_t> rgb, alpha;
+    b200_status st = webp_decode_status(in, in_len, wi, rgb, &alpha);
+    if (st.code) return st;
+    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
+    SlotLease s(-1);
+    if (!s) return s.failure();
+    tr.lap(0, nullptr);
+    if (!s->gif_dev()->canvas_from_host(*s->png_dev()->quantiser(), rgb.data(), alpha.empty() ? nullptr : alpha.data(), wi.width, wi.height, s->stream, err))
+        return make_status(B200_ERR_CUDA, err);
+    return gif_code_canvas(s, (uint32_t)wi.width, (uint32_t)wi.height, p, tr, "webp", "host decode", out);
+}
+
+b200_status to_gif(const uint8_t *in, size_t in_len, uint32_t src, const b200_params *p, std::vector<uint8_t> &out)
+{
+    if (p->width || p->height) return make_status(B200_ERR_UNSUPPORTED, "GIF resize is outside the GPU path (route to caesium::convert_in_memory)");
+    if (src == B200_FMT_JPEG) return jpeg_to_gif(in, in_len, p, out);
+    return src == B200_FMT_PNG ? png_to_gif(in, in_len, p, out) : webp_to_gif(in, in_len, p, out);
+}
+
+// libcaesium convert on a GIF source: image::load_from_memory decodes frame 0 alone (GifReader::first_frame), then the target's
+// writer.  The frame takes the back ends of the other host-decoded sources (K3 when width / height are set): a JPEG drops the
+// alpha (to_rgb8), a PNG or WebP keeps it as an alpha plane when some pixel is clear.
+b200_status gif_to(const uint8_t *in, size_t in_len, uint32_t fmt, const b200_params *p, std::vector<uint8_t> &out)
+{
+    if (fmt == B200_FMT_JPEG && p->jpeg_optimize) return make_status(B200_ERR_UNSUPPORTED, "lossless conversion to JPEG is outside the GPU path (route to caesium::convert_in_memory)");
+    if (fmt == B200_FMT_PNG && !p->png_optimize && !g_png_lossy.on()) return make_status(B200_ERR_UNSUPPORTED, "lossy PNG (imagequant) is outside the GPU path (route to caesium::convert_in_memory)");
+    if (fmt == B200_FMT_WEBP && p->webp_lossless) return make_status(B200_ERR_UNSUPPORTED, "lossless WebP (VP8L) is outside the GPU path (route to caesium::convert_in_memory)");
+    std::string err;
+    const auto t0 = std::chrono::steady_clock::now();
+    GifReader rd;
+    std::vector<uint32_t> canvas;
+    if (!rd.first_frame(in, in_len, canvas, err)) return make_status(rd.unsupported ? B200_ERR_UNSUPPORTED : B200_ERR_CORRUPT_INPUT, err);
+    const uint32_t w = (uint32_t)rd.width, h = (uint32_t)rd.height;
+    const size_t n = (size_t)w * h;
+    std::vector<uint8_t> rgb(3 * n), alpha(n);
+    bool clear = false;
+    for (size_t i = 0; i < n; i++) {
+        const uint32_t v = canvas[i];
+        rgb[i] = (uint8_t)v; rgb[n + i] = (uint8_t)(v >> 8); rgb[2 * n + i] = (uint8_t)(v >> 16); alpha[i] = (uint8_t)(v >> 24);
+        clear |= !alpha[i];
+    }
+    const auto t1 = std::chrono::steady_clock::now();
+    const b200_status st = fmt == B200_FMT_JPEG ? planes_to_jpeg(rgb, w, h, 3, p, -1, out)
+                         : fmt == B200_FMT_PNG  ? rgb_to_png(rgb, w, h, p, -1, out, clear ? &alpha : nullptr)
+                                                : rgb_to_webp(rgb, w, h, p, -1, out, clear ? &alpha : nullptr);
+    if (!st.code && trace_level() >= 2)
+        fprintf(stderr, "[b200 trace] gif-convert gif %ux%u -> %s: frame 0 host decode %.3f ms, back end %.3f ms\n", w, h,
+                fmt == B200_FMT_JPEG ? "jpeg" : fmt == B200_FMT_PNG ? "png" : "webp", ms_between(t0, t1), ms_between(t1, std::chrono::steady_clock::now()));
+    return st;
+}
+
 // libcaesium convert_in_memory for a source of format src: the conversions this path takes, the refusals in the reference's order
 b200_status convert_dispatch(const uint8_t *in, size_t in_len, uint32_t src, uint32_t fmt, const b200_params *p, std::vector<uint8_t> &out)
 {
     if (src == B200_FMT_UNKNOWN) return make_status(B200_ERR_UNKNOWN_FORMAT, "Unknown file type");
     if (src == fmt) return make_status(B200_ERR_SAME_FORMAT, "Cannot convert to the same format");
+    if (g_gif_convert.on()) {
+        auto jpw = [](uint32_t f) { return f == B200_FMT_JPEG || f == B200_FMT_PNG || f == B200_FMT_WEBP; };
+        if (fmt == B200_FMT_GIF && jpw(src)) return to_gif(in, in_len, src, p, out);
+        if (src == B200_FMT_GIF && jpw(fmt)) return gif_to(in, in_len, fmt, p, out);
+    }
     if (fmt == B200_FMT_PNG && src == B200_FMT_JPEG) return jpeg_to_png(in, in_len, p, -1, out);
     if (src == B200_FMT_WEBP && (fmt == B200_FMT_JPEG || fmt == B200_FMT_PNG)) {
         // WebP source: decoded on the calling thread (vp8_decode.cpp), then the same back ends as a PNG source
@@ -1195,6 +1321,7 @@ int b200_set_gif(int on) { return g_gif.set(on); }
 int b200_set_png_resize(int on) { return g_png_resize.set(on); }
 int b200_set_webp_lossless_convert(int on) { return g_webp_lossless_convert.set(on); }
 int b200_set_png_interlaced(int on) { return g_png_interlaced.set(on); }
+int b200_set_gif_convert(int on) { return g_gif_convert.set(on); }
 int b200_set_jpeg_trellis(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; set_jpeg_trellis(on == 1); return B200_OK; }
 
 uint32_t b200_sniff_format(const uint8_t *d, size_t n)
@@ -1854,6 +1981,24 @@ b200_status b200_gif_decode(const uint8_t *in, size_t in_len, int *width, int *h
         s = give(bytes, rgba, &n);
         if (s.code) { free(*delays); *delays = nullptr; return s; }
         *width = rd.width; *height = rd.height; *nframes = rd.frames; *loop = rd.loop;
+        return s;
+    });
+}
+
+b200_status b200_gif_first_frame(const uint8_t *in, size_t in_len, int *width, int *height, uint8_t **rgba)
+{
+    if (!in || !width || !height || !rgba) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
+    *rgba = nullptr;
+    return guarded([&] {
+        std::string err;
+        GifReader rd;
+        std::vector<uint32_t> px;
+        if (!rd.first_frame(in, in_len, px, err)) return make_status(rd.unsupported ? B200_ERR_UNSUPPORTED : B200_ERR_CORRUPT_INPUT, err);
+        std::vector<uint8_t> bytes(px.size() * 4);
+        memcpy(bytes.data(), px.data(), bytes.size());
+        size_t n = 0;
+        const b200_status s = give(bytes, rgba, &n);
+        if (!s.code) { *width = rd.width; *height = rd.height; }
         return s;
     });
 }

@@ -55,6 +55,10 @@ GIF_HD GifRect gif_union(GifRect a, GifRect b)
 /* the pixel a frame draws at a position inside its rectangle (redraw: the position lies in R, or this is frame 0) */
 GIF_HD uint32_t gif_out_pixel(uint32_t prev, uint32_t cur, int redraw) { return redraw || prev != cur ? cur : 0u; }
 
+/* the canvas pixel of a converted source pixel: clear (0x00000000) where alpha is 0, else opaque -- the gif crate's
+ * Frame::from_rgba_speed makes every other alpha 255 */
+GIF_HD uint32_t gif_canvas_pixel(uint32_t r, uint32_t g, uint32_t b, uint32_t a) { return a ? (r | g << 8 | b << 16 | 0xFF000000u) : 0u; }
+
 /* colour table size field s (2^(s+1) entries hold n) and the LZW minimum code size */
 GIF_HD int gif_table_bits(int n) { int s = 0; while ((1 << (s + 1)) < n) s++; return s; }
 GIF_HD int gif_min_code_size(int n) { const int s = gif_table_bits(n) + 1; return s < 2 ? 2 : s; }

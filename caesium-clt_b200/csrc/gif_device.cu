@@ -50,6 +50,46 @@ bool GifDevice::lzw(const uint8_t *d_idx, size_t n, int m, void *stream_, std::v
     return true;
 }
 
+bool GifDevice::code_frame(PngQuant &q, int quality, int delay, int disposal, GifRect r, void *stream, std::vector<uint8_t> &out, std::string &err)
+{
+    std::vector<uint32_t> pal;
+    if (!q.prepare(stream, err) || !q.quantize(quality, stream, pal, err, quality == 100)) return false;
+    uint8_t head[8 + 10 + 768 + 1];
+    const int hn = gif_put_frame_head(head, delay, disposal, r, pal.data(), (int)pal.size());
+    out.insert(out.end(), head, head + hn);
+    return lzw(q.d_idx, (size_t)(r.x1 - r.x0) * (r.y1 - r.y0), gif_min_code_size((int)pal.size()), stream, out, err);
+}
+
+bool GifDevice::encode_canvas(PngQuant &q, int W, int H, int quality, void *stream, std::vector<uint8_t> &out, std::string &err)
+{
+    out.resize(64);
+    out.resize((size_t)gif_put_header(out.data(), W, H, -1));
+    if (!code_frame(q, quality, 0, 1, GifRect{0, 0, W, H}, stream, out, err)) return false;
+    out.push_back(0x3B);
+    return true;
+}
+
+bool GifDevice::canvas_from_planes(PngQuant &q, const uint8_t *r, const uint8_t *g, const uint8_t *b, const uint8_t *a, int W, int H, void *stream, std::string &err)
+{
+    uint32_t *d_rgba = q.rgba_for(W, H, err);
+    return d_rgba && launch_ok(launch_gif_canvas(r, g, b, a, (size_t)W * H, d_rgba, stream), "k_gif_canvas", err);
+}
+
+bool GifDevice::canvas_from_host(PngQuant &q, const uint8_t *rgb, const uint8_t *a, int W, int H, void *stream, std::string &err)
+{
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t n = (size_t)W * H;
+    if (!grow(d_planes, 4 * n, err)) return false;
+    CU(cudaMemcpyAsync(d_planes, rgb, 3 * n, cudaMemcpyHostToDevice, st));
+    if (a) CU(cudaMemcpyAsync(d_planes + 3 * n, a, n, cudaMemcpyHostToDevice, st));
+    return canvas_from_planes(q, d_planes, d_planes + n, d_planes + 2 * n, a ? d_planes + 3 * n : nullptr, W, H, stream, err);
+}
+
+bool GifDevice::canvas_from_rgba(PngQuant &q, void *stream, std::string &err)
+{
+    return launch_ok(launch_gif_canvas_rgba(q.d_rgba, (size_t)q.w * q.h, stream), "k_gif_canvas_rgba", err);
+}
+
 bool GifDevice::encode(GifReader &rd, PngQuant &q, int quality, void *stream_, std::vector<uint8_t> &out, bool &corrupt, std::string &err)
 {
     cudaStream_t st = (cudaStream_t)stream_;
@@ -67,19 +107,13 @@ bool GifDevice::encode(GifReader &rd, PngQuant &q, int quality, void *stream_, s
     int prev = -1, cur = -1, delay_pending = 0;
     GifRect changed = whole, redraw = none;
     bool first = true;
-    std::vector<uint32_t> pal;
     auto write_frame = [&](GifRect clears) -> bool {
         const GifRect r = first ? whole : gif_union(gif_union(changed, clears), redraw);
         const int disposal = gif_rect_empty(clears) ? 1 : 2;
-        const int rw = r.x1 - r.x0, rh = r.y1 - r.y0;
-        uint32_t *d_rgba = q.rgba_for(rw, rh, err);
+        uint32_t *d_rgba = q.rgba_for(r.x1 - r.x0, r.y1 - r.y0, err);
         if (!d_rgba) return false;
         if (!launch_ok(launch_gif_crop(first ? d_canvas[cur] : d_canvas[prev], d_canvas[cur], W, r, first ? whole : redraw, d_rgba, st), "k_gif_crop", err) ||
-            !q.prepare(st, err) || !q.quantize(quality, st, pal, err, quality == 100)) return false;
-        uint8_t head[8 + 10 + 768 + 1];
-        const int hn = gif_put_frame_head(head, delay_pending, disposal, r, pal.data(), (int)pal.size());
-        out.insert(out.end(), head, head + hn);
-        if (!lzw(q.d_idx, (size_t)rw * rh, gif_min_code_size((int)pal.size()), st, out, err)) return false;
+            !code_frame(q, quality, delay_pending, disposal, r, st, out, err)) return false;
         redraw = disposal == 2 ? r : none;
         first = false;
         return true;

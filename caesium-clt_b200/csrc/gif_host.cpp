@@ -64,9 +64,17 @@ bool lzw_decode(const uint8_t *data, size_t n, int m, uint8_t *out, size_t npix,
     return true;
 }
 
+// row k of the image data of a frame fh rows high -> its row in the frame (interlaced: the four passes of rows 8k, 8k + 4, 4k + 2, 2k + 1)
+int frame_row(int k, int fh, bool interlaced)
+{
+    if (!interlaced) return k;
+    const int p1 = (fh + 7) / 8, p2 = (fh + 3) / 8, p3 = (fh + 1) / 4;
+    return k < p1 ? 8 * k : k < p1 + p2 ? 8 * (k - p1) + 4 : k < p1 + p2 + p3 ? 4 * (k - p1 - p2) + 2 : 2 * (k - p1 - p2 - p3) + 1;
+}
+
 } // namespace
 
-bool GifReader::open(const uint8_t *d, size_t n, std::string &err)
+bool GifReader::read_screen(const uint8_t *d, size_t n, std::string &err)
 {
     d_ = d; n_ = n; frames = 0; loop = -1; unsupported = false;
     if (n < 13 || (memcmp(d, "GIF87a", 6) && memcmp(d, "GIF89a", 6))) { err = "not a GIF"; return false; }
@@ -81,36 +89,78 @@ bool GifReader::open(const uint8_t *d, size_t n, std::string &err)
         pos += (size_t)gct_n_ * 3;
     }
     first_block_ = pos;
+    return true;
+}
+
+bool GifReader::walk_block(size_t &pos, uint8_t &kind, std::string &err)
+{
+    const uint8_t *d = d_;
+    const size_t n = n_;
+    if (pos >= n) { err = "GIF truncated (no trailer)"; return false; }
+    const uint8_t b = kind = d[pos++];
+    if (b == 0x3B) return true;
+    if (b == 0x21) {
+        if (pos >= n) { err = "GIF extension truncated"; return false; }
+        const uint8_t label = d[pos++];
+        if (label == 0xFF && pos + 12 <= n && d[pos] == 11 && !memcmp(d + pos + 1, "NETSCAPE2.0", 11)) {
+            const size_t q = pos + 12;
+            if (q + 4 <= n && d[q] == 3 && d[q + 1] == 1) loop = (int)rd16(d + q + 2);
+        }
+        if (label == 0xF9 && (pos >= n || d[pos] < 4)) { err = "GIF graphic control extension too short"; return false; }
+        if (!skip_blocks(d, n, pos)) { err = "GIF extension truncated"; return false; }
+        return true;
+    }
+    if (b != 0x2C) { err = "GIF block of unknown type"; return false; }
+    if (n - pos < 9) { err = "GIF image descriptor truncated"; return false; }
+    const uint32_t x = rd16(d + pos), y = rd16(d + pos + 2), w = rd16(d + pos + 4), h = rd16(d + pos + 6);
+    const uint8_t f = d[pos + 8];
+    pos += 9;
+    if (x + w > (uint32_t)width || y + h > (uint32_t)height) { unsupported = true; err = "a GIF frame extends past the logical screen"; return false; }
+    if (f & 0x80) {
+        const size_t t = (size_t)(2 << (f & 7)) * 3;
+        if (t > n - pos) { err = "GIF local colour table truncated"; return false; }
+        pos += t;
+    } else if (!gct_n_) { err = "GIF frame without a colour table"; return false; }
+    if (pos >= n) { err = "GIF image data truncated"; return false; }
+    if (d[pos] < 2 || d[pos] > 8) { err = "GIF LZW minimum code size out of range"; return false; }
+    pos++;
+    if (!skip_blocks(d, n, pos)) { err = "GIF image data truncated"; return false; }
+    return true;
+}
+
+bool GifReader::read_image(Image &im, std::string &err)
+{
+    const uint8_t *d = d_;
+    im.x = (int)rd16(d + pos_); im.y = (int)rd16(d + pos_ + 2); im.w = (int)rd16(d + pos_ + 4); im.h = (int)rd16(d + pos_ + 6);
+    const uint8_t f = d[pos_ + 8];
+    pos_ += 9;
+    im.interlaced = (f & 0x40) != 0;
+    im.table = gct_; im.tn = gct_n_;
+    if (f & 0x80) { im.tn = 2 << (f & 7); read_table(d + pos_, im.tn, im.lct); im.table = im.lct; pos_ += (size_t)im.tn * 3; }
+    const int m = d[pos_++];
+    lzw_.clear();
     for (;;) {
-        if (pos >= n) { err = "GIF truncated (no trailer)"; return false; }
-        const uint8_t b = d[pos++];
-        if (b == 0x3B) break;
-        if (b == 0x21) {
-            if (pos >= n) { err = "GIF extension truncated"; return false; }
-            const uint8_t label = d[pos++];
-            if (label == 0xFF && pos + 12 <= n && d[pos] == 11 && !memcmp(d + pos + 1, "NETSCAPE2.0", 11)) {
-                const size_t q = pos + 12;
-                if (q + 4 <= n && d[q] == 3 && d[q + 1] == 1) loop = (int)rd16(d + q + 2);
-            }
-            if (label == 0xF9 && (pos >= n || d[pos] < 4)) { err = "GIF graphic control extension too short"; return false; }
-            if (!skip_blocks(d, n, pos)) { err = "GIF extension truncated"; return false; }
-        } else if (b == 0x2C) {
-            if (n - pos < 9) { err = "GIF image descriptor truncated"; return false; }
-            const uint32_t x = rd16(d + pos), y = rd16(d + pos + 2), w = rd16(d + pos + 4), h = rd16(d + pos + 6);
-            const uint8_t f = d[pos + 8];
-            pos += 9;
-            if (x + w > (uint32_t)width || y + h > (uint32_t)height) { unsupported = true; err = "a GIF frame extends past the logical screen"; return false; }
-            if (f & 0x80) {
-                const size_t t = (size_t)(2 << (f & 7)) * 3;
-                if (t > n - pos) { err = "GIF local colour table truncated"; return false; }
-                pos += t;
-            } else if (!gct_n_) { err = "GIF frame without a colour table"; return false; }
-            if (pos >= n) { err = "GIF image data truncated"; return false; }
-            if (d[pos] < 2 || d[pos] > 8) { err = "GIF LZW minimum code size out of range"; return false; }
-            pos++;
-            if (!skip_blocks(d, n, pos)) { err = "GIF image data truncated"; return false; }
-            frames++;
-        } else { err = "GIF block of unknown type"; return false; }
+        const size_t len = d[pos_++];
+        if (!len) break;
+        lzw_.insert(lzw_.end(), d + pos_, d + pos_ + len);
+        pos_ += len;
+    }
+    const size_t npix = (size_t)im.w * im.h;
+    idx_.resize(npix);
+    if (!lzw_decode(lzw_.data(), lzw_.size(), m, idx_.data(), npix, err)) return false;
+    for (size_t i = 0; i < npix; i++) if (idx_[i] >= im.tn) { err = "GIF pixel index past its colour table"; return false; }
+    return true;
+}
+
+bool GifReader::open(const uint8_t *d, size_t n, std::string &err)
+{
+    if (!read_screen(d, n, err)) return false;
+    size_t pos = first_block_;
+    for (;;) {
+        uint8_t kind;
+        if (!walk_block(pos, kind, err)) return false;
+        if (kind == 0x3B) break;
+        if (kind == 0x2C) frames++;
     }
     if (!frames) { err = "GIF without frames"; return false; }
     pos_ = first_block_;
@@ -142,45 +192,47 @@ bool GifReader::next(uint32_t *canvas, int &delay, std::string &err)
             continue;
         }
         // 0x2C
-        const int x = (int)rd16(d + pos_), y = (int)rd16(d + pos_ + 2), fw = (int)rd16(d + pos_ + 4), fh = (int)rd16(d + pos_ + 6);
-        const uint8_t f = d[pos_ + 8];
-        pos_ += 9;
-        uint32_t lct[256];
-        const uint32_t *table = gct_;
-        int tn = gct_n_;
-        if (f & 0x80) { tn = 2 << (f & 7); read_table(d + pos_, tn, lct); table = lct; pos_ += (size_t)tn * 3; }
-        const int m = d[pos_++];
-        lzw_.clear();
-        for (;;) {
-            const size_t len = d[pos_++];
-            if (!len) break;
-            lzw_.insert(lzw_.end(), d + pos_, d + pos_ + len);
-            pos_ += len;
-        }
-        const size_t npix = (size_t)fw * fh;
-        idx_.resize(npix);
-        if (!lzw_decode(lzw_.data(), lzw_.size(), m, idx_.data(), npix, err)) return false;
-        for (size_t i = 0; i < npix; i++) if (idx_[i] >= tn) { err = "GIF pixel index past its colour table"; return false; }
+        Image im;
+        if (!read_image(im, err)) return false;
         // the previous frame's disposal, then this frame's save for disposal 3
         if (prev_disposal_ == 2) {
             for (int r = 0; r < prev_h_; r++) memset(&canvas_[(size_t)(prev_y_ + r) * width + prev_x_], 0, (size_t)prev_w_ * 4);
         } else if (prev_disposal_ == 3 && !saved_.empty()) canvas_.swap(saved_);
         if (disposal == 3) saved_ = canvas_;
-        const bool interlaced = (f & 0x40) != 0;
-        for (int k = 0; k < fh; k++) {
-            int row = k;
-            if (interlaced) {
-                const int p1 = (fh + 7) / 8, p2 = (fh + 3) / 8, p3 = (fh + 1) / 4;
-                row = k < p1 ? 8 * k : k < p1 + p2 ? 8 * (k - p1) + 4 : k < p1 + p2 + p3 ? 4 * (k - p1 - p2) + 2 : 2 * (k - p1 - p2 - p3) + 1;
-            }
-            uint32_t *dst = &canvas_[(size_t)(y + row) * width + x];
-            const uint8_t *src = &idx_[(size_t)k * fw];
-            for (int i = 0; i < fw; i++) if (src[i] != tindex) dst[i] = table[src[i]];
+        for (int k = 0; k < im.h; k++) {
+            uint32_t *dst = &canvas_[(size_t)(im.y + frame_row(k, im.h, im.interlaced)) * width + im.x];
+            const uint8_t *src = &idx_[(size_t)k * im.w];
+            for (int i = 0; i < im.w; i++) if (src[i] != tindex) dst[i] = im.table[src[i]];
         }
-        prev_disposal_ = disposal; prev_x_ = x; prev_y_ = y; prev_w_ = fw; prev_h_ = fh;
+        prev_disposal_ = disposal; prev_x_ = im.x; prev_y_ = im.y; prev_w_ = im.w; prev_h_ = im.h;
         memcpy(canvas, canvas_.data(), canvas_.size() * 4);
         return true;
     }
+}
+
+bool GifReader::first_frame(const uint8_t *d, size_t n, std::vector<uint32_t> &canvas, std::string &err)
+{
+    if (!read_screen(d, n, err)) return false;
+    size_t pos = first_block_;
+    int tindex = -1;
+    for (;;) {
+        const size_t at = pos;
+        uint8_t kind;
+        if (!walk_block(pos, kind, err)) return false;
+        if (kind == 0x3B) { err = "GIF without frames"; return false; }
+        if (kind == 0x21 && d[at + 1] == 0xF9) tindex = (d[at + 3] & 1) ? d[at + 6] : -1;      // checked: its block holds 4 bytes or more
+        if (kind == 0x2C) { pos_ = at + 1; break; }
+    }
+    frames = 1;
+    Image im;
+    if (!read_image(im, err)) return false;
+    canvas.assign((size_t)width * height, 0u);
+    for (int k = 0; k < im.h; k++) {
+        uint32_t *dst = &canvas[(size_t)(im.y + frame_row(k, im.h, im.interlaced)) * width + im.x];
+        const uint8_t *src = &idx_[(size_t)k * im.w];
+        for (int i = 0; i < im.w; i++) dst[i] = src[i] == tindex ? im.table[src[i]] & 0x00FFFFFFu : im.table[src[i]];
+    }
+    return true;
 }
 
 } // namespace b200

@@ -28,7 +28,26 @@ public:
     // corrupt data (err says why)
     bool next(uint32_t *canvas, int &delay, std::string &err);
 
+    // Instead of open() / next(): frame 0 alone as the image crate decodes a GIF for a conversion -- width * height words, R in the
+    // low byte; inside the frame's rectangle every pixel is its palette colour, with alpha 0 for the transparent index and 255
+    // otherwise; outside it 0x00000000.  The blocks are checked up to the end of frame 0's image data only, so damage after it is
+    // never seen.  Refusals as open(): `unsupported` for a frame past the logical screen, otherwise the file is corrupt.
+    bool first_frame(const uint8_t *data, size_t n, std::vector<uint32_t> &canvas, std::string &err);
+
 private:
+    struct Image {                          // one frame's descriptor and colour table; its indices are in idx_
+        int x, y, w, h, tn;
+        bool interlaced;
+        const uint32_t *table;
+        uint32_t lct[256];
+    };
+    // the header and global colour table
+    bool read_screen(const uint8_t *data, size_t n, std::string &err);
+    // the block at pos checked against the input and skipped; kind = its introducer (0x21, 0x2C or the trailer 0x3B)
+    bool walk_block(size_t &pos, uint8_t &kind, std::string &err);
+    // the image at pos_ (after its 0x2C, its block checked by walk_block): descriptor, colour table and indices in stream order
+    bool read_image(Image &im, std::string &err);
+
     const uint8_t *d_ = nullptr;
     size_t n_ = 0, pos_ = 0, first_block_ = 0;
     uint32_t gct_[256] = {};

@@ -1,5 +1,5 @@
-// gif_kernels.cu -- the GIF leg's kernels: canvas difference, crop and mask, and the segmented LZW coder (one walker per segment,
-// a prefix sum of the segments' bit lengths, placement with DevBits, sub-blocking).
+// gif_kernels.cu -- the GIF leg's kernels: canvas difference, crop and mask, the canvases of converted sources, and the segmented
+// LZW coder (one walker per segment, a prefix sum of the segments' bit lengths, placement with DevBits, sub-blocking).
 #include <cuda_runtime.h>
 #include <algorithm>
 #include "gif_kernels.h"
@@ -35,6 +35,23 @@ __global__ void k_gif_crop(const uint32_t *__restrict__ prev, const uint32_t *__
         const int x = r.x0 + (int)(i % rw), y = r.y0 + (int)(i / rw);
         const size_t at = (size_t)y * w + x;
         out[i] = gif_out_pixel(prev[at], cur[at], gif_in_rect(redraw, x, y));
+    }
+}
+
+// converted sources: 8-bit planes (a grey source passes its one plane as r, g and b; a == null: opaque) -> canvas words
+__global__ void k_gif_canvas(const uint8_t *__restrict__ r, const uint8_t *__restrict__ g, const uint8_t *__restrict__ b, const uint8_t *__restrict__ a,
+                             size_t n, uint32_t *__restrict__ out)
+{
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+        out[i] = gif_canvas_pixel(r[i], g[i], b[i], a ? a[i] : 255u);
+}
+
+// RGBA8 words (R in the low byte) -> canvas words, in place
+__global__ void k_gif_canvas_rgba(uint32_t *__restrict__ px, size_t n)
+{
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const uint32_t v = px[i];
+        px[i] = gif_canvas_pixel(v & 255u, (v >> 8) & 255u, (v >> 16) & 255u, v >> 24);
     }
 }
 
@@ -79,6 +96,18 @@ int launch_gif_diff(const uint32_t *a, const uint32_t *b, int w, int h, uint32_t
 int launch_gif_crop(const uint32_t *prev, const uint32_t *cur, int w, GifRect r, GifRect redraw, uint32_t *out, void *stream)
 {
     k_gif_crop<<<grid_for((size_t)(r.x1 - r.x0) * (r.y1 - r.y0), 256), 256, 0, (cudaStream_t)stream>>>(prev, cur, w, r, redraw, out);
+    return (int)cudaGetLastError();
+}
+
+int launch_gif_canvas(const uint8_t *r, const uint8_t *g, const uint8_t *b, const uint8_t *a, size_t n, uint32_t *out, void *stream)
+{
+    k_gif_canvas<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(r, g, b, a, n, out);
+    return (int)cudaGetLastError();
+}
+
+int launch_gif_canvas_rgba(uint32_t *px, size_t n, void *stream)
+{
+    k_gif_canvas_rgba<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(px, n);
     return (int)cudaGetLastError();
 }
 

@@ -12,6 +12,11 @@ namespace b200 {
 int launch_gif_diff(const uint32_t *a, const uint32_t *b, int w, int h, uint32_t *box, void *stream);
 // rectangle r of canvas cur, masked against prev as in gif_out_pixel (redraw: the positions drawn whatever they hold), into out
 int launch_gif_crop(const uint32_t *prev, const uint32_t *cur, int w, GifRect r, GifRect redraw, uint32_t *out, void *stream);
+// n pixels of 8-bit planes r, g, b (a grey source passes one plane three times) and an optional alpha plane a -> canvas words
+// (gif_canvas_pixel) in out
+int launch_gif_canvas(const uint8_t *r, const uint8_t *g, const uint8_t *b, const uint8_t *a, size_t n, uint32_t *out, void *stream);
+// n RGBA8 words -> canvas words, in place
+int launch_gif_canvas_rgba(uint32_t *px, size_t n, void *stream);
 // segmented LZW: per segment its codes (GIF_SEG_CODES apart), their count and their bit total (bits[nseg] is left alone)
 int launch_gif_walk(const uint8_t *idx, size_t n, int m, int nseg, uint16_t *codes, uint32_t *ncodes, unsigned long long *bits, void *stream);
 // the codes at their scanned bit offsets into zeroed words
