@@ -7,8 +7,8 @@
 //   classify + inline-symbol histogram + correction-bit counts -> [max-scan: previous event] [sum-scan: trailing correction bits] ->
 //   groups + EOBn histogram -> tables + bits per table -> scan sizes / buffer layout (on the device) | D2H: sizes ->
 //   lengths of the interleaved scans' units -> [sum-scan: their bit offsets] -> zero -> emit (single-component scans: CTA runs into a
-//   staging arena) -> [sum-scan: run offsets] -> place runs -> ffcount -> [sum-scan] -> layout -> scatter (byte stuffing) |
-//   D2H: stuffed scans + DHT payloads.  No host wait in between: see "host orchestration".
+//   staging arena) -> [sum-scan: run offsets] -> place runs -> 0xFF count per chunk of each scan -> layout -> scatter (byte stuffing
+//   through shared memory) | D2H: stuffed scans + DHT payloads.  No host wait in between: see "host orchestration".
 #include <cuda_runtime.h>
 #include <cub/device/device_scan.cuh>
 #include <cuda_pipeline.h>
@@ -16,6 +16,7 @@
 #include <chrono>
 #include <cstring>
 #include "jpeg_gpuenc.h"
+#include "jpeg_gpuenc_stuff_core.h"
 #include "stream_wait.h"
 #include "launch_timer.h"
 
@@ -121,15 +122,16 @@ __global__ void k_ge_tables(const uint32_t *__restrict__ hist, Table *__restrict
 
 // Sizes on the device: bits per scan (its four tables' bits + its correction bits), then every scan's place in the group's bit
 // buffer (word_base) and, for a single-component scan, in the staging arena of its CTA runs (arena_base: a run takes whole words,
-// so a scan takes at most its words plus one per run), its byte / 16-byte-group counts and the group index base -- what the host
+// so a scan takes at most its words plus one per run) and its byte count -- what the host
 // used to compute between two halves of the pipeline (one stream wait per megabatch less).  The buffers are sized from an ESTIMATE of the output (the input's size for a re-encode);
 // if the real sizes do not fit, flags[0] is raised, every scan is given zero length so the back half does nothing, and the host
-// re-runs the back half with exact sizes (flags[1..2] = words / groups needed).  One warp; scans in chunks of 32.
+// re-runs the back half with exact sizes (flags[1] = words needed).  A scan's words are rounded up to a multiple of four, so that
+// every scan starts 16-byte aligned for the stuffing passes' group loads.  One warp; scans in chunks of 32.
 __global__ void k_ge_scanout(const Scan *__restrict__ scans, int nscans, const unsigned long long *__restrict__ tbits, const uint32_t *__restrict__ corr,
-                             uint32_t *__restrict__ total, ScanOut *__restrict__ so, uint32_t words_cap, uint32_t groups_cap, uint32_t *__restrict__ flags)
+                             uint32_t *__restrict__ total, ScanOut *__restrict__ so, uint32_t words_cap, uint32_t *__restrict__ flags)
 {
     const int lane = threadIdx.x;
-    uint32_t wbase = 0, gbase = 0, abase = 0;
+    uint32_t wbase = 0, abase = 0;
     for (int c0 = 0; c0 < nscans; c0 += 32) {
         const int i = c0 + lane;
         uint32_t tb = 0, na = 0;
@@ -137,23 +139,23 @@ __global__ void k_ge_scanout(const Scan *__restrict__ scans, int nscans, const u
             tb = (uint32_t)(tbits[4 * i] + tbits[4 * i + 1] + tbits[4 * i + 2] + tbits[4 * i + 3] + corr[i]);
             na = scans[i].nruns ? (tb + 31) / 32 + scans[i].nruns : 0;
         }
-        const uint32_t nbytes = (tb + 7) / 8, ng = (nbytes + 15) / 16, nw = i < nscans ? (tb + 31) / 32 + 1 : 0;
-        uint32_t wi = nw, gi = i < nscans ? ng : 0, ai = na;        // inclusive warp scans
+        const uint32_t nbytes = (tb + 7) / 8, nw = i < nscans ? ((tb + 31) / 32 + 1 + 3) & ~3u : 0;
+        uint32_t wi = nw, ai = na;          // inclusive warp scans
         for (int d = 1; d < 32; d <<= 1) {
-            const uint32_t a = __shfl_up_sync(0xFFFFFFFFu, wi, d), b = __shfl_up_sync(0xFFFFFFFFu, gi, d), c = __shfl_up_sync(0xFFFFFFFFu, ai, d);
-            if (lane >= d) { wi += a; gi += b; ai += c; }
+            const uint32_t a = __shfl_up_sync(0xFFFFFFFFu, wi, d), c = __shfl_up_sync(0xFFFFFFFFu, ai, d);
+            if (lane >= d) { wi += a; ai += c; }
         }
         if (i < nscans) {
             total[i] = tb;
-            ScanOut o; o.total_bits = tb; o.nbytes = nbytes; o.ngroups = ng; o.group_base = gbase + gi - ng; o.word_base = wbase + wi - nw; o.arena_base = abase + ai - na;
+            ScanOut o; o.total_bits = tb; o.nbytes = nbytes; o.word_base = wbase + wi - nw; o.arena_base = abase + ai - na;
             so[i] = o;
         }
-        wbase += __shfl_sync(0xFFFFFFFFu, wi, 31); gbase += __shfl_sync(0xFFFFFFFFu, gi, 31); abase += __shfl_sync(0xFFFFFFFFu, ai, 31);
+        wbase += __shfl_sync(0xFFFFFFFFu, wi, 31); abase += __shfl_sync(0xFFFFFFFFu, ai, 31);
     }
     __syncwarp();
-    const bool ovf = wbase > words_cap || gbase > groups_cap;       // the arena holds words_cap + total_runs words: it fits when the words do
-    if (lane == 0) { flags[0] = ovf ? 1u : 0u; flags[1] = wbase; flags[2] = gbase; flags[3] = 0; flags[4] = 0; }
-    if (ovf) for (int i = lane; i < nscans; i += 32) { so[i].total_bits = 0; so[i].nbytes = 0; so[i].ngroups = 0; so[i].group_base = 0; so[i].word_base = 0; so[i].arena_base = 0; }
+    const bool ovf = wbase > words_cap;     // the arena holds words_cap + total_runs words: it fits when the words do
+    if (lane == 0) { flags[0] = ovf ? 1u : 0u; flags[1] = wbase; flags[3] = 0; flags[4] = 0; }
+    if (ovf) for (int i = lane; i < nscans; i += 32) { so[i].total_bits = 0; so[i].nbytes = 0; so[i].word_base = 0; so[i].arena_base = 0; }
 }
 
 // a scan's bit buffer, and for a single-component scan its part of the staging arena (the runs' edge words are ORed)
@@ -443,67 +445,88 @@ __global__ void __launch_bounds__(PLACE_THREADS) k_ge_place(const Scan *__restri
                [&](long long w, uint32_t v) { atomicOr(&dst[w], v); }, [&](long long w, uint32_t v) { dst[w] = v; }, threadIdx.x & 31, 32);
 }
 
-// byte i of a scan's unstuffed stream (big-endian within words), with flush_bits' padding ones in the last byte
-__device__ __forceinline__ uint32_t scan_byte(const uint32_t *__restrict__ w, uint32_t i, uint32_t nbytes, uint32_t total_bits)
-{
-    uint32_t b = (w[i >> 2] >> (24 - 8 * (i & 3))) & 0xFF;
-    if (i == nbytes - 1 && (total_bits & 7)) b |= (1u << (8 - (total_bits & 7))) - 1u;
-    return b;
-}
+// ---- 0xFF stuffing: the bodies are in jpeg_gpuenc_stuff_core.h --------------------------------------------------------------
+// Grid (STUFF_CHUNKS, nscans) for both k_ge_ffcount and k_ge_scatter: CTA x of scan y owns chunk x of the scan's 16-byte groups
+// (stuff_chunk: whole tiles of STUFF_THREADS groups) and walks it a tile at a time, one 16-byte load per thread and tile.
+constexpr int STUFF_THREADS = ENC_THREADS;      // groups per tile (the CTA prefix sum is cta_exclusive_sum's)
+constexpr int STUFF_CHUNKS = 32;                // CTAs per scan
+static_assert(STUFF_CHUNKS <= STUFF_THREADS, "k_ge_scatter sums the chunks before its own with one thread each");
+__device__ __forceinline__ ScanGroup load_scan_group(const uint32_t *w, uint32_t g) { const uint4 q = reinterpret_cast<const uint4 *>(w)[g]; return ScanGroup{{q.x, q.y, q.z, q.w}}; }
 
-// 0xFF count per 16-byte group.  Grid (X, nscans + 1): row y < nscans strides over scan y's groups; the extra row zero-fills the
-// group slots past the batch's last group, because the prefix sum that follows runs over the whole (capacity-sized) array.
-__global__ void k_ge_ffcount(const ScanOut *__restrict__ so, int nscans, const uint32_t *__restrict__ words, uint32_t *__restrict__ ffcount, uint32_t groups_cap,
-                             const uint32_t *__restrict__ flags)
+// 0xFF bytes per chunk: chunkff[y * STUFF_CHUNKS + x] (every CTA writes its entry, an empty chunk 0)
+__global__ void __launch_bounds__(STUFF_THREADS) k_ge_ffcount(const ScanOut *__restrict__ so, const uint32_t *__restrict__ words, uint32_t *__restrict__ chunkff)
 {
-    if ((int)blockIdx.y == nscans) {
-        const uint32_t used = flags[0] ? 0u : flags[2];
-        for (uint32_t g = used + blockIdx.x * blockDim.x + threadIdx.x; g < groups_cap; g += gridDim.x * blockDim.x) ffcount[g] = 0;
-        return;
-    }
+    __shared__ uint32_t wsum[STUFF_THREADS / 32];
     const ScanOut o = so[blockIdx.y];
     const uint32_t *w = words + o.word_base;
-    for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < o.ngroups; g += gridDim.x * blockDim.x) {
-        uint32_t n = 0;
-        for (uint32_t i = g * 16; i < g * 16 + 16 && i < o.nbytes; i++) n += scan_byte(w, i, o.nbytes, o.total_bits) == 0xFF;
-        ffcount[o.group_base + g] = n;
+    uint32_t g0, g1;
+    stuff_chunk(o.nbytes, blockIdx.x, STUFF_CHUNKS, STUFF_THREADS, g0, g1);
+    uint32_t n = 0;
+    for (uint32_t g = g0 + threadIdx.x; g < g1; g += STUFF_THREADS) {
+        ScanGroup q = load_scan_group(w, g);
+        stuff_group(q, g, o.nbytes, o.total_bits);
+        n += stuff_ff_count(q);
     }
+    uint32_t total;
+    cta_exclusive_sum(n, wsum, total);
+    if (threadIdx.x == 0) chunkff[blockIdx.y * STUFF_CHUNKS + blockIdx.x] = total;
 }
 
-// per image: lay its scans out back to back in the image's output region; out_off / out_len per scan; an image that outgrows its
-// region raises flags[0] (and flags[3] = the largest image size seen, so the host can size the retry)
-__global__ void k_ge_layout(const ScanOut *__restrict__ so, int scans_per_image, int nimages, const uint32_t *__restrict__ ffcount, const uint32_t *__restrict__ ffoff,
-                            uint32_t *__restrict__ out_off, uint32_t *__restrict__ out_len, uint32_t out_image_stride, uint32_t *__restrict__ flags)
+// One CTA per image: lay its scans out back to back in the image's output region (a scan's stuffed length is its bytes plus its
+// chunks' 0xFF counts; warp k sums scan k's); out_off / out_len per scan; an image that outgrows its region raises flags[4] (and
+// flags[3] = the largest image size seen, so the host can size the retry)
+constexpr int LAYOUT_THREADS = 256;
+__global__ void __launch_bounds__(LAYOUT_THREADS) k_ge_layout(const ScanOut *__restrict__ so, int scans_per_image, const uint32_t *__restrict__ chunkff,
+                                                              uint32_t *__restrict__ out_off, uint32_t *__restrict__ out_len, uint32_t out_image_stride, uint32_t *__restrict__ flags)
 {
-    const int im = blockIdx.x * blockDim.x + threadIdx.x;
-    if (im >= nimages) return;
-    uint32_t off = 0;
-    for (int k = 0; k < scans_per_image; k++) {
-        const int si = im * scans_per_image + k;
-        const ScanOut o = so[si];
+    extern __shared__ uint32_t slen[];      // scans_per_image
+    const int lane = threadIdx.x & 31, s0 = blockIdx.x * scans_per_image;
+    for (int k = threadIdx.x >> 5; k < scans_per_image; k += LAYOUT_THREADS / 32) {
         uint32_t ff = 0;
-        if (o.ngroups) { const uint32_t lastg = o.group_base + o.ngroups - 1; ff = ffoff[lastg] + ffcount[lastg] - ffoff[o.group_base]; }
-        out_off[si] = off; out_len[si] = o.nbytes + ff;
-        off += o.nbytes + ff;
+        for (int x = lane; x < STUFF_CHUNKS; x += 32) ff += chunkff[(s0 + k) * STUFF_CHUNKS + x];
+        ff = __reduce_add_sync(0xFFFFFFFFu, ff);
+        if (lane == 0) slen[k] = so[s0 + k].nbytes + ff;
     }
+    __syncthreads();
+    if (threadIdx.x) return;
+    uint32_t off = 0;
+    for (int k = 0; k < scans_per_image; k++) { out_off[s0 + k] = off; out_len[s0 + k] = slen[k]; off += slen[k]; }
     atomicMax(&flags[3], off);
     if (off > out_image_stride) atomicOr(&flags[4], 1u);
 }
 
-__global__ void k_ge_scatter(const ScanOut *__restrict__ so, const uint32_t *__restrict__ words, const uint32_t *__restrict__ ffoff,
-                             const uint32_t *__restrict__ out_off, uint8_t *__restrict__ out, int scans_per_image, size_t out_image_stride, const uint32_t *__restrict__ flags)
+// The chunk's output starts after its groups' bytes before it and the 0xFF bytes of the chunks before it.  Per tile: each thread
+// re-reads its group, a CTA prefix sum over the stuffed lengths gives its place, the bytes are stuffed into shared memory at the
+// output's word alignment and leave as aligned 4-byte stores, coalesced across the CTA (stuff_store); the next tile starts where
+// this one ended.
+__global__ void __launch_bounds__(STUFF_THREADS) k_ge_scatter(const ScanOut *__restrict__ so, const uint32_t *__restrict__ words, const uint32_t *__restrict__ chunkff,
+                                                              const uint32_t *__restrict__ out_off, uint8_t *__restrict__ out, int scans_per_image, size_t out_image_stride,
+                                                              const uint32_t *__restrict__ flags)
 {
+    __shared__ uint32_t sbuf[STUFF_THREADS * 8 + 1];       // a tile of 0xFF bytes stuffs to 32 bytes a group, after up to 3 bytes of alignment
+    __shared__ uint32_t wsum[STUFF_THREADS / 32];
     if (flags[4]) return;                   // some image does not fit its output region: nothing is written, the host retries
     const ScanOut o = so[blockIdx.y];
+    uint32_t g0, g1;
+    stuff_chunk(o.nbytes, blockIdx.x, STUFF_CHUNKS, STUFF_THREADS, g0, g1);
+    if (g0 >= g1) return;
     const uint32_t *w = words + o.word_base;
-    uint8_t *base = out + (size_t)(blockIdx.y / scans_per_image) * out_image_stride + out_off[blockIdx.y];
-    for (uint32_t g = blockIdx.x * blockDim.x + threadIdx.x; g < o.ngroups; g += gridDim.x * blockDim.x) {
-        uint8_t *dst = base + (size_t)g * 16 + (ffoff[o.group_base + g] - ffoff[o.group_base]);
-        for (uint32_t i = g * 16; i < g * 16 + 16 && i < o.nbytes; i++) {
-            const uint32_t b = scan_byte(w, i, o.nbytes, o.total_bits);
-            *dst++ = (uint8_t)b;
-            if (b == 0xFF) *dst++ = 0;
-        }
+    uint8_t *img = out + (size_t)(blockIdx.y / scans_per_image) * out_image_stride, *sb = reinterpret_cast<uint8_t *>(sbuf);
+    uint32_t ff_before;
+    cta_exclusive_sum(threadIdx.x < blockIdx.x ? chunkff[blockIdx.y * STUFF_CHUNKS + threadIdx.x] : 0u, wsum, ff_before);
+    uint32_t at = out_off[blockIdx.y] + g0 * 16 + ff_before;
+    for (uint32_t t0 = g0; t0 < g1; t0 += STUFF_THREADS) {
+        const uint32_t g = t0 + threadIdx.x;
+        ScanGroup q;
+        uint32_t n = 0, len = 0;
+        if (g < g1) { q = load_scan_group(w, g); n = stuff_group(q, g, o.nbytes, o.total_bits); len = n + stuff_ff_count(q); }
+        __syncthreads();                    // the previous tile's wsum / sbuf reads are done
+        uint32_t L;
+        const uint32_t rel = cta_exclusive_sum(len, wsum, L), aligned = at & ~3u;
+        if (n) stuff_place_group(q, n, at - aligned + rel, sb);
+        __syncthreads();
+        stuff_store(sbuf, aligned, at, at + L, threadIdx.x, STUFF_THREADS, img);
+        at += L;
     }
 }
 
@@ -541,7 +564,7 @@ GpuEncoder::~GpuEncoder()
 // Sizes here depend on image CONTENT (bytes of entropy-coded output): Grow::Pow2Half rounds up to a power of two with headroom so a
 // slot stops reallocating after its first image of a given class (cudaFree / cudaHostAlloc stall every stream).
 bool GpuEncoder::size_back_buffers(size_t image_bytes, std::string &err)
-{   // everything whose size follows the OUTPUT: bit buffer, 16-byte group arrays, stuffed bytes
+{   // everything whose size follows the OUTPUT: bit buffer, stuffed bytes
     const int NS = (int)plan.scans.size();
     // capacities only grow (per image count): they are kernel arguments of the launch sequence, and a sequence whose arguments do
     // not change from megabatch to megabatch can be replayed as a CUDA graph
@@ -552,13 +575,10 @@ bool GpuEncoder::size_back_buffers(size_t image_bytes, std::string &err)
     if (image_bytes <= est_image_bytes && words_cap) return grow_arena();
     est_image_bytes = image_bytes + image_bytes / 8;
     image_bytes = est_image_bytes;
-    words_cap = (uint32_t)std::min<size_t>((size_t)nimg * (image_bytes / 4 + 1) + 2 * (size_t)NS + 64, 0xFFFFFF00u);
-    groups_cap = (uint32_t)((size_t)words_cap / 4 + NS + 1);
+    // a scan takes its bits' words, one more, and up to three to round its words to a multiple of four (k_ge_scanout)
+    words_cap = (uint32_t)std::min<size_t>((size_t)nimg * (image_bytes / 4 + 1) + 5 * (size_t)NS + 64, 0xFFFFFF00u);
     out_stride = align_up(image_bytes + image_bytes / 8 + 1024, 256);
-    if (!grow_arena() || !grow(d_words, (size_t)words_cap * 4 + 64) || !grow(d_ffcount, (size_t)groups_cap * 4 + 4) || !grow(d_ffoff, (size_t)groups_cap * 4 + 4) ||
-        !grow(d_out, out_stride * nimg)) return false;
-    size_t tb3 = 0; cub::DeviceScan::ExclusiveSum((void *)nullptr, tb3, d_ffcount.get(), d_ffoff.get(), (int)groups_cap, (cudaStream_t)0);
-    return grow(d_temp, tb3 + 256);
+    return grow_arena() && grow(d_words, (size_t)words_cap * 4 + 64) && grow(d_out, out_stride * nimg);
 }
 
 bool GpuEncoder::prepare(const JpegGeom &g, bool progressive, int16_t *const *d_coefs, int nimages, void *stream_, size_t out_bytes_hint, std::string &err)
@@ -586,7 +606,7 @@ bool GpuEncoder::prepare(const JpegGeom &g, bool progressive, int16_t *const *d_
         !grow(d_cursor, (size_t)NS * 4) || !grow(d_runlen, (size_t)R * 4) || !grow(d_runoff, (size_t)R * 4) || !grow(d_runpos, (size_t)R * 4) ||
         !grow(d_hist, (size_t)NS * 4 * 256 * 4) || !grow(d_tabs, (size_t)NS * 4 * sizeof(Table)) || !grow(d_dht, (size_t)NS * 4 * sizeof(DhtOut)) ||
         !grow(d_total, (size_t)NS * 4) || !grow(d_so, (size_t)NS * sizeof(ScanOut)) || !grow(d_outoff, (size_t)NS * 4) || !grow(d_outlen, (size_t)NS * 4) ||
-        !grow(d_flags, 64) || !grow(d_masks, (size_t)plan.total_comp_blocks * sizeof(Masks3))) return false;
+        !grow(d_flags, 64) || !grow(d_masks, (size_t)plan.total_comp_blocks * sizeof(Masks3)) || !grow(d_chunkff, (size_t)NS * STUFF_CHUNKS * 4)) return false;
     o_scans = 0; o_total = o_scans + align_up((size_t)NS * sizeof(Scan), 256); o_outlen = o_total + align_up((size_t)NS * 4, 256);
     o_dht = o_outlen + align_up((size_t)NS * 4, 256); o_comps = o_dht + align_up((size_t)NS * 4 * sizeof(DhtOut), 256);
     o_flags = o_comps + align_up((size_t)NC * sizeof(BlockComp), 256);
@@ -626,7 +646,7 @@ unsigned long long GpuEncoder::signature() const
     unsigned long long h = 1469598103934665603ull;
     auto mix = [&](unsigned long long v) { h = (h ^ v) * 1099511628211ull; };
     mix((unsigned long long)nimg); mix((unsigned long long)plan.scans.size()); mix((unsigned long long)plan.comps.size()); mix((unsigned long long)plan.total_units);
-    mix((unsigned long long)plan.max_comp_blocks); mix((unsigned long long)plan.scans_per_image); mix(words_cap); mix(groups_cap); mix(out_stride); mix(generation);
+    mix((unsigned long long)plan.max_comp_blocks); mix((unsigned long long)plan.scans_per_image); mix(words_cap); mix(out_stride); mix(generation);
     mix((unsigned long long)geom.width); mix((unsigned long long)geom.height); mix(prog ? 1 : 0);
     for (int c = 0; c < geom.ncomp; c++) { mix((unsigned long long)geom.bw[c]); mix((unsigned long long)geom.bh[c]); mix((unsigned long long)geom.rbw[c]); mix((unsigned long long)geom.rbh[c]); mix((unsigned long long)geom.hs[c]); }
     for (auto pb : coef_bases) mix((unsigned long long)(uintptr_t)pb);
@@ -642,10 +662,10 @@ bool GpuEncoder::enqueue_sizes(void *stream_, std::string &err)
     cudaStream_t st = (cudaStream_t)stream_;
     const int NS = (int)plan.scans.size();
     uint32_t *h_total = reinterpret_cast<uint32_t *>(h_small + o_total), *h_flags = reinterpret_cast<uint32_t *>(h_small + o_flags);
-    k_ge_scanout<<<1, 32, 0, st>>>(d_scans, NS, d_tbits, d_corr, d_total, d_so, words_cap, groups_cap, d_flags);
+    k_ge_scanout<<<1, 32, 0, st>>>(d_scans, NS, d_tbits, d_corr, d_total, d_so, words_cap, d_flags);
     LT_MARK("k_ge_scanout");
     CU(cudaMemcpyAsync(h_total, d_total, (size_t)NS * 4, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(h_flags, d_flags, 12, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(h_flags, d_flags, 8, cudaMemcpyDeviceToHost, st));
     LT_MARK("copy");
     return true;
 }
@@ -661,7 +681,7 @@ bool GpuEncoder::enqueue_back(void *stream_, std::string &err)
     const int NS = (int)plan.scans.size(), NC = (int)plan.comps.size();
     uint32_t *h_flags = reinterpret_cast<uint32_t *>(h_small + o_flags);
     const dim3 gb(cdiv(plan.max_comp_blocks, ENC_THREADS), NC);
-    int n = 6;
+    int n = 5;
     if (plan.total_lunits) {                // units of the interleaved scans: lengths, then bit offsets
         bool dc_only = true;
         for (auto &sc : plan.scans) if (sc.ns > 1 && sc.mode != MODE_DC_FIRST) dc_only = false;
@@ -691,14 +711,11 @@ bool GpuEncoder::enqueue_back(void *stream_, std::string &err)
         LT_MARK("k_ge_place");
         n += 2;
     }
-    k_ge_ffcount<<<dim3(32, NS + 1), 128, 0, st>>>(d_so, NS, d_words, d_ffcount, groups_cap, d_flags);
+    k_ge_ffcount<<<dim3(STUFF_CHUNKS, NS), STUFF_THREADS, 0, st>>>(d_so, d_words, d_chunkff);
     LT_MARK("k_ge_ffcount");
-    size_t tb = d_temp.capacity();
-    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_ffcount.get(), d_ffoff.get(), (int)groups_cap, st);
-    LT_MARK("cub_scan");
-    k_ge_layout<<<cdiv(nimg, 64), 64, 0, st>>>(d_so, plan.scans_per_image, nimg, d_ffcount, d_ffoff, d_outoff, d_outlen, (uint32_t)out_stride, d_flags);
+    k_ge_layout<<<nimg, LAYOUT_THREADS, plan.scans_per_image * 4, st>>>(d_so, plan.scans_per_image, d_chunkff, d_outoff, d_outlen, (uint32_t)out_stride, d_flags);
     LT_MARK("k_ge_layout");
-    k_ge_scatter<<<dim3(32, NS), 128, 0, st>>>(d_so, d_words, d_ffoff, d_outoff, d_out, plan.scans_per_image, out_stride, d_flags);
+    k_ge_scatter<<<dim3(STUFF_CHUNKS, NS), STUFF_THREADS, 0, st>>>(d_so, d_words, d_chunkff, d_outoff, d_out, plan.scans_per_image, out_stride, d_flags);
     LT_MARK("k_ge_scatter");
     CU(cudaMemcpyAsync(h_small + o_outlen, d_outlen, (size_t)NS * 4, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(h_small + o_dht, d_dht, (size_t)NS * 4 * sizeof(DhtOut), cudaMemcpyDeviceToHost, st));

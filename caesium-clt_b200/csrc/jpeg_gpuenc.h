@@ -10,7 +10,7 @@
 namespace b200 {
 
 struct DhtOut { uint8_t bits[17]; uint8_t vals[256]; int32_t nvals; };
-struct ScanOut { uint32_t total_bits, nbytes, ngroups, group_base, word_base, arena_base; };   // filled on the device (k_ge_scanout)
+struct ScanOut { uint32_t total_bits, nbytes, word_base, arena_base; };   // filled on the device (k_ge_scanout)
 
 // One encoder instance per slot (or per megabatch): owns its device / pinned buffers and grows them on demand.
 class GpuEncoder {
@@ -52,7 +52,7 @@ private:
     JpegGeom geom; bool prog = false;
     std::vector<int16_t *> coef_bases;
     void *ev_sizes = nullptr;
-    uint32_t words_cap = 0, groups_cap = 0;
+    uint32_t words_cap = 0;
     size_t est_image_bytes = 0, learned_image_bytes = 0, learned_for = 0;
     DeviceBuffer<uint32_t> d_flags;
     size_t o_scans = 0, o_total = 0, o_outlen = 0, o_dht = 0, o_comps = 0, o_flags = 0;
@@ -71,7 +71,7 @@ private:
     DeviceBuffer<ScanOut> d_so;
     DeviceBuffer<uint32_t> d_words;
     DeviceBuffer<ge::Masks3> d_masks;                   // threshold masks per block, written by the classify pass
-    DeviceBuffer<uint32_t> d_ffcount, d_ffoff;
+    DeviceBuffer<uint32_t> d_chunkff;                   // 0xFF bytes per chunk of each scan (k_ge_ffcount)
     DeviceBuffer<uint32_t> d_outoff, d_outlen;
     DeviceBuffer<uint8_t> d_out;
     DeviceBuffer<uint8_t> d_temp;
