@@ -6,8 +6,8 @@
 // Passes (one launch each for ANY number of images x scans; blockIdx.y = scan):
 //   classify + inline-symbol histogram + correction-bit counts -> [max-scan: previous event] [sum-scan: trailing correction bits] ->
 //   groups + EOBn histogram -> tables + bits per table -> scan sizes / buffer layout (on the device) | D2H: sizes ->
-//   lengths of the interleaved scans' units -> [sum-scan: their bit offsets] -> zero -> emit (single-component scans: CTA runs into a
-//   staging arena) -> [sum-scan: run offsets] -> place runs -> 0xFF count per chunk of each scan -> layout -> scatter (byte stuffing
+//   lengths of the sequential interleaved scans' units -> [sum-scan: their bit offsets] -> zero -> emit (single-component scans: CTA
+//   runs into a staging arena) -> DC-first interleaved scan (MCU runs into the arena) -> [sum-scan: run offsets] -> place runs -> 0xFF count per chunk of each scan -> layout -> scatter (byte stuffing
 //   through shared memory) | D2H: stuffed scans + DHT payloads.  No host wait in between: see "host orchestration".
 #include <cuda_runtime.h>
 #include <cub/device/device_scan.cuh>
@@ -239,8 +239,11 @@ struct SmemHist {
     __device__ void raw64(int, unsigned long long) {}
 };
 // Also each refinement scan's correction bits (corr[scan]), the one part of a scan's size that is not in its histograms.
+// And, for a script with a DC-first interleaved scan, each block's DC coefficient into the compact DC array (dc != nullptr; component
+// at mask_base, entries in MCU order: enc_dc_index) that k_geb_dc_first codes from.
 __global__ void __launch_bounds__(ENC_THREADS) k_geb_classify(const BlockComp *__restrict__ comps, uint32_t *__restrict__ meta, int *__restrict__ evkey,
-                                                              uint32_t *__restrict__ tail, Masks3 *__restrict__ masks, uint32_t *__restrict__ hist, uint32_t *__restrict__ corr)
+                                                              uint32_t *__restrict__ tail, Masks3 *__restrict__ masks, uint32_t *__restrict__ hist, uint32_t *__restrict__ corr,
+                                                              int16_t *__restrict__ dc)
 {
     __shared__ __align__(16) Tile tile;
     __shared__ uint32_t h[ENC_TAB_ENTRIES];
@@ -258,6 +261,7 @@ __global__ void __launch_bounds__(ENC_THREADS) k_geb_classify(const BlockComp *_
         const int row = i / bc.bw, col = i - row * bc.bw;
         const Masks3 M = make_masks3(tile[threadIdx.x]);
         masks[bc.mask_base + i] = M;
+        if (dc) dc[bc.mask_base + enc_dc_index(bc, row, col)] = tile[threadIdx.x][0];
         for (int j = 0; j < bc.nscan; j++) {
             const EncVisit &v = vis[j];
             const int u = enc_unit_of(bc, v.ns, row, col);
@@ -312,28 +316,6 @@ __global__ void __launch_bounds__(ENC_THREADS) k_geb_len(const BlockComp *__rest
         bitlen[v.lu_base + u] = (uint32_t)sk.bits;
     }
 }
-// The same when every interleaved visit is a DC-first one (the progressive script): a unit is one DC difference, so a thread reads
-// its block's and the predecessor's DC coefficient and one code length from global memory -- no tile, masks or table staging.
-constexpr int LEN_DC_THREADS = 256;
-__global__ void __launch_bounds__(LEN_DC_THREADS) k_geb_len_dc(const BlockComp *__restrict__ comps, const Table *__restrict__ tabs, uint32_t *__restrict__ bitlen)
-{
-    const BlockComp &bc = comps[blockIdx.y];
-    const int nblk = bc.bw * bc.bh, i = blockIdx.x * LEN_DC_THREADS + threadIdx.x;
-    if (i >= nblk) return;
-    const int row = i / bc.bw, col = i - row * bc.bw;
-    const int16_t *cb = bc.coef + bc.comp_off;
-    const Masks3 none{};
-    for (int j = 0; j < bc.nscan; j++) {
-        const EncVisit v = bc.visit[j];
-        if (v.ns == 1) continue;
-        const int p = enc_dc_prev(bc, v.ns, row, col);
-        const BlockRef r{cb + (long long)i * 64, p >= 0 ? cb + (long long)p * 64 : nullptr, 0};
-        LenSinkT<KindTabs<const uint32_t>> sk{KindTabs<const uint32_t>{tabs[bc.tab[ENC_AC_SLOTS]].code_len, nullptr}};
-        gen_block_m(v, v.tbl, r, none, 0, sk);
-        bitlen[v.lu_base + enc_unit_of(bc, v.ns, row, col)] = (uint32_t)sk.bits;
-    }
-}
-
 // exclusive prefix sum of x over the CTA, and the CTA's total; every thread calls it (it has a barrier)
 __device__ __forceinline__ uint32_t cta_exclusive_sum(uint32_t x, uint32_t *wsum /*ENC_THREADS / 32*/, uint32_t &total)
 {
@@ -349,7 +331,8 @@ __device__ __forceinline__ uint32_t cta_exclusive_sum(uint32_t x, uint32_t *wsum
     return base + inc - x;
 }
 
-// Emit.  A visit of an interleaved scan writes each unit at the bit offset k_geb_len's lengths gave it.  A visit of a single-component
+// Emit.  A visit of a sequential interleaved scan writes each unit at the bit offset k_geb_len's lengths gave it (a DC-first
+// interleaved scan is k_geb_dc_first's).  A visit of a single-component
 // scan codes its units once for length and bits together: the CTA's units are consecutive units of the scan, so their offsets inside
 // the CTA's run follow from the lengths, and the run's place in the scan from the other runs' lengths (k_ge_place):
 //   - each thread codes its unit into its slot of ENC_SLOT_WORDS words in shared memory, counting bits past the slot's end;
@@ -380,7 +363,8 @@ __global__ void __launch_bounds__(ENC_THREADS) k_geb_emit(const BlockComp *__res
     if ((int)threadIdx.x < bc.nscan) {
         const EncVisit &v = bc.visit[threadIdx.x];
         const ScanOut &o = so[v.scan];
-        vword[threadIdx.x] = v.ns > 1 ? o.word_base : o.arena_base; vbit0[threadIdx.x] = v.ns > 1 ? bitoff[v.lu_base] : 0;
+        const bool unit = v.ns > 1 && v.mode != MODE_DC_FIRST;
+        vword[threadIdx.x] = unit ? o.word_base : o.arena_base; vbit0[threadIdx.x] = unit ? bitoff[v.lu_base] : 0;
     }
     for (int k = threadIdx.x; k < ENC_TAB_ENTRIES; k += ENC_THREADS) {
         int symbol; const int t = enc_entry_table(bc, k, symbol);
@@ -398,7 +382,7 @@ __global__ void __launch_bounds__(ENC_THREADS) k_geb_emit(const BlockComp *__res
         const EncVisit &v = vis[j];
         const int u = live ? enc_unit_of(bc, v.ns, row, col) : -1;
         if (v.ns > 1) {
-            if (u < 0) continue;
+            if (u < 0 || v.mode == MODE_DC_FIRST) continue;
             EmitSink<decltype(orw), decltype(stw), KT> sk(kind_tabs<const uint32_t>(tc, v), orw, stw, (long long)vword[j], (unsigned long long)(bitoff[v.lu_base + u] - vbit0[j]));
             gen_block_m(v, v.tbl, ref_of(v, bc, tile, i0, row, col), M, gcount[v.unit_base + u], sk);
             sk.finish();
@@ -428,7 +412,55 @@ __global__ void __launch_bounds__(ENC_THREADS) k_geb_emit(const BlockComp *__res
     }
 }
 
-// Runs of the single-component scans to their place in the scan's bit buffer: run r of scan y starts runoff[r] - runoff[first run]
+// The DC-first scan with ns > 1 (the progressive script's first scan): one thread per MCU, whose units are consecutive in the scan,
+// coded from the compact DC array (gen_dc_mcu) into the thread's slot; then the CTA's run into the arena as k_geb_emit does for a
+// single-component visit.  A 4:2:0 MCU is six units of ~6 bits; the largest (10 blocks of 16 + 11 bits) overflows the slot and is
+// coded a second time straight to its place.  Grid (MCU runs, images): the scan is script entry `k` of every image.  The minimum of one
+// CTA per SM in the launch bounds keeps ptxas from capping the kernel at 32 registers, where it spills.
+__global__ void __launch_bounds__(ENC_DC_MCUS, 1) k_geb_dc_first(const Scan *__restrict__ scans, int spi, int k, const int16_t *__restrict__ dc,
+                                                              const Table *__restrict__ tabs, const ScanOut *__restrict__ so, const uint32_t *__restrict__ flags,
+                                                              uint32_t *__restrict__ arena, uint32_t *__restrict__ cursor, uint32_t *__restrict__ runlen,
+                                                              uint32_t *__restrict__ runpos)
+{
+    static_assert(ENC_DC_MCUS == ENC_THREADS, "cta_exclusive_sum sums ENC_THREADS lanes");
+    __shared__ uint32_t tc[2 * ENC_DC_SYMBOLS];                         // DC code words of table ids 0 and 1
+    __shared__ uint32_t slot[ENC_SLOT_WORDS][ENC_DC_MCUS];
+    __shared__ uint32_t wsum[ENC_DC_MCUS / 32], run_word;
+    if (flags[0]) return;
+    const int si = blockIdx.y * spi + k;
+    const Scan &s = scans[si];
+    const int nmcu = s.mcux * s.mcuy, m = blockIdx.x * ENC_DC_MCUS + threadIdx.x;
+    if ((int)(blockIdx.x * ENC_DC_MCUS) >= nmcu) return;
+    if (threadIdx.x < 2 * ENC_DC_SYMBOLS) tc[threadIdx.x] = tabs[s.tab_base + threadIdx.x / ENC_DC_SYMBOLS].code_len[threadIdx.x % ENC_DC_SYMBOLS];
+    __syncthreads();
+    struct DcTabs { const uint32_t *t; __device__ uint32_t operator()(int, int tbl, int symbol) const { return t[tbl * ENC_DC_SYMBOLS + symbol]; } };
+    auto sls = [&](long long w, uint32_t v) { if (w < ENC_SLOT_WORDS) slot[w][threadIdx.x] = v; };
+    auto ora = [&](long long w, uint32_t v) { if (v) atomicOr(&arena[w], v); };
+    auto sta = [&](long long w, uint32_t v) { arena[w] = v; };
+    uint32_t nb = 0;
+    if (m < nmcu) {
+        EmitSink<decltype(sls), decltype(sls), DcTabs> sk(DcTabs{tc}, sls, sls, 0, 0);
+        gen_dc_mcu(s, dc, m, sk);
+        sk.finish();
+        nb = (uint32_t)sk.bits_written(0);
+    }
+    uint32_t L;
+    const uint32_t off = cta_exclusive_sum(nb, wsum, L);
+    if (threadIdx.x == 0) {
+        const uint32_t a = so[si].arena_base + atomicAdd(&cursor[si], (L + 31) / 32);
+        run_word = a; runlen[s.run_base + blockIdx.x] = L; runpos[s.run_base + blockIdx.x] = a;
+    }
+    __syncthreads();
+    const unsigned long long at = (unsigned long long)run_word * 32 + off;
+    if (nb <= ENC_SLOT_WORDS * 32) place_bits([&](long long w) { return slot[w][threadIdx.x]; }, nb, at, ora, sta);
+    else {                                  // rare: the MCU overflowed its slot
+        EmitSink<decltype(ora), decltype(sta), DcTabs> sk(DcTabs{tc}, ora, sta, 0, at);
+        gen_dc_mcu(s, dc, m, sk);
+        sk.finish();
+    }
+}
+
+// Runs (of the single-component scans and of the DC-first interleaved scan) to their place in the scan's bit buffer: run r of scan y starts runoff[r] - runoff[first run]
 // bits into the scan (an exclusive sum over the run lengths); one warp per run, funnel-shifting the run's whole arena words.
 constexpr int PLACE_THREADS = 128;
 __global__ void __launch_bounds__(PLACE_THREADS) k_ge_place(const Scan *__restrict__ scans, const ScanOut *__restrict__ so, const uint32_t *__restrict__ runlen,
@@ -590,7 +622,7 @@ bool GpuEncoder::prepare(const JpegGeom &g, bool progressive, int16_t *const *d_
     gpuenc_plan(g, progressive, bases.data(), nimages, plan);
     nimg = nimages;
     const int NS = (int)plan.scans.size();
-    const long long U = plan.total_units, LU = std::max(plan.total_lunits, 1ll);
+    const long long U = plan.total_units, LU = plan.unit_coded ? std::max(plan.total_lunits, 1ll) : 1;
     const int R = std::max(plan.total_runs, 1);
     if (U >= (1ll << 31)) { err = "batch too large for the entropy encoder"; return false; }
     overflow = false;
@@ -606,7 +638,7 @@ bool GpuEncoder::prepare(const JpegGeom &g, bool progressive, int16_t *const *d_
         !grow(d_cursor, (size_t)NS * 4) || !grow(d_runlen, (size_t)R * 4) || !grow(d_runoff, (size_t)R * 4) || !grow(d_runpos, (size_t)R * 4) ||
         !grow(d_hist, (size_t)NS * 4 * 256 * 4) || !grow(d_tabs, (size_t)NS * 4 * sizeof(Table)) || !grow(d_dht, (size_t)NS * 4 * sizeof(DhtOut)) ||
         !grow(d_total, (size_t)NS * 4) || !grow(d_so, (size_t)NS * sizeof(ScanOut)) || !grow(d_outoff, (size_t)NS * 4) || !grow(d_outlen, (size_t)NS * 4) ||
-        !grow(d_flags, 64) || !grow(d_masks, (size_t)plan.total_comp_blocks * sizeof(Masks3)) || !grow(d_chunkff, (size_t)NS * STUFF_CHUNKS * 4)) return false;
+        !grow(d_flags, 64) || !grow(d_masks, (size_t)plan.total_comp_blocks * sizeof(Masks3)) || !grow(d_dc, (size_t)plan.total_comp_blocks * 2) || !grow(d_chunkff, (size_t)NS * STUFF_CHUNKS * 4)) return false;
     o_scans = 0; o_total = o_scans + align_up((size_t)NS * sizeof(Scan), 256); o_outlen = o_total + align_up((size_t)NS * 4, 256);
     o_dht = o_outlen + align_up((size_t)NS * 4, 256); o_comps = o_dht + align_up((size_t)NS * 4 * sizeof(DhtOut), 256);
     o_flags = o_comps + align_up((size_t)NC * sizeof(BlockComp), 256);
@@ -653,6 +685,7 @@ unsigned long long GpuEncoder::signature() const
     int max_units = 0; for (auto &sc : plan.scans) max_units = std::max(max_units, sc.nblocks);
     mix((unsigned long long)max_units);
     mix((unsigned long long)plan.total_lunits); mix((unsigned long long)plan.total_runs); mix((unsigned long long)plan.max_runs);
+    mix((unsigned long long)(plan.dc_first_scan + 1)); mix(plan.unit_coded ? 1 : 0);
     return h;
 }
 
@@ -682,16 +715,9 @@ bool GpuEncoder::enqueue_back(void *stream_, std::string &err)
     uint32_t *h_flags = reinterpret_cast<uint32_t *>(h_small + o_flags);
     const dim3 gb(cdiv(plan.max_comp_blocks, ENC_THREADS), NC);
     int n = 5;
-    if (plan.total_lunits) {                // units of the interleaved scans: lengths, then bit offsets
-        bool dc_only = true;
-        for (auto &sc : plan.scans) if (sc.ns > 1 && sc.mode != MODE_DC_FIRST) dc_only = false;
-        if (dc_only) {
-            k_geb_len_dc<<<dim3(cdiv(plan.max_comp_blocks, LEN_DC_THREADS), NC), LEN_DC_THREADS, 0, st>>>(d_comps, d_tabs, d_bitlen);
-            LT_MARK("k_geb_len_dc");
-        } else {
-            k_geb_len<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_gcount, d_tabs, d_bitlen, d_masks);
-            LT_MARK("k_geb_len");
-        }
+    if (plan.unit_coded) {                  // units of the sequential interleaved scans: lengths, then bit offsets
+        k_geb_len<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_gcount, d_tabs, d_bitlen, d_masks);
+        LT_MARK("k_geb_len");
         size_t tb = d_temp.capacity();
         cub::DeviceScan::ExclusiveSum(d_temp, tb, d_bitlen.get(), d_bitoff.get(), (int)plan.total_lunits, st);
         LT_MARK("cub_scan");
@@ -703,6 +729,12 @@ bool GpuEncoder::enqueue_back(void *stream_, std::string &err)
     LT_MARK("k_ge_zero");
     k_geb_emit<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_gcount, d_tabs, d_bitoff, d_words, d_masks, d_so, d_flags, d_arena, d_cursor, d_runlen, d_runpos);
     LT_MARK("k_geb_emit");
+    if (plan.dc_first_scan >= 0) {
+        k_geb_dc_first<<<dim3(cdiv((long long)geom.mcux * geom.mcuy, ENC_DC_MCUS), nimg), ENC_DC_MCUS, 0, st>>>(d_scans, plan.scans_per_image, plan.dc_first_scan, d_dc,
+                                                                                                         d_tabs, d_so, d_flags, d_arena, d_cursor, d_runlen, d_runpos);
+        LT_MARK("k_geb_dc_first");
+        n++;
+    }
     if (plan.total_runs) {                  // runs of the single-component scans: offsets, then placement
         size_t tb = d_temp.capacity();
         cub::DeviceScan::ExclusiveSum(d_temp, tb, d_runlen.get(), d_runoff.get(), plan.total_runs, st);
@@ -752,7 +784,7 @@ bool GpuEncoder::enqueue_front(void *stream_, bool fill_dummy, std::string &err)
     LT_MARK("memset");
     CU(cudaMemsetAsync(d_corr, 0, (size_t)NS * 4, st));
     LT_MARK("memset");
-    k_geb_classify<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_meta, d_evkey, d_tail, d_masks, d_hist, d_corr);
+    k_geb_classify<<<gb, ENC_THREADS, 0, st>>>(d_comps, d_meta, d_evkey, d_tail, d_masks, d_hist, d_corr, plan.dc_first_scan >= 0 ? d_dc.get() : nullptr);
     LT_MARK("k_geb_classify");
     size_t tb = d_temp.capacity();
     cub::DeviceScan::ExclusiveScan(d_temp, tb, d_evkey.get(), d_prev.get(), cub::Max(), -1, (int)U, st);

@@ -59,7 +59,8 @@ private:
     DeviceBuffer<ge::Scan> d_scans;
     DeviceBuffer<BlockComp> d_comps;
     DeviceBuffer<uint32_t> d_meta, d_tail, d_tsum, d_gcount;
-    DeviceBuffer<uint32_t> d_bitlen, d_bitoff;          // per unit of the interleaved scans (Scan::lu_base)
+    DeviceBuffer<uint32_t> d_bitlen, d_bitoff;          // per unit of the interleaved scans coded unit by unit (Scan::lu_base)
+    DeviceBuffer<int16_t> d_dc;                         // compact DC arrays for the DC-first interleaved scan (k_geb_classify, k_geb_dc_first)
     DeviceBuffer<uint32_t> d_corr;                      // correction bits per scan (k_geb_classify)
     DeviceBuffer<unsigned long long> d_tbits;           // bits coded with each table (k_ge_tables)
     DeviceBuffer<uint32_t> d_cursor, d_runlen, d_runoff, d_runpos, d_arena;   // CTA runs of the single-component scans (k_geb_emit, k_ge_place)

@@ -45,7 +45,8 @@ struct Scan {
     int nblocks;                // units in this scan
     long long unit_base;        // index of unit 0 in the batch-wide per-unit arrays
     long long lu_base;          // ns > 1: index of unit 0 in the per-unit bit length / offset arrays (only these scans have them)
-    int run_base, nruns;        // ns == 1: the scan's first CTA run in the batch-wide run arrays, and its run count
+    int run_base, nruns;        // ns == 1 or a DC-first scan: the scan's first CTA run in the batch-wide run arrays, and its run count
+    long long dc_base[3];       // DC-first scan with ns > 1: first entry of component i (scan order) in the batch-wide compact DC array
     int tab_base;              // index of this scan's first table in the batch-wide table array (4 per scan: [kind*2+tbl])
     long long word_base;        // first word of this scan's unstuffed bit buffer
     long long word_cap;         // capacity in 32-bit words
@@ -230,6 +231,24 @@ GE_HD void gen_dc(int value_shifted, int pred_shifted, int tbl, Sink &sk)
     if (temp < 0) { temp = -temp; temp2--; }
     const int nb = nbits_of((unsigned)temp);
     sk.sym(0, tbl, nb, nb, (unsigned)temp2);
+}
+
+// The units of MCU m of a DC-first scan with ns > 1, in scan order, from the batch-wide compact DC array: component i of the scan
+// has its DC coefficients at dc + s.dc_base[i], in MCU order, hs * vs per MCU, so the predecessor of every block is the entry
+// before it (0 at the component's start).
+template <class Sink>
+GE_HD void gen_dc_mcu(const Scan &s, const int16_t *dc, int m, Sink &sk)
+{
+#if defined(__CUDA_ARCH__)
+#pragma unroll
+#endif
+    for (int i = 0; i < 3; i++) {
+        if (i >= s.ns) break;
+        const int nb = s.hs[i] * s.vs[i];
+        const int16_t *d = dc + s.dc_base[i] + (long long)m * nb;
+        int prev = m ? d[-1] >> s.Al : 0;
+        for (int q = 0; q < nb; q++) { const int v = d[q] >> s.Al; gen_dc(v, prev, s.tbl[i], sk); prev = v; }
+    }
 }
 
 GE_HD int eob_symbol(unsigned count) { return (nbits_of(count) - 1) << 4; }     // EOBn: AC symbol of a group of `count` blocks

@@ -17,6 +17,9 @@ namespace b200 {
 // A CTA of the block-major passes owns ENC_THREADS consecutive blocks of one component.  In a scan with one component these are
 // consecutive units: the CTA's part of such a scan is one run of the scan's bits, coded in one pass (see k_geb_emit).
 constexpr int ENC_THREADS = 128;
+// The DC-first scan of a progressive colour script is coded one MCU per thread (k_geb_dc_first): a CTA's ENC_DC_MCUS consecutive
+// MCUs are consecutive units of the scan, so it too is one run of the scan's bits.
+constexpr int ENC_DC_MCUS = 128;
 constexpr int ENC_MAX_VISITS = 6, ENC_AC_SLOTS = 3, ENC_DC_SLOTS = 1, ENC_DC_SYMBOLS = 17;
 constexpr int ENC_TAB_ENTRIES = ENC_AC_SLOTS * 256 + ENC_DC_SLOTS * ENC_DC_SYMBOLS;   // entry of (AC slot a, symbol) = a * 256 + symbol
 constexpr int ENC_DC_ENTRY = ENC_AC_SLOTS * 256;                                      // entry of (DC slot, symbol) = ENC_DC_ENTRY + symbol
@@ -27,7 +30,7 @@ struct EncVisit {                       // one scan visiting the component: what
     int tbl;                            // the component's Huffman table id
     int unit_base;                      // Scan::unit_base (a batch has fewer than 2^31 units)
     int lu_base;                        // ns > 1: Scan::lu_base
-    int run_base;                       // ns == 1: Scan::run_base
+    int run_base;                       // Scan::run_base
     int ac_entry;                       // first on-chip entry of the visit's AC table (unused by a DC-only scan)
 };
 
@@ -61,6 +64,13 @@ GE_HD int enc_dc_prev(const BlockComp &bc, int ns, int row, int col)
     return -1;
 }
 
+// entry of component block (row, col) in the component's compact DC array: its blocks in MCU order, hs * vs per MCU (the grid of
+// a component of an interleaved image is whole MCUs)
+GE_HD int enc_dc_index(const BlockComp &bc, int row, int col)
+{
+    return ((row / bc.vs) * bc.mcux + col / bc.hs) * (bc.hs * bc.vs) + (row % bc.vs) * bc.hs + col % bc.hs;
+}
+
 // the table of on-chip entry k and the entry's symbol; -1 for a slot the component does not use
 GE_HD int enc_entry_table(const BlockComp &bc, int k, int &symbol)
 {
@@ -77,8 +87,10 @@ struct GpuEncPlan {
     int scans_per_image = 0;
     long long units_per_image = 0, words_per_image = 0;
     long long total_units = 0, total_words = 0, total_comp_blocks = 0;
-    long long total_lunits = 0;         // units of the scans with ns > 1 (the ones coded unit by unit)
-    int total_runs = 0, max_runs = 0;   // CTA runs of the scans with ns == 1: in all, and in the largest scan
+    long long total_lunits = 0;         // units of the scans with ns > 1
+    bool unit_coded = false;            // some scan with ns > 1 is coded unit by unit (k_geb_len, offsets): a sequential colour script
+    int dc_first_scan = -1;             // index in the script of the DC-first scan with ns > 1, coded in MCU runs (k_geb_dc_first)
+    int total_runs = 0, max_runs = 0;   // CTA runs of the scans coded in runs: in all, and in the largest scan
 };
 
 // coef_base[i] = device (or host) pointer to image i's coefficient buffer (geometry g, zigzag)
@@ -91,7 +103,9 @@ inline void gpuenc_plan(const JpegGeom &g, bool progressive, const int16_t *cons
     p.scans.clear();
     long long unit = 0, word = 0, lunit = 0;
     int run = 0;
-    p.max_runs = 0;
+    p.max_runs = 0; p.unit_coded = false; p.dc_first_scan = -1;
+    long long image_blocks = 0;         // the compact DC arrays of an image's components, back to back (= BlockComp::mask_base)
+    for (int c = 0; c < g.ncomp; c++) image_blocks += (long long)g.bw[c] * g.bh[c];
     for (int im = 0; im < nimages; im++) {
         for (int si = 0; si < ns; si++) {
             const ScanDef &d = sc[si];
@@ -113,6 +127,15 @@ inline void gpuenc_plan(const JpegGeom &g, bool progressive, const int16_t *cons
             s.unit_base = unit; unit += s.nblocks;
             s.lu_base = -1; s.run_base = -1; s.nruns = 0;
             if (d.ns > 1) { s.lu_base = lunit; lunit += s.nblocks; }
+            if (d.ns > 1 && s.mode == ge::MODE_DC_FIRST) {
+                if (im == 0) p.dc_first_scan = si;
+                s.run_base = run; s.nruns = (g.mcux * g.mcuy + ENC_DC_MCUS - 1) / ENC_DC_MCUS; run += s.nruns; p.max_runs = std::max(p.max_runs, s.nruns);
+                for (int i = 0; i < d.ns; i++) {
+                    long long b = im * image_blocks;
+                    for (int c = 0; c < d.ci[i]; c++) b += (long long)g.bw[c] * g.bh[c];
+                    s.dc_base[i] = b;
+                }
+            } else if (d.ns > 1) p.unit_coded = true;
             else { s.run_base = run; s.nruns = (g.bw[d.ci[0]] * g.bh[d.ci[0]] + ENC_THREADS - 1) / ENC_THREADS; run += s.nruns; p.max_runs = std::max(p.max_runs, s.nruns); }
             s.tab_base = (int)p.scans.size() * 4;
             s.word_base = word; s.word_cap = (long long)s.nblocks * 32 + 64; word += s.word_cap;   // 128 B per block: the size of its coefficients
