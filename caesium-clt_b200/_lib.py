@@ -69,7 +69,7 @@ _SYMBOLS = [
     "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_jpeg_pipe_destroy", "b200_device_jobs", "b200_device_numa_node", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba", "b200_webp_alpha_filter", "b200_webp_d2h_bytes",
     "b200_set_png_lossy", "b200_png_quantize", "b200_set_jpeg_trellis", "b200_set_gif", "b200_gif_decode", "b200_gif_lzw",
     "b200_set_png_resize", "b200_png_resize_samples", "b200_set_webp_lossless_convert", "b200_set_png_interlaced",
-    "b200_set_gif_convert", "b200_gif_first_frame",
+    "b200_set_gif_convert", "b200_gif_first_frame", "b200_set_webp_anim", "b200_webp_anim_decode",
 ]
 
 
@@ -87,7 +87,7 @@ def lib():
                   "b200_png_decode", "b200_png_decode_reduced", "b200_png_filter", "b200_png_lz77", "b200_png_deflate_tokens",
                   "b200_webp_encode_rgb", "b200_webp_write_levels", "b200_jpeg_encode_coefficients_device",
                   "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba", "b200_png_quantize",
-                  "b200_gif_decode", "b200_gif_lzw", "b200_png_resize_samples", "b200_gif_first_frame"):
+                  "b200_gif_decode", "b200_gif_lzw", "b200_png_resize_samples", "b200_gif_first_frame", "b200_webp_anim_decode"):
             getattr(L, f).restype = Status
         L.b200_webp_d2h_bytes.restype = C.c_ulonglong
         L.b200_version.restype = C.c_char_p
@@ -303,6 +303,26 @@ def gif_first_frame(data):
     out = np.frombuffer(C.string_at(px, h.value * w.value * 4), np.uint8).reshape(h.value, w.value, 4).copy()
     lib().b200_free(px)
     return out
+
+
+def set_webp_anim(on):
+    """b200_set_webp_anim: compress_in_memory on animated WebP sources runs on the device (1) or is refused with code 3 (0, the
+    default).  Any other value is refused with B200_ERR_INVALID_ARGUMENT."""
+    return lib().b200_set_webp_anim(int(on))
+
+
+def webp_anim_decode(data):
+    """b200_webp_anim_decode (host): -> (canvases uint8 [n, h, w, 4] as R, G, B, A, durations list in ms, loop, background bytes)."""
+    w, h, n, loop = C.c_int(), C.c_int(), C.c_int(), C.c_int()
+    bg = (C.c_uint8 * 4)()
+    px, du = C.POINTER(C.c_uint8)(), C.POINTER(C.c_int)()
+    _check(lib().b200_webp_anim_decode(data, C.c_size_t(len(data)), C.byref(w), C.byref(h), C.byref(n), C.byref(loop), bg, C.byref(px), C.byref(du)))
+    size = n.value * h.value * w.value * 4
+    canv = np.frombuffer(C.string_at(px, size), np.uint8).reshape(n.value, h.value, w.value, 4).copy()
+    durations = [du[i] for i in range(n.value)]
+    lib().b200_free(px)
+    lib().b200_free(du)
+    return canv, durations, loop.value, bytes(bg)
 
 
 def gif_lzw(indices, min_code_size):

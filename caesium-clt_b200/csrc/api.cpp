@@ -9,6 +9,7 @@
 #include "../../include/b200_caesium_webp_lossless.h"
 #include "../../include/b200_caesium_png_interlaced.h"
 #include "../../include/b200_caesium_gif_convert.h"
+#include "../../include/b200_caesium_webp_anim.h"
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -40,6 +41,8 @@
 #include "vp8l_alpha.h"
 #include "gif_host.h"
 #include "gif_device.h"
+#include "webp_anim_host.h"
+#include "webp_anim_device.h"
 #include "jpeg_pipe.h"
 #include "topology.h"
 #include "launch_timer.h"
@@ -96,6 +99,7 @@ OptIn g_png_resize{"B200_PNG_RESIZE"};                        // PNG -> PNG with
 OptIn g_webp_lossless_convert{"B200_WEBP_LOSSLESS_CONVERT"};  // JPEG / PNG -> lossless WebP on the device
 OptIn g_png_interlaced{"B200_PNG_INTERLACED"};                // Adam7 PNG sources on every PNG leg
 OptIn g_gif_convert{"B200_GIF_CONVERT"};                      // JPEG / PNG / WebP -> GIF and GIF -> JPEG / PNG / WebP on the device
+OptIn g_webp_anim{"B200_WEBP_ANIM"};                          // animated WebP re-encoded on the device
 
 // runtime_init is idempotent while initialised, so after b200_shutdown (which frees every slot's device buffers) the next call
 // initialises again: a long-running host can hand the memory of one workload's slots back before starting another
@@ -881,8 +885,37 @@ b200_status webp_lossless_compress(const uint8_t *in, size_t in_len, const b200_
     return ok_status();
 }
 
+// Animated WebP (the switch on): frames decoded one at a time on the calling thread, composited on the device and re-encoded there
+// (VP8L with webp.lossless, else K8 at webp.quality with K7-coded alpha); the container is written here.  B200_TRACE=2 prints where
+// the time went.
+b200_status webp_anim_compress(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
+{
+    if (p->width || p->height) return make_status(B200_ERR_UNSUPPORTED, "animated WebP resize is outside the GPU path (route to caesium::compress_in_memory)");
+    std::string err;
+    WebpAnimReader rd;
+    if (!rd.open(in, in_len, err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
+    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
+    SlotLease s(prefer_dev);
+    if (!s) return s.failure();
+    const auto t0 = std::chrono::steady_clock::now();
+    bool corrupt = false;
+    const int q = (int)std::min<uint32_t>(p->webp_quality, 100);
+    WebpAnimDevice *d = s->webp_anim_dev();
+    if (!d->encode(rd, *s->webp_dev(), *s->vp8l_dev(), *s->png_dev(), p->webp_lossless != 0, q, s->stream, out, corrupt, err))
+        return make_status(corrupt ? B200_ERR_CORRUPT_INPUT : B200_ERR_CUDA, err);
+    if (trace_level() >= 2)
+        fprintf(stderr, "[b200 trace] webp-anim %dx%d, %d frames -> %d, %s: call %.3f ms, host decode %.3f ms, compose + diff %.3f ms, %s %.3f ms (host coder %.3f ms)\n",
+                rd.width, rd.height, rd.frames, d->frames_out, p->webp_lossless ? "lossless" : "lossy", ms_between(t0, std::chrono::steady_clock::now()),
+                d->decode_ms, d->compose_ms, p->webp_lossless ? "VP8L" : "K8", d->encode_ms, d->code_ms);
+    return ok_status();
+}
+
 b200_status webp_compress(const uint8_t *in, size_t in_len, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out)
 {
+    if (g_webp_anim.on()) {
+        WebpInfo info; std::string err;
+        if (webp_probe(in, in_len, info, err) && info.animated) return webp_anim_compress(in, in_len, p, prefer_dev, out);
+    }
     if (p->webp_lossless) return webp_lossless_compress(in, in_len, p, prefer_dev, out);
     WebpInfo info; std::vector<uint8_t> rgb, alpha;
     b200_status st = webp_decode_status(in, in_len, info, rgb, &alpha);
@@ -1322,6 +1355,7 @@ int b200_set_png_resize(int on) { return g_png_resize.set(on); }
 int b200_set_webp_lossless_convert(int on) { return g_webp_lossless_convert.set(on); }
 int b200_set_png_interlaced(int on) { return g_png_interlaced.set(on); }
 int b200_set_gif_convert(int on) { return g_gif_convert.set(on); }
+int b200_set_webp_anim(int on) { return g_webp_anim.set(on); }
 int b200_set_jpeg_trellis(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; set_jpeg_trellis(on == 1); return B200_OK; }
 
 uint32_t b200_sniff_format(const uint8_t *d, size_t n)
@@ -1981,6 +2015,30 @@ b200_status b200_gif_decode(const uint8_t *in, size_t in_len, int *width, int *h
         s = give(bytes, rgba, &n);
         if (s.code) { free(*delays); *delays = nullptr; return s; }
         *width = rd.width; *height = rd.height; *nframes = rd.frames; *loop = rd.loop;
+        return s;
+    });
+}
+
+b200_status b200_webp_anim_decode(const uint8_t *in, size_t in_len, int *width, int *height, int *nframes, int *loop, uint8_t bg[4], uint8_t **rgba,
+                                  int **durations)
+{
+    if (!in || !width || !height || !nframes || !loop || !bg || !rgba || !durations) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
+    *rgba = nullptr; *durations = nullptr;
+    return guarded([&] {
+        std::string err;
+        WebpAnimReader rd;
+        std::vector<uint32_t> px, du;
+        if (!webp_anim_decode_all(in, in_len, rd, px, du, err)) return make_status(B200_ERR_CORRUPT_INPUT, err);
+        std::vector<uint8_t> bytes(px.size() * 4);
+        memcpy(bytes.data(), px.data(), bytes.size());
+        const std::vector<int> dl(du.begin(), du.end());
+        size_t n = 0;
+        b200_status s = give(dl, durations, &n);
+        if (s.code) return s;
+        s = give(bytes, rgba, &n);
+        if (s.code) { free(*durations); *durations = nullptr; return s; }
+        *width = rd.width; *height = rd.height; *nframes = rd.frames; *loop = rd.loop;
+        memcpy(bg, rd.bg, 4);
         return s;
     });
 }

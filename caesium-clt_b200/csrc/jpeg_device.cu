@@ -21,6 +21,7 @@
 #include "webp_device.h"
 #include "vp8l_device.h"
 #include "gif_device.h"
+#include "webp_anim_device.h"
 #include "stream_wait.h"
 #include "launch_timer.h"
 
@@ -211,6 +212,7 @@ PngDevice *Slot::png_dev() { if (!png) png.reset(new PngDevice()); return png.ge
 WebpDevice *Slot::webp_dev() { if (!webp) webp.reset(new WebpDevice()); return webp.get(); }
 Vp8lDevice *Slot::vp8l_dev() { if (!vp8l) vp8l.reset(new Vp8lDevice()); return vp8l.get(); }
 GifDevice *Slot::gif_dev() { if (!gif) gif.reset(new GifDevice()); return gif.get(); }
+WebpAnimDevice *Slot::webp_anim_dev() { if (!webp_anim) webp_anim.reset(new WebpAnimDevice()); return webp_anim.get(); }
 
 int runtime_device_count() { std::lock_guard<std::mutex> lk(g_mu); return g_inited ? (int)g_devs.size() : 0; }
 long long runtime_device_jobs(int i) { return g_devs.empty() || i < 0 || i >= (int)g_devs.size() ? 0 : g_devs[(size_t)i]->jobs.load(); }

@@ -56,6 +56,7 @@ struct PngDevice;
 struct WebpDevice;
 struct Vp8lDevice;
 struct GifDevice;
+struct WebpAnimDevice;
 struct Slot {
     int dev = 0;
     void *stream = nullptr;
@@ -70,6 +71,7 @@ struct Slot {
     std::unique_ptr<WebpDevice> webp;                                                    // WebP / VP8 state (lazy, webp_device.cu)
     std::unique_ptr<Vp8lDevice> vp8l;                                                    // lossless WebP / VP8L state (lazy, vp8l_encode.cpp)
     std::unique_ptr<GifDevice> gif;                                                      // GIF state (lazy, gif_device.cu)
+    std::unique_ptr<WebpAnimDevice> webp_anim;                                           // animated WebP state (lazy, webp_anim_device.cu)
     // megabatch path: transform work lists of the current megabatch, and the captured launch sequence (two CUDA graphs, see
     // slot_run_group) with the signature it was captured for
     WorkLists group_wl; size_t group_par_bytes = 0, group_work_off = 0;
@@ -83,6 +85,7 @@ struct Slot {
     WebpDevice *webp_dev();
     Vp8lDevice *vp8l_dev();
     GifDevice *gif_dev();
+    WebpAnimDevice *webp_anim_dev();
     Resampler resampler{Grow::Slot};                                                     // K3 of the sample stages
     Slot();
     Slot(const Slot &) = delete;

@@ -350,10 +350,17 @@ int webp_decode_rgb(const uint8_t *data, size_t len, WebpInfo &info, std::vector
     if (alpha) alpha->clear();
     if (!find_vp8(data, len, &f, &flen, info, err, &oc)) return 2;
     if (info.animated) { err = "animated WebP is outside the GPU path (route to caesium::compress_in_memory)"; return 1; }
+    return webp_decode_chunks(f, flen, oc.alph, oc.alph_len, oc.vp8l, oc.vp8l_len, info, rgb, err, alpha);
+}
+
+int webp_decode_chunks(const uint8_t *f, size_t flen, const uint8_t *alph, size_t alph_len, const uint8_t *vp8l, size_t vp8l_len, WebpInfo &info,
+                       std::vector<uint8_t> &rgb, std::string &err, std::vector<uint8_t> *alpha)
+{
+    if (alpha) alpha->clear();
     if (info.lossless && !f) {
         // lossless file: the VP8L decoder gives ARGB; the alpha plane is reported only if some pixel is not opaque
         std::vector<uint32_t> argb; int W = 0, H = 0; bool hint = false;
-        if (!vp8l_decode_file_chunk(oc.vp8l, oc.vp8l_len, W, H, hint, argb, err)) return 2;
+        if (!vp8l_decode_file_chunk(vp8l, vp8l_len, W, H, hint, argb, err)) return 2;
         info.width = W; info.height = H;
         const size_t n = (size_t)W * H;
         rgb.resize(3 * n);
@@ -640,8 +647,8 @@ int webp_decode_rgb(const uint8_t *data, size_t len, WebpInfo &info, std::vector
         }
     }
     if (info.has_alpha) {
-        // the ALPH chunk describes the canvas, which for a still image is the frame
-        if (!webp_alpha_decode(oc.alph, oc.alph_len, W, H, *alpha, err)) return 2;
+        // the ALPH chunk has the frame's size (for a still image, the canvas's)
+        if (!webp_alpha_decode(alph, alph_len, W, H, *alpha, err)) return 2;
         bool any = false;
         for (uint8_t a : *alpha) if (a != 0xFF) { any = true; break; }
         if (!any) { alpha->clear(); info.has_alpha = false; }

@@ -19,5 +19,10 @@ bool webp_probe(const uint8_t *data, size_t len, WebpInfo &info, std::string &er
 // (optional) receives the alpha plane [h][w] when some pixel is not opaque (info.has_alpha), else it is left empty; without it a
 // file with transparency is refused.  Returns 0 ok, 1 unsupported feature (animation; alpha not asked for), 2 corrupt.
 int webp_decode_rgb(const uint8_t *data, size_t len, WebpInfo &info, std::vector<uint8_t> &rgb_planar, std::string &err, std::vector<uint8_t> *alpha = nullptr);
+// The same decode from one image's chunk payloads once the container is walked (a still file's, or one animation frame's): vp8 /
+// vp8_len the 'VP8 ' payload and alph / alph_len its ALPH payload, or vp8l / vp8l_len a VP8L payload.  info.lossless and
+// info.has_alpha say which of them the caller found; the rest of info is filled in.  Returns as webp_decode_rgb.
+int webp_decode_chunks(const uint8_t *vp8, size_t vp8_len, const uint8_t *alph, size_t alph_len, const uint8_t *vp8l, size_t vp8l_len, WebpInfo &info,
+                       std::vector<uint8_t> &rgb_planar, std::string &err, std::vector<uint8_t> *alpha = nullptr);
 
 } // namespace b200
