@@ -70,6 +70,7 @@ _SYMBOLS = [
     "b200_set_png_lossy", "b200_png_quantize", "b200_set_jpeg_trellis", "b200_set_gif", "b200_gif_decode", "b200_gif_lzw",
     "b200_set_png_resize", "b200_png_resize_samples", "b200_set_webp_lossless_convert", "b200_set_png_interlaced",
     "b200_set_gif_convert", "b200_gif_first_frame", "b200_set_webp_anim", "b200_webp_anim_decode",
+    "b200_set_png_zopfli", "b200_png_lz77_zopfli",
 ]
 
 
@@ -87,7 +88,8 @@ def lib():
                   "b200_png_decode", "b200_png_decode_reduced", "b200_png_filter", "b200_png_lz77", "b200_png_deflate_tokens",
                   "b200_webp_encode_rgb", "b200_webp_write_levels", "b200_jpeg_encode_coefficients_device",
                   "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba", "b200_png_quantize",
-                  "b200_gif_decode", "b200_gif_lzw", "b200_png_resize_samples", "b200_gif_first_frame", "b200_webp_anim_decode"):
+                  "b200_gif_decode", "b200_gif_lzw", "b200_png_resize_samples", "b200_gif_first_frame", "b200_webp_anim_decode",
+                  "b200_png_lz77_zopfli"):
             getattr(L, f).restype = Status
         L.b200_webp_d2h_bytes.restype = C.c_ulonglong
         L.b200_version.restype = C.c_char_p
@@ -309,6 +311,22 @@ def set_webp_anim(on):
     """b200_set_webp_anim: compress_in_memory on animated WebP sources runs on the device (1) or is refused with code 3 (0, the
     default).  Any other value is refused with B200_ERR_INVALID_ARGUMENT."""
     return lib().b200_set_webp_anim(int(on))
+
+
+def set_png_zopfli(on):
+    """b200_set_png_zopfli: png_force_zopfli takes the iterated optimal LZ77 parse on every PNG output (1) or is accepted and
+    ignored (0, the default).  Any other value is refused with B200_ERR_INVALID_ARGUMENT."""
+    return lib().b200_set_png_zopfli(int(on))
+
+
+def png_lz77_zopfli(stream, bpp, stride):
+    """b200_png_lz77_zopfli: the optimal parse of a filtered stream on the device -> tokens uint32[nt] in png_lz77's format."""
+    s = np.ascontiguousarray(stream, dtype=np.uint8).reshape(-1)
+    tok, nt = C.POINTER(C.c_uint32)(), C.c_size_t()
+    _check(lib().b200_png_lz77_zopfli(s.ctypes.data_as(C.c_void_p), C.c_size_t(s.size), int(bpp), int(stride), C.byref(tok), C.byref(nt)))
+    out = np.frombuffer(C.string_at(tok, nt.value * 4), dtype=np.uint32).copy()
+    lib().b200_free(tok)
+    return out
 
 
 def webp_anim_decode(data):

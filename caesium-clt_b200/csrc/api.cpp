@@ -10,6 +10,7 @@
 #include "../../include/b200_caesium_png_interlaced.h"
 #include "../../include/b200_caesium_gif_convert.h"
 #include "../../include/b200_caesium_webp_anim.h"
+#include "../../include/b200_caesium_png_zopfli.h"
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -100,6 +101,7 @@ OptIn g_webp_lossless_convert{"B200_WEBP_LOSSLESS_CONVERT"};  // JPEG / PNG -> l
 OptIn g_png_interlaced{"B200_PNG_INTERLACED"};                // Adam7 PNG sources on every PNG leg
 OptIn g_gif_convert{"B200_GIF_CONVERT"};                      // JPEG / PNG / WebP -> GIF and GIF -> JPEG / PNG / WebP on the device
 OptIn g_webp_anim{"B200_WEBP_ANIM"};                          // animated WebP re-encoded on the device
+OptIn g_png_zopfli{"B200_PNG_ZOPFLI"};                        // png_force_zopfli: the iterated optimal LZ77 parse on PNG outputs
 
 // runtime_init is idempotent while initialised, so after b200_shutdown (which frees every slot's device buffers) the next call
 // initialises again: a long-running host can hand the memory of one workload's slots back before starting another
@@ -428,6 +430,15 @@ void jpeg_compress_group(const uint8_t *const *in, const size_t *in_len, const s
 
 b200_status png_lossy_compress(PngInfo &info, const PngIdat &idat, const b200_params *p, int prefer_dev, std::vector<uint8_t> &out, uint32_t nw, uint32_t nh);
 
+// The slot's PNG back end for a call with params p.  The one place --zopfli is decided: png_force_zopfli takes the optimal parse
+// only while the switch is on (off, the flag is accepted and ignored, as before).
+PngDevice *png_back_end(Slot *s, const b200_params *p)
+{
+    PngDevice *png = s->png_dev();
+    png->zopfli = p->png_force_zopfli && g_png_zopfli.on();
+    return png;
+}
+
 // a failed PngDevice call: the input's fault (code 4); with a resize, a failed allocation is out of memory (code 7); else a CUDA error
 b200_status png_device_status(const PngDevice *png, bool resize, const std::string &err)
 {
@@ -484,7 +495,7 @@ b200_status png_compress(const uint8_t *in, size_t in_len, const b200_params *p,
     {   // the slot goes back before the container is written
         SlotLease s(prefer_dev);
         if (!s) return s.failure();
-        PngDevice *png = s->png_dev();
+        PngDevice *png = png_back_end(s, p);
         // the IDAT stream is inflated straight into the slot's pinned staging buffer; from there on everything is device work
         // (un-filter, checksum, reductions, filter trials, LZ77, DEFLATE coding) until the finished zlib stream comes back
         size_t nfilt; uint32_t stored_adler;
@@ -529,14 +540,15 @@ void drop_colour_chunks(std::vector<uint8_t> &kept, bool grey_source)
 
 // One lossy PNG try: the quantiser already holds the image (histogram built); palette at `quality`, dithering, indexed coding, file.
 // B200_TRACE=2 prints the per-kernel event times.
-b200_status png_lossy_code(Slot *s, PngInfo info, int quality, int level, std::vector<uint8_t> &out)
+b200_status png_lossy_code(Slot *s, PngInfo info, int quality, const b200_params *p, std::vector<uint8_t> &out)
 {
+    const int level = (int)p->png_optimization_level;
     const bool verbose = trace_level() >= 2;
     std::string err;
     std::vector<uint8_t> z;
     LaunchTrace tr(s->stream, verbose);
     const auto t0 = std::chrono::steady_clock::now();
-    if (!s->png_dev()->code_quantized(info, quality < 0 ? 0 : quality > 100 ? 100 : quality, std::min(level, 6), s->stream, z, err)) return make_status(B200_ERR_CUDA, err);
+    if (!png_back_end(s, p)->code_quantized(info, quality < 0 ? 0 : quality > 100 ? 100 : quality, std::min(level, 6), s->stream, z, err)) return make_status(B200_ERR_CUDA, err);
     if (verbose) {
         const std::string kt = tr.kernel_ms();
         fprintf(stderr, "[b200 trace] png-lossy %ux%u q%d: %d colours, device %.3f ms (median cut %.3f); kernels ms:%s\n", info.width, info.height, quality,
@@ -571,7 +583,7 @@ b200_status png_lossy_compress(PngInfo &info, const PngIdat &idat, const b200_pa
     if (!s) return s.failure();
     const b200_status st = png_lossy_load(s, info, idat, nw, nh);
     if (st.code) return st;
-    return png_lossy_code(s, info, (int)p->png_quality, (int)p->png_optimization_level, out);
+    return png_lossy_code(s, info, (int)p->png_quality, p, out);
 }
 
 // 8-bit planar samples ([nc][h][w], nc = 1 or 3) and an optional alpha plane -> lossless PNG (K6 filter selection, K7 LZ77) on the
@@ -583,7 +595,7 @@ b200_status png_from_planes(Slot *s, const uint8_t *planes, int nc, const uint8_
         PngQuant *q = s->png_dev()->quantiser();
         if (!q->load_planes(planes, nc, alpha, (int)w, (int)h, s->stream, err) || !q->prepare(s->stream, err)) return make_status(B200_ERR_CUDA, err);
         PngInfo info; info.width = w; info.height = h;
-        return png_lossy_code(s, info, (int)p->png_quality, (int)p->png_optimization_level, out);
+        return png_lossy_code(s, info, (int)p->png_quality, p, out);
     }
     const size_t n = (size_t)w * h;
     const int ch = nc + (alpha ? 1 : 0);
@@ -600,7 +612,7 @@ b200_status png_from_planes(Slot *s, const uint8_t *planes, int nc, const uint8_
     info.bits_per_pixel = 8 * ch; info.bpp = ch; info.row_bytes = (size_t)w * ch;
     if (palette) png_reduce_palette(info, raw);
     std::vector<uint8_t> z;
-    if (!s->png_dev()->compress(info, raw, std::min((int)p->png_optimization_level, 6), s->stream, z, nullptr, err)) return make_status(B200_ERR_CUDA, err);
+    if (!png_back_end(s, p)->compress(info, raw, std::min((int)p->png_optimization_level, 6), s->stream, z, nullptr, err)) return make_status(B200_ERR_CUDA, err);
     png_write(info, z, out);
     return ok_status();
 }
@@ -1356,6 +1368,7 @@ int b200_set_webp_lossless_convert(int on) { return g_webp_lossless_convert.set(
 int b200_set_png_interlaced(int on) { return g_png_interlaced.set(on); }
 int b200_set_gif_convert(int on) { return g_gif_convert.set(on); }
 int b200_set_webp_anim(int on) { return g_webp_anim.set(on); }
+int b200_set_png_zopfli(int on) { return g_png_zopfli.set(on); }
 int b200_set_jpeg_trellis(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; set_jpeg_trellis(on == 1); return B200_OK; }
 
 uint32_t b200_sniff_format(const uint8_t *d, size_t n)
@@ -1523,7 +1536,7 @@ static b200_status png_to_size(const uint8_t *in, size_t in_len, b200_params *pa
     if (st.code) return st;
     auto size_at = [&](int q, auto want, size_t &sz, std::vector<uint8_t> &cur) -> b200_status {
         (void)want;
-        const b200_status r = png_lossy_code(s, info, q, (int)params->png_optimization_level, cur);
+        const b200_status r = png_lossy_code(s, info, q, params, cur);
         sz = cur.size();
         return r;
     };
@@ -1832,6 +1845,17 @@ b200_status b200_png_lz77(const uint8_t *filtered, size_t n, int bpp, int stride
     if (!png_stage_lz77(filtered, n, bpp, stride, t, hist, err)) return make_status(B200_ERR_CUDA, err);
     return give(t, tokens, ntokens);
 }
+b200_status b200_png_lz77_zopfli(const uint8_t *filtered, size_t n, int bpp, int stride, uint32_t **tokens, size_t *ntokens)
+{
+    if (!filtered || !n || !tokens || !ntokens || bpp < 1 || bpp > 8 || stride < 1) return make_status(B200_ERR_INVALID_ARGUMENT, "invalid argument");
+    std::string err;
+    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
+    SlotLease s(-1);
+    if (!s) return s.failure();
+    std::vector<uint32_t> t;
+    if (!s->png_dev()->lz77_tokens(filtered, n, bpp, stride, true, s->stream, t, err)) return make_status(B200_ERR_CUDA, err);
+    return give(t, tokens, ntokens);
+}
 b200_status b200_png_deflate_tokens(const uint32_t *tokens, size_t ntokens, uint32_t adler, uint8_t **out, size_t *out_len)
 {
     if ((!tokens && ntokens) || !out || !out_len) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
@@ -1928,7 +1952,8 @@ b200_status b200_png_device_times(const uint8_t *in, size_t in_len, int level, i
     {
         SlotLease s(-1);
         if (!s) return s.failure();
-        PngDevice *png = s->png_dev();
+        b200_params p; b200_params_default(&p);
+        PngDevice *png = png_back_end(s, &p);
         size_t nfilt; uint32_t adler;
         const b200_status ist = png_inflate(png, info0, idat, nfilt, adler);
         if (ist.code) return ist;

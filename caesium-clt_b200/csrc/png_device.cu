@@ -11,6 +11,7 @@
 #include "png_kernels.h"
 #include "png_deflate.h"
 #include "png_quant.h"
+#include "png_zopfli.h"
 #include "png_resize.h"
 #include "resize_kernels.h"
 #include <chrono>
@@ -346,11 +347,26 @@ bool PngDevice::reduce_and_code(PngInfo &info, bool probed, const uint32_t *h_fl
         rc = launch_png_deflate(d_out, d_ntok, n, kBlockTokens, d_dfl, reinterpret_cast<uint32_t *>(d_z.get()), z_cap, d_total, st);
         if (!launch_ok(rc, "png deflate", err)) return false;
         CU(cudaMemcpyAsync(h_total, d_total, 16, cudaMemcpyDeviceToHost, st));
+        if (zopfli) {   // --zopfli: the optimal parse of the same stream, coded into its own buffer behind the greedy one
+            if (!zop) zop.reset(new PngZopfli());
+            unsigned long long *d_ztotal = reinterpret_cast<unsigned long long *>(d_hist + 1036);
+            uint32_t *d_zntok = d_hist + 1034;
+            if (!grow(zop->d_z, z_cap + 64, err) || !zop->tokens(wfilt, n, bpp, (int)rb + 1, d_tok, d_counts, kChunk, d_out, st, err)) return false;
+            k_png_ntok<<<1, 32, 0, st>>>(zop->d_segn, zop->d_offsets, PngZopfli::nseg(n), d_zntok);
+            rc = launch_png_deflate(d_out, d_zntok, n, kBlockTokens, d_dfl, reinterpret_cast<uint32_t *>(zop->d_z.get()), z_cap, d_ztotal, st);
+            if (!launch_ok(rc, "png zopfli deflate", err)) return false;
+            CU(cudaMemcpyAsync(h_total + 2, d_ztotal, 16, cudaMemcpyDeviceToHost, st));
+        }
         CU(cudaMemcpyAsync(h_sums, d_sums, npieces * 16, cudaMemcpyDeviceToHost, st));
         CU(stream_wait(st)); LT_MARK("host_wait");
-        const size_t zbytes = (size_t)((h_total[0] + 7) / 8);
+        size_t zbytes = (size_t)((h_total[0] + 7) / 8);
+        const uint8_t *zsrc = d_z;
+        if (zopfli) {   // the smaller payload; the greedy one on a tie
+            const size_t zz = (size_t)((h_total[2] + 7) / 8);
+            if (zz < zbytes && zz + 8 <= z_cap) { zbytes = zz; zsrc = zop->d_z; }
+        }
         if (zbytes + 8 <= z_cap) {
-            CU(cudaMemcpyAsync(h_z, d_z, zbytes, cudaMemcpyDeviceToHost, st)); LT_MARK("d2h");
+            CU(cudaMemcpyAsync(h_z, zsrc, zbytes, cudaMemcpyDeviceToHost, st)); LT_MARK("d2h");
             CU(stream_wait(st)); LT_MARK("host_wait");
             const uint32_t adler = combine_adler(h_sums, n);
             zlib_stream.resize(zbytes + 4);
@@ -381,6 +397,11 @@ bool PngDevice::reduce_and_code(PngInfo &info, bool probed, const uint32_t *h_fl
 // its pixel / row candidates and the hash chains, parallel parse, compaction; the tokens come back to the host (vp8l_alpha.cpp codes them).
 bool PngDevice::plane_tokens(const uint8_t *plane, size_t n, int stride, void *stream_, std::vector<uint32_t> &tokens, std::string &err)
 {
+    return lz77_tokens(plane, n, 1, stride, false, stream_, tokens, err);
+}
+
+bool PngDevice::lz77_tokens(const uint8_t *plane, size_t n, int bpp, int stride, bool optimal, void *stream_, std::vector<uint32_t> &tokens, std::string &err)
+{
     cudaStream_t st = (cudaStream_t)stream_;
     if (!n || stride < 1) { err = "empty plane"; return false; }
     if (!ensure_buffers(n, n, (size_t)stride, st, err)) return false;
@@ -388,18 +409,24 @@ bool PngDevice::plane_tokens(const uint8_t *plane, size_t n, int stride, void *s
     memcpy(h_raw, plane, n);
     CU(cudaMemcpyAsync(d_filt, h_raw, n, cudaMemcpyHostToDevice, st));
     const size_t nchunks = (n + kChunk - 1) / kChunk;
-    int rc = launch_png_match(d_filt, d_best, n, 1, stride, st);
+    int rc = launch_png_match(d_filt, d_best, n, bpp, stride, st);
     if (!rc) rc = launch_png_hashmatch(d_filt, d_best, n, d_hist + 2048, st);
     if (!launch_ok(rc, "png kernels", err)) return false;
     CU(cudaMemsetAsync(d_hist, 0, 316 * 4, st));
     rc = launch_png_parse(d_best, d_filt, n, kChunk, d_tok, d_counts, d_hist, st);
     if (!launch_ok(rc, "png parse", err)) return false;
-    size_t tb = d_temp.capacity();
-    cub::DeviceScan::ExclusiveSum(d_temp, tb, d_counts.get(), d_offsets.get(), (int)nchunks, st);
-    rc = launch_png_compact(d_tok, d_counts, d_offsets, nchunks, kChunk, d_out, st);
-    if (!launch_ok(rc, "png compact", err)) return false;
     uint32_t *d_ntok = d_hist + 1032;
-    k_png_ntok<<<1, 32, 0, st>>>(d_counts, d_offsets, nchunks, d_ntok);
+    if (optimal) {
+        if (!zop) zop.reset(new PngZopfli());
+        if (!zop->tokens(d_filt, n, bpp, stride, d_tok, d_counts, kChunk, d_out, st, err)) return false;
+        k_png_ntok<<<1, 32, 0, st>>>(zop->d_segn, zop->d_offsets, PngZopfli::nseg(n), d_ntok);
+    } else {
+        size_t tb = d_temp.capacity();
+        cub::DeviceScan::ExclusiveSum(d_temp, tb, d_counts.get(), d_offsets.get(), (int)nchunks, st);
+        rc = launch_png_compact(d_tok, d_counts, d_offsets, nchunks, kChunk, d_out, st);
+        if (!launch_ok(rc, "png compact", err)) return false;
+        k_png_ntok<<<1, 32, 0, st>>>(d_counts, d_offsets, nchunks, d_ntok);
+    }
     uint32_t *h_n = reinterpret_cast<uint32_t *>(h_small + 64);
     CU(cudaMemcpyAsync(h_n, d_ntok, 4, cudaMemcpyDeviceToHost, st));
     CU(stream_wait(st));

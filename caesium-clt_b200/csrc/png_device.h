@@ -13,6 +13,7 @@
 namespace b200 {
 
 struct PngQuant;
+struct PngZopfli;
 
 // strategies tried per oxipng optimisation level 0..6 (PngStrategy values)
 std::vector<int> png_level_strategies(int level);
@@ -27,6 +28,10 @@ struct PngDevice {
     size_t z_cap = 0;
     bool corrupt = false;                                // the last failure was the INPUT's fault (bad filter byte, Adler-32 mismatch)
     size_t tlog_n = 0;
+    // --zopfli (png_force_zopfli with the switch on, decided by the caller): reduce_and_code also codes the winner's filtered stream
+    // from the iterated optimal parse (png_zopfli.cu) and keeps the smaller zlib payload, the greedy / lazy one on a tie
+    bool zopfli = false;
+    std::unique_ptr<PngZopfli> zop;
     double last_deflate_ms = 0;                          // host Huffman/bit-packing time of the last compress() (tracing)
     PngDevice();
     ~PngDevice();
@@ -61,6 +66,8 @@ struct PngDevice {
     bool run_strategy(int strategy, int h, int rb, int bpp, void *stream, std::string &err, uint8_t *filt = nullptr, bool do_filter = true, bool with_hash = true);
     // K7 over a byte plane on the host (bpp 1, stride = width) -> compacted LZ77 tokens on the host
     bool plane_tokens(const uint8_t *plane, size_t n, int stride, void *stream, std::vector<uint32_t> &tokens, std::string &err);
+    // the same over a filtered stream with filter distance bpp; optimal: the --zopfli parse instead of the greedy / lazy one
+    bool lz77_tokens(const uint8_t *s, size_t n, int bpp, int stride, bool optimal, void *stream, std::vector<uint32_t> &tokens, std::string &err);
     DeviceBuffer<uint8_t> d_filt_all;                   // the trials' filtered streams, one after another
     // the resize: source planes, resized planes, and K3's tables and intermediate
     DeviceBuffer<uint8_t> d_planes, d_rplanes;

@@ -13,6 +13,7 @@
 #include <cstdint>
 #include "png_kernels.h"
 #include "png_match_core.h"
+#include "png_zopfli_core.h"
 #include "launch_timer.h"
 
 namespace b200 {
@@ -306,20 +307,14 @@ constexpr int HM_SEG = 16384, HM_THREADS = 512, HM_ITEMS = HM_SEG / HM_THREADS, 
 // replaces are: in photographic residuals (3 - 4 bits per byte after Huffman coding) a 5-byte repeat 10,000 bytes back costs more
 // than its literals and flattens the distance statistics of the matches that matter; in text or flat art the bytes a repeat covers
 // are the rare, expensive ones.  So the stream is measured first -- a byte histogram, from it the order-0 cost of every byte value
-// in 1024ths of a bit (integer arithmetic, the same on the device and in the oracle) -- and a hash candidate is accepted when the
+// in 1024ths of a bit (pz_log2_q10: integer arithmetic, the same on the device and in the oracle) -- and a hash candidate is accepted when the
 // literals it would replace cost at least 1.25 x (7 bits of length code + 5 of distance code + the distance's extra bits).
 // (zlib's TOO_FAR rule, made proportional.)  The fixed pixel / row candidates are not subject to it.
-__host__ __device__ inline uint32_t log2_q10(unsigned long long x)
-{   // 1024 * log2(x), piecewise linear between powers of two (exact at them, at most 0.09 low in between); x >= 1
-    int e = 63; while (!((x >> e) & 1ull)) e--;
-    const unsigned long long frac = e >= 10 ? (x >> (e - 10)) & 1023ull : (x << (10 - e)) & 1023ull;
-    return (uint32_t)e * 1024u + (uint32_t)frac;
-}
 // cost[0..255] = literal costs, cost[256..285] = match cost per distance code
 __host__ __device__ inline void hash_cost_tables(const uint32_t *hist256, unsigned long long n, uint32_t *cost /*286*/)
 {
-    const uint32_t ln = log2_q10(n ? n : 1);
-    for (int v = 0; v < 256; v++) { const uint32_t c = hist256[v] ? ln - log2_q10(hist256[v]) : 16u * 1024u; cost[v] = c < 256u ? 256u : c; }
+    const uint32_t ln = pz_log2_q10(n ? n : 1);
+    for (int v = 0; v < 256; v++) { const uint32_t c = hist256[v] ? ln - pz_log2_q10(hist256[v]) : 16u * 1024u; cost[v] = c < 256u ? 256u : c; }
     for (int ds = 0; ds < 30; ds++) cost[256 + ds] = (uint32_t)(7 + 5 + (ds < 4 ? 0 : (ds >> 1) - 1)) * 1280u;
 }
 __global__ void __launch_bounds__(256) k_png_bytehist(const uint8_t *__restrict__ s, size_t n, uint32_t *__restrict__ hist)

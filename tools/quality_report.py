@@ -3,8 +3,8 @@ writes the same bytes as the CUDA path -- that equality is what the GPU tests as
 quality number, standard tables, optimised Huffman, progressive) and, for the WebP leg, libwebp (Pillow) at equal -q.
 The reference (libcaesium -> mozjpeg with trellis quantisation, deringing and scan optimisation) is expected to produce
 SMALLER files than ours at equal -q; libjpeg-turbo, its parent without those three, is the closest stand-in that exists here.
-CPU only.  Writes profiles/quality.json.  usage: python tools/quality_report.py [jpeg_trellis]
-(with `jpeg_trellis`, only that section is recomputed and the others are kept as they are)"""
+CPU only.  Writes profiles/quality.json.  usage: python tools/quality_report.py [jpeg_trellis | png_zopfli]
+(with a section's name, only that section is recomputed and the others are kept as they are)"""
 import io
 import json
 import os
@@ -93,6 +93,7 @@ def main():
                 row[f"pillow_mediancut_256_{k}_blur_mae"] = round(blur_mae(v, rgba), 3)
             out["png_lossy"].append(row)
     out["jpeg_trellis"] = jpeg_trellis()
+    out["png_zopfli"] = png_zopfli()
     with open(os.path.join(ROOT, "profiles", "quality.json"), "w") as f:
         json.dump(out, f, indent=1)
     for r in out["jpeg"] + out["webp"] + out["png_lossy"] + out["jpeg_trellis"]["rows"]:
@@ -127,15 +128,42 @@ def jpeg_trellis():
             "rows": rows, "bd_rate_percent": bd}
 
 
+def png_zopfli():
+    """PNG --zopfli (b200_set_png_zopfli; the twin's tokens are the device's, and the device's DEFLATE writer is the host writer's twin):
+    zlib payload bytes of one filtered stream coded from the default greedy / lazy parse, from the optimal parse (what the device emits
+    is the smaller of the two), and by zlib level 9, on the seeded flat-art and text images of the tests at two filter strategies"""
+    import zlib
+    import png_zopfli_cases as cases
+    from oracle import png_zopfli as Z
+    import __graft_entry__ as G
+    L = G._pkg()
+    rows = []
+    for name, img in (("flat art 320x200", cases.flat(320, 200)), ("text 320x160", cases.text(320, 160)), ("photograph 256x192", cases.photo(256, 192))):
+        for strategy, sname in ((0, "None"), (5, "MinSum")):
+            st, bpp, stride = cases.filtered(img, strategy)
+            ad = zlib.adler32(st.tobytes())
+            greedy = len(L.png_deflate_tokens(O.png_lz77(st, bpp, stride)[0], ad))
+            optimal = len(L.png_deflate_tokens(Z.lz77_zopfli(st, bpp, stride), ad))
+            z9 = len(zlib.compress(st.tobytes(), 9))
+            rows.append({"input": name, "filter": sname, "stream_bytes": int(st.size), "default_bytes": greedy, "zopfli_bytes": optimal,
+                         "emitted_bytes": min(greedy, optimal), "zlib9_bytes": z9, "emitted_over_zlib9": round(min(greedy, optimal) / z9, 4),
+                         "default_over_zlib9": round(greedy / z9, 4)})
+    return {"what": "zlib payload bytes of one filtered stream: the default parse, the --zopfli parse, the smaller of the two (what the device "
+                    "emits with the switch and flag on) and zlib level 9; CPU twin, identical to the device's bytes", "rows": rows}
+
+
+SECTIONS = {"jpeg_trellis": (jpeg_trellis, lambda r: r["bd_rate_percent"]), "png_zopfli": (png_zopfli, lambda r: r["rows"])}
+
 if __name__ == "__main__":
-    if sys.argv[1:] == ["jpeg_trellis"]:
+    if len(sys.argv) == 2 and sys.argv[1] in SECTIONS:
         O.lib()
+        fn, show = SECTIONS[sys.argv[1]]
         path = os.path.join(ROOT, "profiles", "quality.json")
         with open(path) as f:
             rep = json.load(f)
-        rep["jpeg_trellis"] = jpeg_trellis()
+        rep[sys.argv[1]] = fn()
         with open(path, "w") as f:
             json.dump(rep, f, indent=1)
-        print(json.dumps(rep["jpeg_trellis"]["bd_rate_percent"]))
+        print(json.dumps(show(rep[sys.argv[1]])))
     else:
         main()
