@@ -70,7 +70,7 @@ _SYMBOLS = [
     "b200_set_png_lossy", "b200_png_quantize", "b200_set_jpeg_trellis", "b200_set_gif", "b200_gif_decode", "b200_gif_lzw",
     "b200_set_png_resize", "b200_png_resize_samples", "b200_set_webp_lossless_convert", "b200_set_png_interlaced",
     "b200_set_gif_convert", "b200_gif_first_frame", "b200_set_webp_anim", "b200_webp_anim_decode",
-    "b200_set_png_zopfli", "b200_png_lz77_zopfli",
+    "b200_set_png_zopfli", "b200_png_lz77_zopfli", "b200_set_webp_palette",
 ]
 
 
@@ -317,6 +317,12 @@ def set_png_zopfli(on):
     """b200_set_png_zopfli: png_force_zopfli takes the iterated optimal LZ77 parse on every PNG output (1) or is accepted and
     ignored (0, the default).  Any other value is refused with B200_ERR_INVALID_ARGUMENT."""
     return lib().b200_set_png_zopfli(int(on))
+
+
+def set_webp_palette(on):
+    """b200_set_webp_palette: every lossless WebP output also tries the colour-indexing (palette) transform on images of at most 256
+    colours and keeps the smaller file (1), or never does (0, the default).  Any other value is refused with B200_ERR_INVALID_ARGUMENT."""
+    return lib().b200_set_webp_palette(int(on))
 
 
 def png_lz77_zopfli(stream, bpp, stride):

@@ -11,6 +11,7 @@
 #include "../../include/b200_caesium_gif_convert.h"
 #include "../../include/b200_caesium_webp_anim.h"
 #include "../../include/b200_caesium_png_zopfli.h"
+#include "../../include/b200_caesium_webp_palette.h"
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -102,6 +103,7 @@ OptIn g_png_interlaced{"B200_PNG_INTERLACED"};                // Adam7 PNG sourc
 OptIn g_gif_convert{"B200_GIF_CONVERT"};                      // JPEG / PNG / WebP -> GIF and GIF -> JPEG / PNG / WebP on the device
 OptIn g_webp_anim{"B200_WEBP_ANIM"};                          // animated WebP re-encoded on the device
 OptIn g_png_zopfli{"B200_PNG_ZOPFLI"};                        // png_force_zopfli: the iterated optimal LZ77 parse on PNG outputs
+OptIn g_webp_palette{"B200_WEBP_PALETTE"};                    // lossless WebP: the colour-indexing variant for <= 256 colours
 
 // runtime_init is idempotent while initialised, so after b200_shutdown (which frees every slot's device buffers) the next call
 // initialises again: a long-running host can hand the memory of one workload's slots back before starting another
@@ -128,6 +130,8 @@ int entropy_mode()
 
 // asked by png_parse_chunks (png_host.cpp), which every PNG leg goes through
 bool b200::png_interlaced() { return g_png_interlaced.on(); }
+// asked by Vp8lDevice::encode_packed (vp8l_encode.cpp), which every lossless WebP leg goes through
+bool b200::webp_palette() { return g_webp_palette.on(); }
 
 namespace {
 
@@ -891,8 +895,9 @@ b200_status webp_lossless_compress(const uint8_t *in, size_t in_len, const b200_
     if (!v->encode(src, ap, (int)nw, (int)nh, s->stream, out, err)) return make_status(B200_ERR_CUDA, err);
     if (verbose) {
         const std::string kt = tr.kernel_ms();
-        fprintf(stderr, "[b200 trace] webp-lossless %ux%u -> %ux%u: host decode %.3f ms, resize %.3f ms, device encode %.3f ms (analysis wait %.3f, cache bits %d, codes + emission %.3f); kernels ms:%s\n",
-                w, h, nw, nh, ms_between(t0, t1), ms_between(t1, t2), ms_between(t2, std::chrono::steady_clock::now()), v->last_analyse_ms, v->last_cache_bits, v->last_code_ms, kt.c_str());
+        fprintf(stderr, "[b200 trace] webp-lossless %ux%u -> %ux%u: host decode %.3f ms, resize %.3f ms, device encode %.3f ms (analysis wait %.3f, cache bits %d, codes + emission %.3f%s); kernels ms:%s\n",
+                w, h, nw, nh, ms_between(t0, t1), ms_between(t1, t2), ms_between(t2, std::chrono::steady_clock::now()), v->last_analyse_ms, v->last_cache_bits, v->last_code_ms,
+                v->palette_trace().c_str(), kt.c_str());
     }
     return ok_status();
 }
@@ -971,9 +976,9 @@ struct ConvertStages {
     void print(const char *src, uint32_t w, uint32_t h, uint32_t nw, uint32_t nh, const Vp8lDevice *v, const char *stage0) const
     {
         if (!verbose()) return;
-        fprintf(stderr, "[b200 trace] webp-lossless-convert %s %ux%u -> %ux%u: %s %.3f ms, front end %.3f ms, resize %.3f ms, encode %.3f ms (cache bits %d); "
+        fprintf(stderr, "[b200 trace] webp-lossless-convert %s %ux%u -> %ux%u: %s %.3f ms, front end %.3f ms, resize %.3f ms, encode %.3f ms (cache bits %d%s); "
                         "fetched %zu bytes (encoder), sample planes fetched 0\n",
-                src, w, h, nw, nh, stage0, ms[0], ms[1], ms[2], ms[3], v->last_cache_bits, v->last_d2h_bytes);
+                src, w, h, nw, nh, stage0, ms[0], ms[1], ms[2], ms[3], v->last_cache_bits, v->palette_trace().c_str(), v->last_d2h_bytes);
     }
 };
 
@@ -1369,6 +1374,7 @@ int b200_set_png_interlaced(int on) { return g_png_interlaced.set(on); }
 int b200_set_gif_convert(int on) { return g_gif_convert.set(on); }
 int b200_set_webp_anim(int on) { return g_webp_anim.set(on); }
 int b200_set_png_zopfli(int on) { return g_png_zopfli.set(on); }
+int b200_set_webp_palette(int on) { return g_webp_palette.set(on); }
 int b200_set_jpeg_trellis(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; set_jpeg_trellis(on == 1); return B200_OK; }
 
 uint32_t b200_sniff_format(const uint8_t *d, size_t n)

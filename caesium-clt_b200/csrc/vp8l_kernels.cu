@@ -11,6 +11,8 @@
 //   k_vp8l_len          per chunk: bits of every thread's tokens under the chosen codes -> offsets inside the chunk
 //   k_vp8l_scan         chunk sizes -> start bit of every chunk after the header (one CTA)
 //   k_vp8l_emit         LSB-first emission of the tokens with atomic ORs into zeroed words
+// The palette variant (vp8l_palette.cu) writes its packed index image into the residual image and runs everything after
+// k_vp8l_predict over it.
 #include <cuda_runtime.h>
 #include <cstdint>
 #include "vp8l_enc_core.h"
@@ -371,10 +373,17 @@ int launch_vp8l_pack(const uint8_t *r, const uint8_t *g, const uint8_t *b, const
 int launch_vp8l_analyse(const Vp8lBuffers &B, int w, int h, void *stream_)
 {
     cudaStream_t st = (cudaStream_t)stream_;
-    const uint32_t n = (uint32_t)w * (uint32_t)h;
-    const int nchunks = (int)cdiv(n, VP8L_CHUNK), tiles_x = (w + VP8L_TILE - 1) >> VP8L_TILE_BITS, tiles = tiles_x * ((h + VP8L_TILE - 1) >> VP8L_TILE_BITS);
-    cudaMemsetAsync(B.hist, 0, sizeof(uint32_t) * VP8L_NCACHE * VP8L_HIST, st); LT_MARK("memset");
+    const int tiles_x =(w + VP8L_TILE - 1) >> VP8L_TILE_BITS, tiles = tiles_x * ((h + VP8L_TILE - 1) >> VP8L_TILE_BITS);
     k_vp8l_predict<<<tiles, V_THREADS, 0, st>>>(B.argb, w, h, tiles_x, B.res, B.modes); LT_MARK("k_vp8l_predict");
+    return launch_vp8l_analyse_res(B, w, h, stream_);
+}
+
+int launch_vp8l_analyse_res(const Vp8lBuffers &B, int w, int h, void *stream_)
+{
+    cudaStream_t st = (cudaStream_t)stream_;
+    const uint32_t n = (uint32_t)w * (uint32_t)h;
+    const int nchunks = (int)cdiv(n, VP8L_CHUNK);
+    cudaMemsetAsync(B.hist, 0, sizeof(uint32_t) * VP8L_NCACHE * VP8L_HIST, st); LT_MARK("memset");
     k_vp8l_cache_last<<<dim3(nchunks, VP8L_NCACHE - 1), V_THREADS, 0, st>>>(B.res, n, nchunks, B.cache_tab); LT_MARK("k_vp8l_cache_last");
     k_vp8l_cache_carry<<<dim3(cdiv(1 << VP8L_MAX_CACHE_BITS, V_THREADS), VP8L_NCACHE - 1), V_THREADS, 0, st>>>(nchunks, B.cache_tab); LT_MARK("k_vp8l_cache_carry");
     k_vp8l_cache_hits<<<dim3(nchunks, VP8L_NCACHE - 1), 32, 0, st>>>(B.res, n, nchunks, B.cache_tab, B.hits); LT_MARK("k_vp8l_cache_hits");
