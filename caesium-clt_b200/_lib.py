@@ -71,6 +71,7 @@ _SYMBOLS = [
     "b200_set_png_resize", "b200_png_resize_samples", "b200_set_webp_lossless_convert", "b200_set_png_interlaced",
     "b200_set_gif_convert", "b200_gif_first_frame", "b200_set_webp_anim", "b200_webp_anim_decode",
     "b200_set_png_zopfli", "b200_png_lz77_zopfli", "b200_set_webp_palette",
+    "b200_set_webp_bpred", "b200_webp_encode_rgb_bpred", "b200_webp_write_levels_bpred",
 ]
 
 
@@ -89,7 +90,7 @@ def lib():
                   "b200_webp_encode_rgb", "b200_webp_write_levels", "b200_jpeg_encode_coefficients_device",
                   "b200_jpeg_pipe_create", "b200_jpeg_pipe_run", "b200_jpeg_pipe_finish", "b200_jpeg_pipe_fetch", "b200_jpeg_pipe_kernel_times", "b200_png_device_times", "b200_webp_decode", "b200_webp_alpha_chunk", "b200_webp_wrap_alpha", "b200_webp_decode_rgba", "b200_png_quantize",
                   "b200_gif_decode", "b200_gif_lzw", "b200_png_resize_samples", "b200_gif_first_frame", "b200_webp_anim_decode",
-                  "b200_png_lz77_zopfli"):
+                  "b200_png_lz77_zopfli", "b200_webp_encode_rgb_bpred", "b200_webp_write_levels_bpred"):
             getattr(L, f).restype = Status
         L.b200_webp_d2h_bytes.restype = C.c_ulonglong
         L.b200_version.restype = C.c_char_p
@@ -325,6 +326,12 @@ def set_webp_palette(on):
     return lib().b200_set_webp_palette(int(on))
 
 
+def set_webp_bpred(on):
+    """b200_set_webp_bpred: every lossy WebP output lets macroblocks take 4x4 intra prediction (B_PRED) where it scores lower in
+    distortion + lambda * rate (1), or never (0, the default).  Any other value is refused with B200_ERR_INVALID_ARGUMENT."""
+    return lib().b200_set_webp_bpred(int(on))
+
+
 def png_lz77_zopfli(stream, bpp, stride):
     """b200_png_lz77_zopfli: the optimal parse of a filtered stream on the device -> tokens uint32[nt] in png_lz77's format."""
     s = np.ascontiguousarray(stream, dtype=np.uint8).reshape(-1)
@@ -476,6 +483,31 @@ def webp_encode_rgb(rgb, quality, want_stage=False):
                                       levels.ctypes.data_as(C.c_void_p) if want_stage else None, modes.ctypes.data_as(C.c_void_p) if want_stage else None))
     data = _take(outp, outl)
     return (data, levels, modes) if want_stage else data
+
+
+def webp_encode_rgb_bpred(rgb, quality, want_stage=False):
+    """The B_PRED encoder whatever the switch says: planar uint8 [3, h, w] -> .webp bytes (and, if asked, (levels [nmb,25,16],
+    modes [nmb,4], bmodes [nmb,16]))."""
+    rgb = np.ascontiguousarray(rgb, dtype=np.uint8)
+    _, h, w = rgb.shape
+    nmb = ((w + 15) // 16) * ((h + 15) // 16)
+    levels = np.zeros((nmb, 25, 16), np.int16) if want_stage else None
+    modes = np.zeros((nmb, 4), np.uint8) if want_stage else None
+    bmodes = np.zeros((nmb, 16), np.uint8) if want_stage else None
+    p = lambda a: a.ctypes.data_as(C.c_void_p) if a is not None else None
+    outp, outl = C.POINTER(C.c_uint8)(), C.c_size_t()
+    _check(lib().b200_webp_encode_rgb_bpred(p(rgb), w, h, int(quality), C.byref(outp), C.byref(outl), p(levels), p(modes), p(bmodes)))
+    data = _take(outp, outl)
+    return (data, levels, modes, bmodes) if want_stage else data
+
+
+def webp_write_levels_bpred(w, h, quality, levels, modes, bmodes):
+    """Host writer with sub-block modes: (levels [nmb,25,16], modes [nmb,4], bmodes [nmb,16]) -> .webp bytes."""
+    lv = np.ascontiguousarray(levels, dtype=np.int16); md = np.ascontiguousarray(modes, dtype=np.uint8); bm = np.ascontiguousarray(bmodes, dtype=np.uint8)
+    outp, outl = C.POINTER(C.c_uint8)(), C.c_size_t()
+    _check(lib().b200_webp_write_levels_bpred(int(w), int(h), int(quality), lv.ctypes.data_as(C.c_void_p), md.ctypes.data_as(C.c_void_p),
+                                              bm.ctypes.data_as(C.c_void_p), C.byref(outp), C.byref(outl)))
+    return _take(outp, outl)
 
 
 def webp_decode(data):

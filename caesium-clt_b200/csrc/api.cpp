@@ -12,6 +12,7 @@
 #include "../../include/b200_caesium_webp_anim.h"
 #include "../../include/b200_caesium_png_zopfli.h"
 #include "../../include/b200_caesium_webp_palette.h"
+#include "../../include/b200_caesium_webp_bpred.h"
 #include <atomic>
 #include <chrono>
 #include <condition_variable>
@@ -104,6 +105,7 @@ OptIn g_gif_convert{"B200_GIF_CONVERT"};                      // JPEG / PNG / We
 OptIn g_webp_anim{"B200_WEBP_ANIM"};                          // animated WebP re-encoded on the device
 OptIn g_png_zopfli{"B200_PNG_ZOPFLI"};                        // png_force_zopfli: the iterated optimal LZ77 parse on PNG outputs
 OptIn g_webp_palette{"B200_WEBP_PALETTE"};                    // lossless WebP: the colour-indexing variant for <= 256 colours
+OptIn g_webp_bpred{"B200_WEBP_BPRED"};                        // lossy WebP: 4x4 intra prediction (B_PRED) by rate and distortion
 
 // runtime_init is idempotent while initialised, so after b200_shutdown (which frees every slot's device buffers) the next call
 // initialises again: a long-running host can hand the memory of one workload's slots back before starting another
@@ -132,6 +134,8 @@ int entropy_mode()
 bool b200::png_interlaced() { return g_png_interlaced.on(); }
 // asked by Vp8lDevice::encode_packed (vp8l_encode.cpp), which every lossless WebP leg goes through
 bool b200::webp_palette() { return g_webp_palette.on(); }
+// asked by WebpDevice::encode_planes (webp_device.cu), which every lossy WebP leg goes through
+bool b200::webp_bpred() { return g_webp_bpred.on(); }
 
 namespace {
 
@@ -1375,6 +1379,7 @@ int b200_set_gif_convert(int on) { return g_gif_convert.set(on); }
 int b200_set_webp_anim(int on) { return g_webp_anim.set(on); }
 int b200_set_png_zopfli(int on) { return g_png_zopfli.set(on); }
 int b200_set_webp_palette(int on) { return g_webp_palette.set(on); }
+int b200_set_webp_bpred(int on) { return g_webp_bpred.set(on); }
 int b200_set_jpeg_trellis(int on) { if (on < 0 || on > 1) return B200_ERR_INVALID_ARGUMENT; set_jpeg_trellis(on == 1); return B200_OK; }
 
 uint32_t b200_sniff_format(const uint8_t *d, size_t n)
@@ -1903,6 +1908,18 @@ b200_status b200_webp_encode_rgb(const uint8_t *rgb, int w, int h, int quality, 
     if (!s->webp_dev()->encode_host_rgb(rgb, w, h, quality, s->stream, v, err, levels, modes)) return make_status(B200_ERR_CUDA, err);
     return give(v, out, out_len);
 }
+b200_status b200_webp_encode_rgb_bpred(const uint8_t *rgb, int w, int h, int quality, uint8_t **out, size_t *out_len, int16_t *levels, uint8_t *modes, uint8_t *bmodes)
+{
+    if (!rgb || !out || !out_len || w < 1 || h < 1 || w > 16383 || h > 16383) return make_status(B200_ERR_INVALID_ARGUMENT, "invalid argument");
+    *out = nullptr; *out_len = 0;
+    std::string err;
+    if (!ensure_runtime(err)) return make_status(B200_ERR_NO_DEVICE, err);
+    SlotLease s(-1);
+    if (!s) return s.failure();
+    std::vector<uint8_t> v;
+    if (!s->webp_dev()->encode_host_rgb(rgb, w, h, quality, s->stream, v, err, levels, modes, bmodes, true)) return make_status(B200_ERR_CUDA, err);
+    return give(v, out, out_len);
+}
 b200_status b200_webp_decode(const uint8_t *in, size_t in_len, int *width, int *height, uint8_t **rgb)
 {
     if (!in || !width || !height || !rgb) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
@@ -1937,6 +1954,13 @@ b200_status b200_webp_write_levels(int w, int h, int quality, const int16_t *lev
     if (!levels || !modes || !out || !out_len) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
     std::vector<uint8_t> v;
     if (!vp8_write_file(w, h, vp8_qindex(quality < 0 ? 0 : quality > 100 ? 100 : quality), levels, modes, v)) return make_status(B200_ERR_INVALID_ARGUMENT, "frame cannot be written as VP8");
+    return give(v, out, out_len);
+}
+b200_status b200_webp_write_levels_bpred(int w, int h, int quality, const int16_t *levels, const uint8_t *modes, const uint8_t *bmodes, uint8_t **out, size_t *out_len)
+{
+    if (!levels || !modes || !bmodes || !out || !out_len) return make_status(B200_ERR_INVALID_ARGUMENT, "null argument");
+    std::vector<uint8_t> v;
+    if (!vp8_write_file(w, h, vp8_qindex(quality < 0 ? 0 : quality > 100 ? 100 : quality), levels, modes, v, bmodes)) return make_status(B200_ERR_INVALID_ARGUMENT, "frame cannot be written as VP8");
     return give(v, out, out_len);
 }
 unsigned long long b200_webp_d2h_bytes(void) { return webp_d2h_bytes_total(); }

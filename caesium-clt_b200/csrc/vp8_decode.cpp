@@ -6,137 +6,12 @@
 #include <algorithm>
 #include <cstring>
 #include "vp8_tables.h"
+#include "vp8_bpred_core.h"
 
 namespace b200 {
 namespace {
 
-// 4x4 sub-block mode probabilities of key frames, indexed [mode above][mode to the left][tree node] (RFC 6386 section 11.5's
-// kf_bmode_probs in libwebp's mode numbering: DC, TM, VE, HE, RD, VR, LD, VL, HD, HU).  Normative constants.
-const uint8_t kBModesProba[10][10][9] = {
-    {
-     {231, 120, 48, 89, 115, 113, 120, 152, 112},
-     {152, 179, 64, 126, 170, 118, 46, 70, 95},
-     {175, 69, 143, 80, 85, 82, 72, 155, 103},
-     {56, 58, 10, 171, 218, 189, 17, 13, 152},
-     {114, 26, 17, 163, 44, 195, 21, 10, 173},
-     {121, 24, 80, 195, 26, 62, 44, 64, 85},
-     {144, 71, 10, 38, 171, 213, 144, 34, 26},
-     {170, 46, 55, 19, 136, 160, 33, 206, 71},
-     {63, 20, 8, 114, 114, 208, 12, 9, 226},
-     {81, 40, 11, 96, 182, 84, 29, 16, 36},
-    },
-    {
-     {134, 183, 89, 137, 98, 101, 106, 165, 148},
-     {72, 187, 100, 130, 157, 111, 32, 75, 80},
-     {66, 102, 167, 99, 74, 62, 40, 234, 128},
-     {41, 53, 9, 178, 241, 141, 26, 8, 107},
-     {74, 43, 26, 146, 73, 166, 49, 23, 157},
-     {65, 38, 105, 160, 51, 52, 31, 115, 128},
-     {104, 79, 12, 27, 217, 255, 87, 17, 7},
-     {87, 68, 71, 44, 114, 51, 15, 186, 23},
-     {47, 41, 14, 110, 182, 183, 21, 17, 194},
-     {66, 45, 25, 102, 197, 189, 23, 18, 22},
-    },
-    {
-     {88, 88, 147, 150, 42, 46, 45, 196, 205},
-     {43, 97, 183, 117, 85, 38, 35, 179, 61},
-     {39, 53, 200, 87, 26, 21, 43, 232, 171},
-     {56, 34, 51, 104, 114, 102, 29, 93, 77},
-     {39, 28, 85, 171, 58, 165, 90, 98, 64},
-     {34, 22, 116, 206, 23, 34, 43, 166, 73},
-     {107, 54, 32, 26, 51, 1, 81, 43, 31},
-     {68, 25, 106, 22, 64, 171, 36, 225, 114},
-     {34, 19, 21, 102, 132, 188, 16, 76, 124},
-     {62, 18, 78, 95, 85, 57, 50, 48, 51},
-    },
-    {
-     {193, 101, 35, 159, 215, 111, 89, 46, 111},
-     {60, 148, 31, 172, 219, 228, 21, 18, 111},
-     {112, 113, 77, 85, 179, 255, 38, 120, 114},
-     {40, 42, 1, 196, 245, 209, 10, 25, 109},
-     {88, 43, 29, 140, 166, 213, 37, 43, 154},
-     {61, 63, 30, 155, 67, 45, 68, 1, 209},
-     {100, 80, 8, 43, 154, 1, 51, 26, 71},
-     {142, 78, 78, 16, 255, 128, 34, 197, 171},
-     {41, 40, 5, 102, 211, 183, 4, 1, 221},
-     {51, 50, 17, 168, 209, 192, 23, 25, 82},
-    },
-    {
-     {138, 31, 36, 171, 27, 166, 38, 44, 229},
-     {67, 87, 58, 169, 82, 115, 26, 59, 179},
-     {63, 59, 90, 180, 59, 166, 93, 73, 154},
-     {40, 40, 21, 116, 143, 209, 34, 39, 175},
-     {47, 15, 16, 183, 34, 223, 49, 45, 183},
-     {46, 17, 33, 183, 6, 98, 15, 32, 183},
-     {57, 46, 22, 24, 128, 1, 54, 17, 37},
-     {65, 32, 73, 115, 28, 128, 23, 128, 205},
-     {40, 3, 9, 115, 51, 192, 18, 6, 223},
-     {87, 37, 9, 115, 59, 77, 64, 21, 47},
-    },
-    {
-     {104, 55, 44, 218, 9, 54, 53, 130, 226},
-     {64, 90, 70, 205, 40, 41, 23, 26, 57},
-     {54, 57, 112, 184, 5, 41, 38, 166, 213},
-     {30, 34, 26, 133, 152, 116, 10, 32, 134},
-     {39, 19, 53, 221, 26, 114, 32, 73, 255},
-     {31, 9, 65, 234, 2, 15, 1, 118, 73},
-     {75, 32, 12, 51, 192, 255, 160, 43, 51},
-     {88, 31, 35, 67, 102, 85, 55, 186, 85},
-     {56, 21, 23, 111, 59, 205, 45, 37, 192},
-     {55, 38, 70, 124, 73, 102, 1, 34, 98},
-    },
-    {
-     {125, 98, 42, 88, 104, 85, 117, 175, 82},
-     {95, 84, 53, 89, 128, 100, 113, 101, 45},
-     {75, 79, 123, 47, 51, 128, 81, 171, 1},
-     {57, 17, 5, 71, 102, 57, 53, 41, 49},
-     {38, 33, 13, 121, 57, 73, 26, 1, 85},
-     {41, 10, 67, 138, 77, 110, 90, 47, 114},
-     {115, 21, 2, 10, 102, 255, 166, 23, 6},
-     {101, 29, 16, 10, 85, 128, 101, 196, 26},
-     {57, 18, 10, 102, 102, 213, 34, 20, 43},
-     {117, 20, 15, 36, 163, 128, 68, 1, 26},
-    },
-    {
-     {102, 61, 71, 37, 34, 53, 31, 243, 192},
-     {69, 60, 71, 38, 73, 119, 28, 222, 37},
-     {68, 45, 128, 34, 1, 47, 11, 245, 171},
-     {62, 17, 19, 70, 146, 85, 55, 62, 70},
-     {37, 43, 37, 154, 100, 163, 85, 160, 1},
-     {63, 9, 92, 136, 28, 64, 32, 201, 85},
-     {75, 15, 9, 9, 64, 255, 184, 119, 16},
-     {86, 6, 28, 5, 64, 255, 25, 248, 1},
-     {56, 8, 17, 132, 137, 255, 55, 116, 128},
-     {58, 15, 20, 82, 135, 57, 26, 121, 40},
-    },
-    {
-     {164, 50, 31, 137, 154, 133, 25, 35, 218},
-     {51, 103, 44, 131, 131, 123, 31, 6, 158},
-     {86, 40, 64, 135, 148, 224, 45, 183, 128},
-     {22, 26, 17, 131, 240, 154, 14, 1, 209},
-     {45, 16, 21, 91, 64, 222, 7, 1, 197},
-     {56, 21, 39, 155, 60, 138, 23, 102, 213},
-     {83, 12, 13, 54, 192, 255, 68, 47, 28},
-     {85, 26, 85, 85, 128, 128, 32, 146, 171},
-     {18, 11, 7, 63, 144, 171, 4, 4, 246},
-     {35, 27, 10, 146, 174, 171, 12, 26, 128},
-    },
-    {
-     {190, 80, 35, 99, 180, 80, 126, 54, 45},
-     {85, 126, 47, 87, 176, 51, 41, 20, 32},
-     {101, 75, 128, 139, 118, 146, 116, 128, 85},
-     {56, 41, 15, 176, 236, 85, 37, 9, 62},
-     {71, 30, 17, 119, 118, 255, 17, 18, 138},
-     {101, 38, 60, 138, 55, 70, 43, 26, 142},
-     {146, 36, 19, 30, 171, 255, 97, 27, 20},
-     {138, 45, 61, 62, 219, 1, 81, 188, 64},
-     {32, 41, 20, 117, 151, 142, 20, 21, 163},
-     {112, 19, 12, 61, 195, 128, 48, 4, 24},
-    },
-};
-// the sub-block mode tree in the same numbering (leaf = -mode)
-const int8_t kYModesIntra4[18] = {-0, 1, -1, 2, -2, 3, 4, 6, -3, 5, -4, -5, -6, 7, -7, 8, -8, -9};
-enum { B_DC = 0, B_TM, B_VE, B_HE, B_RD, B_VR, B_LD, B_VL, B_HD, B_HU };
+enum { B_DC = 0 };
 enum { DC_PRED = 0, TM_PRED = 1, V_PRED = 2, H_PRED = 3 };
 const uint8_t kZigzag4[16] = {0, 1, 4, 8, 5, 2, 3, 6, 9, 12, 13, 10, 7, 11, 14, 15};
 const uint8_t kBands4[17] = {0, 1, 2, 3, 6, 4, 5, 6, 6, 6, 6, 6, 6, 6, 6, 7, 0};
@@ -199,46 +74,6 @@ void iwht(const int16_t *in, int16_t *out /* 16 blocks x 16 coefficients: DC slo
 }
 
 // ---- intra prediction on a bordered work area (row -1 / column -1 hold the neighbours) ---------------------------------------------
-#define AVG3(a, b, c) ((uint8_t)(((a) + 2 * (b) + (c) + 2) >> 2))
-#define AVG2(a, b) ((uint8_t)(((a) + (b) + 1) >> 1))
-void pred4(int mode, uint8_t *d, int s)
-{   // d = top-left pixel of the 4x4 block inside the work area, s = its stride; top row d[-s + (-1..7)], left column d[-1 + y * s]
-    const uint8_t *top = d - s;
-    const int X = top[-1], A = top[0], B = top[1], C = top[2], D = top[3], E = top[4], F = top[5], G = top[6], H = top[7];
-    const int I = d[-1], J = d[-1 + s], K = d[-1 + 2 * s], L = d[-1 + 3 * s];
-#define DST(x, y) d[(x) + (y) * s]
-    switch (mode) {
-        case B_DC: { int dc = 4; for (int i = 0; i < 4; i++) dc += top[i] + d[-1 + i * s]; dc >>= 3; for (int y = 0; y < 4; y++) for (int x = 0; x < 4; x++) DST(x, y) = (uint8_t)dc; break; }
-        case B_TM: for (int y = 0; y < 4; y++) for (int x = 0; x < 4; x++) DST(x, y) = clip8(top[x] + d[-1 + y * s] - X); break;
-        case B_VE: { const uint8_t v[4] = {AVG3(X, A, B), AVG3(A, B, C), AVG3(B, C, D), AVG3(C, D, E)}; for (int y = 0; y < 4; y++) for (int x = 0; x < 4; x++) DST(x, y) = v[x]; break; }
-        case B_HE: { const uint8_t v[4] = {AVG3(X, I, J), AVG3(I, J, K), AVG3(J, K, L), AVG3(K, L, L)}; for (int y = 0; y < 4; y++) for (int x = 0; x < 4; x++) DST(x, y) = v[y]; break; }
-        case B_RD:
-            DST(0, 3) = AVG3(J, K, L); DST(1, 3) = DST(0, 2) = AVG3(I, J, K); DST(2, 3) = DST(1, 2) = DST(0, 1) = AVG3(X, I, J);
-            DST(3, 3) = DST(2, 2) = DST(1, 1) = DST(0, 0) = AVG3(A, X, I); DST(3, 2) = DST(2, 1) = DST(1, 0) = AVG3(B, A, X);
-            DST(3, 1) = DST(2, 0) = AVG3(C, B, A); DST(3, 0) = AVG3(D, C, B); break;
-        case B_VR:
-            DST(0, 0) = DST(1, 2) = AVG2(X, A); DST(1, 0) = DST(2, 2) = AVG2(A, B); DST(2, 0) = DST(3, 2) = AVG2(B, C); DST(3, 0) = AVG2(C, D);
-            DST(0, 3) = AVG3(K, J, I); DST(0, 2) = AVG3(J, I, X); DST(0, 1) = DST(1, 3) = AVG3(I, X, A); DST(1, 1) = DST(2, 3) = AVG3(X, A, B);
-            DST(2, 1) = DST(3, 3) = AVG3(A, B, C); DST(3, 1) = AVG3(B, C, D); break;
-        case B_LD:
-            DST(0, 0) = AVG3(A, B, C); DST(1, 0) = DST(0, 1) = AVG3(B, C, D); DST(2, 0) = DST(1, 1) = DST(0, 2) = AVG3(C, D, E);
-            DST(3, 0) = DST(2, 1) = DST(1, 2) = DST(0, 3) = AVG3(D, E, F); DST(3, 1) = DST(2, 2) = DST(1, 3) = AVG3(E, F, G);
-            DST(3, 2) = DST(2, 3) = AVG3(F, G, H); DST(3, 3) = AVG3(G, H, H); break;
-        case B_VL:
-            DST(0, 0) = AVG2(A, B); DST(1, 0) = DST(0, 2) = AVG2(B, C); DST(2, 0) = DST(1, 2) = AVG2(C, D); DST(3, 0) = DST(2, 2) = AVG2(D, E);
-            DST(0, 1) = AVG3(A, B, C); DST(1, 1) = DST(0, 3) = AVG3(B, C, D); DST(2, 1) = DST(1, 3) = AVG3(C, D, E); DST(3, 1) = DST(2, 3) = AVG3(D, E, F);
-            DST(3, 2) = AVG3(E, F, G); DST(3, 3) = AVG3(F, G, H); break;
-        case B_HU:
-            DST(0, 0) = AVG2(I, J); DST(2, 0) = DST(0, 1) = AVG2(J, K); DST(2, 1) = DST(0, 2) = AVG2(K, L); DST(1, 0) = AVG3(I, J, K);
-            DST(3, 0) = DST(1, 1) = AVG3(J, K, L); DST(3, 1) = DST(1, 2) = AVG3(K, L, L);
-            DST(3, 2) = DST(2, 2) = DST(0, 3) = DST(1, 3) = DST(2, 3) = DST(3, 3) = (uint8_t)L; break;
-        default: /* B_HD */
-            DST(0, 0) = DST(2, 1) = AVG2(I, X); DST(0, 1) = DST(2, 2) = AVG2(J, I); DST(0, 2) = DST(2, 3) = AVG2(K, J); DST(0, 3) = AVG2(L, K);
-            DST(3, 0) = AVG3(A, B, C); DST(2, 0) = AVG3(X, A, B); DST(1, 0) = DST(3, 1) = AVG3(I, X, A); DST(1, 1) = DST(3, 2) = AVG3(J, I, X);
-            DST(1, 2) = DST(3, 3) = AVG3(K, J, I); DST(1, 3) = AVG3(L, K, J); break;
-    }
-#undef DST
-}
 // whole-block predictors (16x16 luma / 8x8 chroma); have_top / have_left only matter for DC (the other modes read the 127 / 129 borders)
 void pred_block(int mode, uint8_t *d, int s, int n, bool have_top, bool have_left)
 {
@@ -483,9 +318,9 @@ int webp_decode_chunks(const uint8_t *f, size_t flen, const uint8_t *alph, size_
                 for (int y = 0; y < 4; y++) {
                     int ym = left_modes[y];
                     for (int x = 0; x < 4; x++) {
-                        const uint8_t *prob = kBModesProba[tm[x]][ym];
-                        int i = kYModesIntra4[br.bit(prob[0])];
-                        while (i > 0) i = kYModesIntra4[2 * i + br.bit(prob[i])];
+                        const uint8_t *prob = VP8_BMODES_PROBA[tm[x]][ym];
+                        int i = VP8_YMODES_INTRA4[br.bit(prob[0])];
+                        while (i > 0) i = VP8_YMODES_INTRA4[2 * i + br.bit(prob[i])];
                         ym = -i; tm[x] = (uint8_t)ym; imodes[y * 4 + x] = (uint8_t)ym;
                     }
                     left_modes[y] = (uint8_t)ym;
@@ -575,10 +410,14 @@ int webp_decode_chunks(const uint8_t *f, size_t flen, const uint8_t *alph, size_
                 } else memset(yd - WS - 1, 127, 21);
                 for (int j = 0; j < 16; j++) yd[j * WS - 1] = mx > 0 ? Y[(size_t)(my * 16 + j) * ys + (size_t)mx * 16 - 1] : 129;
                 if (i4) {
-                    for (int r = 1; r < 4; r++) memcpy(yd + (4 * r - 1) * WS + 16, yd - WS + 16, 4);      // the top-right pixels, replicated below
+                    uint8_t top[21], left[16], e[13], p[16];
+                    memcpy(top, yd - WS - 1, 21);
+                    for (int j = 0; j < 16; j++) left[j] = yd[j * WS - 1];
                     for (int n = 0; n < 16; n++) {
                         uint8_t *d = yd + (n >> 2) * 4 * WS + (n & 3) * 4;
-                        pred4(imodes[n], d, WS);
+                        vp8bp_edges(top, left, yd, WS, n & 3, n >> 2, e);
+                        vp8bp_pred4(imodes[n], e, p);
+                        for (int y = 0; y < 4; y++) memcpy(d + y * WS, p + 4 * y, 4);
                         idct_add(coeffs + n * 16, d, WS);
                     }
                 } else {

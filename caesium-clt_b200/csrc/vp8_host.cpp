@@ -4,6 +4,7 @@
 #include <cstring>
 #include "vp8_tables.h"
 #include "vp8_tokens_core.h"
+#include "vp8_bpred_core.h"
 
 namespace b200 {
 
@@ -89,7 +90,10 @@ void host_tokens(int mbw, int mbh, bool use_skip, const int16_t *levels, const u
 {
     const size_t nmb = (size_t)mbw * mbh;
     std::vector<uint32_t> mask(nmb);
-    for (size_t mb = 0; mb < nmb; mb++) mask[mb] = (use_skip && modes[4 * mb + 2]) ? 0u : vt::mb_mask(levels + mb * 400);
+    std::vector<uint8_t> y2top(nmb), y2left(nmb);
+    for (size_t mb = 0; mb < nmb; mb++) mask[mb] = (use_skip && modes[4 * mb + 2]) ? 0u : vt::mb_mask(levels + mb * 400, modes[4 * mb] == 4);
+    for (int x = 0; x < mbw; x++) vt::y2_carry_col(mask.data(), modes, mbw, mbh, x, y2top.data());
+    for (int y = 0; y < mbh; y++) vt::y2_carry_row(mask.data(), modes, mbw, y, y2left.data());
     tokens.resize(nmb * 128 + vt::kMaxDecisionsPerMb);
     TokenRecorder tc{reinterpret_cast<uint32_t (*)[2]>(cnt), tokens};
     for (int my = 0; my < mbh; my++)
@@ -97,7 +101,7 @@ void host_tokens(int mbw, int mbh, bool use_skip, const int16_t *levels, const u
             const size_t mb = (size_t)my * mbw + mx;
             if (use_skip && modes[4 * mb + 2]) continue;
             tc.begin_mb();
-            vt::walk_mb(tc, levels + mb * 400, my ? mask[mb - mbw] : 0u, mx ? mask[mb - 1] : 0u);
+            vt::walk_mb(tc, levels + mb * 400, vt::with_y2(my ? mask[mb - mbw] : 0u, y2top[mb]), vt::with_y2(mx ? mask[mb - 1] : 0u, y2left[mb]), modes[4 * mb] == 4);
         }
     tokens.resize(tc.size());
 }
@@ -116,22 +120,28 @@ bool vp8_frame_uses_skip(int width, int height, const uint8_t *modes)
     return false;
 }
 
-bool vp8_write_file(int width, int height, int qindex, const int16_t *levels, const uint8_t *modes, std::vector<uint8_t> &out)
+bool vp8_write_file(int width, int height, int qindex, const int16_t *levels, const uint8_t *modes, std::vector<uint8_t> &out, const uint8_t *bmodes)
 {
     if (width < 1 || height < 1 || width > 16383 || height > 16383) return false;
     const int mbw = (width + 15) >> 4, mbh = (height + 15) >> 4;
+    for (int i = 0; i < mbw * mbh; i++) {                            // modes index the sub-block mode probabilities: refuse any out of range
+        if (modes[4 * i] > 4 || modes[4 * i + 1] > 3) return false;
+        if (modes[4 * i] == 4) { if (!bmodes) return false; for (int k = 0; k < 16; k++) if (bmodes[16 * i + k] > 9) return false; }
+    }
     std::vector<uint32_t> cnt((size_t)kNumProbs * 2, 0);
     std::vector<uint16_t> tokens;
     host_tokens(mbw, mbh, vp8_frame_uses_skip(width, height, modes), levels, modes, cnt.data(), tokens);
-    return vp8_write_file_tokens(width, height, qindex, modes, cnt.data(), tokens.data(), tokens.size(), out);
+    return vp8_write_file_tokens(width, height, qindex, modes, cnt.data(), tokens.data(), tokens.size(), out, bmodes);
 }
 
-bool vp8_write_file_tokens(int width, int height, int qindex, const uint8_t *modes, const uint32_t *cnt, const uint16_t *tokens, size_t ntokens, std::vector<uint8_t> &out)
+bool vp8_write_file_tokens(int width, int height, int qindex, const uint8_t *modes, const uint32_t *cnt, const uint16_t *tokens, size_t ntokens, std::vector<uint8_t> &out,
+                           const uint8_t *bmodes)
 {
     const int mbw = (width + 15) >> 4, mbh = (height + 15) >> 4, nmb = mbw * mbh;
     if (width < 1 || height < 1 || width > 16383 || height > 16383) return false;
-    int nskip = 0;
-    for (int i = 0; i < nmb; i++) nskip += modes[4 * i + 2];
+    int nskip = 0, nbpred = 0;
+    for (int i = 0; i < nmb; i++) { nskip += modes[4 * i + 2]; nbpred += modes[4 * i] == 4; }
+    if (nbpred && !bmodes) return false;
     const bool use_skip = nskip > 0;
     int skip_p = (int)(((long long)(nmb - nskip) * 255) / nmb); if (skip_p < 1) skip_p = 1; if (skip_p > 255) skip_p = 255;
     // ---- token probabilities (13.4): from the tallies of this frame's tree decisions, replace a default wherever the frame's
@@ -147,7 +157,8 @@ bool vp8_write_file_tokens(int width, int height, int qindex, const uint8_t *mod
         if (newp != oldp && change < keep) { probs[i] = (uint8_t)newp; updated[i] = 1; }
     }
     // ---- first partition: frame header (RFC 6386 9.2-9.11, 19.2) and the per-macroblock modes (19.3)
-    BoolWriter hd((size_t)kNumProbs * 9 + (size_t)nmb * 8 + 256);
+    // decisions: a 16x16 macroblock takes at most 8, a B_PRED one at most 3 + 16 * 7 (sub-block modes HD and HU are 7 deep) + 3
+    BoolWriter hd((size_t)kNumProbs * 9 + (size_t)nmb * 8 + (size_t)nbpred * 120 + 256);
     hd.literal(0, 1);                   // color_space
     hd.literal(0, 1);                   // clamping_type
     hd.literal(0, 1);                   // segmentation_enabled
@@ -162,13 +173,31 @@ bool vp8_write_file_tokens(int width, int height, int qindex, const uint8_t *mod
     for (int i = 0; i < kNumProbs; i++) { hd.put(updated[i], VP8_COEF_UPDATE_PROBS[i]); if (updated[i]) hd.literal(probs[i], 8); }
     hd.literal(use_skip, 1);            // mb_no_coeff_skip
     if (use_skip) hd.literal(skip_p, 8);
+    // sub-block mode contexts (11.3): the modes above / to the left, a 16x16 macroblock's luma mode standing for all its sub-blocks,
+    // DC beyond the frame's edges
+    std::vector<uint8_t> top_modes((size_t)mbw * 4, 0);
+    uint8_t left_modes[4] = {0, 0, 0, 0};
     for (int i = 0; i < nmb; i++) {
         const int ym = modes[4 * i], uvm = modes[4 * i + 1];
+        uint8_t *tm = &top_modes[(size_t)(i % mbw) * 4];
+        if (i % mbw == 0) memset(left_modes, 0, 4);
         if (use_skip) hd.put(modes[4 * i + 2], skip_p);
-        hd.put(1, 145);                                                                 // a 16x16 mode, not B_PRED
-        const bool tm_or_h = ym == 1 || ym == 3;
-        hd.put(tm_or_h, 156);
-        if (tm_or_h) hd.put(ym == 1, 128); else hd.put(ym == 2, 163);
+        if (ym == 4) {
+            hd.put(0, 145);                                                             // B_PRED
+            const uint8_t *bm = bmodes + (size_t)i * 16;
+            for (int k = 0; k < 16; k++) {
+                uint8_t p[8], b[8];
+                const int n = vp8bp_bmode_bits(tm[k & 3], left_modes[k >> 2], bm[k], p, b);
+                for (int j = 0; j < n; j++) hd.put(b[j], p[j]);
+                tm[k & 3] = left_modes[k >> 2] = bm[k];
+            }
+        } else {
+            hd.put(1, 145);                                                             // a 16x16 mode, not B_PRED
+            const bool tm_or_h = ym == 1 || ym == 3;
+            hd.put(tm_or_h, 156);
+            if (tm_or_h) hd.put(ym == 1, 128); else hd.put(ym == 2, 163);
+            memset(tm, ym, 4); memset(left_modes, ym, 4);
+        }
         hd.put(uvm != 0, 142);
         if (uvm != 0) { hd.put(uvm != 2, 114); if (uvm != 2) hd.put(uvm != 3, 183); }
     }

@@ -97,19 +97,21 @@ template <class Sink> VT_HD int put_block(Sink &w, const int16_t *lv, int type, 
     return 1;
 }
 
-// which of a macroblock's 25 blocks have coded coefficients: bit 0 Y2, bits 1..16 the Y blocks (AC only: their DC lives in Y2),
-// bits 17..20 U, 21..24 V
-VT_HD uint32_t mb_mask(const int16_t *lv)
+// which of a macroblock's 25 blocks have coded coefficients: bit 0 Y2, bits 1..16 the Y blocks (AC only: their DC lives in Y2; all
+// 16 coefficients in a B_PRED macroblock, which has no Y2), bits 17..20 U, 21..24 V
+VT_HD uint32_t mb_mask(const int16_t *lv, bool bpred = false)
 {
-    uint32_t m = last_nonzero(lv, 0) >= 0 ? 1u : 0u;
-    for (int b = 0; b < 16; b++) if (last_nonzero(lv + 16 * (1 + b), 1) >= 0) m |= 1u << (1 + b);
+    uint32_t m = !bpred && last_nonzero(lv, 0) >= 0 ? 1u : 0u;
+    for (int b = 0; b < 16; b++) if (last_nonzero(lv + 16 * (1 + b), bpred ? 0 : 1) >= 0) m |= 1u << (1 + b);
     for (int b = 0; b < 8; b++) if (last_nonzero(lv + 16 * (17 + b), 0) >= 0) m |= 1u << (17 + b);
     return m;
 }
 
 // every residual block of one macroblock in coding order (13): the contexts of its first row / column of blocks come from the masks
-// of the macroblock above / to the left (0 at the frame edge and for a skipped macroblock)
-template <class Sink> VT_HD void walk_mb(Sink &sk, const int16_t *lv, uint32_t top, uint32_t left_mask)
+// of the macroblock above / to the left (0 at the frame edge and for a skipped macroblock).  Bit 0 of `top` / `left_mask` is the Y2
+// context, which is NOT the neighbour's own bit 0: a decoder updates it on 16x16-coded macroblocks only (y2_carry).  A B_PRED
+// macroblock codes no Y2 and its luma blocks as type 3 from coefficient 0.
+template <class Sink> VT_HD void walk_mb(Sink &sk, const int16_t *lv, uint32_t top, uint32_t left_mask, bool bpred = false)
 {
     uint8_t t[9], l[9];
     for (int x = 0; x < 4; x++) { t[x] = (uint8_t)((top >> (1 + 12 + x)) & 1u); l[x] = (uint8_t)((left_mask >> (1 + 4 * x + 3)) & 1u); }
@@ -118,11 +120,36 @@ template <class Sink> VT_HD void walk_mb(Sink &sk, const int16_t *lv, uint32_t t
         t[6 + x] = (uint8_t)((top >> (21 + 2 + x)) & 1u); l[6 + x] = (uint8_t)((left_mask >> (21 + 2 * x + 1)) & 1u);
     }
     t[8] = (uint8_t)(top & 1u); l[8] = (uint8_t)(left_mask & 1u);
-    t[8] = l[8] = (uint8_t)put_block(sk, lv, 1, 0, t[8] + l[8]);
-    for (int b = 0; b < 16; b++) { const int x = b & 3, y = b >> 2; t[x] = l[y] = (uint8_t)put_block(sk, lv + 16 * (1 + b), 0, 1, t[x] + l[y]); }
+    if (!bpred) t[8] = l[8] = (uint8_t)put_block(sk, lv, 1, 0, t[8] + l[8]);
+    for (int b = 0; b < 16; b++) { const int x = b & 3, y = b >> 2; t[x] = l[y] = (uint8_t)put_block(sk, lv + 16 * (1 + b), bpred ? 3 : 0, bpred ? 0 : 1, t[x] + l[y]); }
     for (int c = 0; c < 2; c++)
         for (int b = 0; b < 4; b++) { const int x = 4 + 2 * c + (b & 1), y = 4 + 2 * c + (b >> 1); t[x] = l[y] = (uint8_t)put_block(sk, lv + 16 * (17 + 4 * c + b), 2, 0, t[x] + l[y]); }
 }
+
+// The Y2 contexts of macroblock mb = y * mbw + x: the Y2 flag of the nearest 16x16-coded macroblock above in the same column
+// (y2top[mb]) and to the left in the same row (y2left[mb]), 0 if there is none.  A skipped 16x16 macroblock's flag is 0 (its mask
+// is); a B_PRED macroblock, skipped or not, leaves the flag alone.  modes[4 * mb] == 4 marks B_PRED.  Every column and every row
+// is an independent walk: the device runs one thread per column and one per row.
+VT_HD void y2_carry_col(const uint32_t *mask, const uint8_t *modes, int mbw, int mbh, int col, uint8_t *y2top)
+{
+    uint8_t c = 0;
+    for (int y = 0; y < mbh; y++) {
+        const int mb = y * mbw + col;
+        y2top[mb] = c;
+        if (modes[4 * mb] != 4) c = (uint8_t)(mask[mb] & 1u);
+    }
+}
+VT_HD void y2_carry_row(const uint32_t *mask, const uint8_t *modes, int mbw, int row, uint8_t *y2left)
+{
+    uint8_t c = 0;
+    for (int x = 0; x < mbw; x++) {
+        const int mb = row * mbw + x;
+        y2left[mb] = c;
+        if (modes[4 * mb] != 4) c = (uint8_t)(mask[mb] & 1u);
+    }
+}
+// a neighbour's mask with bit 0 replaced by the carried Y2 context
+VT_HD uint32_t with_y2(uint32_t mask, uint8_t y2) { return (mask & ~1u) | (y2 & 1u); }
 
 VT_HD uint16_t rec_node(int s, bool bit) { return (uint16_t)((s << 1) | (bit ? 1 : 0)); }
 VT_HD uint16_t rec_fixed(bool bit, int prob) { return (uint16_t)(0x8000u | ((unsigned)prob << 1) | (bit ? 1u : 0u)); }

@@ -215,7 +215,8 @@ b200_status b200_webp_decode(const uint8_t *in, size_t in_len, int *width, int *
 b200_status b200_webp_decode_rgba(const uint8_t *in, size_t in_len, int *width, int *height, uint8_t **rgb, uint8_t **alpha);
 /* diagnostics: bytes the WebP leg has copied device -> host since the library was loaded (modes, tallies and decision records per frame) */
 unsigned long long b200_webp_d2h_bytes(void);
-/* host only: boolean-code levels + modes (layout above) into a .webp file -- the entropy-coding half on its own */
+/* host only: boolean-code levels + modes (layout above) into a .webp file -- the entropy-coding half on its own.  A ymode of 4 (B_PRED)
+ * needs sub-block modes and is refused here with B200_ERR_INVALID_ARGUMENT (b200_webp_write_levels_bpred writes it). */
 b200_status b200_webp_write_levels(int w, int h, int quality, const int16_t *levels, const uint8_t *modes, uint8_t **out, size_t *out_len);
 /* libwebp's quality -> quantiser index curve and the six dequantisation factors (y1 dc/ac, y2 dc/ac, uv dc/ac) it selects */
 int b200_webp_qindex(int quality, int factors[6]);

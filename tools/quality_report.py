@@ -3,7 +3,7 @@ writes the same bytes as the CUDA path -- that equality is what the GPU tests as
 quality number, standard tables, optimised Huffman, progressive) and, for the WebP leg, libwebp (Pillow) at equal -q.
 The reference (libcaesium -> mozjpeg with trellis quantisation, deringing and scan optimisation) is expected to produce
 SMALLER files than ours at equal -q; libjpeg-turbo, its parent without those three, is the closest stand-in that exists here.
-CPU only.  Writes profiles/quality.json.  usage: python tools/quality_report.py [jpeg_trellis | png_zopfli]
+CPU only.  Writes profiles/quality.json.  usage: python tools/quality_report.py [jpeg_trellis | png_zopfli | webp_bpred]
 (with a section's name, only that section is recomputed and the others are kept as they are)"""
 import io
 import json
@@ -94,6 +94,7 @@ def main():
             out["png_lossy"].append(row)
     out["jpeg_trellis"] = jpeg_trellis()
     out["png_zopfli"] = png_zopfli()
+    out["webp_bpred"] = webp_bpred()
     with open(os.path.join(ROOT, "profiles", "quality.json"), "w") as f:
         json.dump(out, f, indent=1)
     for r in out["jpeg"] + out["webp"] + out["png_lossy"] + out["jpeg_trellis"]["rows"]:
@@ -152,7 +153,39 @@ def png_zopfli():
                     "emits with the switch and flag on) and zlib level 9; CPU twin, identical to the device's bytes", "rows": rows}
 
 
-SECTIONS = {"jpeg_trellis": (jpeg_trellis, lambda r: r["bd_rate_percent"]), "png_zopfli": (png_zopfli, lambda r: r["rows"])}
+def webp_bpred():
+    """Lossy WebP with B_PRED (b200_set_webp_bpred; the twin writes the device's bytes) against the switch-off encoder and libwebp
+    (Pillow, method 4): bytes and RGB PSNR (decoded by libwebp) at q 30..90, and the BD-rates (bytes at equal PSNR) per image.  Lambda
+    is libwebp's 4x4 one, untuned; the reference samples are held out all the same."""
+    from oracle import webp_bpred as B
+    from test_webp_bpred_host import bd_rate
+    srcs = [(f"synthetic 1280x720 seed {i}", synth_rgb(1280, 720, i)) for i in range(3)]
+    for n in ("j0.JPG", "j1.jpg", "w0.webp", "w1.webp"):
+        srcs.append((f"reference samples/{n}", decode_rgb(open(os.path.join(ROOT, "tests", "golden", "reference_samples", n), "rb").read())))
+    rows, bd_off, bd_lib = [], {}, {}
+    for name, rgb in srcs:
+        planar = np.ascontiguousarray(rgb.transpose(2, 0, 1))
+        curve = {"off": ([], []), "bpred": ([], []), "libwebp": ([], [])}
+        for q in (30, 45, 60, 75, 90):
+            b = io.BytesIO(); Image.fromarray(rgb).save(b, "WEBP", quality=q, method=4)
+            files = {"off": O.webp_encode(planar, q)[0], "bpred": B.webp_bpred_encode(planar, q), "libwebp": b.getvalue()}
+            row = {"input": name, "quality": q}
+            for k, data in files.items():
+                p = psnr(decode_rgb(data), rgb)
+                curve[k][0].append(len(data)); curve[k][1].append(p)
+                row[f"{k}_bytes"], row[f"{k}_psnr"] = len(data), round(p, 3)
+            rows.append(row)
+        # a BD-rate needs the two PSNR ranges to overlap; where they do not, there is none to state
+        bd = lambda a, b: round(float(bd_rate(*curve[a], *curve[b])), 3) if max(min(curve[a][1]), min(curve[b][1])) < min(max(curve[a][1]), max(curve[b][1])) else None
+        bd_off[name], bd_lib[name] = bd("off", "bpred"), bd("libwebp", "bpred")
+    return {"what": "lossy WebP with B_PRED vs the switch-off encoder and vs libwebp (Pillow, method 4) at equal -q; PSNR of RGB against "
+                    "the source pixels, decoded by libwebp; BD-rate: Bjontegaard delta of bytes at equal PSNR over q 30-90 (negative = B_PRED smaller), "
+                    "null where the PSNR ranges do not overlap",
+            "rows": rows, "bd_rate_percent_vs_switch_off": bd_off, "bd_rate_percent_vs_libwebp": bd_lib}
+
+
+SECTIONS = {"jpeg_trellis": (jpeg_trellis, lambda r: r["bd_rate_percent"]), "png_zopfli": (png_zopfli, lambda r: r["rows"]),
+            "webp_bpred": (webp_bpred, lambda r: [r["bd_rate_percent_vs_switch_off"], r["bd_rate_percent_vs_libwebp"]])}
 
 if __name__ == "__main__":
     if len(sys.argv) == 2 and sys.argv[1] in SECTIONS:
